@@ -1,4 +1,4 @@
-"""amphion_b200 — B200-native (sm_100a) vocoder-inference hot path for Amphion recipes.
+"""amphion_b200 — H100-native (sm_90a) vocoder-inference hot path for Amphion recipes.
 
 Host code is Python with PyTorch tensors at the boundary; all arithmetic runs
 in hand-written CUDA behind the C ABI declared in ``include/amphion_b200.h``

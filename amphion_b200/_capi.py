@@ -61,7 +61,7 @@ _I64P = C.POINTER(C.c_int64)
 SIGNATURES = {
     "ab_last_error": (C.c_char_p, []),
     "ab_version": (C.c_int, []),
-    "ab_device_is_sm100": (C.c_int, []),
+    "ab_device_is_sm90": (C.c_int, []),
     "ab_generator_create": (C.c_int, [C.POINTER(GeneratorConfig), C.POINTER(_P)]),
     "ab_generator_destroy": (None, [_P]),
     "ab_generator_param_bytes": (C.c_size_t, [_P]),

@@ -1,4 +1,4 @@
-"""Build libamphion_b200.so in-tree with nvcc for sm_100a (no torch headers, plain C ABI).
+"""Build libamphion_b200.so in-tree with nvcc for sm_90a (H100; no torch headers, plain C ABI).
 
 Each .cu is compiled to an object in `_build/` (in parallel, only when it or a header changed) and the
 objects are linked into the shared library next to this file, so the `.so` travels with the tree."""
@@ -14,9 +14,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libamphion_b200.so")
-SOURCES = ["ab_capi.cu", "ab_kernels_fp32.cu", "ab_kernels_tc.cu", "ab_kernels_rb.cu", "ab_kernels_gemmconv.cu",
-           "ab_mel.cu", "ab_pcm.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+SOURCES = ["ab_capi.cu", "ab_kernels_fp32.cu", "ab_kernels_tc.cu", "ab_mel.cu", "ab_pcm.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc() -> str:

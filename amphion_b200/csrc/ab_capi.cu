@@ -97,7 +97,7 @@ struct ab_generator {
   int precision = AB_PREC_FP32;
   int hop = 1;
   int launches = 0;
-  int rb_mode = 2;          // "resblock_fusion" option; AB_RB in the environment sets the initial value
+  int rb_mode = 2;          // "resblock_fusion" option
   std::vector<cudaEvent_t> tail_events;   // ab_generator_set_tail_events: consumed by the next forward
   int64_t source_frames = 0;              // NSF-HiFiGAN: frames of the f0 track of the next forward (0 = covers the mel)
 
@@ -223,11 +223,11 @@ extern "C" {
 const char* ab_last_error(void) { return g_err; }
 int ab_version(void) { return 100; }
 
-int ab_device_is_sm100(void) {
+int ab_device_is_sm90(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10;
+  return major == 9;
 }
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
@@ -236,7 +236,6 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
   if (rc != AB_OK) return rc;
   ab_generator* g = new ab_generator();
   g->cfg = *cfg;
-  if (const char* e = getenv("AB_RB")) g->rb_mode = std::min(std::max(atoi(e), 0), 4);
   const bool big = cfg->kind == AB_GEN_BIGVGAN;
   const bool has_beta = cfg->activation == AB_ACT_SNAKEBETA;
   const int c0 = cfg->upsample_initial_channel;
@@ -414,7 +413,7 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
     return fail(AB_ERR_ARG, "finalize: unknown precision %d", precision);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (precision != AB_PREC_FP32) {
-    if (!ab_device_is_sm100()) return fail(AB_ERR_UNSUPPORTED, "finalize: tensor-core precision needs an sm_100 device");
+    if (!ab_device_is_sm90()) return fail(AB_ERR_UNSUPPORTED, "finalize: tensor-core precision needs an sm_90 (Hopper) device");
     for (size_t i = 0; i < g->slots.size(); ++i) {
       Slot& s = g->slots[i];
       int rc = AB_OK;
@@ -507,7 +506,7 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
   return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
-         NIMG * align_up(stage_max_image_bytes(g, B, T), 256) + align_up(rb_scratch_bytes(), 256);
+         NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
 }
 
 int ab_generator_last_launches(const ab_generator* g) { return g ? g->launches : 0; }
@@ -576,6 +575,9 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
 }
 
 
+// block mode (resblock_fusion 2) is chosen when it computes at most this many tile rows per output row
+static constexpr double kChainMaxRecompute = 1.5;
+
 static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
                         const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
                         size_t workspace_bytes, void* stream) {
@@ -598,7 +600,6 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   for (int i = 0; i < NIMG; ++i)
     img[i] = reinterpret_cast<uint16_t*>(static_cast<char*>(dev_workspace) + NBUF * bufsz + i * imgsz);
   uint16_t *U16 = img[0], *P16[2] = {img[1], img[2]}, *R16 = img[3];
-  float* rb_scratch = reinterpret_cast<float*>(static_cast<char*>(dev_workspace) + NBUF * bufsz + NIMG * imgsz);
   const uint16_t* r_img = nullptr;   // operand image of lrelu(stage input, 0.1) when the previous stage emitted it
   float *R[2] = {buf[0], buf[1]}, *U = buf[2], *P[2] = {buf[3], buf[4]}, *TMP = buf[5], *ACT = buf[6];
   const bool big = g->cfg.kind == AB_GEN_BIGVGAN;
@@ -685,39 +686,6 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     prof_end();
     return r;
   };
-
-  // a chain of `np` (c1[, c2]) pairs of one ResBlock on the persistent fused kernel (ab_kernels_rb.cu)
-  auto rb_chain = [&](const BlockRef& blk, int p0, int np, const float* x, const uint16_t* ximg, float* y, int C, int Tn,
-                      const float* acc_prev, float out_div, uint16_t* yimg, int split = 0) -> int {
-    RbParams rp;
-    memset(&rp, 0, sizeof(rp));
-    const bool pair = !blk.c2.empty();
-    rp.x = x; rp.ximg = ximg; rp.y = y; rp.acc_prev = acc_prev; rp.yimg = yimg;
-    rp.npairs = np; rp.nconv = pair ? 2 : 1;
-    for (int q = 0; q < np; ++q) {
-      rp.dil[q] = blk.c1[p0 + q].d;
-      rp.w[q * rp.nconv] = g->tcptr(blk.c1[p0 + q].w);
-      rp.bias[q * rp.nconv] = g->fptr(blk.c1[p0 + q].b);
-      if (pair) {
-        rp.w[q * 2 + 1] = g->tcptr(blk.c2[p0 + q].w);
-        rp.bias[q * 2 + 1] = g->fptr(blk.c2[p0 + q].b);
-      }
-    }
-    rp.B = (int)B; rp.C = C; rp.T = Tn; rp.k = blk.k;
-    rp.slope = 0.1f; rp.img_slope = 0.1f; rp.out_div = out_div; rp.precision = g->precision;
-    rp.scratch = rb_scratch;
-    rp.split = split;
-    ++launches;
-    const double el = (double)B * C * Tn;
-    prof_begin(0, 2.0 * el * C * blk.k * rp.nconv * np,
-               4.0 * (el * (2 + (acc_prev != nullptr)) + (double)rp.nconv * np * C * C * blk.k));
-    const int r = launch_rb(rp, st);
-    prof_end();
-    return r;
-  };
-  // AB_RB: 0 = per-pair kernel of ab_kernels_tc.cu only, 1 = persistent kernel one pair per launch,
-  //        2 (default) = persistent kernel, whole block fused when the cost model prefers it, 3 = always fused
-  const int rb_mode = g->rb_mode;
 
   // wide single conv on the streaming tensor-core kernel (operand image in)
   auto gs_conv = [&](const ConvRef& c, const uint16_t* ximg, float* y, int Tn, const float* residual,
@@ -819,27 +787,33 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       const uint16_t* cur_img = u_img;
       int pp = 0;
       const int nd = (int)blk.dil.size();
-      const bool blk_rb = use_tc && !big && rb_mode > 0 && rb_supported(C, blk.k) && tc_conv_supported(C, blk.k);
-      if (blk_rb && rb_mode >= 2 && nd <= AB_RB_MAX_PAIRS) {
-        // whole block in one launch when the halo recompute costs less than the per-pair HBM round trips; with the
-        // residual stream resident in TMEM (split accumulators) when that is cheaper still
+      if (use_tc && !big && g->rb_mode >= 2 && nd <= AB_TC_CHAIN_MAX_PAIRS) {
+        // whole block in one launch when the halo recompute costs less than the per-pair HBM round trips of x
         const int ncv = blk.c2.empty() ? 1 : 2;
-        const double fused = rb_cost_per_row(C, blk.k, blk.dil.data(), nd, ncv, 0);
-        const double fsplit = rb_cost_per_row(C, blk.k, blk.dil.data(), nd, ncv, 1);
-        double split = 0.0;
-        for (int p = 0; p < nd; ++p) split += rb_cost_per_row(C, blk.k, &blk.dil[p], 1, ncv, 0);
-        int plan = 0;   // 0 per pair, 1 fused, 2 fused + split accumulators
-        if (rb_mode == 3) plan = fused > 0.0 ? 1 : 0;
-        else if (rb_mode == 4) plan = fsplit > 0.0 ? 2 : (fused > 0.0 ? 1 : 0);
-        else {
-          double best = split;
-          if (fused > 0.0 && fused < best) { best = fused; plan = 1; }
-          if (fsplit > 0.0 && fsplit < best) { best = fsplit; plan = 2; }
-        }
-        if (plan) {
+        const double recompute = tc_chain_recompute(C, blk.k, blk.dil.data(), nd, ncv);
+        if (recompute > 0.0 && (g->rb_mode >= 3 || recompute <= kChainMaxRecompute)) {
           const bool stage_img = j == nk - 1 && i + 1 < g->stages.size();
-          rc = rb_chain(blk, 0, nd, U, u_img, Rout, C, Tn, j > 0 ? Rout : nullptr, j == nk - 1 ? (float)nk : 1.0f,
-                        stage_img ? R16 : nullptr, plan == 2);
+          TcChainParams cp;
+          memset(&cp, 0, sizeof(cp));
+          cp.x = U; cp.ximg = u_img; cp.y = Rout; cp.acc_prev = j > 0 ? Rout : nullptr;
+          cp.yimg = stage_img ? R16 : nullptr;
+          for (int q = 0; q < nd; ++q) {
+            cp.dil[q] = blk.dil[q];
+            cp.w[q * ncv] = g->tcptr(blk.c1[q].w);
+            cp.bias[q * ncv] = g->fptr(blk.c1[q].b);
+            if (ncv == 2) {
+              cp.w[q * 2 + 1] = g->tcptr(blk.c2[q].w);
+              cp.bias[q * 2 + 1] = g->fptr(blk.c2[q].b);
+            }
+          }
+          cp.npairs = nd; cp.nconv = ncv; cp.B = (int)B; cp.C = C; cp.T = Tn; cp.k = blk.k;
+          cp.slope = 0.1f; cp.img_slope = 0.1f; cp.out_div = j == nk - 1 ? (float)nk : 1.0f;
+          cp.precision = g->precision;
+          ++launches;
+          const double el = (double)B * C * Tn;
+          prof_begin(0, 2.0 * el * C * blk.k * ncv * nd, 4.0 * (el * (2 + (j > 0)) + (double)ncv * nd * C * C * blk.k));
+          rc = launch_tc_chain(cp, st);
+          prof_end();
           if (rc != AB_OK) return rc;
           if (stage_img) stage_img_written = true;
           continue;
@@ -861,12 +835,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
         // wide layers (C > 256): streaming kernel, BigVGAN only (it needs the activation as an operand image)
         const bool blk_gs = tc && big && !blk_tc && g->slots[blk.c1[0].w].tc_kind == 3;
         if (!big) {
-          if (blk_rb) {
-            rc = rb_chain(blk, p, 1, cur, cur_img, dst, C, Tn, accp, div, dst_img);
-            if (rc != AB_OK) return rc;
-            cur_img = dst_img;
-            if (stage_img) stage_img_written = true;
-          } else if (blk_tc) {
+          if (blk_tc) {
             rc = tc_convs(blk.c1[p], pair ? &blk.c2[p] : nullptr, cur, dst, C, Tn, 0.1f, 0.1f, cur, accp, div,
                           cur_img, dst_img);
             if (rc != AB_OK) return rc;

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libamphion_b200 (sm_100a only).
+// Shared host/device helpers for libamphion_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -71,8 +71,9 @@ struct ConvTParams {
 };
 
 #ifdef __CUDACC__
-// Packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2: one issue slot for two lanes of work).  A pair lives in an
-// aligned 64-bit register; 8- and 16-byte shared-memory loads deliver pairs without any move.
+// fp32 pairs in an aligned 64-bit register, so that 8- and 16-byte shared-memory loads deliver pairs without any
+// move.  Hopper has no packed fp32 arithmetic: each op is two scalar IEEE round-to-nearest ops (the explicit
+// intrinsics keep the compiler from contracting a mul and an add into one FMA).
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pk2(float lo, float hi) {
   f32x2 r;
@@ -83,14 +84,14 @@ __device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ float hsum2(f32x2 v) {
   float lo, hi;
@@ -99,9 +100,9 @@ __device__ __forceinline__ float hsum2(f32x2 v) {
 }
 
 __device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 
 #endif

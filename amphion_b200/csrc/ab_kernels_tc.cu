@@ -1,35 +1,31 @@
-// tcgen05 implicit-GEMM convolution for the ResBlock / AMPBlock convs (sm_100a).
+// wgmma implicit-GEMM convolutions (sm_90a): the ResBlock / AMPBlock convs, ConvTranspose1d and the
+// non-square / wide Conv1d layers.
 //
-// Mapping (DESIGN.md §4):  D[t, co] += sum_{tap j} A_j[t, ci] * W_j[co, ci]
-//   M = time (128 rows per MMA, m M-tiles per CTA), N = C_out (<= 256), K = C_in per tap.
-//   A (activations): fp16/bf16 in shared memory, SWIZZLE_32B K-major rows [ci/16][row][32 B]: a tap
-//     shift of j*d time steps is a +j*d*32 B move of the descriptor start address, so one resident
-//     activation tile serves all k taps.
-//   B (weights): pre-packed in global memory in exactly the shared-memory image and streamed stage
-//     by stage with cp.async.bulk (TMA, 1-D) into an mbarrier ring.
-//   D: fp32 in TMEM, m * Np columns; read back with tcgen05.ld for the epilogues.
-// Phases per CTA tile:
-//   prologue   activated operand tile -> smem A.  Either a register-free cp.async burst from the fp16
-//              operand image the producing kernel left in HBM (ximg), or fp32 loads + lrelu + cvt.
-//   conv1      k * C/16 MMAs per M-tile
-//   epilogue 1 TMEM -> +bias, lrelu, cvt -> A (aliased; zero outside [0,T))      [pair mode only]
-//   conv2      same, dilation 1
-//   epilogue 2 TMEM -> +bias +residual (+branch sum, /nk) -> fp32 y and the fp16 operand image of
-//              lrelu(y) for the next kernel.  The residual / branch-sum tiles are streamed through a
-//              per-warp cp.async ring placed in the (now free) A region.
-// Warp roles: WW worker warps, 1 TMA producer warp, 1 MMA-issue warp.  Configurations:
-//   <8,1>: full tile (m*Np = 512 TMEM columns), one CTA per SM (C = 256: the tile does not fit twice);
-//   <8,2>: half tile (<= 256 columns, <= 113 KB smem, 96 registers), two CTAs per SM so one CTA's
-//          global-memory phases overlap the other's MMA phases (default whenever it fits);
-//   <4,2>, <4,3>: the same with 4 worker warps / third-size tiles (measured slower or equal; knobs only).
+// Mapping (DESIGN.md §4):  D[row, n] += sum_{tap} A[row + shift(tap), ci] * W[tap][n, ci]
+//   M = time rows, N = output channels (<= 256 per N block), K = C_in per tap.
+//   Conv1d ("same", dilation d): row = output time, n = c_out, tap j reads row + j*d.
+//   ConvTranspose1d (stride u, padding (k-u)/2, polyphase):
+//     y[co, s*u - p + phi] = b[co] + sum_m sum_ci act(x)[ci, s - m] * W[ci, co, phi + u*m]
+//     -> row = input time s, virtual channel n = co_local*u + phi, taps m = 0..ceil(k/u)-1; every MAC is useful.
+//   Conv pair (one ResBlock1 step, hifigan.py:93-100): conv1 -> +b1, lrelu -> a shared-memory operand tile ->
+//     conv2 -> +b2 + residual (+ branch sum, / num_kernels) in one launch; the intermediate never leaves the SM.
+//
+// Operands (ab_tc_ptx.cuh): fp16/bf16, K-major 8x16-byte core matrices without swizzle, so a tap is a row shift of
+// the descriptor start and one activation tile serves all taps.
+//   A: streamed in 32-channel chunks [4][rowsA][16 B]: lrelu + cvt of fp32 input in the loader, or a cp.async copy
+//      of the 16-bit operand image the producing kernel left in HBM.
+//   W: pre-packed in global memory in exactly the shared-memory image of one (N block, K chunk, tap) stage and
+//      streamed with cp.async.bulk (TMA 1-D) through an mbarrier ring; thread 0 refills a stage once every warp
+//      has released it.
+//   D: fp32 in the registers of two consumer warpgroups (MT m64 tiles each); the epilogues run on the fragments.
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "ab_tc.cuh"
 #include "ab_tc_ptx.cuh"
-#include "ab_tc_issue.cuh"
+#include "ab_wgmma.cuh"
 
 namespace ab {
 
@@ -37,690 +33,762 @@ using namespace tcx;
 
 namespace {
 
-constexpr int TC_MAX_STAGES = 8;
+constexpr int HC_WG = 2;                      // consumer warpgroups per CTA
+constexpr int HC_THREADS = HC_WG * 128;
+constexpr int HC_STAGES_MAX = 6;
 constexpr int TC_MAX_C = 256;
-constexpr uint32_t TC_SMEM_LIMIT = 227 * 1024;
-constexpr int RING_DEPTH_MAX = 4;             // per-warp residual ring: slots of (16 ch x 32 rows) x 2 tensors
-constexpr uint32_t RING_SLOT_BYTES = 4096;    // 2 KB residual + 2 KB branch sum
+constexpr uint32_t HC_SMEM_1CTA = 227 * 1024;  // N = 256: 128 accumulator registers per thread, one CTA per SM
+constexpr uint32_t HC_SMEM_2CTA = 113 * 1024;  // N <= 128: two CTAs per SM overlap one's loads with the other's MMAs
 
-struct TcGeom {
-  int Np;          // channels padded to 16 (N and K extent)
-  int nkc;         // 32-channel K chunks per tap
-  int m;           // M tiles (128 rows each) per CTA
-  int V;           // valid output rows per CTA tile
-  int rowsA;       // allocated activation rows (multiple of 8)
-  int tiles;       // tiles per sequence
-  int nstages;
-  uint32_t stage_bytes;
-  uint32_t off_w, off_bias, off_bar;  // byte offsets in dynamic smem (A at 0)
-  uint32_t smem_bytes;
-  int hh;          // time of A row 0 is T0 - hh
-  int h2;          // time of the intermediate row 0 is T0 - h2 (pair mode)
-  uint32_t idesc;
-  int tmem_cols;   // TMEM columns to allocate (power of two >= m*Np)
-  int dual;        // 0: full tile, 8 worker warps, 1 CTA/SM; n >= 2: 1/n tile, 4 worker warps, n CTAs per SM
-  int ww;          // worker warps of the chosen configuration (4 or 8)
-  int ring_depth;  // slots per worker warp in the epilogue-2 ring (2..4)
-  int staged;      // 1: epilogue 2 streams residual / branch sum through the cp.async ring (needs T % 4 == 0)
-  int stagger_groups, first_wave;   // first-wave CTAs start (blockIdx % groups) * stagger_cycles late so that the
-  long long stagger_cycles;         // HBM-bound phases of identical tiles do not run in lock-step chip-wide
-  float out_scale; // 1 / out_div (the reference divides, hifigan.py:214; <= 1 ulp apart)
-  int korder;      // MMA issue order within a weight stage: 1 = K-half outer / M-tile inner
-  int skip;        // debug timing experiments (AB_TC_DEBUG_SKIP bitmask): 1 no fp32 y store, 2 no image store, 4 no residual loads
-  long long* dbg;  // debug: per-CTA phase timestamps (AB_TC_DEBUG_TIMING=1), else nullptr
+// m64 tiles per warpgroup: at most 64 accumulator registers per thread below N = 256
+__host__ __device__ constexpr int mt_of(int nw) { return nw >= 128 ? 1 : (nw == 64 ? 2 : 4); }
+
+struct HcArgs {
+  const float* x;          // fp32 input with element strides (used when ximg is null)
+  int64_t xsb, xsc, xst;
+  const uint16_t* ximg;    // operand image [B][c8n_in][Tin][8] of the already activated input, or null
+  float pre_slope;
+  int B, Cin, Cout;
+  const void* w;           // weight image (stages in (N block, K chunk, tap) order)
+  const void* w2;          // pair mode: conv2's image
+  const void* ws[2 * AB_TC_CHAIN_MAX_PAIRS];     // block mode: weight image of step s = pair * nconv + conv
+  const float* bs[2 * AB_TC_CHAIN_MAX_PAIRS];    // block mode: biases (nullable)
+  const float* bias;
+  const float* bias2;      // pair mode
+  float* y;                // [B, Cout, Tout]
+  const float* residual;   // nullable, [B, Cout, Tout]
+  const float* acc_prev;   // nullable, may alias y
+  int post_tanh;
+  uint16_t* yimg;          // nullable: operand image of lrelu(y, img_slope), [B][c8n_out][Tout][8]
+  float img_slope;
 };
 
-constexpr int DBG_BLOCKS = 2048, DBG_SLOTS = 10;   // 0-5 phase stamps, 6 smid, 7 globaltimer, 8 weight-wait cycles, 9 A-wait cycles
+struct HcGeom {
+  int mode;                // 0 conv, 1 conv-transpose, 2 conv pair
+  int NB, cc;              // N blocks; output channels per block
+  int R, V, tiles;         // rows per CTA tile, valid output rows per tile, tiles per sequence
+  int ntaps, d;            // taps of the (first) conv and the row step between them
+  int a0, rowsA, nkc;      // time of A row 0 = tile origin - a0; rows of the A chunk; 32-channel chunks of C_in
+  int h2, rowsI, nkc2;     // pair mode: intermediate row 0 = origin - h2; its rows; conv2's K chunks
+  int c8n_in, c8n_out;
+  int nstages;
+  uint32_t stage_bytes, off_i, off_w, off_bias, off_bar, smem_bytes;
+  int Tin, Tout, u, pad;
+  float out_scale, mid_slope;
+  // block mode (3): nsteps = npairs * nconv convs of one ResBlock; output row r is time origin - H + r, the operand
+  // tiles keep G guard rows on both sides so that every tap shift is a non-negative row offset
+  int nsteps, nconv, H, G, rowsX, k;
+  int dil[AB_TC_CHAIN_MAX_PAIRS];
+};
 
-template <int WW, int MINB, int BF16>
-__global__ void __launch_bounds__(WW * 32 + 64, MINB) tc_conv_kernel(TcConvParams p, TcGeom g) {
-  constexpr int WORKERS = WW * 32;
-  constexpr int NWG = WW / 4;   // worker warps per TMEM lane quarter
+// CHAIN: block mode — the residual stream x_p of a whole ResBlock stays in registers in the accumulator fragment
+// layout (one CTA per SM for the doubled register use); otherwise modes 0-2.
+template <int NW, int BF16, bool CHAIN>
+__global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
+  constexpr int MT = mt_of(NW);
+  constexpr int NACC = NW / 2;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31, wq = (tid >> 5) & 3;
   const int b = blockIdx.x / g.tiles, tile = blockIdx.x - b * g.tiles;
-  const int T0 = tile * g.V;
-  constexpr int bf16 = BF16;
-
-  const uint32_t sA = smem_u32(smem);
-  const uint32_t sW = sA + g.off_w;
-  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);   // [2][Np]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + g.off_bar);
-  const uint32_t bar0 = smem_u32(bars);
+  const int O = tile * g.V;   // output time (conv) / input time (conv-transpose) of row 0
+  const uint32_t sA = smem_u32(smem), sI = sA + g.off_i, sW = sA + g.off_w;
+  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
+  const uint32_t bar0 = smem_u32(smem + g.off_bar);
   auto bar_full = [&](int s) { return bar0 + 8u * s; };
-  auto bar_empty = [&](int s) { return bar0 + 8u * (TC_MAX_STAGES + s); };
-  const uint32_t bar_aready = bar0 + 8u * (2 * TC_MAX_STAGES);
-  const uint32_t bar_accfull = bar0 + 8u * (2 * TC_MAX_STAGES + 1);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TC_MAX_STAGES + 2);
+  auto bar_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
 
-  if (threadIdx.x == 0) {
+  const int total1 = g.NB * g.nkc * g.ntaps;
+  const int total = CHAIN ? g.nsteps * total1 : total1 + (g.mode == 2 ? g.nkc2 * g.ntaps : 0);
+  auto stage_src = [&](int it) -> const uint8_t* {
+    if (CHAIN) return static_cast<const uint8_t*>(p.ws[it / total1]) + (size_t)(it % total1) * g.stage_bytes;
+    return it < total1 ? static_cast<const uint8_t*>(p.w) + (size_t)it * g.stage_bytes
+                       : static_cast<const uint8_t*>(p.w2) + (size_t)(it - total1) * g.stage_bytes;
+  };
+
+  if (tid == 0) {
     for (int s = 0; s < g.nstages; ++s) {
       mbar_init(bar_full(s), 1);
-      mbar_init(bar_empty(s), 1);
+      mbar_init(bar_empty(s), HC_THREADS / 32);
     }
-    mbar_init(bar_aready, WORKERS);
-    mbar_init(bar_accfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    fence_proxy_async();
   }
-  if (warp == WW + 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)g.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  const int nbias = CHAIN ? g.nsteps * NW : g.mode == 2 ? 2 * NW : g.NB * NW;
+  for (int i = tid; i < nbias; i += HC_THREADS) {
+    float v = 0.f;
+    if (CHAIN) {
+      const int st = i / NW, c = i - st * NW;
+      v = (p.bs[st] && c < p.Cout) ? __ldg(p.bs[st] + c) : 0.f;
+    } else if (g.mode == 2) v = i < NW ? ((p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f)
+                                : ((p.bias2 && i - NW < p.Cout) ? __ldg(p.bias2 + i - NW) : 0.f);
+    else v = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
+    bias_s[i] = v;
   }
-  tc_fence_before();
+  if (g.mode == 2 || CHAIN) {   // channels of the intermediate beyond the accumulator width stay zero
+    const int n16 = CHAIN ? g.nkc * 4 * g.rowsX : g.nkc2 * 4 * g.rowsI;
+    for (int i = tid; i < n16; i += HC_THREADS) *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  auto stamp = [&](int slot) {
-    if (g.dbg != nullptr && threadIdx.x == 0 && blockIdx.x < DBG_BLOCKS)
-      g.dbg[blockIdx.x * DBG_SLOTS + slot] = clock64();
-  };
-  if (g.stagger_groups > 1 && (int)blockIdx.x < g.first_wave) {
-    const long long wait = (long long)(blockIdx.x % (unsigned)g.stagger_groups) * g.stagger_cycles;
-    const long long t0 = clock64();
-    while (clock64() - t0 < wait) __nanosleep(500);
-  }
-  stamp(0);
-  if (g.dbg != nullptr && threadIdx.x == 0 && blockIdx.x < DBG_BLOCKS) {   // debug: which SM, absolute time
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-    g.dbg[blockIdx.x * DBG_SLOTS + 6] = smid;
-    long long gt;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(gt));
-    g.dbg[blockIdx.x * DBG_SLOTS + 7] = gt;
+  if (tid == 0) {
+    for (int s = 0; s < g.nstages && s < total; ++s) {
+      mbar_arrive_expect_tx(bar_full(s), g.stage_bytes);
+      bulk_g2s(sW + (uint32_t)s * g.stage_bytes, stage_src(s), g.stage_bytes, bar_full(s));
+    }
   }
 
-  if (warp < WW) {
-    // ===================== worker warps =====================
-    for (int i = threadIdx.x; i < 2 * g.Np; i += WORKERS) {
-      const int which = i / g.Np, c = i - which * g.Np;
-      const float* src = which ? p.b2 : p.b1;
-      bias_s[i] = (src != nullptr && c < p.C) ? __ldg(src + c) : 0.f;
-    }
-    const int c8n = g.Np >> 3;
-    if (p.ximg != nullptr) {
-      // ---- prologue (image): A[row][c8] <- ximg[b][c8][T0 - hh + row], 16 B per unit, zero fill outside [0,T)
-      const uint16_t* xb = p.ximg + (size_t)b * c8n * p.T * 8;
-      for (int c8 = warp; c8 < c8n; c8 += WW) {
-        const uint16_t* xc = xb + (size_t)c8 * p.T * 8;
-        for (int row = lane; row < g.rowsA; row += 32) {
-          const int t = T0 - g.hh + row;
-          const bool ok = t >= 0 && t < p.T;
-          cp_async16(sA + unit_offset(g.rowsA, c8, row), ok ? (const void*)(xc + (size_t)t * 8) : (const void*)xb,
-                     ok ? 16u : 0u);
+  float acc[MT][NACC];
+  int it = 0;
+
+  // the taps of one 32-channel K chunk over the A operand at aBase (aRows rows per c8 plane)
+  auto mma_chunk = [&](uint32_t aBase, int aRows, int ntaps, int tapstep, bool reversed, bool& first) {
+    for (int j = 0; j < ntaps; ++j, ++it) {
+      const int s = it % g.nstages;
+      const uint32_t ph = (uint32_t)(it / g.nstages) & 1u;
+      mbar_wait(bar_full(s), ph);
+      const int shift = reversed ? (ntaps - 1 - j) : j * tapstep;
+      const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
+      wg_fence();
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+          const uint32_t a = aBase + (uint32_t)(2 * ks * aRows + (wg * MT + mt) * 64 + shift) * 16u;
+          const uint32_t w = wS + (uint32_t)(2 * ks * NW) * 16u;
+          Wgmma<NW, BF16>::mma(acc[mt], make_desc(a, (uint32_t)aRows), make_desc(w, (uint32_t)NW), (first && ks == 0) ? 0 : 1);
         }
+      }
+      wg_commit();
+      wg_wait<0>();
+      first = false;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty(s));
+      if (tid == 0 && it + g.nstages < total) {
+        mbar_wait(bar_empty(s), ph);
+        mbar_arrive_expect_tx(bar_full(s), g.stage_bytes);
+        bulk_g2s(wS, stage_src(it + g.nstages), g.stage_bytes, bar_full(s));
+      }
+    }
+  };
+
+  // A chunk kc: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32); zero outside [0, Tin) / C_in
+  auto load_chunk = [&](int kc) {
+    __syncthreads();   // every warp has finished the MMAs that read the previous chunk
+    const int items = 4 * g.rowsA;
+    if (p.ximg != nullptr) {
+      const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
+      for (int idx = tid; idx < items; idx += HC_THREADS) {
+        const int c = idx / g.rowsA, row = idx - c * g.rowsA;
+        const int c8 = kc * 4 + c, t = O - g.a0 + row;
+        const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
+        cp_async16(sA + unit_offset(g.rowsA, c, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
+                   ok ? 16u : 0u);
       }
       cp_async_wait_all();
     } else {
-      // ---- prologue (fp32): A[row][ci] = lrelu(x[b, ci, T0 - hh + row]) (zero outside [0,T) and for ci >= C)
-      // one item = 8 channels x 128 rows; each lane keeps 32 independent loads in flight
-      const int ngrp = (g.rowsA + 127) >> 7;
-      const float* xb = p.x + (int64_t)b * p.C * p.T;
-      for (int item = warp; item < c8n * ngrp; item += WW) {
-        const int c8 = item / ngrp, grp = item - c8 * ngrp;
-        const int row0 = (grp << 7) + lane;
-        float v[4][8];
+      const float* xb = p.x + (int64_t)b * p.xsb;
+      for (int idx = tid; idx < items; idx += HC_THREADS) {
+        const int c = idx / g.rowsA, row = idx - c * g.rowsA;
+        const int t = O - g.a0 + row;
+        const bool ok = t >= 0 && t < g.Tin;
+        float v[8];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int row = row0 + 32 * r;
-          const int t = T0 - g.hh + row;
-          const bool ok = row < g.rowsA && t >= 0 && t < p.T;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int c = c8 * 8 + e;
-            v[r][e] = (ok && c < p.C) ? __ldg(xb + (int64_t)c * p.T + t) : 0.f;
-          }
+        for (int e = 0; e < 8; ++e) {
+          const int ci = kc * 32 + c * 8 + e;
+          v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
         }
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int row = row0 + 32 * r;
-          if (row < g.rowsA) {
-            uint4 q;
-            q.x = pack2t<BF16>(lrelu(v[r][0], p.pre_slope), lrelu(v[r][1], p.pre_slope));
-            q.y = pack2t<BF16>(lrelu(v[r][2], p.pre_slope), lrelu(v[r][3], p.pre_slope));
-            q.z = pack2t<BF16>(lrelu(v[r][4], p.pre_slope), lrelu(v[r][5], p.pre_slope));
-            q.w = pack2t<BF16>(lrelu(v[r][6], p.pre_slope), lrelu(v[r][7], p.pre_slope));
-            *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsA, c8, row)) = q;
-          }
-        }
+        uint4 q;
+        q.x = pack2t<BF16>(v[0], v[1]);
+        q.y = pack2t<BF16>(v[2], v[3]);
+        q.z = pack2t<BF16>(v[4], v[5]);
+        q.w = pack2t<BF16>(v[6], v[7]);
+        *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsA, c, row)) = q;
       }
     }
     fence_proxy_async();
-    mbar_arrive(bar_aready);
-    stamp(1);
+    __syncthreads();
+  };
 
-    const int q4 = warp & 3, hsel = warp >> 2;
-    const int nch = g.Np >> 4;  // 16-column chunks
-    if (p.nconv == 2) {
-      // ---- epilogue 1: intermediate = lrelu(conv1 + b1) -> A (aliased), zero outside [0,T)
-      mbar_wait(bar_accfull, 0, 10);
-      tc_fence_after();
-      stamp(2);
-      for (int i = 0; i < g.m; ++i) {
-        const int row = i * 128 + q4 * 32 + lane;
-        const int t = T0 - g.h2 + row;
-        const bool ok = t >= 0 && t < p.T;
-        for (int ch = hsel; ch < nch; ch += NWG) {
-          uint32_t r[16];
-          tc_ld16(tmem + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(i * g.Np + ch * 16), r);
-          tc_wait_ld();
-          float v[16];
+  // accumulator fragment (m64nNk16, fp32): element [c*4 + 2h + e] of tile mt is row 16*wq + lane/4 + 8h,
+  // column 8c + 2*(lane%4) + e of this warpgroup's mt-th m64 tile
+  auto frag_row = [&](int mt, int h) { return (wg * MT + mt) * 64 + wq * 16 + (lane >> 2) + 8 * h; };
+  const int col_l = 2 * (lane & 3);
+
+  // y = ((acc + bias) + residual + acc_prev) * out_scale [tanh] ; yimg = cvt(lrelu(y, img_slope))
+  auto epilogue_conv = [&](int nb, const float* bias_blk) {
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float a = __uint_as_float(r[e]) + bias_s[ch * 16 + e];
-            v[e] = ok ? lrelu(a, p.mid_slope) : 0.f;
-          }
+    for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint4 q;
-            q.x = pack2t<BF16>(v[8 * h + 0], v[8 * h + 1]);
-            q.y = pack2t<BF16>(v[8 * h + 2], v[8 * h + 3]);
-            q.z = pack2t<BF16>(v[8 * h + 4], v[8 * h + 5]);
-            q.w = pack2t<BF16>(v[8 * h + 6], v[8 * h + 7]);
-            *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsA, ch * 2 + h, row)) = q;
+      for (int h = 0; h < 2; ++h) {
+        const int row = frag_row(mt, h), t = O + row;
+        if (row >= g.V || t >= g.Tout) continue;
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c) {
+          const int co = nb * NW + c * 8 + col_l;
+          float ve[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            ve[e] = 0.f;
+            if (co + e < p.Cout) {
+              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
+              float v = acc[mt][c * 4 + 2 * h + e] + bias_blk[c * 8 + col_l + e];
+              if (p.residual) v += __ldg(p.residual + idx);
+              if (p.acc_prev) v += p.acc_prev[idx];
+              v *= g.out_scale;
+              if (p.post_tanh) v = tanhf(v);
+              p.y[idx] = v;
+              ve[e] = v;
+            }
           }
+          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
+            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
         }
       }
-      tc_fence_before();
-      fence_proxy_async();
-      mbar_arrive(bar_aready);
-      stamp(3);
     }
-    // ---- epilogue 2: y = ((acc + bias) + residual + acc_prev) / out_div ; yimg = cvt(lrelu(y, img_slope))
-    mbar_wait(bar_accfull, (uint32_t)(p.nconv - 1), 11);
-    tc_fence_after();
-    stamp(4);
-    const float* bias2 = bias_s + (p.nconv == 2 ? g.Np : 0);
-    const int64_t bCT = (int64_t)b * p.C * p.T;
-    if (g.staged) {
-      // All MMAs have completed, so the A region is free: each warp streams the residual / branch-sum
-      // values of its own (32 rows x 16 channels) items through a private cp.async ring there.
-      const bool has_res = p.residual != nullptr && !(g.skip & 4), has_acc = p.acc_prev != nullptr && !(g.skip & 4);
-      const int nchw = (nch - hsel + NWG - 1) / NWG;     // column chunks owned by this warp
-      const int nitems = g.m * nchw;
-      const int RD = g.ring_depth;
-      uint8_t* ring = smem + (size_t)warp * ((size_t)RD * RING_SLOT_BYTES);
-      const uint32_t ring_u32 = smem_u32(ring);
-      // item = (M-tile i, 16-column chunk ch); no divisions in the loop: both the issue side and the consume
-      // side walk (i, ch, slot) incrementally.  The four 16-byte units a lane copies per item are
-      // (channel c0 + 4k, rows 4*r4 .. 4*r4+3), k = 0..3.
-      const int r4 = lane & 7, c0 = lane >> 3;
-      const uint32_t sm_lane = (uint32_t)(c0 * 128 + r4 * 16);
-      const int64_t g_lane = bCT + (int64_t)c0 * p.T + 4 * r4;
-      const int64_t kT4 = 4 * (int64_t)p.T;
-      int ii = 0, ich = hsel, islot = 0;             // issue cursor
-      auto issue = [&]() {
-        const int tb = T0 + ii * 128 + q4 * 32;
-        const uint32_t slot = ring_u32 + (uint32_t)islot * RING_SLOT_BYTES + sm_lane;
-        const int64_t base = g_lane + (int64_t)(ich * 16) * p.T + tb;
-        const bool tok = tb + 4 * r4 < p.T;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const bool ok = tok && (ich * 16 + c0 + 4 * k) < p.C;
-          const int64_t off = base + k * kT4;
-          if (has_res) cp_async16(slot + (uint32_t)(k * 512), ok ? p.residual + off : p.residual, ok ? 16u : 0u);
-          if (has_acc) cp_async16(slot + 2048u + (uint32_t)(k * 512), ok ? p.acc_prev + off : p.acc_prev, ok ? 16u : 0u);
-        }
-        cp_async_commit();
-        ich += NWG;
-        if (ich >= nch) { ich = hsel; ++ii; }
-        islot = islot + 1 == RD ? 0 : islot + 1;
-      };
-      int issued = 0;
-      for (; issued < RD - 1; ++issued) {
-        if (issued < nitems) issue(); else cp_async_commit();
-      }
-      int i = 0, ch = hsel, cslot = 0;               // consume cursor
-      for (int it = 0; it < nitems; ++it) {
-        if (issued < nitems) { issue(); ++issued; } else cp_async_commit();
-        uint32_t r[16];
-        tc_ld16(tmem + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(i * g.Np + ch * 16), r);
-        if (RD == 4) cp_async_wait_group<3>(); else if (RD == 3) cp_async_wait_group<2>(); else cp_async_wait_group<1>();
-        __syncwarp();
-        tc_wait_ld();
-        const float* rs = reinterpret_cast<const float*>(ring + (size_t)cslot * RING_SLOT_BYTES);
-        const int row = i * 128 + q4 * 32 + lane;
-        const int t = T0 + row;
-        const bool ok = row < g.V && t < p.T;
-        const bool full = ch * 16 + 16 <= p.C;
-        float bv[16];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 b4 = *reinterpret_cast<const float4*>(bias2 + ch * 16 + 4 * q);
-          bv[4 * q] = b4.x; bv[4 * q + 1] = b4.y; bv[4 * q + 2] = b4.z; bv[4 * q + 3] = b4.w;
-        }
-        float* yp = p.y + bCT + (int64_t)(ch * 16) * p.T + t;
-        float v[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          float a = __uint_as_float(r[e]) + bv[e];
-          if (has_res) a += rs[e * 32 + lane];
-          if (has_acc) a += rs[512 + e * 32 + lane];
-          a *= g.out_scale;
-          v[e] = a;
-          if (ok && (full || ch * 16 + e < p.C) && !(g.skip & 1)) *yp = a;
-          yp += p.T;
-        }
-        if (p.yimg != nullptr && ok && !(g.skip & 2)) {
-          uint16_t* yi = p.yimg + (((size_t)b * c8n + (size_t)ch * 2) * p.T + (size_t)t) * 8;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint4 q;
-            q.x = pack2t<BF16>(lrelu(v[8 * h + 0], p.img_slope), lrelu(v[8 * h + 1], p.img_slope));
-            q.y = pack2t<BF16>(lrelu(v[8 * h + 2], p.img_slope), lrelu(v[8 * h + 3], p.img_slope));
-            q.z = pack2t<BF16>(lrelu(v[8 * h + 4], p.img_slope), lrelu(v[8 * h + 5], p.img_slope));
-            q.w = pack2t<BF16>(lrelu(v[8 * h + 6], p.img_slope), lrelu(v[8 * h + 7], p.img_slope));
-            *reinterpret_cast<uint4*>(yi + (size_t)h * p.T * 8) = q;
-          }
-        }
-        ch += NWG;
-        if (ch >= nch) { ch = hsel; ++i; }
-        cslot = cslot + 1 == RD ? 0 : cslot + 1;
-        __syncwarp();
+  };
+
+  if constexpr (CHAIN) {
+    // operand tile X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row
+    const int n16 = g.nkc * 4 * g.rowsX;
+    if (p.ximg != nullptr) {
+      const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
+      for (int idx = tid; idx < n16; idx += HC_THREADS) {
+        const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX;
+        const int t = O - g.H - g.G + row;
+        const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
+        cp_async16(sA + unit_offset(g.rowsX, c8, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
+                   ok ? 16u : 0u);
       }
       cp_async_wait_all();
     } else {
-      for (int i = 0; i < g.m; ++i) {
-        const int row = i * 128 + q4 * 32 + lane;
-        const int t = T0 + row;
-        const bool ok = row < g.V && t < p.T;
-        for (int ch = hsel; ch < nch; ch += NWG) {
-          uint32_t r[16];
-          tc_ld16(tmem + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(i * g.Np + ch * 16), r);
-          float res[16], acp[16];
+      const float* xb = p.x + (int64_t)b * p.xsb;
+      for (int idx = tid; idx < n16; idx += HC_THREADS) {
+        const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX;
+        const int t = O - g.H - g.G + row;
+        const bool ok = t >= 0 && t < g.Tin;
+        float v[8];
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int co = ch * 16 + e;
-            const bool w = ok && co < p.C;
-            const int64_t off = bCT + (int64_t)co * p.T + t;
-            res[e] = (w && p.residual) ? __ldg(p.residual + off) : 0.f;
-            acp[e] = (w && p.acc_prev) ? __ldg(p.acc_prev + off) : 0.f;
+        for (int e = 0; e < 8; ++e) {
+          const int ci = c8 * 8 + e;
+          v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
+        }
+        uint4 q;
+        q.x = pack2t<BF16>(v[0], v[1]);
+        q.y = pack2t<BF16>(v[2], v[3]);
+        q.z = pack2t<BF16>(v[4], v[5]);
+        q.w = pack2t<BF16>(v[6], v[7]);
+        *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsX, c8, row)) = q;
+      }
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // residual stream in the fragment layout: xr = x at (row, column) of this thread's accumulators
+    float xr[MT][NACC];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = O - g.H + frag_row(mt, h);
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = c * 8 + col_l + e;
+            xr[mt][c * 4 + 2 * h + e] = (t >= 0 && t < g.Tin && co < p.Cout) ? __ldg(p.x + ((int64_t)b * p.Cout + co) * g.Tin + t) : 0.f;
           }
-          tc_wait_ld();
-          float v[16];
+      }
+    // lrelu(v, slope) of the fragment -> operand tile at base (rows offset by G), zero outside [0, T)
+    auto store_tile = [&](uint32_t off, const float (&v)[MT][NACC], const float* bb) {
+      __syncthreads();   // ResBlock2 (one conv per step) overwrites the tile its own MMAs just read
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int co = ch * 16 + e;
-            float a = __uint_as_float(r[e]) + bias2[co];
-            a += res[e];
-            a += acp[e];
-            a *= g.out_scale;
-            v[e] = a;
-            if (ok && co < p.C) p.y[bCT + (int64_t)co * p.T + t] = a;
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frag_row(mt, h), t = O - g.H + row;
+          const bool ok = t >= 0 && t < g.Tin;
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c) {
+            if (c >= g.nkc * 4) continue;
+            const int col = c * 8 + col_l;
+            const float a0 = bb ? v[mt][c * 4 + 2 * h] + bb[col] : v[mt][c * 4 + 2 * h];
+            const float a1 = bb ? v[mt][c * 4 + 2 * h + 1] + bb[col + 1] : v[mt][c * 4 + 2 * h + 1];
+            const uint32_t q = ok ? pack2t<BF16>(lrelu(a0, g.mid_slope), lrelu(a1, g.mid_slope)) : 0u;
+            *reinterpret_cast<uint32_t*>(smem + off + unit_offset(g.rowsX, c, row + g.G) + 2 * col_l) = q;
           }
-          if (p.yimg != nullptr && ok) {
-            uint16_t* yi = p.yimg + (((size_t)b * c8n + (size_t)ch * 2) * p.T + (size_t)t) * 8;
+        }
+      fence_proxy_async();
+      __syncthreads();
+    };
+    for (int st = 0; st < g.nsteps; ++st) {
+      const int pr = st / g.nconv, cv = st - pr * g.nconv;
+      const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.k - 1) * d / 2;
+      const uint32_t aT = cv == 0 ? sA : sI;
+      bool first = true;
+      for (int kc = 0; kc < g.nkc; ++kc)
+        mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.rowsX, g.k, d, false, first);
+      const float* bb = bias_s + st * NW;
+      if (g.nconv == 2 && cv == 0) {
+        store_tile(g.off_i, acc, bb);
+      } else {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              uint4 q;
-              q.x = pack2t<BF16>(lrelu(v[8 * h + 0], p.img_slope), lrelu(v[8 * h + 1], p.img_slope));
-              q.y = pack2t<BF16>(lrelu(v[8 * h + 2], p.img_slope), lrelu(v[8 * h + 3], p.img_slope));
-              q.z = pack2t<BF16>(lrelu(v[8 * h + 4], p.img_slope), lrelu(v[8 * h + 5], p.img_slope));
-              q.w = pack2t<BF16>(lrelu(v[8 * h + 6], p.img_slope), lrelu(v[8 * h + 7], p.img_slope));
-              *reinterpret_cast<uint4*>(yi + (size_t)h * p.T * 8) = q;
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              float a = acc[mt][c * 4 + i] + bb[c * 8 + col_l + (i & 1)];
+              a += xr[mt][c * 4 + i];
+              xr[mt][c * 4 + i] = a;
+            }
+        if (st + 1 < g.nsteps) store_tile(0, xr, nullptr);
+      }
+    }
+    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); yimg = cvt(lrelu(y, img_slope))
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = frag_row(mt, h), t = O - g.H + row;
+        if (row < g.H || row >= g.H + g.V || t >= g.Tout) continue;
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c) {
+          const int co = c * 8 + col_l;
+          float ve[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            ve[e] = 0.f;
+            if (co + e < p.Cout) {
+              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
+              float v = xr[mt][c * 4 + 2 * h + e];
+              if (p.acc_prev) v += p.acc_prev[idx];
+              v *= g.out_scale;
+              p.y[idx] = v;
+              ve[e] = v;
+            }
+          }
+          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
+            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
+        }
+      }
+  } else if (g.mode != 2) {
+    for (int nb = 0; nb < g.NB; ++nb) {
+      bool first = true;
+      for (int kc = 0; kc < g.nkc; ++kc) {
+        load_chunk(kc);
+        mma_chunk(sA, g.rowsA, g.ntaps, g.d, g.mode == 1, first);
+      }
+      if (g.mode == 0) {
+        epilogue_conv(nb, bias_s + nb * NW);
+      } else {
+        // conv-transpose: column n = cl*u + phi of input time s is y[nb*cc + cl, s*u - pad + phi]
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int s = O + frag_row(mt, h);
+#pragma unroll
+            for (int c = 0; c < NW / 8; ++c) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = c * 8 + col_l + e;
+                const int cl = n / g.u, phi = n - cl * g.u, co = nb * g.cc + cl;
+                const int t = s * g.u - g.pad + phi;
+                if (cl >= g.cc || co >= p.Cout || t < 0 || t >= g.Tout) continue;
+                const float v = acc[mt][c * 4 + 2 * h + e] + bias_s[co];
+                p.y[((int64_t)b * p.Cout + co) * g.Tout + t] = v;
+                if (p.yimg != nullptr)
+                  p.yimg[(((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)] =
+                      (uint16_t)(pack2t<BF16>(lrelu(v, p.img_slope), 0.f) & 0xffffu);
+              }
             }
           }
         }
-      }
-    }
-    tc_fence_before();
-    stamp(5);
-  } else if (warp == WW) {
-    // ===================== TMA weight producer =====================
-    if (lane == 0) {
-      const int per_conv = p.k * g.nkc;
-      const int total = p.nconv * per_conv;
-      for (int it = 0; it < total; ++it) {
-        const int s = it % g.nstages;
-        const uint32_t ph = (uint32_t)(it / g.nstages) & 1u;
-        mbar_wait(bar_empty(s), ph ^ 1u, 20);
-        mbar_arrive_expect_tx(bar_full(s), g.stage_bytes);
-        const int conv = it / per_conv, local = it - conv * per_conv;
-        const uint8_t* src = static_cast<const uint8_t*>(conv ? p.w2 : p.w1) + (size_t)local * g.stage_bytes;
-        bulk_g2s(sW + (uint32_t)s * g.stage_bytes, src, g.stage_bytes, bar_full(s));
       }
     }
   } else {
-    // ===================== MMA issuer =====================
-    // All 32 lanes run the warp-uniform loops; one elected lane issues tcgen05.mma / commit.
-    const uint32_t elected = elect_one_sync();
-    const int nks_total = g.Np >> 4;                    // 16-channel K steps per tap
-    const uint64_t hi = desc_hi_sw32();
-    const uint32_t kstepA = 2u * (uint32_t)g.rowsA;     // one [c16] chunk of A, in 16-byte units
-    const uint32_t kstepB = 2u * (uint32_t)g.Np;
-    const uint32_t a16 = sA >> 4, w16 = sW >> 4, stage16 = g.stage_bytes >> 4;
-    int it = 0;
-    long long wait_w = 0, wait_a = 0;   // debug: cycles the issuer spent waiting for weight stages / the operand tile
-    for (int conv = 0; conv < p.nconv; ++conv) {
-      const long long ta = g.dbg ? clock64() : 0;
-      mbar_wait(bar_aready, (uint32_t)conv & 1u, 30);
-      if (g.dbg) wait_a += clock64() - ta;
-      tc_fence_after();
-      const int dil = conv == 0 ? p.d1 : 1;
-      // the stage loop, specialised once per conv on (tile count, issue order): the issuing thread bounds the MMA
-      // phases, so nothing that is constant over the conv is re-evaluated per weight stage
-      auto run_conv = [&](auto issue_first, auto issue_rest, bool have_first) {
-        for (int j = 0; j < p.k; ++j) {
-          for (int kc = 0; kc < g.nkc; ++kc, ++it) {
-            const int s = it % g.nstages;
-            const uint32_t ph = (uint32_t)(it / g.nstages) & 1u;
-            const long long tw = g.dbg ? clock64() : 0;
-            mbar_wait(bar_full(s), ph, 31);
-            if (g.dbg) wait_w += clock64() - tw;
-            tc_fence_after();
-            const bool two = nks_total - kc * 2 >= 2;
-            const uint32_t alo = desc_lo_sw32(a16 + (uint32_t)(kc * 2) * kstepA + (uint32_t)(j * dil) * 2u);
-            const uint32_t blo = desc_lo_sw32(w16 + (uint32_t)s * stage16);
-            if (have_first && (j | kc) == 0) issue_first(alo, blo, two);
-            else issue_rest(alo, blo, two);
-            if (elected) tc_commit(bar_empty(s));
-            __syncwarp();
-          }
-        }
-      };
-      auto generic = [&](uint32_t alo, uint32_t blo, bool two, uint32_t acc0) {
-        if (g.korder) {
-          for (int h = 0; h < (two ? 2 : 1); ++h) {
-            uint32_t ah = alo + (uint32_t)h * kstepA;
-            const uint32_t bh = blo + (uint32_t)h * kstepB;
-            uint32_t td = tmem;
-            for (int i = 0; i < g.m; ++i) {
-              if (elected) tc_mma_f16(td, hi | ah, hi | bh, g.idesc, h ? 1u : acc0);
-              ah += 256u;   // 128 rows x 32 B
-              td += (uint32_t)g.Np;
-            }
-          }
-        } else {
-          uint32_t td = tmem;
-          for (int i = 0; i < g.m; ++i) {
-            if (elected) {
-              tc_mma_f16(td, hi | alo, hi | blo, g.idesc, acc0);
-              if (two) tc_mma_f16(td, hi | (alo + kstepA), hi | (blo + kstepB), g.idesc, 1u);
-            }
-            alo += 256u;
-            td += (uint32_t)g.Np;
-          }
-        }
-      };
-#define AB_RUN(MM, KO)                                                                                                     \
-  run_conv([&](uint32_t alo, uint32_t blo, bool two) {                                                                     \
-             issue_stage<MM, KO, 1>(elected, tmem, (uint32_t)g.Np, hi, alo, blo, kstepA, kstepB, g.idesc, two);            \
-           },                                                                                                              \
-           [&](uint32_t alo, uint32_t blo, bool two) {                                                                     \
-             issue_stage<MM, KO, 0>(elected, tmem, (uint32_t)g.Np, hi, alo, blo, kstepA, kstepB, g.idesc, two);            \
-           },                                                                                                              \
-           true)
-      if (g.m == 2 && !g.korder) AB_RUN(2, false);
-      else if (g.m == 4 && g.korder) AB_RUN(4, true);
-      else if (g.m == 8 && g.korder) AB_RUN(8, true);
-      else if (g.m == 1 && !g.korder) AB_RUN(1, false);
-      else if (g.m == 16 && g.korder) AB_RUN(16, true);
-      else
-        run_conv([&](uint32_t alo, uint32_t blo, bool two) { generic(alo, blo, two, 0u); },
-                 [&](uint32_t alo, uint32_t blo, bool two) { generic(alo, blo, two, 1u); }, true);
-#undef AB_RUN
-      if (elected) tc_commit(bar_accfull);
-      __syncwarp();
+    bool first = true;
+    for (int kc = 0; kc < g.nkc; ++kc) {
+      load_chunk(kc);
+      mma_chunk(sA, g.rowsA, g.ntaps, g.d, false, first);
     }
-    if (g.dbg != nullptr && elected && blockIdx.x < DBG_BLOCKS) {
-      g.dbg[blockIdx.x * DBG_SLOTS + 8] = wait_w;
-      g.dbg[blockIdx.x * DBG_SLOTS + 9] = wait_a;
+    // intermediate = lrelu(conv1 + b1, mid_slope) -> shared-memory operand tile, zero outside [0, T)
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = frag_row(mt, h), t = O - g.h2 + row;
+        const bool ok = t >= 0 && t < g.Tin;
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c) {
+          if (c >= g.nkc2 * 4) continue;
+          const int col = c * 8 + col_l;
+          const float v0 = ok ? lrelu(acc[mt][c * 4 + 2 * h] + bias_s[col], g.mid_slope) : 0.f;
+          const float v1 = ok ? lrelu(acc[mt][c * 4 + 2 * h + 1] + bias_s[col + 1], g.mid_slope) : 0.f;
+          *reinterpret_cast<uint32_t*>(smem + g.off_i + unit_offset(g.rowsI, c, row) + 2 * col_l) = pack2t<BF16>(v0, v1);
+        }
+      }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == WW + 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)g.tmem_cols)
-                 : "memory");
+    fence_proxy_async();
+    __syncthreads();
+    first = true;
+    for (int kc = 0; kc < g.nkc2; ++kc)
+      mma_chunk(sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, g.ntaps, 1, false, first);
+    epilogue_conv(0, bias_s + NW);
   }
 }
 
 // ---------------------------------------------------------------------------
-// weight image: stage (tap j, kc) = channels [32*kc, 32*kc+32) x Np rows in the SWIZZLE_32B layout
+// weight images: stage (nb, kc, tap) = [4 c8][NW rows][8] — the A/B operand layout of ab_tc_ptx.cuh
 // ---------------------------------------------------------------------------
-__global__ void tc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* __restrict__ img, int cin,
-                                      int cout, int k, int Np, int nkc, int bf16) {
-  const int64_t total = (int64_t)k * nkc * 4 * Np * 8;
+struct HcLayer {
+  int mode, NW, NB, cc, ntaps, nkc, u;
+};
+
+int rup(int x, int a) { return (x + a - 1) / a * a; }
+int pow2_at_least(int x) {
+  int n = 16;
+  while (n < x) n <<= 1;
+  return n;
+}
+
+// mode 0 conv (d_or_u = dilation), 1 conv-transpose (d_or_u = stride)
+int layer_geom(int mode, int cin, int cout, int k, int d_or_u, HcLayer& L) {
+  if (cin <= 0 || cout <= 0 || k <= 0 || d_or_u <= 0) return fail(AB_ERR_ARG, "tc conv: bad layer shape");
+  L.mode = mode;
+  L.nkc = (cin + 31) / 32;
+  if (mode == 0) {
+    if (!(k & 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv: conv kernel size must be odd");
+    L.NW = std::min(256, pow2_at_least(rup(cout, 16)));
+    L.NB = (cout + L.NW - 1) / L.NW;
+    L.cc = L.NW;
+    L.ntaps = k;
+    L.u = 1;
+  } else {
+    const int u = d_or_u;
+    if (k < u || ((k - u) & 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv: conv-transpose needs k >= stride, k-stride even");
+    if (u > 64) return fail(AB_ERR_UNSUPPORTED, "tc conv: stride %d too large", u);
+    L.cc = std::min(256 / u, cout);
+    L.NW = pow2_at_least(L.cc * u);
+    L.NB = (cout + L.cc - 1) / L.cc;
+    L.ntaps = (k + u - 1) / u;
+    L.u = u;
+  }
+  return AB_OK;
+}
+
+size_t layer_image_bytes(const HcLayer& L) { return (size_t)L.NB * L.nkc * L.ntaps * 64u * L.NW; }
+
+__global__ void hc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* __restrict__ img, HcLayer L, int cin,
+                                      int cout, int k, int bf16) {
+  const int64_t total = (int64_t)L.NB * L.nkc * L.ntaps * 32 * L.NW;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
     const int e = (int)(idx & 7);
     int64_t r = idx >> 3;
-    const int co = (int)(r % Np);
-    r /= Np;
+    const int n = (int)(r % L.NW);
+    r /= L.NW;
     const int c8l = (int)(r & 3);
     r >>= 2;
-    const int kc = (int)(r % nkc);
-    const int j = (int)(r / nkc);
+    const int tap = (int)(r % L.ntaps);
+    r /= L.ntaps;
+    const int kc = (int)(r % L.nkc);
+    const int nb = (int)(r / L.nkc);
     const int ci = kc * 32 + c8l * 8 + e;
     float v = 0.f;
-    if (ci < cin && co < cout) v = w_t[((int64_t)ci * k + j) * cout + co];
-    uint16_t bits;
-    if (bf16) {
-      __nv_bfloat16 h = __float2bfloat16_rn(v);
-      bits = *reinterpret_cast<uint16_t*>(&h);
+    if (L.mode == 0) {
+      const int co = nb * L.NW + n;
+      if (ci < cin && co < cout) v = w_t[((int64_t)ci * k + tap) * cout + co];
     } else {
-      v = fminf(fmaxf(v, -65504.f), 65504.f);
-      __half h = __float2half_rn(v);
-      bits = *reinterpret_cast<uint16_t*>(&h);
+      const int cl = n / L.u, phi = n - cl * L.u, co = nb * L.cc + cl, j = phi + L.u * tap;
+      if (ci < cin && cl < L.cc && co < cout && j < k) v = w_t[((int64_t)ci * k + j) * cout + co];
     }
-    const int64_t stage = (int64_t)j * nkc + kc;
-    const int unit = (c8l & 1) ^ ((co >> 2) & 1);
-    img[stage * (4 * Np * 8) + (int64_t)(c8l >> 1) * Np * 16 + (int64_t)co * 16 + unit * 8 + e] = bits;
+    img[idx] = (uint16_t)(pack2(v, 0.f, bf16) & 0xffffu);
   }
 }
 
-int round_up(int x, int a) { return (x + a - 1) / a * a; }
-
-int make_geom(const TcConvParams& p, TcGeom& g) {
-  if (p.C <= 0 || p.C > TC_MAX_C) return fail(AB_ERR_UNSUPPORTED, "tc_conv: C=%d not in [1,%d]", p.C, TC_MAX_C);
-  if (p.k <= 0 || !(p.k & 1) || p.d1 <= 0) return fail(AB_ERR_UNSUPPORTED, "tc_conv: need odd k and positive dilation");
-  if (p.nconv != 1 && p.nconv != 2) return fail(AB_ERR_ARG, "tc_conv: nconv must be 1 or 2");
-  g.Np = round_up(p.C, 16);
-  g.nkc = (g.Np + 31) / 32;
-  g.stage_bytes = (uint32_t)g.Np * 64u;
-  const int h1 = (p.k - 1) * p.d1 / 2, h2 = (p.k - 1) / 2;
-  g.h2 = h2;
-  g.hh = p.nconv == 2 ? h1 + h2 : h1;
-  const int lost = p.nconv == 2 ? (p.k - 1) : 0;   // rows of the tile that conv2 cannot produce
-  const int halo = (p.k - 1) * p.d1;
-  static const int dual_ok = [] { const char* e = getenv("AB_TC_DUAL"); return (e && e[0] == '0') ? 0 : 1; }();
-  static const int staged_ok = [] { const char* e = getenv("AB_TC_STAGED"); return (e && e[0] == '0') ? 0 : 1; }();
-  const uint32_t misc = 2u * g.Np * 4u + 8u * (2 * TC_MAX_STAGES + 2) + 16u;
-  auto try_fit = [&](int m, int ww, uint32_t limit, int min_stages) -> bool {
-    if (m < 1 || m * 128 - lost < 8) return false;
-    g.rowsA = round_up(m * 128 + halo, 8);
-    // the A region also hosts the epilogue-2 residual ring (ring_depth slots per worker warp)
-    const uint32_t tile_bytes = (uint32_t)g.rowsA * (uint32_t)g.Np * 2u;
-    uint32_t abytes = 0;
-    int rd = RING_DEPTH_MAX;
-    for (; rd >= 2; --rd) {
-      abytes = std::max<uint32_t>(tile_bytes, (uint32_t)ww * rd * RING_SLOT_BYTES);
-      if (abytes + (uint32_t)min_stages * g.stage_bytes + misc + 1280u <= limit) break;
-    }
-    if (rd < 2) return false;
-    g.ring_depth = rd;
-    g.m = m;
-    int ns = (int)((limit - abytes - misc - 1280u) / g.stage_bytes);
-    g.nstages = std::min(ns, TC_MAX_STAGES);
-    g.off_w = (abytes + 1023u) & ~1023u;
-    g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
-    g.off_bar = (g.off_bias + 2u * g.Np * 4u + 15u) & ~15u;
-    g.smem_bytes = g.off_bar + 8u * (2 * TC_MAX_STAGES + 2) + 16u;
-    return true;
-  };
-  g.dual = 0;
-  // preferred: 1/n-size tiles so that n CTAs share an SM and one CTA's global-memory phases overlap the
-  // others' MMA phases (n = 3 when the 108-register kernel, 512 TMEM columns and 227 KB smem allow it)
-  static const int ncta_pref = [] { const char* e = getenv("AB_TC_NCTA"); return e ? atoi(e) : 2; }();
-  for (int n = std::min(std::max(ncta_pref, 2), 3); n >= 2 && dual_ok && !g.dual; --n) {
-    const int cols = n == 2 ? 256 : 128;
-    int m2 = std::min(cols / g.Np, 16);
-    while (m2 > 1 && (m2 - 1) * 128 - lost >= p.T) --m2;
-    const uint32_t limit = n == 2 ? 113u * 1024u : 74u * 1024u;
-    static const int ww_pref = [] { const char* e = getenv("AB_TC_WW"); return e ? atoi(e) : 8; }();
-    const int ww = (n == 2 && ww_pref == 8) ? 8 : 4;
-    if (m2 >= 1 && try_fit(m2, ww, limit, 3)) {
-      g.dual = n;
-      g.ww = ww;
-      g.tmem_cols = 32;
-      while (g.tmem_cols < g.m * g.Np) g.tmem_cols *= 2;
-    }
-  }
-  if (g.dual) {
-  } else {
-    int m = std::min(512 / g.Np, 16);
-    while (m > 1 && (m - 1) * 128 - lost >= p.T) --m;
-    for (;; --m) {
-      if (m < 1) return fail(AB_ERR_UNSUPPORTED, "tc_conv: C=%d k=%d d=%d does not fit shared memory", p.C, p.k, p.d1);
-      if (try_fit(m, 8, TC_SMEM_LIMIT, 2)) break;
-    }
-    g.ww = 8;
-    g.tmem_cols = 512;
-  }
-  g.V = ((g.m * 128 - lost) / 8) * 8;
-  g.tiles = (p.T + g.V - 1) / g.V;
-  // 16-byte cp.async of fp32 rows needs T % 4 == 0 (tile origins are multiples of 8)
-  g.staged = (staged_ok && (p.T % 4) == 0 && (p.residual != nullptr || p.acc_prev != nullptr)) ? 1 : 0;
-  const uint32_t fmt = p.precision == AB_PREC_TC_BF16 ? 1u : 0u;
-  // cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a_format @7, b_format @10, K-major A and B,
-  // N>>3 @17, M>>4 @24
-  g.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(g.Np >> 3) << 17) | ((128u >> 4) << 24);
-  g.dbg = nullptr;
-  g.out_scale = 1.0f / p.out_div;
-  static const int skip = [] { const char* e = getenv("AB_TC_DEBUG_SKIP"); return e ? atoi(e) : 0; }();
-  g.skip = skip;
-  // measured (profiles/r1_tc_phase_timing_v9.txt): K-half-outer issue is 19 % faster at m = 8 and 7 % slower at m = 2
-  static const int korder = [] { const char* e = getenv("AB_TC_KORDER"); return e ? atoi(e) : 2; }();
-  g.korder = korder == 2 ? (g.m >= 4 ? 1 : 0) : korder;
-  // stagger: period model = MMA issue time + HBM time of the tile at ~4.5 TB/s chip-wide (DESIGN.md §6)
-  static const int stag = [] { const char* e = getenv("AB_TC_STAGGER"); return e ? atoi(e) : 0; }();
-  g.stagger_groups = stag;
-  g.first_wave = 148 * (g.dual ? g.dual : 1);
-  const double mma = (double)p.nconv * p.k * g.nkc * g.m * 2.0 * (64.0 + g.Np / 2.0) * (g.dual ? 2.0 : 1.0);
-  const double mem = (double)g.m * 128.0 * g.Np * 12.0 / (g.dual ? 7.7 : 15.4);
-  g.stagger_cycles = stag > 1 ? (long long)((mma + mem + 8000.0) / stag) : 0;
+int pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u, int precision,
+                cudaStream_t s) {
+  HcLayer L;
+  int rc = layer_geom(mode, cin, cout, k, d_or_u, L);
+  if (rc != AB_OK) return rc;
+  const int64_t total = (int64_t)layer_image_bytes(L) / 2;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 132 * 8);
+  hc_pack_weight_kernel<<<blocks, 256, 0, s>>>(w_t, static_cast<uint16_t*>(image), L, cin, cout, k,
+                                               precision == AB_PREC_TC_BF16 ? 1 : 0);
+  AB_LAUNCH_CHECK("hc_pack_weight_kernel");
   return AB_OK;
+}
+
+// Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.
+int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g) {
+  HcLayer L;
+  int rc = layer_geom(mode == 2 ? 0 : mode, cin, cout, k, d_or_u, L);
+  if (rc != AB_OK) return rc;
+  if (mode == 2 && (cin != cout || L.NB != 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv pair: C=%d not in [1,%d]", cin, TC_MAX_C);
+  g.mode = mode;
+  g.NB = L.NB;
+  g.cc = L.cc;
+  g.ntaps = L.ntaps;
+  g.nkc = L.nkc;
+  g.u = L.u;
+  g.R = HC_WG * mt_of(L.NW) * 64;
+  g.Tin = Tin;
+  g.c8n_in = rup(cin, 16) / 8;
+  g.c8n_out = rup(cout, 16) / 8;
+  g.h2 = 0;
+  g.rowsI = 0;
+  g.nkc2 = 0;
+  int maxshift, rows_total;
+  if (mode == 1) {
+    g.d = 1;
+    g.pad = (k - L.u) / 2;
+    g.Tout = Tin * L.u;
+    maxshift = g.ntaps - 1;
+    g.a0 = maxshift;
+    g.V = g.R;
+    rows_total = (g.Tout - 1 + g.pad) / L.u + 1;
+  } else {
+    g.d = d_or_u;
+    g.pad = 0;
+    g.Tout = Tin;
+    maxshift = (k - 1) * d_or_u;
+    g.a0 = maxshift / 2;
+    g.V = g.R;
+    rows_total = Tin;
+    if (mode == 2) {
+      g.h2 = (k - 1) / 2;
+      g.a0 += g.h2;
+      g.V = g.R - (k - 1);
+      g.rowsI = rup(g.R + k - 1, 8);
+      g.nkc2 = L.nkc;
+    }
+  }
+  if (g.V < 8) return fail(AB_ERR_UNSUPPORTED, "tc conv: kernel size %d too large for a tile", k);
+  g.rowsA = rup(g.R + maxshift, 8);
+  if (g.rowsA > 16383 || g.rowsI > 16383) return fail(AB_ERR_UNSUPPORTED, "tc conv: tap reach %d too large", maxshift);
+  g.tiles = (rows_total + g.V - 1) / g.V;
+  g.stage_bytes = 64u * (uint32_t)L.NW;
+  g.off_i = ((uint32_t)g.rowsA * 64u + 127u) & ~127u;
+  const uint32_t ibytes = (uint32_t)g.nkc2 * 4u * (uint32_t)g.rowsI * 16u;
+  g.off_w = (g.off_i + ibytes + 127u) & ~127u;
+  const uint32_t nbias = (uint32_t)(mode == 2 ? 2 * L.NW : g.NB * L.NW);
+  const uint32_t limit = L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA;
+  const uint32_t fixed = g.off_w + nbias * 4u + 16u + 16u * HC_STAGES_MAX;
+  if (fixed + 2u * g.stage_bytes > limit)
+    return fail(AB_ERR_UNSUPPORTED, "tc conv: C=%d k=%d reach %d does not fit shared memory", cin, k, maxshift);
+  g.nstages = (int)std::min<uint32_t>((limit - fixed) / g.stage_bytes, HC_STAGES_MAX);
+  g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
+  g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
+  g.smem_bytes = g.off_bar + 16u * HC_STAGES_MAX;
+  g.out_scale = 1.0f;
+  g.mid_slope = 1.0f;
+  return AB_OK;
+}
+
+template <int NW, bool CHAIN = false>
+int launch_nw(const HcArgs& a, const HcGeom& g, int bf16, cudaStream_t s) {
+  static DeviceOnce configured;
+  if (configured.need()) {
+    const int lim = (int)((NW >= 256 || CHAIN) ? HC_SMEM_1CTA : HC_SMEM_2CTA);
+    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 0, CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 1, CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+  }
+  const int64_t grid = (int64_t)a.B * g.tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
+  if (bf16) hconv_kernel<NW, 1, CHAIN><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
+  else hconv_kernel<NW, 0, CHAIN><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
+  AB_LAUNCH_CHECK("hconv_kernel");
+  return AB_OK;
+}
+
+// Block-mode geometry: npairs x nconv convs of one ResBlock (C <= 64) with the halo recomputed inside the tile.
+int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, HcGeom& g) {
+  if (npairs < 1 || npairs > AB_TC_CHAIN_MAX_PAIRS || (nconv != 1 && nconv != 2) || !tc_conv_supported(C, k))
+    return fail(AB_ERR_UNSUPPORTED, "tc block: unsupported block");
+  HcLayer L;
+  int rc = layer_geom(0, C, C, k, 1, L);
+  if (rc != AB_OK) return rc;
+  if (L.NW > AB_TC_CHAIN_MAX_C) return fail(AB_ERR_UNSUPPORTED, "tc block: C=%d > %d", C, AB_TC_CHAIN_MAX_C);
+  memset(&g, 0, sizeof(g));
+  g.mode = 3;
+  g.NB = 1; g.cc = L.NW; g.ntaps = k; g.k = k; g.nkc = L.nkc; g.u = 1; g.d = 1;
+  g.nconv = nconv; g.nsteps = npairs * nconv;
+  g.H = 0; g.G = 0;
+  for (int q = 0; q < npairs; ++q) {
+    if (dil[q] <= 0) return fail(AB_ERR_ARG, "tc block: dilation must be positive");
+    g.dil[q] = dil[q];
+    g.H += (k - 1) * dil[q] / 2 + (nconv == 2 ? (k - 1) / 2 : 0);
+    g.G = std::max(g.G, (k - 1) * dil[q] / 2);
+  }
+  g.R = HC_WG * mt_of(L.NW) * 64;
+  g.V = g.R - 2 * g.H;
+  if (g.V < 8) return fail(AB_ERR_UNSUPPORTED, "tc block: halo %d too wide for %d rows", g.H, g.R);
+  g.rowsX = rup(g.R + 2 * g.G, 8);
+  if (g.rowsX > 16383) return fail(AB_ERR_UNSUPPORTED, "tc block: halo too wide");
+  g.Tin = g.Tout = T;
+  g.tiles = (T + g.V - 1) / g.V;
+  g.c8n_in = g.c8n_out = rup(C, 16) / 8;
+  g.stage_bytes = 64u * (uint32_t)L.NW;
+  const uint32_t xbytes = (uint32_t)g.nkc * 4u * (uint32_t)g.rowsX * 16u;
+  g.off_i = (xbytes + 127u) & ~127u;
+  g.off_w = (g.off_i + xbytes + 127u) & ~127u;
+  const uint32_t nbias = (uint32_t)(g.nsteps * L.NW);
+  const uint32_t fixed = g.off_w + nbias * 4u + 16u + 16u * HC_STAGES_MAX;
+  if (fixed + 2u * g.stage_bytes > HC_SMEM_1CTA) return fail(AB_ERR_UNSUPPORTED, "tc block: does not fit shared memory");
+  g.nstages = (int)std::min<uint32_t>((HC_SMEM_1CTA - fixed) / g.stage_bytes, HC_STAGES_MAX);
+  g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
+  g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
+  g.smem_bytes = g.off_bar + 16u * HC_STAGES_MAX;
+  g.out_scale = 1.0f;
+  g.mid_slope = 1.0f;
+  return AB_OK;
+}
+
+int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s) {
+  if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
+  const int bf16 = precision == AB_PREC_TC_BF16;
+  switch ((int)(g.stage_bytes / 64u)) {
+    case 16: return launch_nw<16>(a, g, bf16, s);
+    case 32: return launch_nw<32>(a, g, bf16, s);
+    case 64: return launch_nw<64>(a, g, bf16, s);
+    case 128: return launch_nw<128>(a, g, bf16, s);
+    case 256: return launch_nw<256>(a, g, bf16, s);
+  }
+  return fail(AB_ERR_UNSUPPORTED, "tc conv: N block %u", g.stage_bytes / 64u);
+}
+
+HcArgs base_args(const float* x, int64_t xsb, int64_t xsc, int64_t xst, const uint16_t* ximg, float pre_slope, int B,
+                 int cin, int cout) {
+  HcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.xsb = xsb; a.xsc = xsc; a.xst = xst; a.ximg = ximg; a.pre_slope = pre_slope;
+  a.B = B; a.Cin = cin; a.Cout = cout; a.img_slope = 1.0f;
+  return a;
 }
 
 }  // namespace
 
 int tc_max_channels() { return TC_MAX_C; }
 
+double tc_chain_recompute(int C, int k, const int* dil, int npairs, int nconv) {
+  HcGeom g;
+  if (make_chain_geom(C, k, dil, npairs, nconv, 1 << 20, g) != AB_OK) return 0.0;
+  return (double)g.R / g.V;
+}
+
+int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
+  if (!p.x || !p.y) return fail(AB_ERR_ARG, "tc block: null argument");
+  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "tc block: bad shape");
+  if (p.precision != AB_PREC_TC_F16 && p.precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc block: bad precision");
+  HcGeom g;
+  int rc = make_chain_geom(p.C, p.k, p.dil, p.npairs, p.nconv, p.T, g);
+  if (rc != AB_OK) return rc;
+  g.out_scale = 1.0f / p.out_div;
+  g.mid_slope = p.slope;
+  HcArgs a = base_args(p.x, (int64_t)p.C * p.T, p.T, 1, p.ximg, p.slope, p.B, p.C, p.C);
+  for (int i = 0; i < g.nsteps; ++i) {
+    if (!p.w[i]) return fail(AB_ERR_ARG, "tc block: null weight image");
+    a.ws[i] = p.w[i];
+    a.bs[i] = p.bias[i];
+  }
+  a.y = p.y; a.acc_prev = p.acc_prev; a.yimg = p.yimg; a.img_slope = p.img_slope;
+  const int bf16 = p.precision == AB_PREC_TC_BF16;
+  switch ((int)(g.stage_bytes / 64u)) {
+    case 16: return launch_nw<16, true>(a, g, bf16, s);
+    case 32: return launch_nw<32, true>(a, g, bf16, s);
+    case 64: return launch_nw<64, true>(a, g, bf16, s);
+  }
+  return fail(AB_ERR_UNSUPPORTED, "tc block: N block %u", g.stage_bytes / 64u);
+}
+
 bool tc_conv_supported(int C, int k) { return C > 0 && C <= TC_MAX_C && (k & 1) && k <= 31; }
 
 size_t tc_weight_image_bytes(int cin, int cout, int k) {
   if (cin != cout || !tc_conv_supported(cin, k)) return 0;
-  const int Np = round_up(cout, 16), nkc = (Np + 31) / 32;
-  return (size_t)k * nkc * Np * 64;
+  return gc_weight_image_bytes(0, cin, cout, k, 1);
 }
 
-size_t tc_act_image_bytes(int64_t B, int C, int64_t T) { return (size_t)B * round_up(C, 16) * (size_t)T * 2; }
+size_t tc_act_image_bytes(int64_t B, int C, int64_t T) { return (size_t)B * rup(C, 16) * (size_t)T * 2; }
 
-int launch_tc_pack_weight(const float* w_t, void* image, int cin, int cout, int k, int precision,
-                          cudaStream_t s) {
-  const size_t bytes = tc_weight_image_bytes(cin, cout, k);
-  if (bytes == 0) return AB_OK;  // shape not served by the tensor-core path
-  const int Np = round_up(cout, 16), nkc = (Np + 31) / 32;
-  const int64_t total = (int64_t)bytes / 2;
-  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 8);
-  tc_pack_weight_kernel<<<blocks, 256, 0, s>>>(w_t, static_cast<uint16_t*>(image), cin, cout, k, Np, nkc,
-                                               precision == AB_PREC_TC_BF16 ? 1 : 0);
-  AB_LAUNCH_CHECK("tc_pack_weight_kernel");
-  return AB_OK;
+int launch_tc_pack_weight(const float* w_t, void* image, int cin, int cout, int k, int precision, cudaStream_t s) {
+  if (tc_weight_image_bytes(cin, cout, k) == 0) return AB_OK;  // shape not served by the tensor-core path
+  return pack_weight(w_t, image, 0, cin, cout, k, 1, precision, s);
 }
 
 int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   if (!p.x || !p.y || !p.w1 || (p.nconv == 2 && !p.w2)) return fail(AB_ERR_ARG, "tc_conv: null argument");
   if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "tc_conv: bad shape");
-  if (p.precision != AB_PREC_TC_F16 && p.precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc_conv: bad precision");
-  TcGeom g;
-  int rc = make_geom(p, g);
+  if (p.nconv != 1 && p.nconv != 2) return fail(AB_ERR_ARG, "tc_conv: nconv must be 1 or 2");
+  if (!tc_conv_supported(p.C, p.k) || p.d1 <= 0) return fail(AB_ERR_UNSUPPORTED, "tc_conv: C=%d k=%d d=%d", p.C, p.k, p.d1);
+  HcGeom g;
+  int rc = make_geom(p.nconv == 2 ? 2 : 0, p.C, p.C, p.k, p.d1, p.T, g);
   if (rc != AB_OK) return rc;
-  static DeviceOnce configured;
-  if (configured.need()) {
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<8, 1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_LIMIT));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<8, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_LIMIT));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<4, 2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 113 * 1024));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<4, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 113 * 1024));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<8, 2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_LIMIT));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<8, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_LIMIT));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<4, 3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 74 * 1024));
-    AB_CUDA_TRY(cudaFuncSetAttribute(tc_conv_kernel<4, 3, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 74 * 1024));
-  }
-  const int64_t grid = (int64_t)p.B * g.tiles;
-  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc_conv: grid too large");
-  // single mode: request > half of the SM's shared memory so exactly one CTA (512 TMEM columns) is resident
-  // debug: AB_TC_SOLO=1 keeps the half-tile geometry but lets only one CTA reside per SM (stand-alone phase times)
-  static const bool solo = [] { const char* e = getenv("AB_TC_SOLO"); return e && e[0] == '1'; }();
-  const uint32_t smem = (g.dual && !(solo && g.dual == 2)) ? g.smem_bytes : std::max<uint32_t>(g.smem_bytes, 120u * 1024u);
-  static const bool dbg_on = [] { const char* e = getenv("AB_TC_DEBUG_TIMING"); return e && e[0] == '1'; }();
-  static long long* dbg_buf = nullptr;
-  if (dbg_on) {  // debug only: the one place the library allocates, never on the product path
-    if (!dbg_buf) AB_CUDA_TRY(cudaMalloc(&dbg_buf, sizeof(long long) * DBG_BLOCKS * DBG_SLOTS));
-    AB_CUDA_TRY(cudaMemsetAsync(dbg_buf, 0, sizeof(long long) * DBG_BLOCKS * DBG_SLOTS, s));
-    g.dbg = dbg_buf;
-  }
-  const bool bf = p.precision == AB_PREC_TC_BF16;
-  if (g.dual == 3) {
-    if (bf) tc_conv_kernel<4, 3, 1><<<(unsigned)grid, 4 * 32 + 64, smem, s>>>(p, g);
-    else tc_conv_kernel<4, 3, 0><<<(unsigned)grid, 4 * 32 + 64, smem, s>>>(p, g);
-  } else if (g.dual == 2 && g.ww == 8) {
-    if (bf) tc_conv_kernel<8, 2, 1><<<(unsigned)grid, 8 * 32 + 64, smem, s>>>(p, g);
-    else tc_conv_kernel<8, 2, 0><<<(unsigned)grid, 8 * 32 + 64, smem, s>>>(p, g);
-  } else if (g.dual == 2) {
-    if (bf) tc_conv_kernel<4, 2, 1><<<(unsigned)grid, 4 * 32 + 64, smem, s>>>(p, g);
-    else tc_conv_kernel<4, 2, 0><<<(unsigned)grid, 4 * 32 + 64, smem, s>>>(p, g);
-  } else {
-    if (bf) tc_conv_kernel<8, 1, 1><<<(unsigned)grid, 8 * 32 + 64, smem, s>>>(p, g);
-    else tc_conv_kernel<8, 1, 0><<<(unsigned)grid, 8 * 32 + 64, smem, s>>>(p, g);
-  }
-  AB_LAUNCH_CHECK("tc_conv_kernel");
-  if (dbg_on) {
-    AB_CUDA_TRY(cudaStreamSynchronize(s));
-    static std::vector<long long> h(DBG_BLOCKS * DBG_SLOTS);
-    AB_CUDA_TRY(cudaMemcpy(h.data(), dbg_buf, sizeof(long long) * h.size(), cudaMemcpyDeviceToHost));
-    const int nb = (int)std::min<int64_t>(grid, DBG_BLOCKS);
-    if (const char* dump = getenv("AB_TC_DEBUG_DUMP")) {   // raw per-CTA records: block smid globaltimer t0..t5
-      if (FILE* f = fopen(dump, "a")) {
-        fprintf(f, "# launch C=%d k=%d d=%d nconv=%d dual=%d grid=%lld\n", p.C, p.k, p.d1, p.nconv, g.dual, (long long)grid);
-        for (int i = 0; i < nb; ++i) {
-          const long long* r = &h[(size_t)i * DBG_SLOTS];
-          fprintf(f, "%d %lld %lld %lld %lld %lld %lld %lld %lld\n", i, r[6], r[7], r[0], r[1], r[2], r[3], r[4], r[5]);
-        }
-        fclose(f);
-      }
-    }
-    double ph[5] = {0, 0, 0, 0, 0}, ww = 0, wa = 0;
-    int cnt = 0;
-    for (int i = 0; i < nb; ++i) {
-      const long long* r = &h[(size_t)i * DBG_SLOTS];
-      if (r[5] == 0) continue;
-      ++cnt;
-      ww += (double)r[8];
-      wa += (double)r[9];
-      ph[0] += (double)(r[1] - r[0]);
-      if (p.nconv == 2) {
-        ph[1] += (double)(r[2] - r[1]);
-        ph[2] += (double)(r[3] - r[2]);
-        ph[3] += (double)(r[4] - r[3]);
-      } else {
-        ph[1] += (double)(r[4] - r[1]);
-      }
-      ph[4] += (double)(r[5] - r[4]);
-    }
-    if (cnt) {
-      const double ideal = (double)g.m * (g.Np / 2.0) * (g.Np / 16.0) * p.k;   // cycles per conv at 8192 flop/clk/SM
-      fprintf(stderr,
-              "[tc_timing] C=%d k=%d d=%d nconv=%d dual=%d img=%d staged=%d m=%d V=%d tiles=%lld stages=%d | cycles: "
-              "prologue %.0f conv1 %.0f epi1 %.0f conv2 %.0f epi2 %.0f | ideal MMA/conv %.0f | issuer waited: weights %.0f operand tile %.0f\n",
-              p.C, p.k, p.d1, p.nconv, g.dual, p.ximg != nullptr, g.staged, g.m, g.V, (long long)grid, g.nstages,
-              ph[0] / cnt, ph[1] / cnt, ph[2] / cnt, ph[3] / cnt, ph[4] / cnt, ideal, ww / cnt, wa / cnt);
-    }
-  }
-  return AB_OK;
+  g.out_scale = 1.0f / p.out_div;
+  g.mid_slope = p.mid_slope;
+  HcArgs a = base_args(p.x, (int64_t)p.C * p.T, p.T, 1, p.ximg, p.pre_slope, p.B, p.C, p.C);
+  a.w = p.w1; a.w2 = p.w2; a.bias = p.b1; a.bias2 = p.b2;
+  a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev;
+  a.yimg = p.yimg; a.img_slope = p.img_slope;
+  return launch_hconv(a, g, p.precision, s);
+}
+
+bool gc_can_emit_image(int cout, int k, int u) {
+  HcLayer L;
+  return layer_geom(1, 16, cout, k, u, L) == AB_OK && (cout % 16) == 0;
+}
+bool gs_can_emit_image(int cout, int k, int u) { return gc_can_emit_image(cout, k, u); }
+
+size_t gc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u) {
+  HcLayer L;
+  if (layer_geom(mode, cin, cout, k, d_or_u, L) != AB_OK) return 0;
+  return layer_image_bytes(L);
+}
+size_t gs_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u) {
+  return gc_weight_image_bytes(mode, cin, cout, k, d_or_u);
+}
+
+int launch_gc_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u,
+                          int precision, cudaStream_t s) {
+  return pack_weight(w_t, image, mode, cin, cout, k, d_or_u, precision, s);
+}
+int launch_gs_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u,
+                          int precision, cudaStream_t s) {
+  return pack_weight(w_t, image, mode, cin, cout, k, d_or_u, precision, s);
+}
+
+int launch_gemmconv(const GcParams& p, cudaStream_t s) {
+  if ((!p.x && !p.ximg) || !p.y || !p.w) return fail(AB_ERR_ARG, "gemmconv: null argument");
+  if (p.ximg && (p.Cin % 16) != 0) return fail(AB_ERR_UNSUPPORTED, "gemmconv: operand-image input needs C_in %% 16 == 0");
+  if (p.B <= 0 || p.Tin <= 0) return fail(AB_ERR_ARG, "gemmconv: bad shape");
+  if (p.mode == 0 && ((p.k - 1) * p.d) & 1) return fail(AB_ERR_UNSUPPORTED, "gemmconv: (k-1)*dilation must be even");
+  if (p.yimg != nullptr && !(p.mode == 1 && (p.Cout % 16) == 0))
+    return fail(AB_ERR_UNSUPPORTED, "gemmconv: cannot emit an operand image for this layer");
+  HcGeom g;
+  int rc = make_geom(p.mode, p.Cin, p.Cout, p.k, p.mode ? p.u : p.d, p.Tin, g);
+  if (rc != AB_OK) return rc;
+  HcArgs a = base_args(p.x, p.xsb, p.xsc, p.xst, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
+  a.w = p.w; a.bias = p.bias; a.y = p.y; a.residual = p.mode == 0 ? p.residual : nullptr;
+  a.post_tanh = p.mode == 0 ? p.post_tanh : 0;
+  a.yimg = p.yimg; a.img_slope = p.img_slope;
+  return launch_hconv(a, g, p.precision, s);
+}
+
+int launch_gemmconv_stream(const GsParams& p, cudaStream_t s) {
+  if ((!p.ximg && !p.x) || !p.y || !p.w) return fail(AB_ERR_ARG, "gemmconv(stream): null argument");
+  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "gemmconv(stream): bad shape");
+  if (p.mode == 0 && ((p.k - 1) * p.d) & 1) return fail(AB_ERR_UNSUPPORTED, "gemmconv(stream): (k-1)*dilation must be even");
+  if (p.yimg != nullptr && !(p.mode == 1 && (p.Cout % 16) == 0))
+    return fail(AB_ERR_UNSUPPORTED, "gemmconv(stream): cannot emit an operand image for this layer");
+  HcGeom g;
+  int rc = make_geom(p.mode, p.Cin, p.Cout, p.k, p.mode ? p.u : p.d, p.T, g);
+  if (rc != AB_OK) return rc;
+  g.out_scale = 1.0f / p.out_div;
+  HcArgs a = base_args(p.x, (int64_t)p.Cin * p.T, p.T, 1, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
+  a.w = p.w; a.bias = p.bias; a.y = p.y;
+  a.residual = p.mode == 0 ? p.residual : nullptr;
+  a.acc_prev = p.mode == 0 ? p.acc_prev : nullptr;
+  a.yimg = p.yimg; a.img_slope = p.img_slope;
+  return launch_hconv(a, g, p.precision, s);
 }
 
 }  // namespace ab

@@ -1,4 +1,5 @@
-// Tensor-core (tcgen05 / TMEM / bulk-TMA) convolution path — interface.
+// Tensor-core (wgmma / bulk-TMA) convolution path — interface.  One kernel (ab_kernels_tc.cu) serves the three
+// parameter sets below; the weight image of a layer depends only on (mode, C_in, C_out, k, dilation | stride).
 #pragma once
 #include "ab_common.cuh"
 
@@ -30,7 +31,7 @@ struct TcConvParams {
   float img_slope;
 };
 
-// N-blocked implicit GEMM (ab_kernels_gemmconv.cu): ConvTranspose1d (mode 1) and wide Conv1d (mode 0)
+// Non-square Conv1d (mode 0) and polyphase ConvTranspose1d (mode 1), N-blocked over C_out
 struct GcParams {
   const float* x;         // [B, Cin, Tin] fp32 with element strides xsb / xsc / xst
   int64_t xsb, xsc, xst;
@@ -50,11 +51,11 @@ struct GcParams {
 };
 bool gc_can_emit_image(int cout, int k, int u);
 
-// Streaming N-blocked conv for wide layers (C_in beyond a resident tile): operand-image input only.
-//   y = ((conv(ximg, d) + bias) + residual + acc_prev) / out_div
+// Wide layers (C > 256, several N blocks): like GcParams with a contiguous input, the branch sum and out_div.
+//   y = ((conv(act(x), d) + bias) + residual + acc_prev) / out_div
 struct GsParams {
   const uint16_t* ximg;   // [B][ceil16(Cin)/8][T][8] already activated operands, or nullptr ->
-  const float* x;         //   fp32 [B, Cin, T] contiguous, activated with lrelu(., pre_slope) by the loader warps
+  const float* x;         //   fp32 [B, Cin, T] contiguous, activated with lrelu(., pre_slope) in the loader
   float pre_slope;
   int mode;               // 0 conv ("same", dilation d); 1 conv-transpose (stride u, padding (k-u)/2)
   int u;
@@ -81,32 +82,31 @@ int launch_gc_pack_weight(const float* w_t, void* image, int mode, int cin, int 
 int launch_gemmconv(const GcParams& p, cudaStream_t s);
 
 
-// Persistent fused ResBlock chain (ab_kernels_rb.cu): npairs x nconv k-tap convs with the residual stream kept
-// on chip / in a thread-private L2-resident scratch, C <= 128.
-//   for p < npairs:  x <- x + conv[p][1](lrelu(conv[p][0](lrelu(x, slope), dil[p]) + b, slope), 1) + b   (nconv == 2)
-//                    x <- x + conv[p][0](lrelu(x, slope), dil[p]) + b                                      (nconv == 1)
+// One whole ResBlock per launch ("block mode", C <= 64): npairs x nconv k-tap convs with the residual stream x_p in
+// registers and the halo recomputed inside the time tile, so the block reads its input once and writes its output once.
+//   for q < npairs:  x <- x + conv[q][1](lrelu(conv[q][0](lrelu(x, slope), dil[q]) + b, slope), 1) + b   (nconv == 2)
+//                    x <- x + conv[q][0](lrelu(x, slope), dil[q]) + b                                      (nconv == 1)
 //   y = (x + acc_prev) / out_div ; yimg = cvt(lrelu(y, img_slope))
-constexpr int AB_RB_MAX_PAIRS = 3;
-struct RbParams {
+// Same arithmetic in the same order as npairs launches of launch_tc_conv: the results are bit-equal.
+constexpr int AB_TC_CHAIN_MAX_PAIRS = 3;
+constexpr int AB_TC_CHAIN_MAX_C = 64;
+struct TcChainParams {
   const float* x;          // contiguous [B, C, T] fp32 (block input = first residual)
-  const uint16_t* ximg;    // nullable: operand image of lrelu(x, slope), [B][Np/8][T][8]
+  const uint16_t* ximg;    // nullable: operand image of lrelu(x, slope), [B][ceil16(C)/8][T][8]
   float* y;                // contiguous [B, C, T] fp32
   const float* acc_prev;   // nullable (may alias y)
   uint16_t* yimg;          // nullable
-  const void* w[2 * AB_RB_MAX_PAIRS];      // tc weight images, step = pair * nconv + conv
-  const float* bias[2 * AB_RB_MAX_PAIRS];  // nullable entries
-  int dil[AB_RB_MAX_PAIRS];
+  const void* w[2 * AB_TC_CHAIN_MAX_PAIRS];      // tc weight images, step = pair * nconv + conv
+  const float* bias[2 * AB_TC_CHAIN_MAX_PAIRS];  // nullable entries
+  int dil[AB_TC_CHAIN_MAX_PAIRS];
   int npairs, nconv;
   int B, C, T, k;
   float slope, img_slope, out_div;
   int precision;
-  float* scratch;          // rb_scratch_bytes() bytes; required when npairs > 1 (shared-accumulator layout)
-  int split;               // 1: keep the residual stream in TMEM (two accumulators per slot, half the tile rows; C <= 64)
 };
-bool rb_supported(int C, int k);
-size_t rb_scratch_bytes();
-double rb_cost_per_row(int C, int k, const int* dil, int npairs, int nconv, int split = 0);
-int launch_rb(const RbParams& p, cudaStream_t s);
+// rows computed per valid output row (>= 1) of the block-mode tile, 0 when the block is not served
+double tc_chain_recompute(int C, int k, const int* dil, int npairs, int nconv);
+int launch_tc_chain(const TcChainParams& p, cudaStream_t s);
 
 int tc_max_channels();
 bool tc_conv_supported(int C, int k);

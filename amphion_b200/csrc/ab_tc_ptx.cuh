@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / mbarrier / bulk-TMA PTX wrappers shared by the tensor-core kernels (sm_100a).
+// mbarrier / bulk-copy (TMA 1-D) / wgmma PTX wrappers shared by the tensor-core kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -10,9 +10,6 @@
 namespace ab {
 namespace tcx {
 
-// ---------------------------------------------------------------------------
-// PTX helpers
-// ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -36,25 +33,17 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
-// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag) {
+// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.  No printf here: a
+// call inside the MMA loop would make ptxas serialise the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 22)) {
-      printf("amphion_b200: mbarrier timeout tag=%d block=%d thread=%d parity=%u\n", tag, blockIdx.x,
-             threadIdx.x, parity);
-      __trap();
-    }
+    if (++spins > (1u << 24)) __trap();
   }
 }
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile(
@@ -62,61 +51,34 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
       "l"(src), "r"(bytes), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with the accumulate flag as a compile-time constant: no register -> uniform-register move per MMA
-template <int ACC>
-__device__ __forceinline__ void tc_mma_f16_c(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "n"(ACC)
-      : "memory");
-}
-// Ampere-style async copies (LDGSTS): register-free, so the bytes in flight are not bounded by the
-// register file.  src_bytes = 0 zero-fills the 16-byte destination (used for out-of-range rows).
+// Ampere-style async copies: src_bytes = 0 zero-fills the 16-byte destination (out-of-range rows).
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait_group() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
+// warpgroup MMA ordering: fence before the first wgmma that touches the accumulator registers, commit after a
+// batch, wait until at most N batches are in flight
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+
+// Operand tiles are K-major without swizzle, in 8-row x 16-byte core matrices:
+//   [c8][row][8 x 16 bit]  — unit (c8, row) at (c8 * rows + row) * 16 bytes.
+// Rows are linear in memory, so a tap shift of s time steps is a +16*s byte move of the descriptor start, and one
+// resident activation tile serves every tap.  Consecutive rows of one c8 are consecutive 16-byte units: the
+// row-per-lane loaders and epilogues write 512 contiguous bytes per warp.
+__device__ __forceinline__ uint32_t unit_offset(int rows, int c8, int row) {
+  return ((uint32_t)c8 * (uint32_t)rows + (uint32_t)row) * 16u;
 }
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+// sm_90 matrix descriptor for that layout: start >> 4 @0, leading byte offset (next core matrix along K =
+// rows * 16 B) >> 4 @16, stride byte offset (next 8 rows = 128 B) >> 4 @32, no swizzle (0 @62).
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t rows) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(rows & 0x3FFFu) << 16) | ((uint64_t)(128u >> 4) << 32);
 }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // two fp32 -> packed 16-bit pair (first argument in the low half = lower address), round to nearest,
 // saturating to the largest finite value: operands must never become inf (DESIGN.md §5).  One F2FP.
@@ -133,33 +95,6 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi, int bf16) {
 
 // leaky_relu for 0 <= slope <= 1 (slope 1 = identity): max(v, slope*v)
 __device__ __forceinline__ float lrelu(float v, float slope) { return fmaxf(v, v * slope); }
-
-// Operand tile addressing: SWIZZLE_32B K-major rows.  `rows` = rows of the tile (A: rowsA, B: N block).
-//   [c16][row][32 B]; within a row the two 16-byte halves (8 channels each) are XOR-ed with address
-//   bit 7 (= (row>>2)&1 for a 256-byte aligned chunk), so each row's K=16 slice is 32 contiguous bytes
-//   and 8 consecutive rows hit 32 distinct banks.  (A no-swizzle interleaved variant was measured to
-//   give identical MMA rates: the operand path is 64 B/clk either way — DESIGN.md §6.)
-__device__ __forceinline__ uint32_t unit_offset(int rows, int c8, int row) {
-  return (uint32_t)(c8 >> 1) * (uint32_t)rows * 32u + (uint32_t)row * 32u +
-         ((uint32_t)((c8 & 1) ^ ((row >> 2) & 1)) << 4);
-}
-// descriptor constants for that layout (cute::UMMA::SmemDescriptor): SBO = 256 B (next 8-row group),
-// version 1, layout_type 6 (SWIZZLE_32B); LBO field 1 (unused for swizzled K-major)
-__device__ __forceinline__ uint64_t desc_hi_sw32() { return ((uint64_t)(16u | (1u << 14)) << 32) | (6ull << 61); }
-__device__ __forceinline__ uint32_t desc_lo_sw32(uint32_t addr16) { return addr16 | (1u << 16); }
-
-// one lane of a converged warp (the canonical way to issue tcgen05.mma / commit)
-__device__ __forceinline__ uint32_t elect_one_sync() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-      "elect.sync rx|px, %1;\n\t"
-      "@px mov.s32 %0, 1;\n\t}"
-      : "+r"(pred)
-      : "r"(0xffffffffu));
-  return pred;
-}
-
 
 }  // namespace tcx
 }  // namespace ab

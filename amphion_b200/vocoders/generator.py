@@ -220,7 +220,7 @@ class NativeGenerator(nn.Module):
         return wav
 
     def set_option(self, key: str, value: int):
-        """Execution-plan knob of the C ABI (`ab_generator_set_option`), e.g. ("resblock_fusion", 0..3)."""
+        """Execution-plan knob of the C ABI (`ab_generator_set_option`), e.g. ("nsf_source_frames", n)."""
         _capi.check(_capi.lib.ab_generator_set_option(self._ensure_handle(), key.encode(), int(value)), "set_option")
 
     # ---- per-kernel-class device timing (bench.py roofline) ------------------------

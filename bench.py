@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — vocoder audio samples/s on B200 (BASELINE.json metric, headline = config 2).
+"""bench.py — vocoder audio samples/s on one H100 (BASELINE.json metric, headline = config 2).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port)
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # + DIR/<output>.npy: what each timed path returned last
 
 Headline workload (config.workload): HiFi-GAN V1 22.05 kHz generator forward, batch 64 per GPU, 80x1024
 synthetic mel (random-init weights, torch.manual_seed(1234)).  A "step" is one generator forward over the
@@ -49,12 +50,20 @@ WORKLOADS = {
                           label="BigVGAN-large 24kHz", config="config 5 (per-GPU shard: 32 of 256 utterances)"),
 }
 N_MEL = 80   # kept for scripts that import it
+DUMP_BYTES = 8 << 20   # per dumped array; at most 6 arrays (4 generator workloads, mel and energy): <= 48 MB in all
+
+
+def _positive(v):
+    n = int(v)
+    if n < 1:
+        raise argparse.ArgumentTypeError("must be >= 1")
+    return n
 
 
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=_positive, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--batch", type=int, default=0, help="utterances per GPU (default: the workload's)")
@@ -64,6 +73,9 @@ def parse():
     ap.add_argument("--no-also", action="store_true", help="only the headline workload (quick iteration)")
     ap.add_argument("--workload", default="hifigan_v1", choices=list(WORKLOADS),
                     help="headline workload of the line; hifigan_v1 = BASELINE config 2 (default)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what each timed path returned in its last step to DIR/<name>.npy "
+                         "(float32; a fixed seeded sample of utterances when an array exceeds %d MB)" % (DUMP_BYTES >> 20))
     return ap.parse_args()
 
 
@@ -80,7 +92,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"], tensor=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 3.35 TB/s, dense FP16/BF16 989 TFLOP/s; not measured here
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor=989.0, source="H100 SXM data sheet")
 
 
 # --------------------------------------------------------------------------
@@ -237,20 +250,6 @@ class ClockSampler:
                     power_w_max=max(pw), samples=len(sm))
 
 
-def _traffic(workload, B, T, precision, dom):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture of the same workload
-    (profiles/r2_traffic.json, written by scripts/ncu_traffic.py); None when no capture matches."""
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        e = tr[workload]
-        if (e["batch"], e["frames"], e["precision"]) == (B, T, precision) and dom in e["kernels"]:
-            k = e["kernels"][dom]
-            return k["bytes_per_launch"], "profiles/r2_traffic.json (ncu dram__bytes_read+write, mean of the %d %s launches of one forward)" % (k["launches"], dom)
-    except (OSError, KeyError, ValueError, TypeError):
-        pass
-    return None, None
-
-
 def _roofline(prof, ms_total, samples_rank_step, flop, workload, B, T, precision):
     pk = peaks()
     dom = max(prof, key=lambda k: prof[k]["ms"])
@@ -271,13 +270,26 @@ def _roofline(prof, ms_total, samples_rank_step, flop, workload, B, T, precision
                       note="algorithmic bytes: fp32 x read + y write (+ branch sum) + weights once"),
              classes={k: dict(launches=v["launches"], ms=round(v["ms"], 3)) for k, v in prof.items() if v["launches"]})
     r["algorithmic_bytes_per_launch"] = d["bytes"] / max(d["launches"], 1)
-    r["traffic"], src = _traffic(workload, B, T, precision, dom)
-    if src:
-        r["traffic_source"] = src
     return r
 
 
-def measure_generator(workload, args, dev, rank, world, steps, warmup, want_cpu, clocks_on_rank0=True, shape=None):
+def dump_output(out_dir, name, t):
+    """One output as float32 DIR/<name>.npy.  Above DUMP_BYTES: a seeded, sorted sample of utterances (dim 0), and
+    if one utterance alone is larger, the first DUMP_BYTES of each sampled utterance."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    a = t.float().cpu().numpy()
+    per = a[0].size * 4
+    n = max(1, min(a.shape[0], DUMP_BYTES // max(per, 1)))
+    if n < a.shape[0]:
+        a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], n, replace=False))]
+    if per > DUMP_BYTES:
+        a = a.reshape(a.shape[0], -1)[:, : DUMP_BYTES // 4]
+    np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
+def measure_generator(workload, args, dev, rank, world, steps, warmup, want_cpu, clocks_on_rank0=True, shape=None,
+                      dump_dir=None, dump_name=None):
     """One workload on the native path: device-resident `value` (CUDA events, max over ranks), `e2e` through the
     reference-facing call with pinned host buffers, per-class roofline from the C ABI's launch events."""
     import torch
@@ -328,10 +340,13 @@ def measure_generator(workload, args, dev, rank, world, steps, warmup, want_cpu,
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            step()
+            last = step()
         e1.record()
         torch.cuda.synchronize(); barrier()
         ms_total = e0.elapsed_time(e1)
+        if dump_dir and rank == 0:
+            dump_output(dump_dir, dump_name or workload, last)
+        del last
         prof = model.get_profile()
         model.set_profiling(False)
         clocks = sampler.stop() if (rank == 0 and clocks_on_rank0) else None
@@ -385,7 +400,7 @@ def measure_generator(workload, args, dev, rank, world, steps, warmup, want_cpu,
     return res
 
 
-def measure_mel(dev, steps=10, want_cpu=True):
+def measure_mel(dev, steps=10, want_cpu=True, dump_dir=None):
     """Config 4: TacotronSTFT(1024,256,1024,80,22050,0,8000).mel_spectrogram on 64 x 10 s @ 22.05 kHz."""
     import torch
     from amphion_b200 import mel as M
@@ -409,6 +424,9 @@ def measure_mel(dev, steps=10, want_cpu=True):
         flush.zero_()                      # inputs (56 MB) fit in L2: flush between timed iterations
         e0.record(); out = step(); e1.record(); torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
     ms = statistics.median(ts)
+    if dump_dir:
+        dump_output(dump_dir, "mel", out[1])
+        dump_output(dump_dir, "mel_energy", out[2])
     F = out[1].shape[-1]
     algo = yd.numel() * 4 + out[1].numel() * 4 + out[2].numel() * 4
     pk = peaks()
@@ -432,9 +450,6 @@ def measure_mel(dev, steps=10, want_cpu=True):
                e2e=dict(value=yd.numel() / e2e_ms * 1e3, unit=UNIT, ms_per_step=e2e_ms, h2d_bytes_per_step=yd.numel() * 4,
                         d2h_bytes_per_step=(mel_h.numel() + en_h.numel()) * 4,
                         api="TacotronSTFT.mel_spectrogram(pinned_host_wav) -> CPU (mel, energy)"))
-    tr, src = _traffic("mel", 64, 220500, "fp32", "mel")
-    if tr:
-        res["roofline"]["traffic"], res["roofline"]["traffic_source"] = tr, src
     if want_cpu:
         import numpy as np
         from oracle import mel as om
@@ -519,29 +534,33 @@ def run_native(args, rank, local_rank, world):
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     want_cpu = world == 1 and not args.no_cpu_baseline
-    main = measure_generator(args.workload, args, dev, rank, world, args.steps, args.warmup, want_cpu)
+    main = measure_generator(args.workload, args, dev, rank, world, args.steps, args.warmup, want_cpu,
+                             dump_dir=args.dump_outputs)
     also, eager = {}, None
     if not args.no_also and not os.environ.get("AB_BENCH_PROFILE"):
         if world == 1:
             for wl in ("bigvgan_base", "bigvgan_large"):
                 if wl != args.workload:
-                    also[wl] = measure_generator(wl, args, dev, rank, world, 3, 3, want_cpu, clocks_on_rank0=False)
-            also["mel"] = measure_mel(dev, want_cpu=want_cpu)
+                    also[wl] = measure_generator(wl, args, dev, rank, world, 3, 3, want_cpu, clocks_on_rank0=False,
+                                                 dump_dir=args.dump_outputs)
+            also["mel"] = measure_mel(dev, want_cpu=want_cpu, dump_dir=args.dump_outputs)
             # BASELINE config 1: HiFi-GAN V1, batch 1, 80x200 mel through the egs/vocoder plumbing (CPU leg timed in full)
-            r = measure_generator("hifigan_v1", args, dev, rank, world, 20, 3, want_cpu, clocks_on_rank0=False, shape=(1, 200))
+            r = measure_generator("hifigan_v1", args, dev, rank, world, 20, 3, want_cpu, clocks_on_rank0=False, shape=(1, 200),
+                                  dump_dir=args.dump_outputs, dump_name="hifigan_v1_b1_t200")
             r["baseline_config"] = "config 1 (batch 1, 80x200 mel; the reference runs it on the CPU)"
             also["hifigan_v1_b1_t200"] = r
             eager = measure_gpu_eager(args, dev)
         elif args.workload != "bigvgan_large":
             # BASELINE config 5: BigVGAN-large, 32 utterances per GPU, 100x2048 mel, gather to rank 0
-            r = measure_generator("bigvgan_large", args, dev, rank, world, 3, 3, False, clocks_on_rank0=False)
+            r = measure_generator("bigvgan_large", args, dev, rank, world, 3, 3, False, clocks_on_rank0=False,
+                                  dump_dir=args.dump_outputs)
             if rank == 0:
                 r["baseline_config"] = "config 5 (batch %d sharded 32/GPU across %d GPUs, gather to rank 0)" % (32 * world, world)
                 also["bigvgan_large"] = r
     if rank == 0:
         w = WORKLOADS[args.workload]
-        dt = {"fp32": "f32", "tc_f16": "f16 operands, f32 accumulate (tcgen05); f32 elsewhere",
-              "tc_bf16": "bf16 operands, f32 accumulate (tcgen05); f32 elsewhere"}[args.precision]
+        dt = {"fp32": "f32", "tc_f16": "f16 operands, f32 accumulate (wgmma); f32 elsewhere",
+              "tc_bf16": "bf16 operands, f32 accumulate (wgmma); f32 elsewhere"}[args.precision]
         line = dict(metric=METRIC, value=main["value"], unit=UNIT, n_gpus=world, steps=args.steps,
                     warmup=max(args.warmup, 3), ms_per_step=main["ms_per_step"], higher_is_better=True, scaling="weak",
                     vs_baseline=None, dtype=dt, data="synthetic",
@@ -549,7 +568,7 @@ def run_native(args, rank, local_rank, world):
                                 frames=main["frames"], hop=HOP, precision=args.precision,
                                 parallelism="utterance-batch sharding dp%d, gather of the wav shards to rank 0 (NCCL send/recv, chunked under the last layer)" % world
                                 if world > 1 else "single GPU",
-                                l2="no explicit flush: each step streams > 8 GB of stage tensors (>> 126 MB L2)"),
+                                l2="no explicit flush: each step streams > 8 GB of stage tensors (>> 50 MB L2)"),
                     e2e=main["e2e"], gpu_launches=main["gpu_launches"], clocks=main["clocks"],
                     roofline=main["roofline"], cpu_baseline=main.get("cpu_baseline"), impl="native")
         if also:
@@ -568,7 +587,7 @@ def main():
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.gpus > 1 and world == 1 and "RANK" not in os.environ:
-        # convenience: re-launch under torchrun exactly as the driver does
+        # convenience: re-launch under torchrun, one process per GPU
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}",
                "--master-addr", "127.0.0.1", "--master-port", os.environ.get("MASTER_PORT", "29533"),
                os.path.abspath(__file__)] + sys.argv[1:]

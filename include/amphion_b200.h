@@ -1,5 +1,5 @@
 /*
- * amphion_b200 — C ABI of the B200-native vocoder-inference hot path.
+ * amphion_b200 — C ABI of the H100-native vocoder-inference hot path.
  *
  * The reference (open-mmlab/Amphion) is pure Python: it has no FFI.  Its
  * "operator API" for this path is the duck-typed Python surface listed in
@@ -55,14 +55,14 @@ enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
   AB_PREC_FP32 = 0,   /* CUDA-core FFMA, fp32 operands and accumulation */
-  AB_PREC_TC_F16 = 1, /* tcgen05.mma kind::f16, fp16 operands (saturating cvt), fp32 accumulation in TMEM */
-  AB_PREC_TC_BF16 = 2 /* tcgen05.mma kind::f16, bf16 operands, fp32 accumulation in TMEM */
+  AB_PREC_TC_F16 = 1, /* wgmma, fp16 operands (saturating cvt), fp32 accumulation */
+  AB_PREC_TC_BF16 = 2 /* wgmma, bf16 operands, fp32 accumulation */
 };
 
 const char* ab_last_error(void);
 int ab_version(void);
-/* 1 if the current device is compute capability 10.x (tcgen05 path usable) */
-int ab_device_is_sm100(void);
+/* 1 if the current device is compute capability 9.x (wgmma path usable) */
+int ab_device_is_sm90(void);
 
 /* ------------------------------------------------------------------------
  * Generator: HiFiGAN.forward     (models/vocoders/gan/generator/hifigan.py:203-219)
@@ -156,10 +156,10 @@ typedef struct ab_profile_entry {
 } ab_profile_entry;
 int ab_generator_set_profiling(ab_generator* g, int32_t enable);
 /* Execution-plan options (no reference counterpart; tuning / test knobs, results stay within the stated tolerance):
- *   "resblock_fusion": 0 = one launch per (c1, c2) pair on the per-tile kernel, 1 = persistent kernel with one
- *   pair per launch, 2 (default) = persistent kernel, a whole ResBlock per launch when the cost model prefers
- *   it (with the residual stream resident in TMEM where that is cheaper still), 3 = always a whole ResBlock per
- *   launch with the shared accumulator, 4 = always a whole ResBlock per launch, TMEM-resident residual where served.
+ *   "resblock_fusion": 0, 1 = one launch per (c1, c2) pair (the intermediate stays in shared memory); 2 (default) = a
+ *   whole ResBlock per launch (residual stream in registers, halo recomputed in the tile) where served (C <= 64) and
+ *   the recompute is small, else per pair; 3, 4 = a whole ResBlock per launch wherever served.  All plans run the same
+ *   arithmetic in the same order: their outputs are bit-equal.
  *   "nsf_source_frames" (NSF-HiFiGAN, one-shot, consumed by the next forward): frames of the f0 track when it does
  *   not cover the mel; every stage is then truncated to the harmonic source's length as the reference does
  *   (nsfhifigan.py:264-268) and the output holds ab_generator_output_samples() samples per utterance.

@@ -7,7 +7,7 @@ package: only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s
 The oracle is a restatement, in numpy / CPU-torch primitives, of the algorithm
 in the reference files cited function by function.  It is pinned against
 outputs of the reference modules themselves (``tests/golden/*.npz``, generated
-by ``tests/golden/gen_golden.py`` which imports ``/root/reference``); the
+by ``tests/golden/gen_golden.py`` which imports the reference (open-mmlab/Amphion)); the
 reference ships no golden vectors or tests of its own for this path
 (SURVEY.md §4), so those fixtures are the pin.
 """

@@ -11,7 +11,7 @@ Two sets of primitives are provided:
   * default   : the same maths through ``torch.nn.functional`` on CPU fp32,
                 used for speed; cross-checked against ``*_np`` in
                 tests/test_oracle.py.
-All citations are to files under /root/reference.
+All citations are to files of the reference (open-mmlab/Amphion).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Oracle: the arithmetic of save_audio (/root/reference/utils/io.py:49-76) in numpy.
+"""Oracle: the arithmetic of save_audio (utils/io.py of the reference:49-76) in numpy.
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 

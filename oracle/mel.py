@@ -2,11 +2,11 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
-Third-party arithmetic not present under /root/reference is restated here from
+Third-party arithmetic not present of the reference (open-mmlab/Amphion) is restated here from
 its published algorithm (the reference pins ``librosa==0.9.1`` in env.sh:13):
   * ``librosa.filters.mel`` (Slaney scale, ``norm="slaney"``)  -> ``slaney_mel_filterbank``
   * ``librosa.util.pad_center``                                  -> ``pad_center``
-All citations are to files under /root/reference.
+All citations are to files of the reference (open-mmlab/Amphion).
 """
 from __future__ import annotations
 

@@ -25,7 +25,7 @@ F = out[1].shape[-1]
 algo_bytes = y.numel() * 4 + out[1].numel() * 4 + out[2].numel() * 4
 print(json.dumps(dict(workload="TacotronSTFT mel 64x10s@22.05kHz", frames=int(64 * F), ms=ms, best_ms=min(ts),
                       frames_per_s=64 * F / ms * 1e3, audio_samples_per_s=y.numel() / ms * 1e3,
-                      algorithmic_GBs=algo_bytes / ms / 1e6, hbm_frac=algo_bytes / ms / 1e6 / 6574.1)))
+                      algorithmic_GBs=algo_bytes / ms / 1e6, hbm_frac=algo_bytes / ms / 1e6 / 3350.0)))   # H100 SXM data-sheet HBM3 GB/s
 # torch eager (the reference's ops on the same GPU, TF32 off) for context
 torch.backends.cuda.matmul.allow_tf32 = False
 def ref():

@@ -1,3 +1,4 @@
+import glob
 import os
 import sys
 
@@ -20,12 +21,15 @@ except Exception:  # pragma: no cover
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 def load_golden(name):
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
-    d = {k: z[k] for k in z.files}
+    # a fixture may be split over name.npz and name.part<N>.npz (every stored file stays under 1 MB)
+    d = {}
+    for f in [name + ".npz"] + sorted(glob.glob(os.path.join(GOLDEN, glob.escape(name) + ".part*.npz"))):
+        z = np.load(os.path.join(GOLDEN, f))
+        d.update({k: z[k] for k in z.files})
     sd = {k[3:]: v for k, v in d.items() if k.startswith("sd:")}
     rest = {k: v for k, v in d.items() if not k.startswith("sd:")}
     return rest, sd

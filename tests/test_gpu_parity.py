@@ -206,7 +206,7 @@ def test_generator_tensor_core_matches_reference_fixture(name):
 
 
 TC_CASES = [
-    # C, T, k, d   (single conv through the tcgen05 kernel)
+    # C, T, k, d   (single conv through the wgmma kernel)
     (64, 128, 1, 1),      # pure GEMM: no tap shifts
     (64, 200, 3, 1),      # tap shifts of one row
     (32, 1000, 3, 3),
@@ -603,7 +603,7 @@ def test_hifigan_vits_decoder_size_matches_oracle():
     assert np.abs(got - want).max() <= 1e-3, np.abs(got - want).max()
 
 
-# ---- persistent fused ResBlock kernel (ab_kernels_rb.cu): execution-plan modes -------------------------------
+# ---- ResBlock execution plans (ab_kernels_tc.cu): one launch per pair vs a whole block per launch -------------------------------
 def _fusion_outputs(model, mel, modes):
     outs = {}
     for mode in modes:
@@ -615,10 +615,10 @@ def _fusion_outputs(model, mel, modes):
 
 @pytest.mark.parametrize("B,T", [(2, 40), (3, 150), (1, 37)])
 def test_resblock_fusion_modes_agree_on_v1(B, T):
-    """HiFi-GAN V1 (stages of 256/128/64/32 channels).  The persistent kernel one pair per launch (1), the
-    cost-model plan (2) and whole-block fusion with halo recompute (3) run the same arithmetic in the same order
-    and must agree to the last bit (recomputed halo rows == the rows another tile owns).  The per-pair kernel (0)
-    adds the residual after the convolution instead of accumulating on top of it: fp32 summation order only.
+    """HiFi-GAN V1 (stages of 256/128/64/32 channels).  One launch per pair (0, 1), the cost-model plan (2) and
+    whole-block launches with the residual stream in registers and the halo recomputed (3, 4; the 64- and 32-channel
+    stages) run the same arithmetic in the same order and must agree to the last bit (recomputed halo rows == the
+    rows another tile owns).
     T=150 gives several tiles per sequence and an odd tile count, T=37 a ragged single tile."""
     model = build_model("hifigan", HP_V1, 80, seed=4321).to(DEV)
     mel = torch.randn(B, 80, T, generator=torch.Generator().manual_seed(T)).to(DEV)
@@ -626,8 +626,6 @@ def test_resblock_fusion_modes_agree_on_v1(B, T):
     for mode in (1, 2, 3, 4):
         assert torch.isfinite(outs[mode]).all()
     assert torch.equal(outs[1], outs[3])
-    # the per-pair kernel (0) adds the residual after the convolution; plans with the TMEM-resident residual (2, 4)
-    # accumulate every conv2 of a block on top of x without intermediate rounding of x_p: fp32 summation order only
     for mode in (0, 2, 4):
         diff = (outs[mode] - outs[3]).abs().max().item()
         assert diff <= 3e-5, (mode, diff)
