@@ -81,10 +81,9 @@ struct HcGeom {
   int dil[AB_TC_CHAIN_MAX_PAIRS];
 };
 
-// CHAIN: block mode — the residual stream x_p of a whole ResBlock stays in registers in the accumulator fragment
-// layout (one CTA per SM for the doubled register use); otherwise modes 0-2.
-template <int NW, int BF16, bool CHAIN>
-__global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
+// modes 0-2; block mode runs on hchain_kernel below
+template <int NW, int BF16>
+__global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -98,9 +97,8 @@ __global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hcon
   auto bar_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
 
   const int total1 = g.NB * g.nkc * g.ntaps;
-  const int total = CHAIN ? g.nsteps * total1 : total1 + (g.mode == 2 ? g.nkc2 * g.ntaps : 0);
+  const int total = total1 + (g.mode == 2 ? g.nkc2 * g.ntaps : 0);
   auto stage_src = [&](int it) -> const uint8_t* {
-    if (CHAIN) return static_cast<const uint8_t*>(p.ws[it / total1]) + (size_t)(it % total1) * g.stage_bytes;
     return it < total1 ? static_cast<const uint8_t*>(p.w) + (size_t)it * g.stage_bytes
                        : static_cast<const uint8_t*>(p.w2) + (size_t)(it - total1) * g.stage_bytes;
   };
@@ -112,19 +110,16 @@ __global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hcon
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  const int nbias = CHAIN ? g.nsteps * NW : g.mode == 2 ? 2 * NW : g.NB * NW;
+  const int nbias = g.mode == 2 ? 2 * NW : g.NB * NW;
   for (int i = tid; i < nbias; i += HC_THREADS) {
     float v = 0.f;
-    if (CHAIN) {
-      const int st = i / NW, c = i - st * NW;
-      v = (p.bs[st] && c < p.Cout) ? __ldg(p.bs[st] + c) : 0.f;
-    } else if (g.mode == 2) v = i < NW ? ((p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f)
+    if (g.mode == 2) v = i < NW ? ((p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f)
                                 : ((p.bias2 && i - NW < p.Cout) ? __ldg(p.bias2 + i - NW) : 0.f);
     else v = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
     bias_s[i] = v;
   }
-  if (g.mode == 2 || CHAIN) {   // channels of the intermediate beyond the accumulator width stay zero
-    const int n16 = CHAIN ? g.nkc * 4 * g.rowsX : g.nkc2 * 4 * g.rowsI;
+  if (g.mode == 2) {   // channels of the intermediate beyond the accumulator width stay zero
+    const int n16 = g.nkc2 * 4 * g.rowsI;
     for (int i = tid; i < n16; i += HC_THREADS) *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
   }
   __syncthreads();
@@ -246,131 +241,7 @@ __global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hcon
     }
   };
 
-  if constexpr (CHAIN) {
-    // operand tile X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row
-    const int n16 = g.nkc * 4 * g.rowsX;
-    if (p.ximg != nullptr) {
-      const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
-      for (int idx = tid; idx < n16; idx += HC_THREADS) {
-        const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX;
-        const int t = O - g.H - g.G + row;
-        const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
-        cp_async16(sA + unit_offset(g.rowsX, c8, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
-                   ok ? 16u : 0u);
-      }
-      cp_async_wait_all();
-    } else {
-      const float* xb = p.x + (int64_t)b * p.xsb;
-      for (int idx = tid; idx < n16; idx += HC_THREADS) {
-        const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX;
-        const int t = O - g.H - g.G + row;
-        const bool ok = t >= 0 && t < g.Tin;
-        float v[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int ci = c8 * 8 + e;
-          v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
-        }
-        uint4 q;
-        q.x = pack2t<BF16>(v[0], v[1]);
-        q.y = pack2t<BF16>(v[2], v[3]);
-        q.z = pack2t<BF16>(v[4], v[5]);
-        q.w = pack2t<BF16>(v[6], v[7]);
-        *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsX, c8, row)) = q;
-      }
-    }
-    fence_proxy_async();
-    __syncthreads();
-    // residual stream in the fragment layout: xr = x at (row, column) of this thread's accumulators
-    float xr[MT][NACC];
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int t = O - g.H + frag_row(mt, h);
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int co = c * 8 + col_l + e;
-            xr[mt][c * 4 + 2 * h + e] = (t >= 0 && t < g.Tin && co < p.Cout) ? __ldg(p.x + ((int64_t)b * p.Cout + co) * g.Tin + t) : 0.f;
-          }
-      }
-    // lrelu(v, slope) of the fragment -> operand tile at base (rows offset by G), zero outside [0, T)
-    auto store_tile = [&](uint32_t off, const float (&v)[MT][NACC], const float* bb) {
-      __syncthreads();   // ResBlock2 (one conv per step) overwrites the tile its own MMAs just read
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = frag_row(mt, h), t = O - g.H + row;
-          const bool ok = t >= 0 && t < g.Tin;
-#pragma unroll
-          for (int c = 0; c < NW / 8; ++c) {
-            if (c >= g.nkc * 4) continue;
-            const int col = c * 8 + col_l;
-            const float a0 = bb ? v[mt][c * 4 + 2 * h] + bb[col] : v[mt][c * 4 + 2 * h];
-            const float a1 = bb ? v[mt][c * 4 + 2 * h + 1] + bb[col + 1] : v[mt][c * 4 + 2 * h + 1];
-            const uint32_t q = ok ? pack2t<BF16>(lrelu(a0, g.mid_slope), lrelu(a1, g.mid_slope)) : 0u;
-            *reinterpret_cast<uint32_t*>(smem + off + unit_offset(g.rowsX, c, row + g.G) + 2 * col_l) = q;
-          }
-        }
-      fence_proxy_async();
-      __syncthreads();
-    };
-    for (int st = 0; st < g.nsteps; ++st) {
-      const int pr = st / g.nconv, cv = st - pr * g.nconv;
-      const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.k - 1) * d / 2;
-      const uint32_t aT = cv == 0 ? sA : sI;
-      bool first = true;
-      for (int kc = 0; kc < g.nkc; ++kc)
-        mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.rowsX, g.k, d, false, first);
-      const float* bb = bias_s + st * NW;
-      if (g.nconv == 2 && cv == 0) {
-        store_tile(g.off_i, acc, bb);
-      } else {
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-          for (int c = 0; c < NW / 8; ++c)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float a = acc[mt][c * 4 + i] + bb[c * 8 + col_l + (i & 1)];
-              a += xr[mt][c * 4 + i];
-              xr[mt][c * 4 + i] = a;
-            }
-        if (st + 1 < g.nsteps) store_tile(0, xr, nullptr);
-      }
-    }
-    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); yimg = cvt(lrelu(y, img_slope))
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = frag_row(mt, h), t = O - g.H + row;
-        if (row < g.H || row >= g.H + g.V || t >= g.Tout) continue;
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c) {
-          const int co = c * 8 + col_l;
-          float ve[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            ve[e] = 0.f;
-            if (co + e < p.Cout) {
-              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
-              float v = xr[mt][c * 4 + 2 * h + e];
-              if (p.acc_prev) v += p.acc_prev[idx];
-              v *= g.out_scale;
-              p.y[idx] = v;
-              ve[e] = v;
-            }
-          }
-          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
-            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
-                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
-        }
-      }
-  } else if (g.mode != 2) {
+  if (g.mode != 2) {
     for (int nb = 0; nb < g.NB; ++nb) {
       bool first = true;
       for (int kc = 0; kc < g.nkc; ++kc) {
@@ -434,6 +305,268 @@ __global__ void __launch_bounds__(HC_THREADS, (NW >= 256 || CHAIN) ? 1 : 2) hcon
     for (int kc = 0; kc < g.nkc2; ++kc)
       mma_chunk(sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, g.ntaps, 1, false, first);
     epilogue_conv(0, bias_s + NW);
+  }
+}
+
+// Block mode (launch_tc_chain): warp-specialised and persistent.  One CTA of three warpgroups per SM walks the
+// (utterance, time tile) work items with a static stride.
+//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams the weight stages of every tile through the W ring;
+//     warps 1-3 load the operand tile X of the next work item as soon as the consumers release it, so that load
+//     overlaps the current tile's output epilogue.
+//   warpgroups 1-2 (consumers, setmaxnreg 232): one wgmma batch per tap with the previous batch still in flight; a
+//     W slot is released once the batch that read it has completed.  Consumer-only synchronisation is a named
+//     barrier.  The residual stream x_p of the whole ResBlock stays in registers in the accumulator fragment layout.
+// The accumulation order of every output element is that of hconv_kernel's per-pair mode (K chunk -> tap -> k16).
+constexpr int HB_THREADS = 3 * 128;
+constexpr int HB_LOADERS = 96;
+constexpr int HB_PRODUCER_REGS = 40;
+constexpr int HB_CONSUMER_REGS = 232;
+static_assert(128 * HB_PRODUCER_REGS + 256 * HB_CONSUMER_REGS <= 65536, "setmaxnreg split of the register file");
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+template <int NW, int BF16>
+__global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom g) {
+  constexpr int MT = mt_of(NW);
+  constexpr int NACC = NW / 2;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const uint32_t sX = smem_u32(smem), sI = sX + g.off_i, sW = sX + g.off_w;
+  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
+  const uint32_t bar0 = smem_u32(smem + g.off_bar);
+  auto w_full = [&](int s) { return bar0 + 8u * s; };
+  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
+  const uint32_t x_full = bar0 + 16u * HC_STAGES_MAX, x_empty = x_full + 8u;
+  const int nwork = p.B * g.tiles;
+  const int total1 = g.nkc * g.ntaps;
+  const int total = g.nsteps * total1;
+
+  if (tid == 0) {
+    for (int s = 0; s < g.nstages; ++s) {
+      mbar_init(w_full(s), 1);
+      mbar_init(w_empty(s), 8);
+    }
+    mbar_init(x_full, HB_LOADERS);
+    mbar_init(x_empty, 8);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < g.nsteps * NW; i += HB_THREADS) {
+    const int st = i / NW, c = i - st * NW;
+    bias_s[i] = (p.bs[st] && c < p.Cout) ? __ldg(p.bs[st] + c) : 0.f;
+  }
+  // rows and channels of the intermediate that no step writes stay zero for every tile
+  for (int i = tid; i < g.nkc * 4 * g.rowsX; i += HB_THREADS)
+    *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
+  fence_proxy_async();
+  __syncthreads();
+
+  // ------------------------------------------------------------------------------------------------ producer
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+    if (tid == 0) {
+      int wi = 0;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+        for (int i = 0; i < total; ++i, ++wi) {
+          const int s = wi % g.nstages;
+          if (wi >= g.nstages) mbar_wait(w_empty(s), (uint32_t)(wi / g.nstages - 1) & 1u);
+          mbar_arrive_expect_tx(w_full(s), g.stage_bytes);
+          bulk_g2s(sW + (uint32_t)s * g.stage_bytes,
+                   static_cast<const uint8_t*>(p.ws[i / total1]) + (size_t)(i % total1) * g.stage_bytes,
+                   g.stage_bytes, w_full(s));
+        }
+      }
+    } else if (tid >= 32) {
+      // X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row, zero outside [0, Tin)
+      const int lt = tid - 32, n16 = g.nkc * 4 * g.rowsX;
+      int n = 0;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
+        const int b = w / g.tiles, t0 = (w - b * g.tiles) * g.V - g.H - g.G;
+        if (n > 0) mbar_wait(x_empty, (uint32_t)(n - 1) & 1u);
+        if (p.ximg != nullptr) {
+          const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
+          for (int idx = lt; idx < n16; idx += HB_LOADERS) {
+            const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX, t = t0 + row;
+            const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
+            cp_async16(sX + unit_offset(g.rowsX, c8, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
+                       ok ? 16u : 0u);
+          }
+          cp_async_wait_all();
+        } else {
+          const float* xb = p.x + (int64_t)b * p.xsb;
+          for (int idx = lt; idx < n16; idx += HB_LOADERS) {
+            const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX, t = t0 + row;
+            const bool ok = t >= 0 && t < g.Tin;
+            float v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int ci = c8 * 8 + e;
+              v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
+            }
+            uint4 q;
+            q.x = pack2t<BF16>(v[0], v[1]);
+            q.y = pack2t<BF16>(v[2], v[3]);
+            q.z = pack2t<BF16>(v[4], v[5]);
+            q.w = pack2t<BF16>(v[6], v[7]);
+            *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsX, c8, row)) = q;
+          }
+        }
+        fence_proxy_async();
+        mbar_arrive(x_full);
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------------------------------------ consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
+  const int cw = wg - 1, wq = (tid >> 5) & 3;
+  float acc[MT][NACC];
+  int it = 0;        // weight stages consumed so far
+  int pw = -1;       // W slot read by the batch still in flight (-1: none)
+
+  // keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
+  auto fence_acc = [&]() {
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
+  };
+  auto release_w = [&]() {
+    __syncwarp();
+    if (lane == 0 && pw >= 0) mbar_arrive(w_empty(pw));
+  };
+  // the taps of one 32-channel K chunk over the operand at aBase
+  auto mma_chunk = [&](uint32_t aBase, int ntaps, int tapstep, bool& first) {
+    for (int j = 0; j < ntaps; ++j, ++it) {
+      const int s = it % g.nstages;
+      mbar_wait(w_full(s), (uint32_t)(it / g.nstages) & 1u);
+      const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
+      fence_acc();
+      wg_fence();
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+          const uint32_t a = aBase + (uint32_t)(2 * ks * g.rowsX + (cw * MT + mt) * 64 + j * tapstep) * 16u;
+          const uint32_t w = wS + (uint32_t)(2 * ks * NW) * 16u;
+          Wgmma<NW, BF16>::mma(acc[mt], make_desc(a, (uint32_t)g.rowsX), make_desc(w, (uint32_t)NW), (first && ks == 0) ? 0 : 1);
+        }
+      }
+      wg_commit();
+      wg_wait<1>();      // the previous batch has completed: its W slot can be refilled
+      fence_acc();
+      release_w();
+      pw = s;
+      first = false;
+    }
+  };
+  auto drain = [&]() {
+    wg_wait<0>();
+    fence_acc();
+    release_w();
+    pw = -1;
+  };
+
+  // accumulator fragment (m64nNk16, fp32): element [c*4 + 2h + e] of tile mt is row 16*wq + lane/4 + 8h,
+  // column 8c + 2*(lane%4) + e of this warpgroup's mt-th m64 tile
+  auto frag_row = [&](int mt, int h) { return (cw * MT + mt) * 64 + wq * 16 + (lane >> 2) + 8 * h; };
+  const int col_l = 2 * (lane & 3);
+  int n = 0;
+  for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
+    const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
+    // residual stream in the fragment layout: xr = x at (row, column) of this thread's accumulators
+    float xr[MT][NACC];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = O - g.H + frag_row(mt, h);
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = c * 8 + col_l + e;
+            xr[mt][c * 4 + 2 * h + e] = (t >= 0 && t < g.Tin && co < p.Cout) ? __ldg(p.x + ((int64_t)b * p.Cout + co) * g.Tin + t) : 0.f;
+          }
+      }
+    mbar_wait(x_full, (uint32_t)n & 1u);
+    // lrelu(v, slope) of the fragment -> operand tile at off (rows offset by G), zero outside [0, T)
+    auto store_tile = [&](uint32_t off, const float (&v)[MT][NACC], const float* bb) {
+      consumer_sync();   // both warpgroups have finished the MMAs that read the tile (ResBlock2 overwrites X)
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frag_row(mt, h), t = O - g.H + row;
+          const bool ok = t >= 0 && t < g.Tin;
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c) {
+            if (c >= g.nkc * 4) continue;
+            const int col = c * 8 + col_l;
+            const float a0 = bb ? v[mt][c * 4 + 2 * h] + bb[col] : v[mt][c * 4 + 2 * h];
+            const float a1 = bb ? v[mt][c * 4 + 2 * h + 1] + bb[col + 1] : v[mt][c * 4 + 2 * h + 1];
+            const uint32_t q = ok ? pack2t<BF16>(lrelu(a0, g.mid_slope), lrelu(a1, g.mid_slope)) : 0u;
+            *reinterpret_cast<uint32_t*>(smem + off + unit_offset(g.rowsX, c, row + g.G) + 2 * col_l) = q;
+          }
+        }
+      fence_proxy_async();
+      consumer_sync();
+    };
+    for (int st = 0; st < g.nsteps; ++st) {
+      const int pr = st / g.nconv, cv = st - pr * g.nconv;
+      const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.k - 1) * d / 2;
+      const uint32_t aT = cv == 0 ? sX : sI;
+      bool first = true;
+      for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.k, d, first);
+      drain();
+      const float* bb = bias_s + st * NW;
+      if (g.nconv == 2 && cv == 0) {
+        store_tile(g.off_i, acc, bb);
+      } else {
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              float a = acc[mt][c * 4 + i] + bb[c * 8 + col_l + (i & 1)];
+              a += xr[mt][c * 4 + i];
+              xr[mt][c * 4 + i] = a;
+            }
+        if (st + 1 < g.nsteps) store_tile(0, xr, nullptr);
+      }
+    }
+    // every MMA of this tile has completed: the producer may load the next X
+    __syncwarp();
+    if (lane == 0) mbar_arrive(x_empty);
+    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); yimg = cvt(lrelu(y, img_slope))
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = frag_row(mt, h), t = O - g.H + row;
+        if (row < g.H || row >= g.H + g.V || t >= g.Tout) continue;
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c) {
+          const int co = c * 8 + col_l;
+          float ve[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            ve[e] = 0.f;
+            if (co + e < p.Cout) {
+              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
+              float v = xr[mt][c * 4 + 2 * h + e];
+              if (p.acc_prev) v += p.acc_prev[idx];
+              v *= g.out_scale;
+              p.y[idx] = v;
+              ve[e] = v;
+            }
+          }
+          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
+            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
+        }
+      }
   }
 }
 
@@ -585,19 +718,38 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
   return AB_OK;
 }
 
-template <int NW, bool CHAIN = false>
+template <int NW>
 int launch_nw(const HcArgs& a, const HcGeom& g, int bf16, cudaStream_t s) {
   static DeviceOnce configured;
   if (configured.need()) {
-    const int lim = (int)((NW >= 256 || CHAIN) ? HC_SMEM_1CTA : HC_SMEM_2CTA);
-    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 0, CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 1, CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    const int lim = (int)(NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA);
+    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
   }
   const int64_t grid = (int64_t)a.B * g.tiles;
   if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
-  if (bf16) hconv_kernel<NW, 1, CHAIN><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
-  else hconv_kernel<NW, 0, CHAIN><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
+  if (bf16) hconv_kernel<NW, 1><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
+  else hconv_kernel<NW, 0><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
   AB_LAUNCH_CHECK("hconv_kernel");
+  return AB_OK;
+}
+
+template <int NW>
+int launch_chain(const HcArgs& a, const HcGeom& g, int bf16, cudaStream_t s) {
+  static DeviceOnce configured;
+  if (configured.need()) {
+    AB_CUDA_TRY(cudaFuncSetAttribute(hchain_kernel<NW, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
+    AB_CUDA_TRY(cudaFuncSetAttribute(hchain_kernel<NW, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
+  }
+  const int64_t work = (int64_t)a.B * g.tiles;
+  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc block: too many tiles");
+  int dev = 0, sms = 0;
+  AB_CUDA_TRY(cudaGetDevice(&dev));
+  AB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const unsigned grid = (unsigned)std::min<int64_t>(work, sms);   // persistent: CTAs stride over the work items
+  if (bf16) hchain_kernel<NW, 1><<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g);
+  else hchain_kernel<NW, 0><<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g);
+  AB_LAUNCH_CHECK("hchain_kernel");
   return AB_OK;
 }
 
@@ -633,12 +785,13 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
   g.off_i = (xbytes + 127u) & ~127u;
   g.off_w = (g.off_i + xbytes + 127u) & ~127u;
   const uint32_t nbias = (uint32_t)(g.nsteps * L.NW);
-  const uint32_t fixed = g.off_w + nbias * 4u + 16u + 16u * HC_STAGES_MAX;
+  const uint32_t bars = 16u * HC_STAGES_MAX + 16u;   // W ring full / empty, X full / empty
+  const uint32_t fixed = g.off_w + nbias * 4u + 16u + bars;
   if (fixed + 2u * g.stage_bytes > HC_SMEM_1CTA) return fail(AB_ERR_UNSUPPORTED, "tc block: does not fit shared memory");
   g.nstages = (int)std::min<uint32_t>((HC_SMEM_1CTA - fixed) / g.stage_bytes, HC_STAGES_MAX);
   g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
   g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
-  g.smem_bytes = g.off_bar + 16u * HC_STAGES_MAX;
+  g.smem_bytes = g.off_bar + bars;
   g.out_scale = 1.0f;
   g.mid_slope = 1.0f;
   return AB_OK;
@@ -694,9 +847,9 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
   a.y = p.y; a.acc_prev = p.acc_prev; a.yimg = p.yimg; a.img_slope = p.img_slope;
   const int bf16 = p.precision == AB_PREC_TC_BF16;
   switch ((int)(g.stage_bytes / 64u)) {
-    case 16: return launch_nw<16, true>(a, g, bf16, s);
-    case 32: return launch_nw<32, true>(a, g, bf16, s);
-    case 64: return launch_nw<64, true>(a, g, bf16, s);
+    case 16: return launch_chain<16>(a, g, bf16, s);
+    case 32: return launch_chain<32>(a, g, bf16, s);
+    case 64: return launch_chain<64>(a, g, bf16, s);
   }
   return fail(AB_ERR_UNSUPPORTED, "tc block: N block %u", g.stage_bytes / 64u);
 }
