@@ -50,12 +50,12 @@ struct Slot {
   size_t offset;      // into the arena (fp32 repacked image)
   size_t bytes;
   bool loaded;
-  // tensor-core operand image (built by finalize when precision != fp32)
+  // 16-bit weight image for the wgmma kernel (built by finalize when precision != fp32); tc_bytes > 0 iff the conv
+  // runs there (tc_image_bytes)
   size_t tc_offset;
   size_t tc_bytes;
   int stride;         // ConvTranspose1d stride (SLOT_CONVT_W)
   int dilation;       // Conv1d dilation (SLOT_CONV_W)
-  int tc_kind;        // 0 none, 1 tc_conv image (square, C <= 256), 2 gemmconv image, 3 streaming gemmconv image
   float gain = 1.0f;  // applied to the fp32 image at load time (NSF-HiFiGAN: 2 on every ups weight / bias)
 };
 
@@ -142,7 +142,6 @@ struct ab_generator {
     s.tc_bytes = 0;
     s.stride = 1;
     s.dilation = 1;
-    s.tc_kind = 0;
     fp32_bytes += align_up(s.bytes, 256);
     slots.push_back(s);
     index[name] = (int)slots.size() - 1;
@@ -214,6 +213,20 @@ int validate_config(const ab_generator_config& c) {
   if ((c.gin_channels > 0 || c.conv_post_no_bias) && c.kind != AB_GEN_HIFIGAN)
     return fail(AB_ERR_ARG, "config: gin_channels / conv_post_no_bias belong to the HiFi-GAN kind (HiFiGAN_vits)");
   return AB_OK;
+}
+
+// Routing at tensor-core precision: the size of the slot's 16-bit weight image, 0 when its conv runs on the fp32
+// CUDA-core kernels instead of the wgmma kernel.
+//   ConvTranspose1d and the (square) ResBlock / AMPBlock convs run on the wgmma kernel whenever the shape has an
+//   image; a block of tc_conv_supported convs (C <= 256, k <= 31) runs as pairs or whole blocks, any other as single
+//   convs.  conv_pre / conv_post run there iff C_in != C_out, C_in <= 512 and C_out > 4: the C -> 1 conv_post is
+//   HBM-bound and the last layer, so it stays exact.
+size_t tc_image_bytes(const Slot& s, bool pre_or_post) {
+  if (s.kind == SLOT_CONVT_W) return tc_weight_image_bytes(1, (int)s.shape[0], (int)s.shape[1], (int)s.shape[2], s.stride);
+  if (s.kind != SLOT_CONV_W) return 0;
+  const int cout = (int)s.shape[0], cin = (int)s.shape[1], k = (int)s.shape[2];
+  if (pre_or_post && (cin == cout || cin > 512 || cout <= 4)) return 0;
+  return tc_weight_image_bytes(0, cin, cout, k, s.dilation);
 }
 
 }  // namespace
@@ -305,32 +318,13 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     g->cond_b = g->add_slot("cond.bias", SLOT_VEC, {c0});
   }
 
-  // tensor-core operand images live behind the fp32 images; reserve worst case
+  // tensor-core weight images live behind the fp32 images
   size_t tc = 0;
-  for (auto& s : g->slots) {
-    if (s.kind == SLOT_CONV_W) {
-      s.tc_bytes = tc_weight_image_bytes((int)s.shape[1], (int)s.shape[0], (int)s.shape[2]);
-      s.tc_kind = s.tc_bytes ? 1 : 0;
-      if (!s.tc_bytes && s.shape[0] == s.shape[1] && s.shape[1] > 256) {
-        // wide square convs (BigVGAN-large stages 0/1): streaming N-blocked kernel fed from operand images
-        s.tc_bytes = gs_weight_image_bytes(0, (int)s.shape[1], (int)s.shape[0], (int)s.shape[2], s.dilation);
-        s.tc_kind = s.tc_bytes ? 3 : 0;
-      } else if (!s.tc_bytes && s.shape[1] <= 512) {   // non-square convs (conv_pre, conv_post): N-blocked kernel
-        s.tc_bytes = gc_weight_image_bytes(0, (int)s.shape[1], (int)s.shape[0], (int)s.shape[2], s.dilation);
-        s.tc_kind = s.tc_bytes ? 2 : 0;
-      }
-      s.tc_offset = g->fp32_bytes + tc;
-      tc += align_up(s.tc_bytes, 256);
-    } else if (s.kind == SLOT_CONVT_W) {
-      s.tc_bytes = gc_weight_image_bytes(1, (int)s.shape[0], (int)s.shape[1], (int)s.shape[2], s.stride);
-      s.tc_kind = s.tc_bytes ? 2 : 0;
-      if (!s.tc_bytes) {   // C_in too wide for a resident tile: streaming kernel
-        s.tc_bytes = gs_weight_image_bytes(1, (int)s.shape[0], (int)s.shape[1], (int)s.shape[2], s.stride);
-        s.tc_kind = s.tc_bytes ? 3 : 0;
-      }
-      s.tc_offset = g->fp32_bytes + tc;
-      tc += align_up(s.tc_bytes, 256);
-    }
+  for (size_t i = 0; i < g->slots.size(); ++i) {
+    Slot& s = g->slots[i];
+    s.tc_bytes = tc_image_bytes(s, (int)i == g->conv_pre.w || (int)i == g->conv_post.w);
+    s.tc_offset = g->fp32_bytes + tc;
+    tc += align_up(s.tc_bytes, 256);
   }
   g->arena_need = g->fp32_bytes + tc;
   *out = g;
@@ -415,23 +409,11 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
   if (precision != AB_PREC_FP32) {
     if (!ab_device_is_sm90()) return fail(AB_ERR_UNSUPPORTED, "finalize: tensor-core precision needs an sm_90 (Hopper) device");
     for (size_t i = 0; i < g->slots.size(); ++i) {
-      Slot& s = g->slots[i];
-      int rc = AB_OK;
-      if (s.kind == SLOT_CONV_W && s.tc_kind == 1)
-        rc = launch_tc_pack_weight(g->fptr((int)i), g->tcptr((int)i), (int)s.shape[1], (int)s.shape[0],
-                                   (int)s.shape[2], precision, st);
-      else if (s.kind == SLOT_CONV_W && s.tc_kind == 3)
-        rc = launch_gs_pack_weight(g->fptr((int)i), g->tcptr((int)i), 0, (int)s.shape[1], (int)s.shape[0], (int)s.shape[2],
-                                   s.dilation, precision, st);
-      else if (s.kind == SLOT_CONV_W && s.tc_kind == 2)
-        rc = launch_gc_pack_weight(g->fptr((int)i), g->tcptr((int)i), 0, (int)s.shape[1], (int)s.shape[0],
-                                   (int)s.shape[2], s.dilation, precision, st);
-      else if (s.kind == SLOT_CONVT_W && s.tc_kind == 2)
-        rc = launch_gc_pack_weight(g->fptr((int)i), g->tcptr((int)i), 1, (int)s.shape[0], (int)s.shape[1],
-                                   (int)s.shape[2], s.stride, precision, st);
-      else if (s.kind == SLOT_CONVT_W && s.tc_kind == 3)
-        rc = launch_gs_pack_weight(g->fptr((int)i), g->tcptr((int)i), 1, (int)s.shape[0], (int)s.shape[1],
-                                   (int)s.shape[2], s.stride, precision, st);
+      const Slot& s = g->slots[i];
+      if (!s.tc_bytes) continue;
+      const bool t = s.kind == SLOT_CONVT_W;   // state-dict shape: ConvTranspose1d [C_in, C_out, k], Conv1d [C_out, C_in, k]
+      int rc = launch_tc_pack_weight(g->fptr((int)i), g->tcptr((int)i), t ? 1 : 0, (int)s.shape[t ? 0 : 1],
+                                     (int)s.shape[t ? 1 : 0], (int)s.shape[2], t ? s.stride : s.dilation, precision, st);
       if (rc != AB_OK) return rc;
     }
   }
@@ -621,6 +603,12 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     cudaEventRecord(g->prof_recs.back().e1, st);
   };
 
+  // algorithmic HBM bytes of a Conv1d launch with fp32 activations and weights (profile)
+  auto conv_bytes = [&](const ConvRef& c, int Tn, const float* residual, const float* acc_prev) {
+    const double el = (double)B * Tn;
+    return 4.0 * (el * c.cin + el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + (double)c.cin * c.cout * c.k);
+  };
+  // fp32 CUDA-core Conv1d
   auto conv = [&](const ConvRef& c, const float* x, int64_t xsb, int64_t xsc, int64_t xst, float* y,
                   int Tn, float pre_slope, const float* residual, const float* acc_prev, float out_div,
                   int post_tanh) -> int {
@@ -631,22 +619,30 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d = c.d;
     p.pre_slope = pre_slope; p.out_div = out_div; p.post_tanh = post_tanh;
     ++launches;
-    const double el = (double)B * Tn;
-    // conv_post (C -> 1, then tanh) stays on the exact fp32 kernel: it is HBM-bound and the last layer
-    const bool gc = tc && g->slots[c.w].tc_kind == 2 && acc_prev == nullptr && out_div == 1.0f && c.cout > 4;
-    prof_begin(gc ? 4 : 1, 2.0 * el * c.cout * c.cin * c.k,
-               4.0 * (el * c.cin + el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + (double)c.cin * c.cout * c.k));
-    int r;
-    if (gc) {
-      GcParams gp;
-      gp.x = x; gp.xsb = xsb; gp.xsc = xsc; gp.xst = xst; gp.ximg = nullptr; gp.y = y; gp.w = g->tcptr(c.w); gp.bias = g->fptr(c.b);
-      gp.residual = residual; gp.B = (int)B; gp.Cin = c.cin; gp.Cout = c.cout; gp.Tin = Tn; gp.mode = 0;
-      gp.k = c.k; gp.d = c.d; gp.u = 1; gp.pre_slope = pre_slope; gp.post_tanh = post_tanh;
-      gp.precision = g->precision; gp.yimg = nullptr; gp.img_slope = 1.0f;
-      r = launch_gemmconv(gp, st);
-    } else {
-      r = launch_conv1d_fp32(p, st);
-    }
+    prof_begin(1, 2.0 * B * Tn * c.cout * c.cin * c.k, conv_bytes(c, Tn, residual, acc_prev));
+    const int r = launch_conv1d_fp32(p, st);
+    prof_end();
+    return r;
+  };
+  // whether conv c runs on the wgmma kernel (tc_image_bytes decided it at create)
+  auto on_tc = [&](const ConvRef& c) { return tc && g->slots[c.w].tc_bytes > 0; };
+  // Conv1d c on the wgmma kernel, from fp32 x (lrelu(., pre_slope) in the loader) or the operand image ximg; with c2
+  // the ResBlock1 pair c -> lrelu(., pre_slope) -> c2 in one launch.  bytes: the launch's algorithmic HBM bytes (profile)
+  auto tc_conv = [&](const ConvRef& c, const ConvRef* c2, const float* x, int64_t xsb, int64_t xsc, int64_t xst,
+                     const uint16_t* ximg, float* y, uint16_t* yimg, int Tn, float pre_slope, const float* residual,
+                     const float* acc_prev, float out_div, int post_tanh, double bytes) -> int {
+    TcConvParams p;
+    p.x = x; p.xsb = xsb; p.xsc = xsc; p.xst = xst; p.ximg = ximg; p.pre_slope = pre_slope;
+    p.w = g->tcptr(c.w); p.bias = g->fptr(c.b);
+    if (c2) { p.w2 = g->tcptr(c2->w); p.b2 = g->fptr(c2->b); p.mid_slope = pre_slope; }
+    p.residual = residual; p.acc_prev = acc_prev; p.out_div = out_div; p.post_tanh = post_tanh;
+    p.y = y; p.yimg = yimg; p.img_slope = 0.1f;
+    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d_or_u = c.d;
+    p.precision = g->precision;
+    ++launches;
+    const bool rb = c.cin == c.cout && tc_conv_supported(c.cin, c.k);   // pair / block-mode capable ResBlock conv
+    prof_begin(rb ? 0 : 4, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes);
+    const int r = launch_tc_conv(p, st);
     prof_end();
     return r;
   };
@@ -665,49 +661,13 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     prof_end();
     return r;
   };
-  // one (conv1 -> conv2 -> + x) pair or a single (conv -> + x) on the tensor cores
-  auto tc_convs = [&](const ConvRef& c1, const ConvRef* c2, const float* x, float* y, int C, int Tn,
-                      float pre_slope, float mid_slope, const float* residual, const float* acc_prev,
-                      float out_div, const uint16_t* ximg, uint16_t* yimg) -> int {
-    TcConvParams p;
-    p.ximg = ximg; p.yimg = yimg; p.img_slope = 0.1f;
-    p.x = x; p.y = y; p.residual = residual; p.acc_prev = acc_prev;
-    p.w1 = g->tcptr(c1.w); p.b1 = g->fptr(c1.b);
-    p.w2 = c2 ? g->tcptr(c2->w) : nullptr; p.b2 = c2 ? g->fptr(c2->b) : nullptr;
-    p.B = (int)B; p.C = C; p.T = Tn; p.k = c1.k; p.d1 = c1.d; p.nconv = c2 ? 2 : 1;
-    p.pre_slope = pre_slope; p.mid_slope = mid_slope; p.out_div = out_div;
-    p.precision = g->precision;
-    ++launches;
-    const double el = (double)B * C * Tn;
-    const int ncv = c2 ? 2 : 1;
-    prof_begin(0, 2.0 * el * C * c1.k * ncv,
-               4.0 * (el * (2 + (residual != nullptr && residual != x) + (acc_prev != nullptr)) + (double)ncv * C * C * c1.k));
-    const int r = launch_tc_conv(p, st);
-    prof_end();
-    return r;
-  };
-
-  // wide single conv on the streaming tensor-core kernel (operand image in)
-  auto gs_conv = [&](const ConvRef& c, const uint16_t* ximg, float* y, int Tn, const float* residual,
-                     const float* acc_prev, float out_div, const float* x = nullptr, float pre_slope = 1.0f) -> int {
-    GsParams p;
-    p.x = x; p.pre_slope = pre_slope; p.mode = 0; p.u = 1; p.yimg = nullptr; p.img_slope = 1.0f;
-    p.ximg = ximg; p.y = y; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.residual = residual; p.acc_prev = acc_prev;
-    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d = c.d; p.out_div = out_div;
-    p.precision = g->precision;
-    ++launches;
-    const double el = (double)B * Tn;
-    prof_begin(4, 2.0 * el * c.cout * c.cin * c.k,
-               4.0 * el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + 2.0 * el * c.cin + 4.0 * c.cin * c.cout * c.k);
-    const int r = launch_gemmconv_stream(p, st);
-    prof_end();
-    return r;
-  };
-
   // conv_pre (hifigan.py:204, bigvgan.py:314)
   const int C0 = g->cfg.upsample_initial_channel;
-  rc = conv(g->conv_pre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], R[0], (int)T, 1.0f,
-            nullptr, nullptr, 1.0f, 0);
+  const ConvRef& cpre = g->conv_pre;
+  rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, R[0], nullptr,
+                             (int)T, 1.0f, nullptr, nullptr, 1.0f, 0, conv_bytes(cpre, (int)T, nullptr, nullptr))
+                   : conv(cpre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], R[0], (int)T, 1.0f,
+                          nullptr, nullptr, 1.0f, 0);
   if (rc != AB_OK) return rc;
   if (dev_g != nullptr) {   // x = x + cond(g)  (hifigan.py:429-430)
     ++launches;
@@ -725,41 +685,31 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     if (!sg.has_up) {
       std::swap(U, R[cur_r]);   // AB_GEN_TRUNK: the blocks read conv_pre's output in place
     } else {
-    ConvTParams tp;
-    tp.x = R[cur_r]; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
-    tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u;
-    tp.pre_slope = big ? 1.0f : 0.1f;
-    ++launches;
-    {
+      const bool up_tc = on_tc(sg.up);
+      const float pre_slope = big ? 1.0f : 0.1f;
+      ++launches;
       const double eo = (double)B * sg.ch * Tn * sg.u;
-      prof_begin(2, 2.0 * eo * cin * ((double)sg.up.k / sg.u),
+      prof_begin(up_tc ? 4 : 2, 2.0 * eo * cin * ((double)sg.up.k / sg.u),
                  4.0 * ((double)B * cin * Tn + eo + (double)cin * sg.ch * sg.up.k));
-    }
-    if (tc && g->slots[sg.up.w].tc_kind == 3) {
-      GsParams sp;
-      sp.ximg = nullptr; sp.x = R[cur_r]; sp.pre_slope = tp.pre_slope; sp.mode = 1; sp.u = sg.u;
-      u_img = (!big && gs_can_emit_image(sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
-      sp.yimg = u_img; sp.img_slope = 0.1f; sp.y = U; sp.w = g->tcptr(sg.up.w); sp.bias = g->fptr(sg.up.b);
-      sp.residual = nullptr; sp.acc_prev = nullptr; sp.B = (int)B; sp.Cin = cin; sp.Cout = sg.ch; sp.T = Tn;
-      sp.k = sg.up.k; sp.d = 1; sp.out_div = 1.0f; sp.precision = g->precision;
-      if (g->profiling) g->prof_recs.back().cls = 4;
-      rc = launch_gemmconv_stream(sp, st);
-    } else if (tc && g->slots[sg.up.w].tc_kind == 2) {
-      GcParams gp;
-      gp.x = R[cur_r]; gp.xsb = (int64_t)cin * Tn; gp.xsc = Tn; gp.xst = 1; gp.y = U; gp.w = g->tcptr(sg.up.w);
-      gp.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr; gp.bias = g->fptr(sg.up.b); gp.residual = nullptr;
-      gp.B = (int)B; gp.Cin = cin; gp.Cout = sg.ch; gp.Tin = Tn; gp.mode = 1; gp.k = sg.up.k; gp.d = 1; gp.u = sg.u;
-      gp.pre_slope = tp.pre_slope; gp.post_tanh = 0; gp.precision = g->precision;
-      // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
-      u_img = (!big && gc_can_emit_image(sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
-      gp.yimg = u_img; gp.img_slope = 0.1f;
-      if (g->profiling) g->prof_recs.back().cls = 4;
-      rc = launch_gemmconv(gp, st);
-    } else {
-      rc = launch_conv_transpose1d_fp32(tp, st);
-    }
-    prof_end();
-    if (rc != AB_OK) return rc;
+      if (up_tc) {
+        TcConvParams p;
+        p.mode = 1;
+        p.x = R[cur_r]; p.xsb = (int64_t)cin * Tn; p.xsc = Tn; p.xst = 1; p.pre_slope = pre_slope;
+        p.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr;
+        p.w = g->tcptr(sg.up.w); p.bias = g->fptr(sg.up.b); p.y = U;
+        // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
+        u_img = (!big && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
+        p.yimg = u_img; p.img_slope = 0.1f;
+        p.B = (int)B; p.Cin = cin; p.Cout = sg.ch; p.T = Tn; p.k = sg.up.k; p.d_or_u = sg.u; p.precision = g->precision;
+        rc = launch_tc_conv(p, st);
+      } else {
+        ConvTParams tp;
+        tp.x = R[cur_r]; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
+        tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u; tp.pre_slope = pre_slope;
+        rc = launch_conv_transpose1d_fp32(tp, st);
+      }
+      prof_end();
+      if (rc != AB_OK) return rc;
     }
     Tn *= sg.u;
     const int C = sg.ch;
@@ -779,7 +729,6 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     }
     float* Rout = R[cur_r ^ 1];
     const int64_t sb = (int64_t)C * Tn, sc = Tn;
-    const bool use_tc = tc && tc_conv_supported(C, sg.blocks[0].k);
     bool stage_img_written = false;
     for (int j = 0; j < nk; ++j) {
       const BlockRef& blk = sg.blocks[j];
@@ -787,9 +736,13 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       const uint16_t* cur_img = u_img;
       int pp = 0;
       const int nd = (int)blk.dil.size();
-      if (use_tc && !big && g->rb_mode >= 2 && nd <= AB_TC_CHAIN_MAX_PAIRS) {
+      const bool pair = !blk.c2.empty();
+      const int ncv = pair ? 2 : 1;
+      // every conv of a block has a weight image or none; fused: pair / block mode (HiFi-GAN) and tc_conv launch class
+      const bool blk_tc = on_tc(blk.c1[0]);
+      const bool fused = blk_tc && tc_conv_supported(C, blk.k);
+      if (fused && !big && g->rb_mode >= 2 && nd <= AB_TC_CHAIN_MAX_PAIRS) {
         // whole block in one launch when the halo recompute costs less than the per-pair HBM round trips of x
-        const int ncv = blk.c2.empty() ? 1 : 2;
         const double recompute = tc_chain_recompute(C, blk.k, blk.dil.data(), nd, ncv);
         if (recompute > 0.0 && (g->rb_mode >= 3 || recompute <= kChainMaxRecompute)) {
           const bool stage_img = j == nk - 1 && i + 1 < g->stages.size();
@@ -819,6 +772,33 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
           continue;
         }
       }
+      // algorithmic HBM bytes of one tensor-core launch (profile): a fused launch counts fp32 activations in and out,
+      // a single conv of a wider or longer-kernel block a 16-bit input
+      auto rb_bytes = [&](const ConvRef& c, int nconv, const float* x, const float* residual, const float* acc_prev) {
+        const double el = (double)B * Tn;
+        if (fused)
+          return 4.0 * (el * C * (2 + (residual != nullptr && residual != x) + (acc_prev != nullptr)) + (double)nconv * C * C * c.k);
+        return 4.0 * el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + 2.0 * el * c.cin + 4.0 * c.cin * c.cout * c.k;
+      };
+      // one conv: y = (c(act(x)) + residual + acc_prev) / out_div, act = the AMPBlock's anti-aliased snake
+      // (bigvgan.py:137-146, :222-228; on tensor cores its kernel writes the 16-bit operand image only) or
+      // lrelu(., 0.1) in the conv's loader (hifigan.py:95-99)
+      auto single = [&](const ConvRef& c, const ActRef* a, const float* x, float* y, const float* residual,
+                        const float* acc_prev, float out_div) -> int {
+        const float* in = x;
+        const uint16_t* img = nullptr;
+        float slope = 0.1f;
+        if (a) {
+          img = blk_tc ? P16[0] : nullptr;
+          in = blk_tc ? x : ACT;
+          slope = 1.0f;
+          const int r = blk_tc ? snake(*a, x, nullptr, C, Tn, P16[0]) : snake(*a, x, ACT, C, Tn);
+          if (r != AB_OK) return r;
+        }
+        if (!blk_tc) return conv(c, in, sb, sc, 1, y, Tn, slope, residual, acc_prev, out_div, 0);
+        return tc_conv(c, nullptr, in, sb, sc, 1, img, y, nullptr, Tn, slope, residual, acc_prev, out_div, 0,
+                       rb_bytes(c, 1, x, residual, acc_prev));
+      };
       for (int p = 0; p < nd; ++p) {
         const bool last = p == nd - 1;
         float* dst = last ? Rout : P[pp];
@@ -830,64 +810,22 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
         // xs = rb_0(x) ; xs += rb_j(x) ; x = xs / num_kernels  (hifigan.py:208-214)
         const float* accp = (last && j > 0) ? Rout : nullptr;
         const float div = (last && j == nk - 1) ? (float)nk : 1.0f;
-        const bool pair = !blk.c2.empty();
-        const bool blk_tc = use_tc && tc_conv_supported(C, blk.k);
-        // wide layers (C > 256): streaming kernel, BigVGAN only (it needs the activation as an operand image)
-        const bool blk_gs = tc && big && !blk_tc && g->slots[blk.c1[0].w].tc_kind == 3;
-        if (!big) {
-          if (blk_tc) {
-            rc = tc_convs(blk.c1[p], pair ? &blk.c2[p] : nullptr, cur, dst, C, Tn, 0.1f, 0.1f, cur, accp, div,
-                          cur_img, dst_img);
-            if (rc != AB_OK) return rc;
-            cur_img = dst_img;
-            if (stage_img) stage_img_written = true;
-          } else if (tc && g->slots[blk.c1[p].w].tc_kind == 3) {
-            // wide ResBlocks (C > 256, e.g. NSF-HiFiGAN's 384-channel stage): streaming kernel, fp32 in, lrelu in the loaders
-            if (pair) {
-              rc = gs_conv(blk.c1[p], nullptr, TMP, Tn, nullptr, nullptr, 1.0f, cur, 0.1f);
-              if (rc != AB_OK) return rc;
-              rc = gs_conv(blk.c2[p], nullptr, dst, Tn, cur, accp, div, TMP, 0.1f);
-            } else {
-              rc = gs_conv(blk.c1[p], nullptr, dst, Tn, cur, accp, div, cur, 0.1f);
-            }
-            if (rc != AB_OK) return rc;
-            cur_img = nullptr;
-          } else if (pair) {
-            rc = conv(blk.c1[p], cur, sb, sc, 1, TMP, Tn, 0.1f, nullptr, nullptr, 1.0f, 0);
-            if (rc != AB_OK) return rc;
-            rc = conv(blk.c2[p], TMP, sb, sc, 1, dst, Tn, 0.1f, cur, accp, div, 0);
-            if (rc != AB_OK) return rc;
-            cur_img = nullptr;
-          } else {
-            rc = conv(blk.c1[p], cur, sb, sc, 1, dst, Tn, 0.1f, cur, accp, div, 0);
-            if (rc != AB_OK) return rc;
-            cur_img = nullptr;
-          }
-        } else {
-          // AMPBlock: anti-aliased snake in front of every conv (bigvgan.py:137-146, :222-228)
-          // tensor-core path: the activation kernel writes the 16-bit operand image only (no fp32 copy)
-          const ActRef& a1 = pair ? blk.acts[2 * p] : blk.acts[p];
-          uint16_t* A16 = P16[0];
-          const bool img = blk_tc || blk_gs;
-          rc = img ? snake(a1, cur, nullptr, C, Tn, A16) : snake(a1, cur, ACT, C, Tn);
+        if (fused && !big) {
+          rc = tc_conv(blk.c1[p], pair ? &blk.c2[p] : nullptr, cur, sb, sc, 1, cur_img, dst, dst_img, Tn, 0.1f, cur, accp,
+                       div, 0, rb_bytes(blk.c1[p], ncv, cur, cur, accp));
           if (rc != AB_OK) return rc;
-          if (pair) {
-            if (blk_tc) rc = tc_convs(blk.c1[p], nullptr, cur, TMP, C, Tn, 1.0f, 1.0f, nullptr, nullptr, 1.0f, A16, nullptr);
-            else if (blk_gs) rc = gs_conv(blk.c1[p], A16, TMP, Tn, nullptr, nullptr, 1.0f);
-            else rc = conv(blk.c1[p], ACT, sb, sc, 1, TMP, Tn, 1.0f, nullptr, nullptr, 1.0f, 0);
-            if (rc != AB_OK) return rc;
-            rc = img ? snake(blk.acts[2 * p + 1], TMP, nullptr, C, Tn, A16) : snake(blk.acts[2 * p + 1], TMP, ACT, C, Tn);
-            if (rc != AB_OK) return rc;
-            if (blk_tc) rc = tc_convs(blk.c2[p], nullptr, TMP, dst, C, Tn, 1.0f, 1.0f, cur, accp, div, A16, nullptr);
-            else if (blk_gs) rc = gs_conv(blk.c2[p], A16, dst, Tn, cur, accp, div);
-            else rc = conv(blk.c2[p], ACT, sb, sc, 1, dst, Tn, 1.0f, cur, accp, div, 0);
-            if (rc != AB_OK) return rc;
-          } else {
-            if (blk_tc) rc = tc_convs(blk.c1[p], nullptr, cur, dst, C, Tn, 1.0f, 1.0f, cur, accp, div, A16, nullptr);
-            else if (blk_gs) rc = gs_conv(blk.c1[p], A16, dst, Tn, cur, accp, div);
-            else rc = conv(blk.c1[p], ACT, sb, sc, 1, dst, Tn, 1.0f, cur, accp, div, 0);
-            if (rc != AB_OK) return rc;
-          }
+          cur_img = dst_img;
+          if (stage_img) stage_img_written = true;
+        } else if (pair) {
+          rc = single(blk.c1[p], big ? &blk.acts[2 * p] : nullptr, cur, TMP, nullptr, nullptr, 1.0f);
+          if (rc != AB_OK) return rc;
+          rc = single(blk.c2[p], big ? &blk.acts[2 * p + 1] : nullptr, TMP, dst, cur, accp, div);
+          if (rc != AB_OK) return rc;
+          cur_img = nullptr;
+        } else {
+          rc = single(blk.c1[p], big ? &blk.acts[p] : nullptr, cur, dst, cur, accp, div);
+          if (rc != AB_OK) return rc;
+          cur_img = nullptr;
         }
         cur = dst;
       }
@@ -909,11 +847,17 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   // final gather of chunk i then runs under conv_post of chunk i+1
   const int nchunk = g->tail_events.empty() ? 1 : (int)std::min<int64_t>((int64_t)g->tail_events.size(), B);
   const int64_t Bfull = B;
+  const ConvRef& cpost = g->conv_post;
+  const float post_slope = big ? 1.0f : 0.01f;
+  const int post_tanh = g->cfg.kind == AB_GEN_TRUNK ? 0 : 1;
   for (int ci = 0; ci < nchunk; ++ci) {
     const int64_t b0 = Bfull * ci / nchunk, b1 = Bfull * (ci + 1) / nchunk;
     B = b1 - b0;
-    rc = conv(g->conv_post, xin + b0 * sb, sb, sc, 1, dev_wav + b0 * g->conv_post.cout * Tn, Tn, big ? 1.0f : 0.01f, nullptr,
-              nullptr, 1.0f, g->cfg.kind == AB_GEN_TRUNK ? 0 : 1);
+    const float* x = xin + b0 * sb;
+    float* y = dev_wav + b0 * cpost.cout * Tn;
+    rc = on_tc(cpost) ? tc_conv(cpost, nullptr, x, sb, sc, 1, nullptr, y, nullptr, Tn, post_slope, nullptr, nullptr, 1.0f,
+                                post_tanh, conv_bytes(cpost, Tn, nullptr, nullptr))
+                      : conv(cpost, x, sb, sc, 1, y, Tn, post_slope, nullptr, nullptr, 1.0f, post_tanh);
     B = Bfull;
     if (rc != AB_OK) break;
     if (!g->tail_events.empty()) {
@@ -958,8 +902,7 @@ int ab_activation1d_forward(const float* dev_x, float* dev_y, int64_t B, int64_t
 
 size_t ab_conv1d_workspace_bytes(int64_t cin, int64_t cout, int32_t k, int32_t precision) {
   size_t n = align_up((size_t)cin * cout * k * sizeof(float), 256);
-  if (precision != AB_PREC_FP32)
-    n += align_up(std::max(tc_weight_image_bytes((int)cin, (int)cout, k), gc_weight_image_bytes(0, (int)cin, (int)cout, k, 1)), 256);
+  if (precision != AB_PREC_FP32) n += align_up(tc_weight_image_bytes(0, (int)cin, (int)cout, k, 1), 256);
   return n;
 }
 
@@ -982,34 +925,20 @@ int ab_conv1d_forward(const float* dev_x, const float* dev_w, const float* dev_b
     p.pre_slope = pre_slope; p.out_div = 1.0f; p.post_tanh = post_tanh;
     return launch_conv1d_fp32(p, st);
   }
-  if (cin != cout || post_tanh || !tc_conv_supported((int)cin, k) || cin > tc_max_channels()) {
-    // non-square / wide / tanh: the N-blocked kernel
-    void* gimg = static_cast<char*>(ws) + align_up((size_t)cin * cout * k * sizeof(float), 256);
-    if (gc_weight_image_bytes(0, (int)cin, (int)cout, k, d) == 0) return fail(AB_ERR_UNSUPPORTED, "conv1d: %s", ab_last_error());
-    rc = launch_gc_pack_weight(w_t, gimg, 0, (int)cin, (int)cout, k, d, precision, st);
-    if (rc != AB_OK) return rc;
-    GcParams gp;
-    gp.x = dev_x; gp.xsb = cin * T; gp.xsc = T; gp.xst = 1; gp.ximg = nullptr; gp.y = dev_y; gp.w = gimg; gp.bias = dev_bias;
-    gp.residual = dev_residual; gp.B = (int)B; gp.Cin = (int)cin; gp.Cout = (int)cout; gp.Tin = (int)T; gp.mode = 0;
-    gp.k = k; gp.d = d; gp.u = 1; gp.pre_slope = pre_slope; gp.post_tanh = post_tanh; gp.precision = precision;
-    gp.yimg = nullptr; gp.img_slope = 1.0f;
-    return launch_gemmconv(gp, st);
-  }
   void* img = static_cast<char*>(ws) + align_up((size_t)cin * cout * k * sizeof(float), 256);
-  rc = launch_tc_pack_weight(w_t, img, (int)cin, (int)cout, k, precision, st);
+  if (tc_weight_image_bytes(0, (int)cin, (int)cout, k, d) == 0) return fail(AB_ERR_UNSUPPORTED, "conv1d: %s", ab_last_error());
+  rc = launch_tc_pack_weight(w_t, img, 0, (int)cin, (int)cout, k, d, precision, st);
   if (rc != AB_OK) return rc;
   TcConvParams p;
-  p.x = dev_x; p.y = dev_y; p.residual = dev_residual; p.acc_prev = nullptr;
-  p.w1 = img; p.b1 = dev_bias; p.w2 = nullptr; p.b2 = nullptr;
-  p.B = (int)B; p.C = (int)cin; p.T = (int)T; p.k = k; p.d1 = d; p.nconv = 1;
-  p.pre_slope = pre_slope; p.mid_slope = 1.0f; p.out_div = 1.0f; p.precision = precision;
-  p.ximg = nullptr; p.yimg = nullptr; p.img_slope = 1.0f;
+  p.x = dev_x; p.xsb = cin * T; p.xsc = T; p.xst = 1; p.pre_slope = pre_slope;
+  p.w = img; p.bias = dev_bias; p.residual = dev_residual; p.post_tanh = post_tanh; p.y = dev_y;
+  p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)T; p.k = k; p.d_or_u = d; p.precision = precision;
   return launch_tc_conv(p, st);
 }
 
 size_t ab_conv_transpose1d_workspace_bytes(int64_t cin, int64_t cout, int32_t k, int32_t u, int32_t precision) {
   size_t n = align_up((size_t)cin * cout * k * sizeof(float), 256);
-  if (precision != AB_PREC_FP32) n += align_up(gc_weight_image_bytes(1, (int)cin, (int)cout, k, u), 256);
+  if (precision != AB_PREC_FP32) n += align_up(tc_weight_image_bytes(1, (int)cin, (int)cout, k, u), 256);
   return n;
 }
 
@@ -1026,15 +955,15 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
   if (rc != AB_OK) return rc;
   if (precision != AB_PREC_FP32) {
     void* img = static_cast<char*>(ws) + align_up((size_t)cin * cout * k * sizeof(float), 256);
-    if (gc_weight_image_bytes(1, (int)cin, (int)cout, k, u) == 0) return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: %s", ab_last_error());
-    rc = launch_gc_pack_weight(w_t, img, 1, (int)cin, (int)cout, k, u, precision, st);
+    if (tc_weight_image_bytes(1, (int)cin, (int)cout, k, u) == 0) return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: %s", ab_last_error());
+    rc = launch_tc_pack_weight(w_t, img, 1, (int)cin, (int)cout, k, u, precision, st);
     if (rc != AB_OK) return rc;
-    GcParams gp;
-    gp.x = dev_x; gp.xsb = cin * Tin; gp.xsc = Tin; gp.xst = 1; gp.ximg = nullptr; gp.y = dev_y; gp.w = img; gp.bias = dev_bias; gp.residual = nullptr;
-    gp.B = (int)B; gp.Cin = (int)cin; gp.Cout = (int)cout; gp.Tin = (int)Tin; gp.mode = 1; gp.k = k; gp.d = 1; gp.u = u;
-    gp.pre_slope = pre_slope; gp.post_tanh = 0; gp.precision = precision;
-    gp.yimg = nullptr; gp.img_slope = 1.0f;
-    return launch_gemmconv(gp, st);
+    TcConvParams p;
+    p.mode = 1;
+    p.x = dev_x; p.xsb = cin * Tin; p.xsc = Tin; p.xst = 1; p.pre_slope = pre_slope;
+    p.w = img; p.bias = dev_bias; p.y = dev_y;
+    p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)Tin; p.k = k; p.d_or_u = u; p.precision = precision;
+    return launch_tc_conv(p, st);
   }
   ConvTParams p;
   p.x = dev_x; p.w_t = w_t; p.bias = dev_bias; p.y = dev_y;

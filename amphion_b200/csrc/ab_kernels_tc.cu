@@ -639,19 +639,6 @@ __global__ void hc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* _
   }
 }
 
-int pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u, int precision,
-                cudaStream_t s) {
-  HcLayer L;
-  int rc = layer_geom(mode, cin, cout, k, d_or_u, L);
-  if (rc != AB_OK) return rc;
-  const int64_t total = (int64_t)layer_image_bytes(L) / 2;
-  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 132 * 8);
-  hc_pack_weight_kernel<<<blocks, 256, 0, s>>>(w_t, static_cast<uint16_t*>(image), L, cin, cout, k,
-                                               precision == AB_PREC_TC_BF16 ? 1 : 0);
-  AB_LAUNCH_CHECK("hc_pack_weight_kernel");
-  return AB_OK;
-}
-
 // Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.
 int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g) {
   HcLayer L;
@@ -821,8 +808,6 @@ HcArgs base_args(const float* x, int64_t xsb, int64_t xsc, int64_t xst, const ui
 
 }  // namespace
 
-int tc_max_channels() { return TC_MAX_C; }
-
 double tc_chain_recompute(int C, int k, const int* dil, int npairs, int nconv) {
   HcGeom g;
   if (make_chain_geom(C, k, dil, npairs, nconv, 1 << 20, g) != AB_OK) return 0.0;
@@ -856,90 +841,55 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
 
 bool tc_conv_supported(int C, int k) { return C > 0 && C <= TC_MAX_C && (k & 1) && k <= 31; }
 
-size_t tc_weight_image_bytes(int cin, int cout, int k) {
-  if (cin != cout || !tc_conv_supported(cin, k)) return 0;
-  return gc_weight_image_bytes(0, cin, cout, k, 1);
-}
-
 size_t tc_act_image_bytes(int64_t B, int C, int64_t T) { return (size_t)B * rup(C, 16) * (size_t)T * 2; }
 
-int launch_tc_pack_weight(const float* w_t, void* image, int cin, int cout, int k, int precision, cudaStream_t s) {
-  if (tc_weight_image_bytes(cin, cout, k) == 0) return AB_OK;  // shape not served by the tensor-core path
-  return pack_weight(w_t, image, 0, cin, cout, k, 1, precision, s);
-}
-
-int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
-  if (!p.x || !p.y || !p.w1 || (p.nconv == 2 && !p.w2)) return fail(AB_ERR_ARG, "tc_conv: null argument");
-  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "tc_conv: bad shape");
-  if (p.nconv != 1 && p.nconv != 2) return fail(AB_ERR_ARG, "tc_conv: nconv must be 1 or 2");
-  if (!tc_conv_supported(p.C, p.k) || p.d1 <= 0) return fail(AB_ERR_UNSUPPORTED, "tc_conv: C=%d k=%d d=%d", p.C, p.k, p.d1);
-  HcGeom g;
-  int rc = make_geom(p.nconv == 2 ? 2 : 0, p.C, p.C, p.k, p.d1, p.T, g);
-  if (rc != AB_OK) return rc;
-  g.out_scale = 1.0f / p.out_div;
-  g.mid_slope = p.mid_slope;
-  HcArgs a = base_args(p.x, (int64_t)p.C * p.T, p.T, 1, p.ximg, p.pre_slope, p.B, p.C, p.C);
-  a.w = p.w1; a.w2 = p.w2; a.bias = p.b1; a.bias2 = p.b2;
-  a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev;
-  a.yimg = p.yimg; a.img_slope = p.img_slope;
-  return launch_hconv(a, g, p.precision, s);
-}
-
-bool gc_can_emit_image(int cout, int k, int u) {
-  HcLayer L;
-  return layer_geom(1, 16, cout, k, u, L) == AB_OK && (cout % 16) == 0;
-}
-bool gs_can_emit_image(int cout, int k, int u) { return gc_can_emit_image(cout, k, u); }
-
-size_t gc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u) {
+size_t tc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u) {
   HcLayer L;
   if (layer_geom(mode, cin, cout, k, d_or_u, L) != AB_OK) return 0;
   return layer_image_bytes(L);
 }
-size_t gs_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u) {
-  return gc_weight_image_bytes(mode, cin, cout, k, d_or_u);
-}
 
-int launch_gc_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u,
-                          int precision, cudaStream_t s) {
-  return pack_weight(w_t, image, mode, cin, cout, k, d_or_u, precision, s);
-}
-int launch_gs_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u,
-                          int precision, cudaStream_t s) {
-  return pack_weight(w_t, image, mode, cin, cout, k, d_or_u, precision, s);
-}
-
-int launch_gemmconv(const GcParams& p, cudaStream_t s) {
-  if ((!p.x && !p.ximg) || !p.y || !p.w) return fail(AB_ERR_ARG, "gemmconv: null argument");
-  if (p.ximg && (p.Cin % 16) != 0) return fail(AB_ERR_UNSUPPORTED, "gemmconv: operand-image input needs C_in %% 16 == 0");
-  if (p.B <= 0 || p.Tin <= 0) return fail(AB_ERR_ARG, "gemmconv: bad shape");
-  if (p.mode == 0 && ((p.k - 1) * p.d) & 1) return fail(AB_ERR_UNSUPPORTED, "gemmconv: (k-1)*dilation must be even");
-  if (p.yimg != nullptr && !(p.mode == 1 && (p.Cout % 16) == 0))
-    return fail(AB_ERR_UNSUPPORTED, "gemmconv: cannot emit an operand image for this layer");
-  HcGeom g;
-  int rc = make_geom(p.mode, p.Cin, p.Cout, p.k, p.mode ? p.u : p.d, p.Tin, g);
+int launch_tc_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u, int precision,
+                          cudaStream_t s) {
+  HcLayer L;
+  int rc = layer_geom(mode, cin, cout, k, d_or_u, L);
   if (rc != AB_OK) return rc;
-  HcArgs a = base_args(p.x, p.xsb, p.xsc, p.xst, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
-  a.w = p.w; a.bias = p.bias; a.y = p.y; a.residual = p.mode == 0 ? p.residual : nullptr;
-  a.post_tanh = p.mode == 0 ? p.post_tanh : 0;
-  a.yimg = p.yimg; a.img_slope = p.img_slope;
-  return launch_hconv(a, g, p.precision, s);
+  const int64_t total = (int64_t)layer_image_bytes(L) / 2;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 132 * 8);
+  hc_pack_weight_kernel<<<blocks, 256, 0, s>>>(w_t, static_cast<uint16_t*>(image), L, cin, cout, k,
+                                               precision == AB_PREC_TC_BF16 ? 1 : 0);
+  AB_LAUNCH_CHECK("hc_pack_weight_kernel");
+  return AB_OK;
 }
 
-int launch_gemmconv_stream(const GsParams& p, cudaStream_t s) {
-  if ((!p.ximg && !p.x) || !p.y || !p.w) return fail(AB_ERR_ARG, "gemmconv(stream): null argument");
-  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "gemmconv(stream): bad shape");
-  if (p.mode == 0 && ((p.k - 1) * p.d) & 1) return fail(AB_ERR_UNSUPPORTED, "gemmconv(stream): (k-1)*dilation must be even");
-  if (p.yimg != nullptr && !(p.mode == 1 && (p.Cout % 16) == 0))
-    return fail(AB_ERR_UNSUPPORTED, "gemmconv(stream): cannot emit an operand image for this layer");
+// The conv epilogue zero-fills the image's padding channels; the conv-transpose epilogue writes only c_out < C_out.
+bool tc_can_emit_image(int mode, int cin, int cout, int k, int d_or_u) {
+  if (mode == 0) return cin == cout && tc_conv_supported(cin, k);
+  HcLayer L;
+  return layer_geom(1, cin, cout, k, d_or_u, L) == AB_OK && (cout % 16) == 0;
+}
+
+int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
+  const bool pair = p.w2 != nullptr;
+  if ((!p.x && !p.ximg) || !p.y || !p.w) return fail(AB_ERR_ARG, "tc conv: null argument");
+  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "tc conv: bad shape");
+  if (p.mode != 0 && p.mode != 1) return fail(AB_ERR_ARG, "tc conv: mode must be 0 (conv) or 1 (conv-transpose)");
+  if (p.mode == 1 && (p.residual || p.acc_prev || p.out_div != 1.0f || p.post_tanh))
+    return fail(AB_ERR_ARG, "tc conv-transpose: residual, acc_prev, out_div and tanh belong to conv");
+  if (pair && !(p.mode == 0 && p.Cin == p.Cout && tc_conv_supported(p.Cin, p.k)))
+    return fail(AB_ERR_UNSUPPORTED, "tc conv pair: C_in=%d C_out=%d k=%d", p.Cin, p.Cout, p.k);
+  if (p.mode == 1 && p.ximg && (p.Cin % 16) != 0)
+    return fail(AB_ERR_UNSUPPORTED, "tc conv-transpose: operand-image input needs C_in %% 16 == 0");
+  if (p.yimg && !tc_can_emit_image(p.mode, p.Cin, p.Cout, p.k, p.d_or_u))
+    return fail(AB_ERR_UNSUPPORTED, "tc conv: cannot emit an operand image for this layer");
   HcGeom g;
-  int rc = make_geom(p.mode, p.Cin, p.Cout, p.k, p.mode ? p.u : p.d, p.T, g);
+  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, g);
   if (rc != AB_OK) return rc;
   g.out_scale = 1.0f / p.out_div;
-  HcArgs a = base_args(p.x, (int64_t)p.Cin * p.T, p.T, 1, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
-  a.w = p.w; a.bias = p.bias; a.y = p.y;
-  a.residual = p.mode == 0 ? p.residual : nullptr;
-  a.acc_prev = p.mode == 0 ? p.acc_prev : nullptr;
+  g.mid_slope = p.mid_slope;
+  HcArgs a = base_args(p.x, p.xsb, p.xsc, p.xst, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
+  a.w = p.w; a.w2 = p.w2; a.bias = p.bias; a.bias2 = p.b2;
+  a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev; a.post_tanh = p.post_tanh;
   a.yimg = p.yimg; a.img_slope = p.img_slope;
   return launch_hconv(a, g, p.precision, s);
 }

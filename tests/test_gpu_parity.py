@@ -680,12 +680,17 @@ def _trained_like(model, seed):
     return model
 
 
-@pytest.mark.parametrize("kind,hp,n_mel,B,T,seed", [("hifigan", HP_V1, 80, 2, 40, 21), ("bigvgan", HP_BIGVGAN_BASE, 100, 1, 24, 22)])
+@pytest.mark.parametrize("kind,hp,n_mel,B,T,seed", [
+    ("hifigan", HP_V1, 80, 2, 40, 21), ("bigvgan", HP_BIGVGAN_BASE, 100, 1, 24, 22),
+    ("hifigan", dict(HP_V1, resblock_kernel_sizes=[33, 3], resblock_dilation_sizes=[[1, 3, 5]] * 2), 80, 1, 32, 23),
+    ("bigvgan", dict(HP_BIGVGAN_BASE, resblock_kernel_sizes=[3, 33], resblock_dilation_sizes=[[1, 3, 5]] * 2), 100, 1, 24, 24)])
 @pytest.mark.parametrize("stress", ["logmel_input", "trained_like_weights", "both"])
 def test_tensor_core_path_holds_1e3_under_trained_like_dynamic_range(kind, hp, n_mel, B, T, seed, stress):
     """Full-width V1 / BigVGAN-base on the default tensor-core path (fp16 operands, fp32 accumulate) against the
     fp32 CPU oracle with (i) mel ~ U(-11.5, 2), the log-mel range of utils/mel.py:11 (SURVEY 8d), and (ii) weight-norm
-    gains spanning three decades plus outlier weights.  Bar: 1e-3 max-abs (north star)."""
+    gains spanning three decades plus outlier weights.  Bar: 1e-3 max-abs (north star).
+    The k = 33 ResBlocks (beyond pair and block mode) run as single convs on the wgmma kernel next to a k = 3 block
+    that runs in pair / block mode."""
     model = build_model(kind, hp, n_mel, seed=seed)
     if kind == "bigvgan":
         randomize_snake(model, seed + 1, hp["snake_logscale"])
