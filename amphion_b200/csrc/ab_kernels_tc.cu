@@ -18,10 +18,13 @@
 //      streamed with cp.async.bulk (TMA 1-D) through an mbarrier ring; thread 0 refills a stage once every warp
 //      has released it.
 //   D: fp32 in the registers of two consumer warpgroups (MT m64 tiles each); the epilogues run on the fragments.
+// hconv_kernel (conv, conv-transpose, pair) and hchain_kernel (block mode) share the operand loader, the wgmma batch,
+// the intermediate-tile and output epilogues and the shared-memory layout below; they differ in how they schedule them.
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "ab_tc.cuh"
 #include "ab_tc_ptx.cuh"
@@ -49,12 +52,10 @@ struct HcArgs {
   const uint16_t* ximg;    // operand image [B][c8n_in][Tin][8] of the already activated input, or null
   float pre_slope;
   int B, Cin, Cout;
-  const void* w;           // weight image (stages in (N block, K chunk, tap) order)
-  const void* w2;          // pair mode: conv2's image
-  const void* ws[2 * AB_TC_CHAIN_MAX_PAIRS];     // block mode: weight image of step s = pair * nconv + conv
-  const float* bs[2 * AB_TC_CHAIN_MAX_PAIRS];    // block mode: biases (nullable)
-  const float* bias;
-  const float* bias2;      // pair mode
+  // conv s of the launch (a single conv: 0; pair: 0, 1; block mode: pair * nconv + conv): its weight image, stages in
+  // (N block, K chunk, tap) order, and its bias (nullable)
+  const void* ws[2 * AB_TC_CHAIN_MAX_PAIRS];
+  const float* bs[2 * AB_TC_CHAIN_MAX_PAIRS];
   float* y;                // [B, Cout, Tout]
   const float* residual;   // nullable, [B, Cout, Tout]
   const float* acc_prev;   // nullable, may alias y
@@ -64,22 +65,172 @@ struct HcArgs {
 };
 
 struct HcGeom {
-  int mode;                // 0 conv, 1 conv-transpose, 2 conv pair
+  int mode;                // hconv_kernel: 0 conv, 1 conv-transpose, 2 conv pair
   int NB, cc;              // N blocks; output channels per block
   int R, V, tiles;         // rows per CTA tile, valid output rows per tile, tiles per sequence
-  int ntaps, d;            // taps of the (first) conv and the row step between them
+  int ntaps, d;            // taps of every conv; the row step between the (first) conv's taps
   int a0, rowsA, nkc;      // time of A row 0 = tile origin - a0; rows of the A chunk; 32-channel chunks of C_in
-  int h2, rowsI, nkc2;     // pair mode: intermediate row 0 = origin - h2; its rows; conv2's K chunks
+  int h2, rowsI;           // pair mode: intermediate row 0 = origin - h2; its rows
   int c8n_in, c8n_out;
   int nstages;
   uint32_t stage_bytes, off_i, off_w, off_bias, off_bar, smem_bytes;
   int Tin, Tout, u, pad;
   float out_scale, mid_slope;
-  // block mode (3): nsteps = npairs * nconv convs of one ResBlock; output row r is time origin - H + r, the operand
-  // tiles keep G guard rows on both sides so that every tap shift is a non-negative row offset
-  int nsteps, nconv, H, G, rowsX, k;
+  int nsteps;              // convs of the launch: 1 single conv, 2 pair, npairs * nconv block mode
+  // block mode: output row r is time origin - H + r, the operand tiles keep G guard rows on both sides so that every
+  // tap shift is a non-negative row offset
+  int nconv, H, G, rowsX;
   int dil[AB_TC_CHAIN_MAX_PAIRS];
 };
+
+// ------------------------------------------------------------------------------------------------ shared device code
+
+// Accumulator fragment (m64nNk16, fp32) of consumer warpgroup cw: element [c*4 + 2h + e] of m64 tile mt is tile row
+// row(mt, h) = 64 (cw MT + mt) + 16 wq + lane/4 + 8h and N-block column 8c + col + e, col = 2 (lane % 4).
+template <int MT>
+struct Frag {
+  int row0, col;
+  __device__ __forceinline__ explicit Frag(int cw)
+      : row0(cw * MT * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2)), col(2 * (threadIdx.x & 3)) {}
+  __device__ __forceinline__ int row(int mt, int h) const { return row0 + mt * 64 + 8 * h; }
+};
+
+// Stage i of conv st's weight image; a launch streams its convs' images one after another.
+__device__ __forceinline__ const uint8_t* weight_stage(const HcArgs& p, const HcGeom& g, int st, int i) {
+  return static_cast<const uint8_t*>(p.ws[st]) + (size_t)i * g.stage_bytes;
+}
+
+// Biases of the launch's convs into shared memory, per_step per conv, zero beyond C_out.
+__device__ __forceinline__ void stage_biases(float* bias_s, const HcArgs& p, int nsteps, int per_step, int tid,
+                                             int nthreads) {
+  for (int i = tid; i < nsteps * per_step; i += nthreads) {
+    const int st = i / per_step, c = i - st * per_step;
+    bias_s[i] = (p.bs[st] && c < p.Cout) ? __ldg(p.bs[st] + c) : 0.f;
+  }
+}
+
+// Operand tile at `tile`: c8 planes [c8_0, c8_0 + nplanes) x rows [0, rows), row at time t0 + row, from the operand
+// image or from lrelu(x, pre_slope); zero outside [0, Tin) and C_in.  Thread lt of nthreads cooperating threads.
+template <int BF16>
+__device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int b, uint8_t* tile, int c8_0, int nplanes,
+                                          int rows, int t0, int lt, int nthreads) {
+  const int items = nplanes * rows;
+  if (p.ximg != nullptr) {
+    const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
+    for (int idx = lt; idx < items; idx += nthreads) {
+      const int c = idx / rows, row = idx - c * rows;
+      const int c8 = c8_0 + c, t = t0 + row;
+      const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
+      cp_async16(smem_u32(tile) + unit_offset(rows, c, row),
+                 ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb, ok ? 16u : 0u);
+    }
+    cp_async_wait_all();
+  } else {
+    const float* xb = p.x + (int64_t)b * p.xsb;
+    for (int idx = lt; idx < items; idx += nthreads) {
+      const int c = idx / rows, row = idx - c * rows;
+      const int t = t0 + row;
+      const bool ok = t >= 0 && t < g.Tin;
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int ci = (c8_0 + c) * 8 + e;
+        v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
+      }
+      uint4 q;
+      q.x = pack2t<BF16>(v[0], v[1]);
+      q.y = pack2t<BF16>(v[2], v[3]);
+      q.z = pack2t<BF16>(v[4], v[5]);
+      q.w = pack2t<BF16>(v[6], v[7]);
+      *reinterpret_cast<uint4*>(tile + unit_offset(rows, c, row)) = q;
+    }
+  }
+}
+
+// One tap's wgmma batch over a 32-channel K chunk: acc[mt] (+)= A x W for both k16 halves, A rows starting at
+// row0 + 64 mt of the operand at aBase (aRows rows per c8 plane), W the stage at wS.
+template <int NW, int BF16, int MT>
+__device__ __forceinline__ void mma_batch(float (&acc)[MT][NW / 2], uint32_t aBase, int aRows, int row0, uint32_t wS,
+                                          bool first) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint32_t a = aBase + (uint32_t)(2 * ks * aRows + row0 + mt * 64) * 16u;
+      const uint32_t w = wS + (uint32_t)(2 * ks * NW) * 16u;
+      Wgmma<NW, BF16>::mma(acc[mt], make_desc(a, (uint32_t)aRows), make_desc(w, (uint32_t)NW), (first && ks == 0) ? 0 : 1);
+    }
+  }
+}
+
+// Intermediate tile: lrelu(v [+ bias], slope) of the fragment -> the 16-bit operand tile at `tile` (rows per c8
+// plane), fragment row r to tile row r + roff; zero where time t0 + r is outside [0, T).  Planes >= nplanes are not
+// written.
+template <int NW, int BF16, int MT>
+__device__ __forceinline__ void store_frag_tile(uint8_t* tile, const float (&v)[MT][NW / 2], const float* bias,
+                                                const Frag<MT>& f, int rows, int roff, int t0, int T, int nplanes,
+                                                float slope) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = f.row(mt, h), t = t0 + row;
+      const bool ok = t >= 0 && t < T;
+#pragma unroll
+      for (int c = 0; c < NW / 8; ++c) {
+        if (c >= nplanes) continue;
+        const int col = c * 8 + f.col;
+        float a0 = v[mt][c * 4 + 2 * h], a1 = v[mt][c * 4 + 2 * h + 1];
+        if (bias) {
+          a0 += bias[col];
+          a1 += bias[col + 1];
+        }
+        const uint32_t q = ok ? pack2t<BF16>(lrelu(a0, slope), lrelu(a1, slope)) : 0u;
+        *reinterpret_cast<uint32_t*>(tile + unit_offset(rows, c, row + roff) + 2 * f.col) = q;
+      }
+    }
+}
+
+// Output epilogue on fragment rows [r0, r1) at times t0 + row < Tout, output channels co0 + column < C_out:
+//   y = ((val + residual) + acc_prev) * out_scale [tanh] ; yimg = cvt(lrelu(y, img_slope))
+// where val(mt, c, h, e) is the value of accumulator element [mt][c*4 + 2h + e] before the epilogue.  Without
+// RES_TANH (block mode, whose launches never set them) the residual and tanh are not compiled in.
+template <int NW, int BF16, bool RES_TANH, int MT, class Val>
+__device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, const Frag<MT>& f, int b, int t0, int r0,
+                                             int r1, int co0, Val val) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = f.row(mt, h), t = t0 + row;
+      if (row < r0 || row >= r1 || t >= g.Tout) continue;
+#pragma unroll
+      for (int c = 0; c < NW / 8; ++c) {
+        const int co = co0 + c * 8 + f.col;
+        float ve[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          ve[e] = 0.f;
+          if (co + e < p.Cout) {
+            const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
+            float v = val(mt, c, h, e);
+            if (RES_TANH && p.residual) v += __ldg(p.residual + idx);
+            if (p.acc_prev) v += p.acc_prev[idx];
+            v *= g.out_scale;
+            if (RES_TANH && p.post_tanh) v = tanhf(v);
+            p.y[idx] = v;
+            ve[e] = v;
+          }
+        }
+        if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
+          *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+              pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ kernels
 
 // modes 0-2; block mode runs on hchain_kernel below
 template <int NW, int BF16>
@@ -87,7 +238,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31, wq = (tid >> 5) & 3;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   const int b = blockIdx.x / g.tiles, tile = blockIdx.x - b * g.tiles;
   const int O = tile * g.V;   // output time (conv) / input time (conv-transpose) of row 0
   const uint32_t sA = smem_u32(smem), sI = sA + g.off_i, sW = sA + g.off_w;
@@ -96,11 +247,12 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   auto bar_full = [&](int s) { return bar0 + 8u * s; };
   auto bar_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
 
-  const int total1 = g.NB * g.nkc * g.ntaps;
-  const int total = total1 + (g.mode == 2 ? g.nkc2 * g.ntaps : 0);
-  auto stage_src = [&](int it) -> const uint8_t* {
-    return it < total1 ? static_cast<const uint8_t*>(p.w) + (size_t)it * g.stage_bytes
-                       : static_cast<const uint8_t*>(p.w2) + (size_t)(it - total1) * g.stage_bytes;
+  const int per_step = g.NB * g.nkc * g.ntaps;
+  const int total = g.nsteps * per_step;
+  // stage j of the launch's stream: at most two convs (pair mode), so the conv is one comparison on the per-tap path
+  auto stage_src = [&](int j) {
+    const int st = j >= per_step;
+    return weight_stage(p, g, st, j - st * per_step);
   };
 
   if (tid == 0) {
@@ -110,16 +262,9 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  const int nbias = g.mode == 2 ? 2 * NW : g.NB * NW;
-  for (int i = tid; i < nbias; i += HC_THREADS) {
-    float v = 0.f;
-    if (g.mode == 2) v = i < NW ? ((p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f)
-                                : ((p.bias2 && i - NW < p.Cout) ? __ldg(p.bias2 + i - NW) : 0.f);
-    else v = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
-    bias_s[i] = v;
-  }
+  stage_biases(bias_s, p, g.nsteps, g.NB * NW, tid, HC_THREADS);
   if (g.mode == 2) {   // channels of the intermediate beyond the accumulator width stay zero
-    const int n16 = g.nkc2 * 4 * g.rowsI;
+    const int n16 = g.nkc * 4 * g.rowsI;
     for (int i = tid; i < n16; i += HC_THREADS) *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
   }
   __syncthreads();
@@ -142,15 +287,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
       const int shift = reversed ? (ntaps - 1 - j) : j * tapstep;
       const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
       wg_fence();
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-          const uint32_t a = aBase + (uint32_t)(2 * ks * aRows + (wg * MT + mt) * 64 + shift) * 16u;
-          const uint32_t w = wS + (uint32_t)(2 * ks * NW) * 16u;
-          Wgmma<NW, BF16>::mma(acc[mt], make_desc(a, (uint32_t)aRows), make_desc(w, (uint32_t)NW), (first && ks == 0) ? 0 : 1);
-        }
-      }
+      mma_batch<NW, BF16>(acc, aBase, aRows, wg * MT * 64 + shift, wS, first);
       wg_commit();
       wg_wait<0>();
       first = false;
@@ -164,81 +301,21 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
     }
   };
 
-  // A chunk kc: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32); zero outside [0, Tin) / C_in
+  // A chunk kc: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
   auto load_chunk = [&](int kc) {
     __syncthreads();   // every warp has finished the MMAs that read the previous chunk
-    const int items = 4 * g.rowsA;
-    if (p.ximg != nullptr) {
-      const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
-      for (int idx = tid; idx < items; idx += HC_THREADS) {
-        const int c = idx / g.rowsA, row = idx - c * g.rowsA;
-        const int c8 = kc * 4 + c, t = O - g.a0 + row;
-        const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
-        cp_async16(sA + unit_offset(g.rowsA, c, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
-                   ok ? 16u : 0u);
-      }
-      cp_async_wait_all();
-    } else {
-      const float* xb = p.x + (int64_t)b * p.xsb;
-      for (int idx = tid; idx < items; idx += HC_THREADS) {
-        const int c = idx / g.rowsA, row = idx - c * g.rowsA;
-        const int t = O - g.a0 + row;
-        const bool ok = t >= 0 && t < g.Tin;
-        float v[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int ci = kc * 32 + c * 8 + e;
-          v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
-        }
-        uint4 q;
-        q.x = pack2t<BF16>(v[0], v[1]);
-        q.y = pack2t<BF16>(v[2], v[3]);
-        q.z = pack2t<BF16>(v[4], v[5]);
-        q.w = pack2t<BF16>(v[6], v[7]);
-        *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsA, c, row)) = q;
-      }
-    }
+    load_tile<BF16>(p, g, b, smem, 4 * kc, 4, g.rowsA, O - g.a0, tid, HC_THREADS);
     fence_proxy_async();
     __syncthreads();
   };
 
-  // accumulator fragment (m64nNk16, fp32): element [c*4 + 2h + e] of tile mt is row 16*wq + lane/4 + 8h,
-  // column 8c + 2*(lane%4) + e of this warpgroup's mt-th m64 tile
-  auto frag_row = [&](int mt, int h) { return (wg * MT + mt) * 64 + wq * 16 + (lane >> 2) + 8 * h; };
-  const int col_l = 2 * (lane & 3);
-
-  // y = ((acc + bias) + residual + acc_prev) * out_scale [tanh] ; yimg = cvt(lrelu(y, img_slope))
+  // y = ((acc + bias) + residual + acc_prev) * out_scale [tanh] on the valid rows [0, V).  The fragment coordinates
+  // are built where they are used: kept live across the MMA loops, they make ptxas spill more.
   auto epilogue_conv = [&](int nb, const float* bias_blk) {
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = frag_row(mt, h), t = O + row;
-        if (row >= g.V || t >= g.Tout) continue;
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c) {
-          const int co = nb * NW + c * 8 + col_l;
-          float ve[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            ve[e] = 0.f;
-            if (co + e < p.Cout) {
-              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
-              float v = acc[mt][c * 4 + 2 * h + e] + bias_blk[c * 8 + col_l + e];
-              if (p.residual) v += __ldg(p.residual + idx);
-              if (p.acc_prev) v += p.acc_prev[idx];
-              v *= g.out_scale;
-              if (p.post_tanh) v = tanhf(v);
-              p.y[idx] = v;
-              ve[e] = v;
-            }
-          }
-          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
-            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
-                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
-        }
-      }
-    }
+    const Frag<MT> f(wg);
+    epilogue_out<NW, BF16, true>(p, g, f, b, O, 0, g.V, nb * NW, [&](int mt, int c, int h, int e) {
+      return acc[mt][c * 4 + 2 * h + e] + bias_blk[c * 8 + f.col + e];
+    });
   };
 
   if (g.mode != 2) {
@@ -252,16 +329,17 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
         epilogue_conv(nb, bias_s + nb * NW);
       } else {
         // conv-transpose: column n = cl*u + phi of input time s is y[nb*cc + cl, s*u - pad + phi]
+        const Frag<MT> f(wg);
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int s = O + frag_row(mt, h);
+            const int s = O + f.row(mt, h);
 #pragma unroll
             for (int c = 0; c < NW / 8; ++c) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                const int n = c * 8 + col_l + e;
+                const int n = c * 8 + f.col + e;
                 const int cl = n / g.u, phi = n - cl * g.u, co = nb * g.cc + cl;
                 const int t = s * g.u - g.pad + phi;
                 if (cl >= g.cc || co >= p.Cout || t < 0 || t >= g.Tout) continue;
@@ -283,26 +361,11 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
       mma_chunk(sA, g.rowsA, g.ntaps, g.d, false, first);
     }
     // intermediate = lrelu(conv1 + b1, mid_slope) -> shared-memory operand tile, zero outside [0, T)
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = frag_row(mt, h), t = O - g.h2 + row;
-        const bool ok = t >= 0 && t < g.Tin;
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c) {
-          if (c >= g.nkc2 * 4) continue;
-          const int col = c * 8 + col_l;
-          const float v0 = ok ? lrelu(acc[mt][c * 4 + 2 * h] + bias_s[col], g.mid_slope) : 0.f;
-          const float v1 = ok ? lrelu(acc[mt][c * 4 + 2 * h + 1] + bias_s[col + 1], g.mid_slope) : 0.f;
-          *reinterpret_cast<uint32_t*>(smem + g.off_i + unit_offset(g.rowsI, c, row) + 2 * col_l) = pack2t<BF16>(v0, v1);
-        }
-      }
-    }
+    store_frag_tile<NW, BF16>(smem + g.off_i, acc, bias_s, Frag<MT>(wg), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc, g.mid_slope);
     fence_proxy_async();
     __syncthreads();
     first = true;
-    for (int kc = 0; kc < g.nkc2; ++kc)
+    for (int kc = 0; kc < g.nkc; ++kc)
       mma_chunk(sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, g.ntaps, 1, false, first);
     epilogue_conv(0, bias_s + NW);
   }
@@ -338,8 +401,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
   auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
   const uint32_t x_full = bar0 + 16u * HC_STAGES_MAX, x_empty = x_full + 8u;
   const int nwork = p.B * g.tiles;
-  const int total1 = g.nkc * g.ntaps;
-  const int total = g.nsteps * total1;
+  const int per_step = g.nkc * g.ntaps;
 
   if (tid == 0) {
     for (int s = 0; s < g.nstages; ++s) {
@@ -350,10 +412,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     mbar_init(x_empty, 8);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = tid; i < g.nsteps * NW; i += HB_THREADS) {
-    const int st = i / NW, c = i - st * NW;
-    bias_s[i] = (p.bs[st] && c < p.Cout) ? __ldg(p.bs[st] + c) : 0.f;
-  }
+  stage_biases(bias_s, p, g.nsteps, NW, tid, HB_THREADS);
   // rows and channels of the intermediate that no step writes stay zero for every tile
   for (int i = tid; i < g.nkc * 4 * g.rowsX; i += HB_THREADS)
     *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
@@ -366,50 +425,21 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     if (tid == 0) {
       int wi = 0;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        for (int i = 0; i < total; ++i, ++wi) {
-          const int s = wi % g.nstages;
-          if (wi >= g.nstages) mbar_wait(w_empty(s), (uint32_t)(wi / g.nstages - 1) & 1u);
-          mbar_arrive_expect_tx(w_full(s), g.stage_bytes);
-          bulk_g2s(sW + (uint32_t)s * g.stage_bytes,
-                   static_cast<const uint8_t*>(p.ws[i / total1]) + (size_t)(i % total1) * g.stage_bytes,
-                   g.stage_bytes, w_full(s));
-        }
+        for (int st = 0; st < g.nsteps; ++st)
+          for (int i = 0; i < per_step; ++i, ++wi) {
+            const int s = wi % g.nstages;
+            if (wi >= g.nstages) mbar_wait(w_empty(s), (uint32_t)(wi / g.nstages - 1) & 1u);
+            mbar_arrive_expect_tx(w_full(s), g.stage_bytes);
+            bulk_g2s(sW + (uint32_t)s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(s));
+          }
       }
     } else if (tid >= 32) {
-      // X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row, zero outside [0, Tin)
-      const int lt = tid - 32, n16 = g.nkc * 4 * g.rowsX;
+      // X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row
       int n = 0;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
         const int b = w / g.tiles, t0 = (w - b * g.tiles) * g.V - g.H - g.G;
         if (n > 0) mbar_wait(x_empty, (uint32_t)(n - 1) & 1u);
-        if (p.ximg != nullptr) {
-          const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
-          for (int idx = lt; idx < n16; idx += HB_LOADERS) {
-            const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX, t = t0 + row;
-            const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
-            cp_async16(sX + unit_offset(g.rowsX, c8, row), ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb,
-                       ok ? 16u : 0u);
-          }
-          cp_async_wait_all();
-        } else {
-          const float* xb = p.x + (int64_t)b * p.xsb;
-          for (int idx = lt; idx < n16; idx += HB_LOADERS) {
-            const int c8 = idx / g.rowsX, row = idx - c8 * g.rowsX, t = t0 + row;
-            const bool ok = t >= 0 && t < g.Tin;
-            float v[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const int ci = c8 * 8 + e;
-              v[e] = (ok && ci < p.Cin) ? lrelu(__ldg(xb + (int64_t)ci * p.xsc + (int64_t)t * p.xst), p.pre_slope) : 0.f;
-            }
-            uint4 q;
-            q.x = pack2t<BF16>(v[0], v[1]);
-            q.y = pack2t<BF16>(v[2], v[3]);
-            q.z = pack2t<BF16>(v[4], v[5]);
-            q.w = pack2t<BF16>(v[6], v[7]);
-            *reinterpret_cast<uint4*>(smem + unit_offset(g.rowsX, c8, row)) = q;
-          }
-        }
+        load_tile<BF16>(p, g, b, smem, 0, 4 * g.nkc, g.rowsX, t0, tid - 32, HB_LOADERS);
         fence_proxy_async();
         mbar_arrive(x_full);
       }
@@ -419,7 +449,8 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
 
   // ------------------------------------------------------------------------------------------------ consumers
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
-  const int cw = wg - 1, wq = (tid >> 5) & 3;
+  const int cw = wg - 1;
+  const Frag<MT> f(cw);
   float acc[MT][NACC];
   int it = 0;        // weight stages consumed so far
   int pw = -1;       // W slot read by the batch still in flight (-1: none)
@@ -443,15 +474,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
       const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
       fence_acc();
       wg_fence();
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-        for (int ks = 0; ks < 2; ++ks) {
-          const uint32_t a = aBase + (uint32_t)(2 * ks * g.rowsX + (cw * MT + mt) * 64 + j * tapstep) * 16u;
-          const uint32_t w = wS + (uint32_t)(2 * ks * NW) * 16u;
-          Wgmma<NW, BF16>::mma(acc[mt], make_desc(a, (uint32_t)g.rowsX), make_desc(w, (uint32_t)NW), (first && ks == 0) ? 0 : 1);
-        }
-      }
+      mma_batch<NW, BF16>(acc, aBase, g.rowsX, cw * MT * 64 + j * tapstep, wS, first);
       wg_commit();
       wg_wait<1>();      // the previous batch has completed: its W slot can be refilled
       fence_acc();
@@ -467,10 +490,6 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     pw = -1;
   };
 
-  // accumulator fragment (m64nNk16, fp32): element [c*4 + 2h + e] of tile mt is row 16*wq + lane/4 + 8h,
-  // column 8c + 2*(lane%4) + e of this warpgroup's mt-th m64 tile
-  auto frag_row = [&](int mt, int h) { return (cw * MT + mt) * 64 + wq * 16 + (lane >> 2) + 8 * h; };
-  const int col_l = 2 * (lane & 3);
   int n = 0;
   for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
     const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
@@ -480,44 +499,29 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int t = O - g.H + frag_row(mt, h);
+        const int t = O - g.H + f.row(mt, h);
 #pragma unroll
         for (int c = 0; c < NW / 8; ++c)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int co = c * 8 + col_l + e;
+            const int co = c * 8 + f.col + e;
             xr[mt][c * 4 + 2 * h + e] = (t >= 0 && t < g.Tin && co < p.Cout) ? __ldg(p.x + ((int64_t)b * p.Cout + co) * g.Tin + t) : 0.f;
           }
       }
     mbar_wait(x_full, (uint32_t)n & 1u);
-    // lrelu(v, slope) of the fragment -> operand tile at off (rows offset by G), zero outside [0, T)
+    // lrelu(v [+ bb], mid_slope) of the fragment -> operand tile at off (rows offset by G)
     auto store_tile = [&](uint32_t off, const float (&v)[MT][NACC], const float* bb) {
       consumer_sync();   // both warpgroups have finished the MMAs that read the tile (ResBlock2 overwrites X)
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = frag_row(mt, h), t = O - g.H + row;
-          const bool ok = t >= 0 && t < g.Tin;
-#pragma unroll
-          for (int c = 0; c < NW / 8; ++c) {
-            if (c >= g.nkc * 4) continue;
-            const int col = c * 8 + col_l;
-            const float a0 = bb ? v[mt][c * 4 + 2 * h] + bb[col] : v[mt][c * 4 + 2 * h];
-            const float a1 = bb ? v[mt][c * 4 + 2 * h + 1] + bb[col + 1] : v[mt][c * 4 + 2 * h + 1];
-            const uint32_t q = ok ? pack2t<BF16>(lrelu(a0, g.mid_slope), lrelu(a1, g.mid_slope)) : 0u;
-            *reinterpret_cast<uint32_t*>(smem + off + unit_offset(g.rowsX, c, row + g.G) + 2 * col_l) = q;
-          }
-        }
+      store_frag_tile<NW, BF16>(smem + off, v, bb, f, g.rowsX, g.G, O - g.H, g.Tin, 4 * g.nkc, g.mid_slope);
       fence_proxy_async();
       consumer_sync();
     };
     for (int st = 0; st < g.nsteps; ++st) {
       const int pr = st / g.nconv, cv = st - pr * g.nconv;
-      const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.k - 1) * d / 2;
+      const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.ntaps - 1) * d / 2;
       const uint32_t aT = cv == 0 ? sX : sI;
       bool first = true;
-      for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.k, d, first);
+      for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.ntaps, d, first);
       drain();
       const float* bb = bias_s + st * NW;
       if (g.nconv == 2 && cv == 0) {
@@ -529,7 +533,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
           for (int c = 0; c < NW / 8; ++c)
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-              float a = acc[mt][c * 4 + i] + bb[c * 8 + col_l + (i & 1)];
+              float a = acc[mt][c * 4 + i] + bb[c * 8 + f.col + (i & 1)];
               a += xr[mt][c * 4 + i];
               xr[mt][c * 4 + i] = a;
             }
@@ -539,34 +543,9 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     // every MMA of this tile has completed: the producer may load the next X
     __syncwarp();
     if (lane == 0) mbar_arrive(x_empty);
-    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); yimg = cvt(lrelu(y, img_slope))
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = frag_row(mt, h), t = O - g.H + row;
-        if (row < g.H || row >= g.H + g.V || t >= g.Tout) continue;
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c) {
-          const int co = c * 8 + col_l;
-          float ve[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            ve[e] = 0.f;
-            if (co + e < p.Cout) {
-              const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
-              float v = xr[mt][c * 4 + 2 * h + e];
-              if (p.acc_prev) v += p.acc_prev[idx];
-              v *= g.out_scale;
-              p.y[idx] = v;
-              ve[e] = v;
-            }
-          }
-          if (p.yimg != nullptr && (co >> 3) < g.c8n_out)
-            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
-                pack2t<BF16>(lrelu(ve[0], p.img_slope), lrelu(ve[1], p.img_slope));
-        }
-      }
+    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V)
+    epilogue_out<NW, BF16, false>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
+                           [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
   }
 }
 
@@ -639,6 +618,21 @@ __global__ void hc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* _
   }
 }
 
+// Shared-memory layout of both kernels: the operand tile (abytes) at 0, the intermediate tile (ibytes) at off_i, then
+// the W ring of as many stages as fit (at most HC_STAGES_MAX), nbias fp32 biases and bar_bytes of mbarriers.  Needs
+// g.stage_bytes; false when two W stages do not fit in limit.
+bool layout_smem(HcGeom& g, uint32_t abytes, uint32_t ibytes, uint32_t nbias, uint32_t bar_bytes, uint32_t limit) {
+  g.off_i = (abytes + 127u) & ~127u;
+  g.off_w = (g.off_i + ibytes + 127u) & ~127u;
+  const uint32_t fixed = g.off_w + nbias * 4u + 16u + bar_bytes;
+  if (fixed + 2u * g.stage_bytes > limit) return false;
+  g.nstages = (int)std::min<uint32_t>((limit - fixed) / g.stage_bytes, HC_STAGES_MAX);
+  g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
+  g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
+  g.smem_bytes = g.off_bar + bar_bytes;
+  return true;
+}
+
 // Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.
 int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g) {
   HcLayer L;
@@ -646,6 +640,7 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
   if (rc != AB_OK) return rc;
   if (mode == 2 && (cin != cout || L.NB != 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv pair: C=%d not in [1,%d]", cin, TC_MAX_C);
   g.mode = mode;
+  g.nsteps = mode == 2 ? 2 : 1;
   g.NB = L.NB;
   g.cc = L.cc;
   g.ntaps = L.ntaps;
@@ -657,7 +652,6 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
   g.c8n_out = rup(cout, 16) / 8;
   g.h2 = 0;
   g.rowsI = 0;
-  g.nkc2 = 0;
   int maxshift, rows_total;
   if (mode == 1) {
     g.d = 1;
@@ -680,7 +674,6 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
       g.a0 += g.h2;
       g.V = g.R - (k - 1);
       g.rowsI = rup(g.R + k - 1, 8);
-      g.nkc2 = L.nkc;
     }
   }
   if (g.V < 8) return fail(AB_ERR_UNSUPPORTED, "tc conv: kernel size %d too large for a tile", k);
@@ -688,56 +681,40 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
   if (g.rowsA > 16383 || g.rowsI > 16383) return fail(AB_ERR_UNSUPPORTED, "tc conv: tap reach %d too large", maxshift);
   g.tiles = (rows_total + g.V - 1) / g.V;
   g.stage_bytes = 64u * (uint32_t)L.NW;
-  g.off_i = ((uint32_t)g.rowsA * 64u + 127u) & ~127u;
-  const uint32_t ibytes = (uint32_t)g.nkc2 * 4u * (uint32_t)g.rowsI * 16u;
-  g.off_w = (g.off_i + ibytes + 127u) & ~127u;
-  const uint32_t nbias = (uint32_t)(mode == 2 ? 2 * L.NW : g.NB * L.NW);
-  const uint32_t limit = L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA;
-  const uint32_t fixed = g.off_w + nbias * 4u + 16u + 16u * HC_STAGES_MAX;
-  if (fixed + 2u * g.stage_bytes > limit)
+  if (!layout_smem(g, (uint32_t)g.rowsA * 64u, (uint32_t)g.nkc * 64u * (uint32_t)g.rowsI,
+                   (uint32_t)(g.nsteps * g.NB * L.NW), 16u * HC_STAGES_MAX, L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA))
     return fail(AB_ERR_UNSUPPORTED, "tc conv: C=%d k=%d reach %d does not fit shared memory", cin, k, maxshift);
-  g.nstages = (int)std::min<uint32_t>((limit - fixed) / g.stage_bytes, HC_STAGES_MAX);
-  g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
-  g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
-  g.smem_bytes = g.off_bar + 16u * HC_STAGES_MAX;
   g.out_scale = 1.0f;
   g.mid_slope = 1.0f;
   return AB_OK;
 }
 
-template <int NW>
-int launch_nw(const HcArgs& a, const HcGeom& g, int bf16, cudaStream_t s) {
+// Launches K after raising its dynamic shared-memory limit to `limit`, once per device.
+template <void (*K)(HcArgs, HcGeom)>
+int launch_kernel(const char* name, unsigned grid, int threads, uint32_t limit, const HcArgs& a, const HcGeom& g,
+                  cudaStream_t s) {
   static DeviceOnce configured;
-  if (configured.need()) {
-    const int lim = (int)(NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA);
-    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    AB_CUDA_TRY(cudaFuncSetAttribute(hconv_kernel<NW, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-  }
-  const int64_t grid = (int64_t)a.B * g.tiles;
-  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
-  if (bf16) hconv_kernel<NW, 1><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
-  else hconv_kernel<NW, 0><<<(unsigned)grid, HC_THREADS, g.smem_bytes, s>>>(a, g);
-  AB_LAUNCH_CHECK("hconv_kernel");
+  if (configured.need()) AB_CUDA_TRY(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
+  K<<<grid, threads, g.smem_bytes, s>>>(a, g);
+  AB_LAUNCH_CHECK(name);
   return AB_OK;
 }
 
-template <int NW>
-int launch_chain(const HcArgs& a, const HcGeom& g, int bf16, cudaStream_t s) {
-  static DeviceOnce configured;
-  if (configured.need()) {
-    AB_CUDA_TRY(cudaFuncSetAttribute(hchain_kernel<NW, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
-    AB_CUDA_TRY(cudaFuncSetAttribute(hchain_kernel<NW, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
+template <int V>
+using IntC = std::integral_constant<int, V>;
+
+// f(IntC<NW>(), IntC<BF16>()) for the N width of g and a tensor-core precision: the kernels' template arguments
+template <class F>
+int with_nw(const HcGeom& g, int precision, F f) {
+  auto with_prec = [&](auto nw) { return precision == AB_PREC_TC_BF16 ? f(nw, IntC<1>()) : f(nw, IntC<0>()); };
+  switch ((int)(g.stage_bytes / 64u)) {
+    case 16: return with_prec(IntC<16>());
+    case 32: return with_prec(IntC<32>());
+    case 64: return with_prec(IntC<64>());
+    case 128: return with_prec(IntC<128>());
+    case 256: return with_prec(IntC<256>());
   }
-  const int64_t work = (int64_t)a.B * g.tiles;
-  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc block: too many tiles");
-  int dev = 0, sms = 0;
-  AB_CUDA_TRY(cudaGetDevice(&dev));
-  AB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const unsigned grid = (unsigned)std::min<int64_t>(work, sms);   // persistent: CTAs stride over the work items
-  if (bf16) hchain_kernel<NW, 1><<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g);
-  else hchain_kernel<NW, 0><<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g);
-  AB_LAUNCH_CHECK("hchain_kernel");
-  return AB_OK;
+  return fail(AB_ERR_UNSUPPORTED, "tc conv: N block %u", g.stage_bytes / 64u);
 }
 
 // Block-mode geometry: npairs x nconv convs of one ResBlock (C <= 64) with the halo recomputed inside the tile.
@@ -749,8 +726,7 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
   if (rc != AB_OK) return rc;
   if (L.NW > AB_TC_CHAIN_MAX_C) return fail(AB_ERR_UNSUPPORTED, "tc block: C=%d > %d", C, AB_TC_CHAIN_MAX_C);
   memset(&g, 0, sizeof(g));
-  g.mode = 3;
-  g.NB = 1; g.cc = L.NW; g.ntaps = k; g.k = k; g.nkc = L.nkc; g.u = 1; g.d = 1;
+  g.NB = 1; g.ntaps = k; g.nkc = L.nkc;
   g.nconv = nconv; g.nsteps = npairs * nconv;
   g.H = 0; g.G = 0;
   for (int q = 0; q < npairs; ++q) {
@@ -768,17 +744,10 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
   g.tiles = (T + g.V - 1) / g.V;
   g.c8n_in = g.c8n_out = rup(C, 16) / 8;
   g.stage_bytes = 64u * (uint32_t)L.NW;
-  const uint32_t xbytes = (uint32_t)g.nkc * 4u * (uint32_t)g.rowsX * 16u;
-  g.off_i = (xbytes + 127u) & ~127u;
-  g.off_w = (g.off_i + xbytes + 127u) & ~127u;
-  const uint32_t nbias = (uint32_t)(g.nsteps * L.NW);
-  const uint32_t bars = 16u * HC_STAGES_MAX + 16u;   // W ring full / empty, X full / empty
-  const uint32_t fixed = g.off_w + nbias * 4u + 16u + bars;
-  if (fixed + 2u * g.stage_bytes > HC_SMEM_1CTA) return fail(AB_ERR_UNSUPPORTED, "tc block: does not fit shared memory");
-  g.nstages = (int)std::min<uint32_t>((HC_SMEM_1CTA - fixed) / g.stage_bytes, HC_STAGES_MAX);
-  g.off_bias = g.off_w + (uint32_t)g.nstages * g.stage_bytes;
-  g.off_bar = (g.off_bias + nbias * 4u + 15u) & ~15u;
-  g.smem_bytes = g.off_bar + bars;
+  const uint32_t xbytes = (uint32_t)g.nkc * 64u * (uint32_t)g.rowsX;   // X and the intermediate tile
+  // mbarriers: W ring full / empty, X full / empty
+  if (!layout_smem(g, xbytes, xbytes, (uint32_t)(g.nsteps * L.NW), 16u * HC_STAGES_MAX + 16u, HC_SMEM_1CTA))
+    return fail(AB_ERR_UNSUPPORTED, "tc block: does not fit shared memory");
   g.out_scale = 1.0f;
   g.mid_slope = 1.0f;
   return AB_OK;
@@ -786,15 +755,13 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
 
 int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s) {
   if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
-  const int bf16 = precision == AB_PREC_TC_BF16;
-  switch ((int)(g.stage_bytes / 64u)) {
-    case 16: return launch_nw<16>(a, g, bf16, s);
-    case 32: return launch_nw<32>(a, g, bf16, s);
-    case 64: return launch_nw<64>(a, g, bf16, s);
-    case 128: return launch_nw<128>(a, g, bf16, s);
-    case 256: return launch_nw<256>(a, g, bf16, s);
-  }
-  return fail(AB_ERR_UNSUPPORTED, "tc conv: N block %u", g.stage_bytes / 64u);
+  const int64_t grid = (int64_t)a.B * g.tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
+  return with_nw(g, precision, [&](auto nw, auto bf16) {
+    constexpr int NW = decltype(nw)::value;
+    return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)grid, HC_THREADS,
+                                                                   NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
+  });
 }
 
 HcArgs base_args(const float* x, int64_t xsb, int64_t xsc, int64_t xst, const uint16_t* ximg, float pre_slope, int B,
@@ -830,13 +797,20 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
     a.bs[i] = p.bias[i];
   }
   a.y = p.y; a.acc_prev = p.acc_prev; a.yimg = p.yimg; a.img_slope = p.img_slope;
-  const int bf16 = p.precision == AB_PREC_TC_BF16;
-  switch ((int)(g.stage_bytes / 64u)) {
-    case 16: return launch_chain<16>(a, g, bf16, s);
-    case 32: return launch_chain<32>(a, g, bf16, s);
-    case 64: return launch_chain<64>(a, g, bf16, s);
-  }
-  return fail(AB_ERR_UNSUPPORTED, "tc block: N block %u", g.stage_bytes / 64u);
+  const int64_t work = (int64_t)a.B * g.tiles;
+  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc block: too many tiles");
+  int dev = 0, sms = 0;
+  AB_CUDA_TRY(cudaGetDevice(&dev));
+  AB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const unsigned grid = (unsigned)std::min<int64_t>(work, sms);   // persistent: CTAs stride over the work items
+  return with_nw(g, p.precision, [&](auto nw, auto bf16) {
+    constexpr int NW = decltype(nw)::value;
+    if constexpr (NW > AB_TC_CHAIN_MAX_C)   // make_chain_geom rejects wider blocks
+      return fail(AB_ERR_UNSUPPORTED, "tc block: N block %d", NW);
+    else
+      return launch_kernel<hchain_kernel<NW, decltype(bf16)::value>>("hchain_kernel", grid, HB_THREADS, HC_SMEM_1CTA, a,
+                                                                      g, s);
+  });
 }
 
 bool tc_conv_supported(int C, int k) { return C > 0 && C <= TC_MAX_C && (k & 1) && k <= 31; }
@@ -888,7 +862,8 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   g.out_scale = 1.0f / p.out_div;
   g.mid_slope = p.mid_slope;
   HcArgs a = base_args(p.x, p.xsb, p.xsc, p.xst, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
-  a.w = p.w; a.w2 = p.w2; a.bias = p.bias; a.bias2 = p.b2;
+  a.ws[0] = p.w; a.bs[0] = p.bias;
+  a.ws[1] = p.w2; a.bs[1] = p.b2;
   a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev; a.post_tanh = p.post_tanh;
   a.yimg = p.yimg; a.img_slope = p.img_slope;
   return launch_hconv(a, g, p.precision, s);
