@@ -18,8 +18,9 @@
 //      streamed with cp.async.bulk (TMA 1-D) through an mbarrier ring; thread 0 refills a stage once every warp
 //      has released it.
 //   D: fp32 in the registers of two consumer warpgroups (MT m64 tiles each); the epilogues run on the fragments.
-// hconv_kernel (conv, conv-transpose, pair) and hchain_kernel (block mode) share the operand loader, the wgmma batch,
-// the intermediate-tile and output epilogues and the shared-memory layout below; they differ in how they schedule them.
+// hconv_kernel (conv, conv-transpose), hpair_kernel (conv pair) and hchain_kernel (block mode) share the operand
+// loader, the wgmma batch, the intermediate-tile and output epilogues and the shared-memory layout below; they differ in
+// how they schedule them.
 #include <stdlib.h>
 #include <string.h>
 
@@ -65,7 +66,7 @@ struct HcArgs {
 };
 
 struct HcGeom {
-  int mode;                // hconv_kernel: 0 conv, 1 conv-transpose, 2 conv pair
+  int mode;                // 0 conv, 1 conv-transpose (hconv_kernel), 2 conv pair (hpair_kernel)
   int NB, cc;              // N blocks; output channels per block
   int R, V, tiles;         // rows per CTA tile, valid output rows per tile, tiles per sequence
   int ntaps, d;            // taps of every conv; the row step between the (first) conv's taps
@@ -81,6 +82,7 @@ struct HcGeom {
   // tap shift is a non-negative row offset
   int nconv, H, G, rowsX;
   int dil[AB_TC_CHAIN_MAX_PAIRS];
+  int nabuf;               // pair mode: A chunk buffers
 };
 
 // ------------------------------------------------------------------------------------------------ shared device code
@@ -191,11 +193,15 @@ __device__ __forceinline__ void store_frag_tile(uint8_t* tile, const float (&v)[
     }
 }
 
+// What epilogue_out reads from HBM and applies; a term that is not compiled in is either never set by the kernel's
+// launches (block mode: residual, tanh) or already part of val (hpair_kernel's prefetched residual and branch sum).
+enum : int { EP_RESIDUAL = 1, EP_ACC_PREV = 2, EP_TANH = 4, EP_ALL = 7 };
+
 // Output epilogue on fragment rows [r0, r1) at times t0 + row < Tout, output channels co0 + column < C_out:
 //   y = ((val + residual) + acc_prev) * out_scale [tanh] ; yimg = cvt(lrelu(y, img_slope))
-// where val(mt, c, h, e) is the value of accumulator element [mt][c*4 + 2h + e] before the epilogue.  Without
-// RES_TANH (block mode, whose launches never set them) the residual and tanh are not compiled in.
-template <int NW, int BF16, bool RES_TANH, int MT, class Val>
+// where val(mt, c, h, e) is the value of accumulator element [mt][c*4 + 2h + e] before the epilogue.  EP selects the
+// terms that are compiled in.
+template <int NW, int BF16, int EP, int MT, class Val>
 __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, const Frag<MT>& f, int b, int t0, int r0,
                                              int r1, int co0, Val val) {
 #pragma unroll
@@ -214,10 +220,10 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
           if (co + e < p.Cout) {
             const int64_t idx = ((int64_t)b * p.Cout + co + e) * g.Tout + t;
             float v = val(mt, c, h, e);
-            if (RES_TANH && p.residual) v += __ldg(p.residual + idx);
-            if (p.acc_prev) v += p.acc_prev[idx];
+            if ((EP & EP_RESIDUAL) && p.residual) v += __ldg(p.residual + idx);
+            if ((EP & EP_ACC_PREV) && p.acc_prev) v += p.acc_prev[idx];
             v *= g.out_scale;
-            if (RES_TANH && p.post_tanh) v = tanhf(v);
+            if ((EP & EP_TANH) && p.post_tanh) v = tanhf(v);
             p.y[idx] = v;
             ve[e] = v;
           }
@@ -232,7 +238,11 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
 
 // ------------------------------------------------------------------------------------------------ kernels
 
-// modes 0-2; block mode runs on hchain_kernel below
+// modes 0 (conv) and 1 (conv-transpose); launch_hconv runs pair mode (2) on hpair_kernel, and block mode runs on
+// hchain_kernel.  The mode-2 branch below is no longer launched but stays: without it ptxas (nvcc 12.9, build.py's
+// flags) reports spill stores / loads of 956 / 1220 bytes at N = 256 and 784 / 1020 at N = 128, against 4 / 4 and
+// 16 / 20 with it, which made HiFi-GAN V1's ConvTranspose layers about 5 ms per step slower (H100 80GB HBM3, 400 W
+// power limit).  Re-check those numbers before deleting it.
 template <int NW, int BF16>
 __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
@@ -313,7 +323,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   // are built where they are used: kept live across the MMA loops, they make ptxas spill more.
   auto epilogue_conv = [&](int nb, const float* bias_blk) {
     const Frag<MT> f(wg);
-    epilogue_out<NW, BF16, true>(p, g, f, b, O, 0, g.V, nb * NW, [&](int mt, int c, int h, int e) {
+    epilogue_out<NW, BF16, EP_ALL>(p, g, f, b, O, 0, g.V, nb * NW, [&](int mt, int c, int h, int e) {
       return acc[mt][c * 4 + 2 * h + e] + bias_blk[c * 8 + f.col + e];
     });
   };
@@ -376,7 +386,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
 //   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams the weight stages of every tile through the W ring;
 //     warps 1-3 load the operand tile X of the next work item as soon as the consumers release it, so that load
 //     overlaps the current tile's output epilogue.
-//   warpgroups 1-2 (consumers, setmaxnreg 232): one wgmma batch per tap with the previous batch still in flight; a
+//   warpgroups 1-2 (consumers, setmaxnreg 232): one wgmma batch per tap with the two previous batches still in flight; a
 //     W slot is released once the batch that read it has completed.  Consumer-only synchronisation is a named
 //     barrier.  The residual stream x_p of the whole ResBlock stays in registers in the accumulator fragment layout.
 // The accumulation order of every output element is that of hconv_kernel's per-pair mode (K chunk -> tap -> k16).
@@ -385,8 +395,24 @@ constexpr int HB_LOADERS = 96;
 constexpr int HB_PRODUCER_REGS = 40;
 constexpr int HB_CONSUMER_REGS = 232;
 static_assert(128 * HB_PRODUCER_REGS + 256 * HB_CONSUMER_REGS <= 65536, "setmaxnreg split of the register file");
+constexpr int HP_ABUF_MAX = 3;   // hpair_kernel: A chunk buffers, as many as fit (one for very wide tap reach)
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Position in a ring of n mbarrier slots: the slot, the parity of its current round, and whether the ring has wrapped
+// (the producer waits for a slot's release from the second round on).  Counters instead of a division per tap.
+struct RingPos {
+  int s = 0;
+  uint32_t ph = 0;
+  bool wrapped = false;
+  __device__ __forceinline__ void next(int n) {
+    if (++s == n) {
+      s = 0;
+      ph ^= 1u;
+      wrapped = true;
+    }
+  }
+};
 
 template <int NW, int BF16>
 __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom g) {
@@ -423,14 +449,13 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
     if (tid == 0) {
-      int wi = 0;
+      RingPos r;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
         for (int st = 0; st < g.nsteps; ++st)
-          for (int i = 0; i < per_step; ++i, ++wi) {
-            const int s = wi % g.nstages;
-            if (wi >= g.nstages) mbar_wait(w_empty(s), (uint32_t)(wi / g.nstages - 1) & 1u);
-            mbar_arrive_expect_tx(w_full(s), g.stage_bytes);
-            bulk_g2s(sW + (uint32_t)s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(s));
+          for (int i = 0; i < per_step; ++i, r.next(g.nstages)) {
+            if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
+            mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
+            bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(r.s));
           }
       }
     } else if (tid >= 32) {
@@ -452,8 +477,11 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
   const int cw = wg - 1;
   const Frag<MT> f(cw);
   float acc[MT][NACC];
-  int it = 0;        // weight stages consumed so far
-  int pw = -1;       // W slot read by the batch still in flight (-1: none)
+  RingPos wr;        // W slot of the next weight stage
+  // W slots read by the batches in flight, oldest first (-1: none).  Two batches stay in flight when the ring leaves a
+  // slot to fill next to the two they hold.
+  const bool deep = g.nstages >= 3;
+  int pw0 = -1, pw1 = -1;
 
   // keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
   auto fence_acc = [&]() {
@@ -462,32 +490,41 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
 #pragma unroll
       for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
   };
-  auto release_w = [&]() {
+  auto release_w = [&](int pw) {
     __syncwarp();
     if (lane == 0 && pw >= 0) mbar_arrive(w_empty(pw));
   };
   // the taps of one 32-channel K chunk over the operand at aBase
   auto mma_chunk = [&](uint32_t aBase, int ntaps, int tapstep, bool& first) {
-    for (int j = 0; j < ntaps; ++j, ++it) {
-      const int s = it % g.nstages;
-      mbar_wait(w_full(s), (uint32_t)(it / g.nstages) & 1u);
+    for (int j = 0; j < ntaps; ++j) {
+      const int s = wr.s;
+      mbar_wait(w_full(s), wr.ph);
+      wr.next(g.nstages);
       const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
       fence_acc();
       wg_fence();
       mma_batch<NW, BF16>(acc, aBase, g.rowsX, cw * MT * 64 + j * tapstep, wS, first);
       wg_commit();
-      wg_wait<1>();      // the previous batch has completed: its W slot can be refilled
-      fence_acc();
-      release_w();
-      pw = s;
+      if (deep) {
+        wg_wait<2>();    // the batch before the previous one has completed: its W slot can be refilled
+        fence_acc();
+        release_w(pw0);
+        pw0 = pw1;
+      } else {
+        wg_wait<1>();
+        fence_acc();
+        release_w(pw1);
+      }
+      pw1 = s;
       first = false;
     }
   };
   auto drain = [&]() {
     wg_wait<0>();
     fence_acc();
-    release_w();
-    pw = -1;
+    release_w(pw0);
+    release_w(pw1);
+    pw0 = pw1 = -1;
   };
 
   int n = 0;
@@ -544,8 +581,205 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     __syncwarp();
     if (lane == 0) mbar_arrive(x_empty);
     // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V)
-    epilogue_out<NW, BF16, false>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
-                           [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
+    epilogue_out<NW, BF16, EP_ACC_PREV>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
+                                        [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
+  }
+}
+
+// Pair mode (launch_tc_conv with a second conv; one ResBlock1 step): warp-specialised and persistent like
+// hchain_kernel, with the per-pair tile geometry of make_geom (output row r at time O + r, V = R - (k - 1)).
+//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams both convs' weight stages of every tile through the W
+//     ring; warps 1-3 stream the A operand in 32-channel K chunks through a ring of g.nabuf chunk buffers.  Conv2 reads
+//     only the intermediate tile, so the next tile's chunks load under this tile's conv2 and output epilogue.
+//   warpgroups 1-2 (consumers, setmaxnreg 232): two wgmma batches in flight (one where the rings are too small); a
+//     W slot, and an A buffer after its last tap, is released once the batch that read it has completed.  Below N = 256 each consumer loads the residual
+//     of its fragment into registers at the start of the tile, so that HBM read runs under the MMAs; the branch sum
+//     would need another 64 registers at N = 128 (ptxas spills) and is read in the epilogue.
+// Accumulation order (K chunk -> tap -> k16, conv1 then conv2) and epilogue association are those of the per-pair
+// arithmetic, so the tile shape does not enter any output element.
+template <int NW, int BF16>
+__global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g) {
+  constexpr int MT = mt_of(NW);
+  constexpr int NACC = NW / 2;
+  constexpr bool PREFETCH = MT * NACC <= 64;   // 64 accumulators leave room for 64 prefetched residuals
+  constexpr int PM = PREFETCH ? MT : 1, PN = PREFETCH ? NACC : 1;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const uint32_t sA = smem_u32(smem), sI = sA + g.off_i, sW = sA + g.off_w;
+  const uint32_t abytes = (uint32_t)g.rowsA * 64u;   // one A chunk: 4 c8 planes x rowsA rows
+  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
+  const uint32_t bar0 = smem_u32(smem + g.off_bar);
+  auto w_full = [&](int s) { return bar0 + 8u * s; };
+  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
+  auto a_full = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + s); };
+  auto a_empty = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + HP_ABUF_MAX + s); };
+  const int nwork = p.B * g.tiles;
+  const int per_step = g.nkc * g.ntaps;
+
+  if (tid == 0) {
+    for (int s = 0; s < g.nstages; ++s) {
+      mbar_init(w_full(s), 1);
+      mbar_init(w_empty(s), 8);
+    }
+    for (int s = 0; s < g.nabuf; ++s) {
+      mbar_init(a_full(s), HB_LOADERS);
+      mbar_init(a_empty(s), 8);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  stage_biases(bias_s, p, 2, NW, tid, HB_THREADS);
+  // rows and channels of the intermediate that store_frag_tile does not write stay zero for every tile
+  for (int i = tid; i < g.nkc * 4 * g.rowsI; i += HB_THREADS)
+    *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
+  fence_proxy_async();
+  __syncthreads();
+
+  // ------------------------------------------------------------------------------------------------ producer
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+    if (tid == 0) {
+      RingPos r;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x)
+        for (int st = 0; st < 2; ++st)
+          for (int i = 0; i < per_step; ++i, r.next(g.nstages)) {
+            if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
+            mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
+            bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(r.s));
+          }
+    } else if (tid >= 32) {
+      // A chunk kc of a tile: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
+      int q = 0;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+        const int b = w / g.tiles, t0 = (w - b * g.tiles) * g.V - g.a0;
+        for (int kc = 0; kc < g.nkc; ++kc, ++q) {
+          const int s = q % g.nabuf;
+          if (q >= g.nabuf) mbar_wait(a_empty(s), (uint32_t)(q / g.nabuf - 1) & 1u);
+          load_tile<BF16>(p, g, b, smem + s * abytes, 4 * kc, 4, g.rowsA, t0, tid - 32, HB_LOADERS);
+          fence_proxy_async();
+          mbar_arrive(a_full(s));
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------------------------------------ consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
+  const int cw = wg - 1;
+  float acc[MT][NACC];
+  RingPos wr;             // W slot of the next weight stage
+  int q = 0;              // A chunks consumed so far
+  // Batches in flight, oldest first: the W slot each read, and the A buffer whose last tap it was (-1: none).  Two
+  // stay in flight when the rings allow it: every W slot held by an in-flight batch must leave one to fill
+  // (nstages >= 3), and the loaders must not need the buffer of the last tap of the chunk before the previous one
+  // (ntaps >= 2, or three buffers; one buffer is drained after every chunk).
+  const bool deep = g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2);
+  int pw0 = -1, pw1 = -1, pa0 = -1, pa1 = -1;
+
+  auto fence_acc = [&]() {
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
+  };
+  auto release = [&](int w, int a) {
+    __syncwarp();
+    if (lane == 0) {
+      if (w >= 0) mbar_arrive(w_empty(w));
+      if (a >= 0) mbar_arrive(a_empty(a));
+    }
+  };
+  // the taps of one 32-channel K chunk over the operand at aBase (aRows rows per c8 plane); abuf: the A buffer it
+  // reads, or -1 for the intermediate tile
+  auto mma_chunk = [&](uint32_t aBase, int aRows, int tapstep, int abuf, bool& first) {
+    for (int j = 0; j < g.ntaps; ++j) {
+      const int s = wr.s;
+      mbar_wait(w_full(s), wr.ph);
+      wr.next(g.nstages);
+      const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
+      fence_acc();
+      wg_fence();
+      mma_batch<NW, BF16>(acc, aBase, aRows, cw * MT * 64 + j * tapstep, wS, first);
+      wg_commit();
+      const int a = j == g.ntaps - 1 ? abuf : -1;
+      if (deep) {
+        wg_wait<2>();    // the batch before the previous one has completed: its W slot (and A buffer) can be refilled
+        fence_acc();
+        release(pw0, pa0);
+        pw0 = pw1;
+        pa0 = pa1;
+      } else {
+        wg_wait<1>();
+        fence_acc();
+        release(pw1, pa1);
+      }
+      pw1 = s;
+      pa1 = a;
+      first = false;
+    }
+  };
+  auto drain = [&]() {
+    wg_wait<0>();
+    fence_acc();
+    release(pw0, pa0);
+    release(pw1, pa1);
+    pw0 = pw1 = pa0 = pa1 = -1;
+  };
+
+  for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+    const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
+    // residual of this thread's output elements, in flight under the MMAs
+    float xres[PM][PN];
+    if constexpr (PREFETCH) {
+      const Frag<MT> f(cw);
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = f.row(mt, h), t = O + row;
+          const bool ok = row < g.V && t < g.Tout;
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int co = c * 8 + f.col + e;
+              const bool in = ok && co < p.Cout && p.residual;
+              xres[mt][c * 4 + 2 * h + e] = in ? __ldg(p.residual + ((int64_t)b * p.Cout + co) * g.Tout + t) : 0.f;
+            }
+        }
+    }
+    // conv1 over the A chunks
+    bool first = true;
+    for (int kc = 0; kc < g.nkc; ++kc, ++q) {
+      const int s = q % g.nabuf;
+      mbar_wait(a_full(s), (uint32_t)(q / g.nabuf) & 1u);
+      mma_chunk(sA + (uint32_t)s * abytes, g.rowsA, g.d, s, first);
+      if (g.nabuf == 1) drain();   // the loaders refill the only buffer with the next chunk
+    }
+    drain();
+    // intermediate = lrelu(conv1 + b1, mid_slope) -> operand tile, row 0 at time O - h2, zero outside [0, T)
+    consumer_sync();   // both warpgroups have finished the previous tile's conv2, which read the intermediate
+    store_frag_tile<NW, BF16>(smem + g.off_i, acc, bias_s, Frag<MT>(cw), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc,
+                              g.mid_slope);
+    fence_proxy_async();
+    consumer_sync();
+    first = true;
+    for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, 1, -1, first);
+    drain();
+    // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
+    const Frag<MT> f(cw);
+    const float* b2 = bias_s + NW;
+    if constexpr (PREFETCH) {
+      epilogue_out<NW, BF16, EP_ACC_PREV | EP_TANH>(p, g, f, b, O, 0, g.V, 0, [&](int mt, int c, int h, int e) {
+        const int i = c * 4 + 2 * h + e;
+        const float v = acc[mt][i] + b2[c * 8 + f.col + e];
+        return p.residual ? v + xres[mt][i] : v;
+      });
+    } else {
+      epilogue_out<NW, BF16, EP_ALL>(p, g, f, b, O, 0, g.V, 0, [&](int mt, int c, int h, int e) {
+        return acc[mt][c * 4 + 2 * h + e] + b2[c * 8 + f.col + e];
+      });
+    }
   }
 }
 
@@ -681,9 +915,19 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, HcGeom& g
   if (g.rowsA > 16383 || g.rowsI > 16383) return fail(AB_ERR_UNSUPPORTED, "tc conv: tap reach %d too large", maxshift);
   g.tiles = (rows_total + g.V - 1) / g.V;
   g.stage_bytes = 64u * (uint32_t)L.NW;
-  if (!layout_smem(g, (uint32_t)g.rowsA * 64u, (uint32_t)g.nkc * 64u * (uint32_t)g.rowsI,
-                   (uint32_t)(g.nsteps * g.NB * L.NW), 16u * HC_STAGES_MAX, L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA))
-    return fail(AB_ERR_UNSUPPORTED, "tc conv: C=%d k=%d reach %d does not fit shared memory", cin, k, maxshift);
+  const uint32_t abytes = (uint32_t)g.rowsA * 64u, nbias = (uint32_t)(g.nsteps * g.NB * L.NW);
+  bool fits;
+  if (mode == 2) {   // hpair_kernel: one CTA per SM, as many A chunk buffers as fit next to two W stages
+    const uint32_t ibytes = (uint32_t)g.nkc * 64u * (uint32_t)g.rowsI;
+    g.nabuf = HP_ABUF_MAX;
+    while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, ibytes, nbias,
+                                16u * (HC_STAGES_MAX + HP_ABUF_MAX), HC_SMEM_1CTA)) && g.nabuf > 1)
+      --g.nabuf;
+  } else {
+    g.nabuf = 1;
+    fits = layout_smem(g, abytes, 0, nbias, 16u * HC_STAGES_MAX, L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA);
+  }
+  if (!fits) return fail(AB_ERR_UNSUPPORTED, "tc conv: C=%d k=%d reach %d does not fit shared memory", cin, k, maxshift);
   g.out_scale = 1.0f;
   g.mid_slope = 1.0f;
   return AB_OK;
@@ -753,13 +997,33 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
   return AB_OK;
 }
 
+// Grid of a persistent kernel: min(work items, SMs), the CTAs striding over the items.
+int persistent_grid(int64_t work, const char* what, unsigned& grid) {
+  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "%s: too many tiles", what);
+  int dev = 0, sms = 0;
+  AB_CUDA_TRY(cudaGetDevice(&dev));
+  AB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  grid = (unsigned)std::min<int64_t>(work, sms);
+  return AB_OK;
+}
+
+// modes 0 and 1 on hconv_kernel (one CTA per tile), pair mode on the persistent hpair_kernel
 int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s) {
   if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
-  const int64_t grid = (int64_t)a.B * g.tiles;
-  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
+  const int64_t work = (int64_t)a.B * g.tiles;
+  if (g.mode == 2) {
+    unsigned grid = 0;
+    const int rc = persistent_grid(work, "tc conv pair", grid);
+    if (rc != AB_OK) return rc;
+    return with_nw(g, precision, [&](auto nw, auto bf16) {
+      return launch_kernel<hpair_kernel<decltype(nw)::value, decltype(bf16)::value>>("hpair_kernel", grid, HB_THREADS,
+                                                                                     HC_SMEM_1CTA, a, g, s);
+    });
+  }
+  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
   return with_nw(g, precision, [&](auto nw, auto bf16) {
     constexpr int NW = decltype(nw)::value;
-    return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)grid, HC_THREADS,
+    return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)work, HC_THREADS,
                                                                    NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
   });
 }
@@ -797,12 +1061,9 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
     a.bs[i] = p.bias[i];
   }
   a.y = p.y; a.acc_prev = p.acc_prev; a.yimg = p.yimg; a.img_slope = p.img_slope;
-  const int64_t work = (int64_t)a.B * g.tiles;
-  if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc block: too many tiles");
-  int dev = 0, sms = 0;
-  AB_CUDA_TRY(cudaGetDevice(&dev));
-  AB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const unsigned grid = (unsigned)std::min<int64_t>(work, sms);   // persistent: CTAs stride over the work items
+  unsigned grid = 0;
+  rc = persistent_grid((int64_t)a.B * g.tiles, "tc block", grid);
+  if (rc != AB_OK) return rc;
   return with_nw(g, p.precision, [&](auto nw, auto bf16) {
     constexpr int NW = decltype(nw)::value;
     if constexpr (NW > AB_TC_CHAIN_MAX_C)   // make_chain_geom rejects wider blocks

@@ -5,7 +5,8 @@ trace with CUDA activities.
     python scripts/profile_stages.py [--batch 64] [--frames 1024] [--fusion 2] [--out DIR]
 
 The tensor-core launches of `forward_impl` come in a fixed order: conv_pre, then per stage one ConvTranspose and per
-ResBlock either one block-mode launch (`hchain_kernel`) or one `hconv_kernel` launch per dilation pair.  The script
+ResBlock either one block-mode launch (`hchain_kernel`) or one `hpair_kernel` launch per dilation pair; conv_pre and
+the ConvTranspose layers run on `hconv_kernel`.  The script
 walks that order, attributes each tensor-core launch to (stage, plan) and prints time, share of the step, achieved
 TFLOP/s and algorithmic GB/s per row.  Algorithmic bytes per ResBlock launch: the 16-bit operand image and the fp32
 residual read, the fp32 output and its operand image written, the running branch sum read when it is accumulated, and
@@ -102,7 +103,7 @@ def main():
     kern = sorted((e for e in prof.events() if e.device_type.name == "CUDA" and "memcpy" not in e.name.lower()
                    and "memset" not in e.name.lower()), key=lambda e: e.time_range.start)
     step_us = kern[-1].time_range.end - kern[0].time_range.start
-    tc = ("hconv_kernel", "hchain_kernel")
+    tc = ("hconv_kernel", "hchain_kernel", "hpair_kernel")
     hc = [e for e in kern if any(n in e.name for n in tc)]
     other_us = sum(e.time_range.elapsed_us() for e in kern if not any(n in e.name for n in tc))
 
