@@ -10,7 +10,7 @@ AB_MAX_STAGES = 8
 AB_MAX_KERNELS = 8
 AB_MAX_DILATIONS = 8
 
-GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK = 0, 1, 2, 3
+GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN = 0, 1, 2, 3, 4
 ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA = 0, 1, 2
 PRECISIONS = {"fp32": 0, "tc_f16": 1, "tc_bf16": 2}
 

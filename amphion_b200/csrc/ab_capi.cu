@@ -62,6 +62,7 @@ struct Slot {
 struct ConvRef {   // one weight-normed conv of the model
   int w = -1, b = -1;
   int cin = 0, cout = 0, k = 0, d = 1;
+  bool reflect = false;   // ReflectionPad1d((k-1)*d/2) in front of it instead of zero padding (MelGAN)
 };
 
 struct ActRef {    // one Activation1d module
@@ -73,6 +74,7 @@ struct BlockRef {  // one ResBlock / AMPBlock
   std::vector<int> dil;
   std::vector<ConvRef> c1, c2;  // c2 empty for ResBlock2 / AMPBlock2
   std::vector<ActRef> acts;     // 2*nd (type 1) or nd (type 2); empty for HiFi-GAN
+  ConvRef sc;                   // MelGAN ResnetBlock: the 1x1 shortcut (c1, c2 then hold one conv each)
 };
 
 struct StageRef {
@@ -179,9 +181,11 @@ ActRef make_act(ab_generator* g, const std::string& prefix, int ch, bool has_bet
 }
 
 int validate_config(const ab_generator_config& c) {
-  if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK)
+  if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
+      c.kind != AB_GEN_MELGAN)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   const bool trunk = c.kind == AB_GEN_TRUNK;
+  const bool melgan = c.kind == AB_GEN_MELGAN;
   if (trunk) {
     if (c.num_upsamples != 0) return fail(AB_ERR_ARG, "config: a trunk has no upsampling stages");
     if (c.trunk_out_channels <= 0 || c.trunk_out_channels > 65536) return fail(AB_ERR_ARG, "config: trunk_out_channels %d out of range", c.trunk_out_channels);
@@ -198,7 +202,11 @@ int validate_config(const ab_generator_config& c) {
   if ((c.upsample_initial_channel >> c.num_upsamples) <= 0) return fail(AB_ERR_ARG, "config: upsample_initial_channel too small for %d stages", c.num_upsamples);
   for (int i = 0; i < c.num_upsamples; ++i) {
     const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i];
-    if (u <= 0 || k < u || ((k - u) & 1)) return fail(AB_ERR_UNSUPPORTED, "config: stage %d: kernel %d / rate %d (need k >= u, k-u even)", i, k, u);
+    if (melgan) {
+      if (u <= 0 || k != 2 * u) return fail(AB_ERR_ARG, "config: MelGAN stage %d: kernel %d must be 2 x ratio %d", i, k, u);
+    } else if (u <= 0 || k < u || ((k - u) & 1)) {
+      return fail(AB_ERR_UNSUPPORTED, "config: stage %d: kernel %d / rate %d (need k >= u, k-u even)", i, k, u);
+    }
   }
   for (int j = 0; j < c.num_kernels; ++j) {
     if (c.num_dilations[j] <= 0 || c.num_dilations[j] > AB_MAX_DILATIONS) return fail(AB_ERR_ARG, "config: num_dilations[%d] out of range", j);
@@ -206,6 +214,17 @@ int validate_config(const ab_generator_config& c) {
     if (k <= 0 || !(k & 1)) return fail(AB_ERR_UNSUPPORTED, "config: resblock kernel size %d must be odd", k);
     for (int p = 0; p < c.num_dilations[j]; ++p)
       if (c.resblock_dilation_sizes[j][p] <= 0) return fail(AB_ERR_ARG, "config: dilation must be positive");
+  }
+  if (melgan) {   // ResnetBlock(dim, dilation = 3^j), j < n_residual_layers (melgan.py:34-47, :82-85)
+    if (c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 3)
+      return fail(AB_ERR_ARG, "config: MelGAN has one block kind with kernel 3 (num_kernels %d, kernel %d)", c.num_kernels,
+                  c.resblock_kernel_sizes[0]);
+    for (int p = 0, d = 1; p < c.num_dilations[0]; ++p, d *= 3)
+      if (c.resblock_dilation_sizes[0][p] != d)
+        return fail(AB_ERR_ARG, "config: MelGAN residual layer %d must have dilation %d (got %d)", p, d, c.resblock_dilation_sizes[0][p]);
+    if ((c.upsample_initial_channel >> c.num_upsamples) << c.num_upsamples != c.upsample_initial_channel)
+      return fail(AB_ERR_ARG, "config: MelGAN upsample_initial_channel %d must be ngf * 2^%d", c.upsample_initial_channel, c.num_upsamples);
+    if (c.activation != AB_ACT_LRELU) return fail(AB_ERR_ARG, "config: MelGAN uses LeakyReLU(0.2)");
   }
   if (c.kind == AB_GEN_BIGVGAN && c.activation != AB_ACT_SNAKE && c.activation != AB_ACT_SNAKEBETA)
     return fail(AB_ERR_ARG, "config: BigVGAN activation must be snake or snakebeta");
@@ -229,32 +248,14 @@ size_t tc_image_bytes(const Slot& s, bool pre_or_post) {
   return tc_weight_image_bytes(0, cin, cout, k, s.dilation);
 }
 
-}  // namespace
-
-extern "C" {
-
-const char* ab_last_error(void) { return g_err; }
-int ab_version(void) { return 100; }
-
-int ab_device_is_sm90(void) {
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 9;
-}
-
-int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
-  if (!cfg || !out) return fail(AB_ERR_ARG, "ab_generator_create: null argument");
-  int rc = validate_config(*cfg);
-  if (rc != AB_OK) return rc;
-  ab_generator* g = new ab_generator();
-  g->cfg = *cfg;
+// HiFi-GAN, BigVGAN, NSF-HiFiGAN and trunk tensors (reference state-dict names)
+void add_gan_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
   const bool big = cfg->kind == AB_GEN_BIGVGAN;
   const bool has_beta = cfg->activation == AB_ACT_SNAKEBETA;
   const int c0 = cfg->upsample_initial_channel;
   const bool trunk = cfg->kind == AB_GEN_TRUNK;
   g->conv_pre = make_conv(g, "conv_pre", cfg->n_mel, c0, trunk ? cfg->trunk_in_kernel : 7, 1, false);
-  g->hop = 1;
   int ch = c0;
   if (trunk) {   // one stage at the input rate: no transposed conv, the ResBlock branches read conv_pre's output
     StageRef st;
@@ -317,6 +318,69 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     g->cond_w = g->add_slot("cond.weight", SLOT_VEC, {c0, cfg->gin_channels, 1});
     g->cond_b = g->add_slot("cond.bias", SLOT_VEC, {c0});
   }
+}
+
+// MelGAN tensors (AB_GEN_MELGAN)
+void add_melgan_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int c0 = cfg->upsample_initial_channel;
+  // one nn.Sequential "model" (melgan.py:57-98): [pad, conv_pre], per stage i [lrelu, ConvTranspose, R ResnetBlocks],
+  // [lrelu, pad, conv_post, tanh]; a ResnetBlock's convs are block.2 (k = 3, dilation 3^j), block.4 and shortcut (1x1)
+  const int R = cfg->num_dilations[0], n = cfg->num_upsamples;
+  auto mod = [](int i) { return "model." + std::to_string(i); };
+  g->conv_pre = make_conv(g, mod(1), cfg->n_mel, c0, 7, 1, false);
+  g->conv_pre.reflect = true;
+  for (int i = 0; i < n; ++i) {
+    StageRef st;
+    const int base = 2 + i * (2 + R), cin = c0 >> i;
+    st.ch = c0 >> (i + 1);
+    st.u = cfg->upsample_rates[i];
+    g->hop *= st.u;
+    st.up = make_conv(g, mod(base + 1), cin, st.ch, 2 * st.u, 1, true);
+    g->slots[st.up.w].stride = st.u;
+    for (int j = 0; j < R; ++j) {
+      BlockRef blk;
+      blk.k = 3;
+      const int d = cfg->resblock_dilation_sizes[0][j];
+      blk.dil.push_back(d);
+      const std::string pre = mod(base + 2 + j);
+      blk.c1.push_back(make_conv(g, pre + ".block.2", st.ch, st.ch, 3, d, false));
+      blk.c1.back().reflect = true;
+      blk.c2.push_back(make_conv(g, pre + ".block.4", st.ch, st.ch, 1, 1, false));
+      blk.sc = make_conv(g, pre + ".shortcut", st.ch, st.ch, 1, 1, false);
+      st.blocks.push_back(blk);
+    }
+    g->stages.push_back(st);
+  }
+  g->conv_post = make_conv(g, mod(2 + n * (2 + R) + 2), c0 >> n, 1, 7, 1, false);
+  g->conv_post.reflect = true;
+}
+
+}  // namespace
+
+extern "C" {
+
+const char* ab_last_error(void) { return g_err; }
+int ab_version(void) { return 100; }
+
+int ab_device_is_sm90(void) {
+  int dev = 0, major = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
+  return major == 9;
+}
+
+int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
+  if (!cfg || !out) return fail(AB_ERR_ARG, "ab_generator_create: null argument");
+  int rc = validate_config(*cfg);
+  if (rc != AB_OK) return rc;
+  ab_generator* g = new ab_generator();
+  g->cfg = *cfg;
+  g->hop = 1;
+  if (cfg->kind == AB_GEN_MELGAN)
+    add_melgan_tensors(g);
+  else
+    add_gan_tensors(g);
 
   // tensor-core weight images live behind the fp32 images
   size_t tc = 0;
@@ -573,6 +637,18 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   const size_t need = ab_generator_workspace_bytes(g, B, T);
   if (!dev_workspace || workspace_bytes < need) return fail(AB_ERR_WORKSPACE, "forward: workspace %zu B < required %zu B", workspace_bytes, need);
   if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "forward: workspace must be 256-byte aligned");
+  const bool melgan = g->cfg.kind == AB_GEN_MELGAN;
+  if (melgan) {   // ReflectionPad1d(p) needs more than p samples (the reference raises a RuntimeError)
+    if (T <= 3) return fail(AB_ERR_ARG, "forward: conv_pre's ReflectionPad1d(3) needs more than 3 mel frames (got %lld)", (long long)T);
+    int64_t t = T;
+    for (size_t i = 0; i < g->stages.size(); ++i) {
+      t *= g->stages[i].u;
+      for (auto& blk : g->stages[i].blocks)
+        if (t <= blk.dil[0])
+          return fail(AB_ERR_ARG, "forward: stage %d ResnetBlock's ReflectionPad1d(%d) needs more than %lld samples", (int)i,
+                      blk.dil[0], (long long)t);
+    }
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t bufsz = align_up(stage_max_elems(g, B, T) * sizeof(float), 256);
   const size_t imgsz = align_up(stage_max_image_bytes(g, B, T), 256);
@@ -617,7 +693,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     p.w_t = g->fptr(c.w); p.bias = g->fptr(c.b);
     p.residual = residual; p.acc_prev = acc_prev; p.y = y;
     p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d = c.d;
-    p.pre_slope = pre_slope; p.out_div = out_div; p.post_tanh = post_tanh;
+    p.pre_slope = pre_slope; p.out_div = out_div; p.post_tanh = post_tanh; p.reflect = c.reflect;
     ++launches;
     prof_begin(1, 2.0 * B * Tn * c.cout * c.cin * c.k, conv_bytes(c, Tn, residual, acc_prev));
     const int r = launch_conv1d_fp32(p, st);
@@ -638,7 +714,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     p.residual = residual; p.acc_prev = acc_prev; p.out_div = out_div; p.post_tanh = post_tanh;
     p.y = y; p.yimg = yimg; p.img_slope = 0.1f;
     p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d_or_u = c.d;
-    p.precision = g->precision;
+    p.precision = g->precision; p.reflect = c.reflect;
     ++launches;
     const bool rb = c.cin == c.cout && tc_conv_supported(c.cin, c.k);   // pair / block-mode capable ResBlock conv
     prof_begin(rb ? 0 : 4, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes);
@@ -666,7 +742,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   const ConvRef& cpre = g->conv_pre;
   // HiFi-GAN: a tensor-core stage-0 ConvTranspose reads lrelu(x, 0.1) -> conv_pre emits that operand image, unless the
   // conditioning add changes x after it
-  const bool pre_img = !big && dev_g == nullptr && on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&
+  const bool pre_img = !big && !melgan && dev_g == nullptr && on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&
                        on_tc(g->stages[0].up) && (C0 % 16) == 0 &&
                        tc_can_emit_image(0, cpre.cin, cpre.cout, cpre.k, cpre.d);
   rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, R[0],
@@ -693,7 +769,8 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       std::swap(U, R[cur_r]);   // AB_GEN_TRUNK: the blocks read conv_pre's output in place
     } else {
       const bool up_tc = on_tc(sg.up);
-      const float pre_slope = big ? 1.0f : 0.1f;
+      // x = leaky_relu(x, 0.2) ; x = ConvTranspose1d(k = 2u, padding u//2 + u%2, output_padding u%2) (melgan.py:72-80)
+      const float pre_slope = big ? 1.0f : melgan ? 0.2f : 0.1f;
       ++launches;
       const double eo = (double)B * sg.ch * Tn * sg.u;
       prof_begin(up_tc ? 4 : 2, 2.0 * eo * cin * ((double)sg.up.k / sg.u),
@@ -705,14 +782,16 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
         p.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr;
         p.w = g->tcptr(sg.up.w); p.bias = g->fptr(sg.up.b); p.y = U;
         // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
-        u_img = (!big && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
+        u_img = (!big && !melgan && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
         p.yimg = u_img; p.img_slope = 0.1f;
         p.B = (int)B; p.Cin = cin; p.Cout = sg.ch; p.T = Tn; p.k = sg.up.k; p.d_or_u = sg.u; p.precision = g->precision;
+        p.pad = melgan ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
         rc = launch_tc_conv(p, st);
       } else {
         ConvTParams tp;
         tp.x = R[cur_r]; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
         tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u; tp.pre_slope = pre_slope;
+        tp.pad = melgan ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
         rc = launch_conv_transpose1d_fp32(tp, st);
       }
       prof_end();
@@ -737,7 +816,25 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     float* Rout = R[cur_r ^ 1];
     const int64_t sb = (int64_t)C * Tn, sc = Tn;
     bool stage_img_written = false;
-    for (int j = 0; j < nk; ++j) {
+    // MelGAN: x <- shortcut(x) + c2(lrelu(c1(lrelu(x, 0.2), reflect-padded, dilation 3^j), 0.2)) for each ResnetBlock
+    // (melgan.py:34-47), as three launches: c1 -> TMP, c2 -> P0, shortcut + P0 -> the block output.  The outputs
+    // alternate between P1 and Rout so that the stage's last block writes Rout.
+    for (size_t j = 0; melgan && j < sg.blocks.size(); ++j) {
+      const BlockRef& blk = sg.blocks[j];
+      const float* cur = j == 0 ? U : ((sg.blocks.size() - j) % 2 == 0 ? Rout : P[1]);
+      float* dst = (sg.blocks.size() - 1 - j) % 2 == 0 ? Rout : P[1];
+      auto run = [&](const ConvRef& c, const float* x, float* y, float slope, const float* acc_prev) -> int {
+        if (!on_tc(c)) return conv(c, x, sb, sc, 1, y, Tn, slope, nullptr, acc_prev, 1.0f, 0);
+        const double el = (double)B * Tn;
+        return tc_conv(c, nullptr, x, sb, sc, 1, nullptr, y, nullptr, Tn, slope, nullptr, acc_prev, 1.0f, 0,
+                       4.0 * el * c.cout * (1 + (acc_prev != nullptr)) + 4.0 * el * c.cin + 2.0 * c.cin * c.cout * c.k);
+      };
+      rc = run(blk.c1[0], cur, TMP, 0.2f, nullptr);
+      if (rc == AB_OK) rc = run(blk.c2[0], TMP, P[0], 0.2f, nullptr);
+      if (rc == AB_OK) rc = run(blk.sc, cur, dst, 1.0f, P[0]);   // shortcut(x) + block(x)
+      if (rc != AB_OK) return rc;
+    }
+    for (int j = 0; !melgan && j < nk; ++j) {
       const BlockRef& blk = sg.blocks[j];
       const float* cur = U;
       const uint16_t* cur_img = u_img;
@@ -855,7 +952,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   const int nchunk = g->tail_events.empty() ? 1 : (int)std::min<int64_t>((int64_t)g->tail_events.size(), B);
   const int64_t Bfull = B;
   const ConvRef& cpost = g->conv_post;
-  const float post_slope = big ? 1.0f : 0.01f;
+  const float post_slope = big ? 1.0f : melgan ? 0.2f : 0.01f;
   const int post_tanh = g->cfg.kind == AB_GEN_TRUNK ? 0 : 1;
   for (int ci = 0; ci < nchunk; ++ci) {
     const int64_t b0 = Bfull * ci / nchunk, b1 = Bfull * (ci + 1) / nchunk;
@@ -956,6 +1053,8 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
   if (!dev_x || !dev_w || !dev_y || !ws) return fail(AB_ERR_ARG, "conv_transpose1d: null argument");
   if (ws_bytes < ab_conv_transpose1d_workspace_bytes(cin, cout, k, u, precision)) return fail(AB_ERR_WORKSPACE, "conv_transpose1d: workspace too small");
   if (Tin * u > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: sequence too long");
+  if (k < u || ((k - u) & 1))   // padding (k - u) / 2, hifigan.py:176-186
+    return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: kernel %d / stride %d: need k >= stride and (k - stride) even", k, u);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* w_t = static_cast<float*>(ws);
   int rc = launch_repack_weight(dev_w, nullptr, w_t, (int)cin, (int)cout, k, 1, st);
@@ -975,6 +1074,7 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
   ConvTParams p;
   p.x = dev_x; p.w_t = w_t; p.bias = dev_bias; p.y = dev_y;
   p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.Tin = (int)Tin; p.k = k; p.u = u; p.pre_slope = pre_slope;
+  p.pad = (k - u) / 2;
   return launch_conv_transpose1d_fp32(p, st);
 }
 

@@ -58,6 +58,7 @@ struct ConvParams {
   float pre_slope;      // 1.0f = no activation
   float out_div;        // 1.0f = none (IEEE division, as the reference's xs / num_kernels)
   int post_tanh;
+  int reflect = 0;      // 1: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN, melgan.py:39-40,59-66,90-95)
 };
 
 struct ConvTParams {
@@ -67,10 +68,15 @@ struct ConvTParams {
   float* y;             // contiguous [B, Cout, Tin*u]
   int B, Cin, Cout, Tin;
   int k, u;
+  int pad;              // ConvTranspose1d padding: (k-u)/2 for HiFi-GAN, r//2 + r%2 for MelGAN (melgan.py:73-80)
   float pre_slope;
 };
 
 #ifdef __CUDACC__
+// ReflectionPad1d: the row of a length-T sequence that time t of the padded sequence reads (t in (-T, 2T - 1)); callers
+// zero-fill when the result lies outside [0, T), which only happens for rows no valid output reads.
+__device__ __forceinline__ int reflect_time(int t, int T) { return t < 0 ? -t : (t >= T ? 2 * (T - 1) - t : t); }
+
 // fp32 pairs in an aligned 64-bit register, so that 8- and 16-byte shared-memory loads deliver pairs without any
 // move.  Hopper has no packed fp32 arithmetic: each op is two scalar IEEE round-to-nearest ops (the explicit
 // intrinsics keep the compiler from contracting a mul and an add into one FMA).

@@ -23,6 +23,8 @@ constexpr int TT = 128;
 constexpr int CI_T = 8;
 constexpr int NT = 256;
 
+// REFLECT: ReflectionPad1d(halo / 2) in place of the zero padding (MelGAN's ResnetBlock conv, melgan.py:39-40)
+template <int REFLECT>
 __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
   extern __shared__ float smem[];
   const int halo = (p.k - 1) * p.d;
@@ -44,7 +46,7 @@ __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
   for (int ci0 = 0; ci0 < p.Cin; ci0 += CI_T) {
     for (int idx = threadIdx.x; idx < CI_T * XW; idx += NT) {
       const int ci = idx / XW, n = idx - ci * XW;
-      const int t = t0 - pad + n, c = ci0 + ci;
+      const int t = REFLECT ? reflect_time(t0 - pad + n, p.T) : t0 - pad + n, c = ci0 + ci;
       float v = 0.f;
       if (c < p.Cin && t >= 0 && t < p.T) {
         v = __ldg(xb + (int64_t)c * p.xsc + (int64_t)t * p.xst);
@@ -107,6 +109,7 @@ __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
 // (batch, 1024-sample tile), all Cout (<= 4) per thread; HBM-bound.
 constexpr int PT = 1024;
 constexpr int PCI = 8;
+template <int REFLECT>
 __global__ void __launch_bounds__(NT) conv1d_fewout_fp32_kernel(ConvParams p) {
   extern __shared__ float smem[];
   const int halo = (p.k - 1) * p.d;
@@ -129,7 +132,7 @@ __global__ void __launch_bounds__(NT) conv1d_fewout_fp32_kernel(ConvParams p) {
     __syncthreads();
     for (int idx = threadIdx.x; idx < PCI * XW; idx += NT) {
       const int ci = idx / XW, n = idx - ci * XW;
-      const int t = t0 - pad + n, c = ci0 + ci;
+      const int t = REFLECT ? reflect_time(t0 - pad + n, p.T) : t0 - pad + n, c = ci0 + ci;
       float v = 0.f;
       if (c < p.Cin && t >= 0 && t < p.T) {
         v = __ldg(xb + (int64_t)c * p.xsc + (int64_t)t * p.xst);
@@ -174,7 +177,7 @@ __global__ void __launch_bounds__(NT) conv1d_fewout_fp32_kernel(ConvParams p) {
 // conv_post specialisation: one output channel, k = K taps, dilation 1 (hifigan.py:199,215-217).  Four
 // consecutive outputs per thread from a (4 + K - 1)-sample register window (3 x LDS.128 per input channel),
 // weights of the current 8-channel chunk in registers.  HBM-bound: reads C x T fp32 once.
-template <int K>
+template <int K, int REFLECT = 0>
 __global__ void __launch_bounds__(NT) conv_post_fp32_kernel(ConvParams p) {
   constexpr int XWP = PT + 8;                   // padded row: 1024 outputs + K - 1 (<= 8) halo, 16-byte rows
   __shared__ __align__(16) float xs[PCI][XWP];
@@ -189,7 +192,7 @@ __global__ void __launch_bounds__(NT) conv_post_fp32_kernel(ConvParams p) {
     __syncthreads();
     for (int idx = threadIdx.x; idx < PCI * XWP; idx += NT) {
       const int ci = idx / XWP, n = idx - ci * XWP;
-      const int t = t0 - pad + n, c = ci0 + ci;
+      const int t = REFLECT ? reflect_time(t0 - pad + n, p.T) : t0 - pad + n, c = ci0 + ci;
       float v = 0.f;
       if (c < p.Cin && t >= 0 && t < p.T && n < PT + K - 1) {
         v = __ldg(xb + (int64_t)c * p.xsc + (int64_t)t * p.xst);
@@ -240,7 +243,9 @@ __global__ void __launch_bounds__(NT) conv_post_fp32_kernel(ConvParams p) {
 // superset [t0 - 4, t0 + PT + 4) consists of float4 groups that lie entirely inside or outside the row), the weights
 // are read as two broadcast LDS.128 per channel.  The generic kernel above spent ~25 instructions per staged
 // element (index division, 64-bit address math, scalar LDG/STS): 1575 instructions per output against ~370 here.
-template <int K>
+// REFLECT (MelGAN's ReflectionPad1d(3) before conv_post, melgan.py:90-95): the staged tile is completed at the
+// sequence ends from its own rows, which lie inside it (T % 4 == 0, T >= 4).
+template <int K, int REFLECT = 0>
 __global__ void __launch_bounds__(NT) conv_post_vec_kernel(ConvParams p) {
   static_assert(K <= 8, "weights are padded to 8 per channel");
   constexpr int XG = PT / 4 + 2;                // float4 groups per staged row
@@ -282,6 +287,15 @@ __global__ void __launch_bounds__(NT) conv_post_vec_kernel(ConvParams p) {
       w.z = w.z >= 0.f ? w.z : w.z * slope;
       w.w = w.w >= 0.f ? w.w : w.w * slope;
       if (idx < PCI * XG) *reinterpret_cast<float4*>(&xs[ci][4 * q]) = w;
+    }
+    if (REFLECT) {   // staged index n holds time t0 - 4 + n: x[-r] = x[r], x[T - 1 + r] = x[T - 1 - r], r = 1..pad
+      __syncthreads();
+      if (threadIdx.x < PCI * pad) {
+        const int ci = threadIdx.x / pad, r = threadIdx.x - ci * pad + 1;
+        if (t0 == 0) xs[ci][4 - r] = xs[ci][4 + r];
+        const int n = p.T - 1 + r - t0 + 4;
+        if (n >= 0 && n < XG * 4) xs[ci][n] = xs[ci][n - 2 * r];
+      }
     }
     if (ci0 + PCI < p.Cin) request(ci0 + PCI);
     if (threadIdx.x < PCI * 8) {
@@ -333,45 +347,52 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
                 p.k, p.d);
   if (p.B > 65535) return fail(AB_ERR_UNSUPPORTED, "conv1d: batch %d > 65535", p.B);
   const int halo = (p.k - 1) * p.d;
+  if (p.reflect && halo / 2 >= p.T)
+    return fail(AB_ERR_ARG, "conv1d: reflection padding %d needs more than %d samples", halo / 2, p.T);
   if (p.Cout == 1 && p.k == 7 && p.d == 1 && !p.residual && !p.acc_prev && p.out_div == 1.0f) {
     dim3 grid((unsigned)ceil_div(p.T, PT), 1, (unsigned)p.B);
     const bool vec = p.xst == 1 && (p.T & 3) == 0 && (p.xsc & 3) == 0 && (p.xsb & 3) == 0 &&
                      (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0;
-    if (vec) conv_post_vec_kernel<7><<<grid, NT, 0, s>>>(p);
-    else conv_post_fp32_kernel<7><<<grid, NT, 0, s>>>(p);
+    if (p.reflect) {
+      if (vec) conv_post_vec_kernel<7, 1><<<grid, NT, 0, s>>>(p);
+      else conv_post_fp32_kernel<7, 1><<<grid, NT, 0, s>>>(p);
+    } else {
+      if (vec) conv_post_vec_kernel<7><<<grid, NT, 0, s>>>(p);
+      else conv_post_fp32_kernel<7><<<grid, NT, 0, s>>>(p);
+    }
     AB_LAUNCH_CHECK("conv_post_fp32_kernel");
     return AB_OK;
   }
   if (p.Cout <= 4) {
     const size_t smem = sizeof(float) * ((size_t)PCI * (PT + halo) + (size_t)p.Cin * p.k * p.Cout);
     if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "conv1d(few-out): filter too large for smem");
-    static DeviceOnce configured;
-    if (smem > 48 * 1024 && configured.need())
-      AB_CUDA_TRY(cudaFuncSetAttribute(conv1d_fewout_fp32_kernel,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    static DeviceOnce configured[2];
+    auto kern = p.reflect ? conv1d_fewout_fp32_kernel<1> : conv1d_fewout_fp32_kernel<0>;
+    if (smem > 48 * 1024 && configured[p.reflect ? 1 : 0].need())
+      AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     dim3 grid((unsigned)ceil_div(p.T, PT), 1, (unsigned)p.B);
-    conv1d_fewout_fp32_kernel<<<grid, NT, smem, s>>>(p);
+    kern<<<grid, NT, smem, s>>>(p);
     AB_LAUNCH_CHECK("conv1d_fewout_fp32_kernel");
     return AB_OK;
   }
   const size_t smem = sizeof(float) * ((size_t)CI_T * (TT + halo) + (size_t)CI_T * p.k * CO_T);
   if (smem > 200 * 1024)
     return fail(AB_ERR_UNSUPPORTED, "conv1d: k=%d dilation=%d needs %zu B of shared memory", p.k, p.d, smem);
-  static DeviceOnce configured;
-  if (smem > 48 * 1024 && configured.need()) {
-    AB_CUDA_TRY(cudaFuncSetAttribute(conv1d_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     200 * 1024));
+  static DeviceOnce configured[2];
+  auto kern = p.reflect ? conv1d_fp32_kernel<1> : conv1d_fp32_kernel<0>;
+  if (smem > 48 * 1024 && configured[p.reflect ? 1 : 0].need()) {
+    AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   if (ceil_div(p.Cout, CO_T) > 65535) return fail(AB_ERR_UNSUPPORTED, "conv1d: too many channels");
   dim3 grid((unsigned)ceil_div(p.T, TT), (unsigned)ceil_div(p.Cout, CO_T), (unsigned)p.B);
-  conv1d_fp32_kernel<<<grid, NT, smem, s>>>(p);
+  kern<<<grid, NT, smem, s>>>(p);
   AB_LAUNCH_CHECK("conv1d_fp32_kernel");
   return AB_OK;
 }
 
 // ===========================================================================
-// ConvTranspose1d(stride=u, padding=(k-u)/2) fused with the leaky_relu in
-// front of it (hifigan.py:206-207; bigvgan.py:316-318 has no activation):
+// ConvTranspose1d(stride=u, padding=p) fused with the leaky_relu in front of it (hifigan.py:206-207, p = (k-u)/2;
+// bigvgan.py:316-318 has no activation; melgan.py:73-80, p = u//2 + u%2 with output_padding u%2), Tin*u outputs:
 //   y[co,t] = b[co] + sum_ci sum_{j = (t+p) mod u, +u, ... < k} x[ci,(t+p-j)/u] * W[ci,co,j]
 // ===========================================================================
 namespace {
@@ -382,7 +403,7 @@ __global__ void __launch_bounds__(NT) convT_fp32_kernel(ConvTParams p, int XW, i
   const int Tout = p.Tin * p.u;
   const int t0 = blockIdx.x * TT, co0 = blockIdx.y * CO_T, b = blockIdx.z;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int pd = (p.k - p.u) >> 1;
+  const int pd = p.pad;
   const int s_min = (t0 + pd) / p.u - (M - 1);
   const float slope = p.pre_slope;
   const float* xb = p.x + (int64_t)b * p.Cin * p.Tin;
@@ -461,9 +482,9 @@ __global__ void __launch_bounds__(NT) convT_fp32_kernel(ConvTParams p, int XW, i
 int launch_conv_transpose1d_fp32(const ConvTParams& p, cudaStream_t s) {
   if (p.B <= 0 || p.Cin <= 0 || p.Cout <= 0 || p.Tin <= 0 || p.k <= 0 || p.u <= 0)
     return fail(AB_ERR_ARG, "conv_transpose1d: bad shape");
-  if (p.k < p.u || ((p.k - p.u) & 1))
-    return fail(AB_ERR_UNSUPPORTED,
-                "conv_transpose1d: kernel %d / stride %d: need k >= stride and (k - stride) even", p.k, p.u);
+  if (p.k < p.u || p.pad < 0 || p.pad > p.k)
+    return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: kernel %d / stride %d / padding %d: need k >= stride, 0 <= padding <= k",
+                p.k, p.u, p.pad);
   if (p.B > 65535) return fail(AB_ERR_UNSUPPORTED, "conv_transpose1d: batch %d > 65535", p.B);
   const int M = (p.k + p.u - 1) / p.u;
   const int XW = TT / p.u + 2 + M;

@@ -113,7 +113,9 @@ __device__ __forceinline__ void stage_biases(float* bias_s, const HcArgs& p, int
 
 // Operand tile at `tile`: c8 planes [c8_0, c8_0 + nplanes) x rows [0, rows), row at time t0 + row, from the operand
 // image or from lrelu(x, pre_slope); zero outside [0, Tin) and C_in.  Thread lt of nthreads cooperating threads.
-template <int BF16>
+// REFLECT: time t outside [0, Tin) reads row -t or 2 (Tin - 1) - t instead (ReflectionPad1d, MelGAN), zero where that
+// row does not exist either (rows no valid output reads).
+template <int BF16, int REFLECT = 0>
 __device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int b, uint8_t* tile, int c8_0, int nplanes,
                                           int rows, int t0, int lt, int nthreads) {
   const int items = nplanes * rows;
@@ -121,7 +123,7 @@ __device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int 
     const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
     for (int idx = lt; idx < items; idx += nthreads) {
       const int c = idx / rows, row = idx - c * rows;
-      const int c8 = c8_0 + c, t = t0 + row;
+      const int c8 = c8_0 + c, t = REFLECT ? reflect_time(t0 + row, g.Tin) : t0 + row;
       const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
       cp_async16(smem_u32(tile) + unit_offset(rows, c, row),
                  ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb, ok ? 16u : 0u);
@@ -131,7 +133,7 @@ __device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int 
     const float* xb = p.x + (int64_t)b * p.xsb;
     for (int idx = lt; idx < items; idx += nthreads) {
       const int c = idx / rows, row = idx - c * rows;
-      const int t = t0 + row;
+      const int t = REFLECT ? reflect_time(t0 + row, g.Tin) : t0 + row;
       const bool ok = t >= 0 && t < g.Tin;
       float v[8];
 #pragma unroll
@@ -243,7 +245,8 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
 // flags) reports spill stores / loads of 956 / 1220 bytes at N = 256 and 784 / 1020 at N = 128, against 4 / 4 and
 // 16 / 20 with it, which made HiFi-GAN V1's ConvTranspose layers about 5 ms per step slower (H100 80GB HBM3, 400 W
 // power limit).  Re-check those numbers before deleting it.
-template <int NW, int BF16>
+// REFLECT (mode 0 only): ReflectionPad1d in place of the zero "same" padding (MelGAN's conv_pre and ResnetBlock conv).
+template <int NW, int BF16, int REFLECT = 0>
 __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
@@ -314,7 +317,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   // A chunk kc: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
   auto load_chunk = [&](int kc) {
     __syncthreads();   // every warp has finished the MMAs that read the previous chunk
-    load_tile<BF16>(p, g, b, smem, 4 * kc, 4, g.rowsA, O - g.a0, tid, HC_THREADS);
+    load_tile<BF16, REFLECT>(p, g, b, smem, 4 * kc, 4, g.rowsA, O - g.a0, tid, HC_THREADS);
     fence_proxy_async();
     __syncthreads();
   };
@@ -1152,7 +1155,7 @@ int layer_geom(int mode, int cin, int cout, int k, int d_or_u, HcLayer& L) {
     L.u = 1;
   } else {
     const int u = d_or_u;
-    if (k < u || ((k - u) & 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv: conv-transpose needs k >= stride, k-stride even");
+    if (k < u) return fail(AB_ERR_UNSUPPORTED, "tc conv: conv-transpose needs k >= stride");
     if (u > 64) return fail(AB_ERR_UNSUPPORTED, "tc conv: stride %d too large", u);
     L.cc = std::min(256 / u, cout);
     L.NW = pow2_at_least(L.cc * u);
@@ -1208,8 +1211,9 @@ bool layout_smem(HcGeom& g, uint32_t abytes, uint32_t ibytes, uint32_t nbias, ui
   return true;
 }
 
-// Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.
-int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg, HcGeom& g) {
+// Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.  mode 1: padding
+// pad (-1: (k - u) / 2), Tin * u outputs.
+int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg, HcGeom& g, int pad = -1) {
   HcLayer L;
   int rc = layer_geom(mode == 2 ? 0 : mode, cin, cout, k, d_or_u, L);
   if (rc != AB_OK) return rc;
@@ -1230,7 +1234,7 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg
   int maxshift, rows_total;
   if (mode == 1) {
     g.d = 1;
-    g.pad = (k - L.u) / 2;
+    g.pad = pad < 0 ? (k - L.u) / 2 : pad;
     g.Tout = Tin * L.u;
     maxshift = g.ntaps - 1;
     g.a0 = maxshift;
@@ -1353,7 +1357,7 @@ int persistent_grid(int64_t work, const char* what, unsigned& grid) {
 // on the persistent hconvt_kernel, pair mode on the persistent hpair_kernel.  From fp32 input, hconvt_kernel's 96 loader
 // threads (8 scattered loads in flight each) cannot keep up with the MMAs and it is slower than hconv_kernel, whose
 // 256 threads all load.
-int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s) {
+int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s, bool reflect = false) {
   if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
   const int64_t work = (int64_t)a.B * g.tiles;
   if (g.mode == 1 && a.ximg) {
@@ -1377,6 +1381,9 @@ int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s
   if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
   return with_nw(g, precision, [&](auto nw, auto bf16) {
     constexpr int NW = decltype(nw)::value;
+    if (reflect)
+      return launch_kernel<hconv_kernel<NW, decltype(bf16)::value, 1>>("hconv_kernel", (unsigned)work, HC_THREADS,
+                                                                        NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
     return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)work, HC_THREADS,
                                                                    NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
   });
@@ -1471,9 +1478,15 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
     return fail(AB_ERR_UNSUPPORTED, "tc conv-transpose: operand-image input needs C_in %% 16 == 0");
   if (p.yimg && !tc_can_emit_image(p.mode, p.Cin, p.Cout, p.k, p.d_or_u))
     return fail(AB_ERR_UNSUPPORTED, "tc conv: cannot emit an operand image for this layer");
+  if (p.mode == 1 && (p.pad < -1 || p.pad >= p.k))
+    return fail(AB_ERR_ARG, "tc conv-transpose: padding %d outside [0, k = %d)", p.pad, p.k);
+  if (p.reflect && (p.mode != 0 || pair))
+    return fail(AB_ERR_UNSUPPORTED, "tc conv: reflection padding belongs to a single conv (mode 0)");
   HcGeom g;
-  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, p.ximg != nullptr, g);
+  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, p.ximg != nullptr, g, p.pad);
   if (rc != AB_OK) return rc;
+  if (p.reflect && g.a0 >= p.T)
+    return fail(AB_ERR_ARG, "tc conv: reflection padding %d needs more than %d samples", g.a0, p.T);
   g.out_scale = 1.0f / p.out_div;
   g.mid_slope = p.mid_slope;
   HcArgs a = base_args(p.x, p.xsb, p.xsc, p.xst, p.ximg, p.pre_slope, p.B, p.Cin, p.Cout);
@@ -1481,7 +1494,7 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   a.ws[1] = p.w2; a.bs[1] = p.b2;
   a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev; a.post_tanh = p.post_tanh;
   a.yimg = p.yimg; a.img_slope = p.img_slope;
-  return launch_hconv(a, g, p.precision, s);
+  return launch_hconv(a, g, p.precision, s, p.reflect != 0);
 }
 
 }  // namespace ab

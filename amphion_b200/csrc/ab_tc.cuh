@@ -11,7 +11,7 @@ namespace ab {
 //   pair (mode 0 with w2):  y = ((conv2(lrelu(conv(act(x), d) + bias, mid_slope), 1) + b2) + residual + acc_prev) / out_div
 //     i.e. one (c1, c2) step of ResBlock1.forward (hifigan.py:93-100); a single conv is one step of ResBlock2
 //     (:139-144); residual, acc_prev and out_div are the branch mix of hifigan.py:208-214
-//   conv-transpose (mode 1, stride u = d_or_u, padding (k-u)/2):  y = conv_transpose(act(x), u) + bias
+//   conv-transpose (mode 1, stride u = d_or_u, padding `pad`, T*u outputs):  y = conv_transpose(act(x), u) + bias
 struct TcConvParams {
   int mode = 0;                      // 0 conv, 1 conv-transpose
   const float* x = nullptr;          // fp32 [B, Cin, T] with element strides xsb / xsc / xst (unused when ximg is given)
@@ -32,6 +32,8 @@ struct TcConvParams {
   float img_slope = 1.0f;
   int B = 0, Cin = 0, Cout = 0, T = 0, k = 0, d_or_u = 1;
   int precision = AB_PREC_FP32;      // set to AB_PREC_TC_F16 | AB_PREC_TC_BF16 (fp32 is rejected)
+  int reflect = 0;                   // conv only, no w2: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN)
+  int pad = -1;                      // conv-transpose padding, 0 <= pad < k; -1 = (k-u)/2 (HiFi-GAN; MelGAN: u//2 + u%2)
 };
 // 16-bit weight image of a layer, 0 when hconv_kernel cannot run it
 size_t tc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u);

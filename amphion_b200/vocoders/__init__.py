@@ -3,16 +3,17 @@
 from .apnet import APNet, ISTFT, ISTFTHead
 from .bigvgan import BigVGAN
 from .hifigan import HiFiGAN, HiFiGAN_vits
+from .melgan import MelGAN
 from .nsfhifigan import NSFHiFiGAN
 from .gan_vocoder_inference import synthesis_audios, synthesize_to_files
 from .gan_vocoder_inference import vocoder_inference as _gan_vocoder_inference
 
 # same shape as the reference's registries: generator name -> class / functions
-_vocoders = {"hifigan": HiFiGAN, "bigvgan": BigVGAN, "nsfhifigan": NSFHiFiGAN, "apnet": APNet}
+_vocoders = {"hifigan": HiFiGAN, "bigvgan": BigVGAN, "nsfhifigan": NSFHiFiGAN, "melgan": MelGAN, "apnet": APNet}
 _vocoder_forward_funcs = {k: _gan_vocoder_inference for k in _vocoders}
 _vocoder_infer_funcs = {k: synthesis_audios for k in _vocoders}
 
-__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "NSFHiFiGAN", "APNet", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
+__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "NSFHiFiGAN", "MelGAN", "APNet", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
            "_vocoder_forward_funcs", "_vocoder_infer_funcs"]
 
 # `amphion_b200.vocoders.vocoder_inference` is the MODULE (synthesis, load_nnvocoder), as

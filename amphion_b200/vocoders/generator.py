@@ -87,6 +87,10 @@ class NativeGenerator(nn.Module):
     def _hp(self):
         return getattr(self.cfg.model, self.hp_key)
 
+    def _upsample_rates(self):
+        """Upsampling factor of each stage; their product is the hop."""
+        return [int(u) for u in self._hp().upsample_rates]
+
     def _c_config(self):
         hp = self._hp()
         c = _capi.GeneratorConfig()
@@ -188,8 +192,8 @@ class NativeGenerator(nn.Module):
             self._sync_params(x.device)
             lib, h = _capi.lib, self._handle
             hop = 1
-            for u in self._hp().upsample_rates:
-                hop *= int(u)
+            for u in self._upsample_rates():
+                hop *= u
             need = lib.ab_generator_workspace_bytes(h, B, T)
             if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != x.device:
                 self._workspace = None

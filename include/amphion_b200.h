@@ -49,8 +49,18 @@ extern "C" {
  * (models/vocoders/gan/generator/apnet.py:283-375): x = conv_pre(mel) [k = trunk_in_kernel]; xs = sum_j ResBlock1_j(x)
  * / num_kernels; y = conv_post(leaky_relu(xs, 0.01)) [C -> trunk_out_channels, k = trunk_out_kernel], no tanh.
  * num_upsamples = 0, upsample_initial_channel = the trunk width; tensors "conv_pre", "resblocks.j.convs{1,2}.p",
- * "conv_post" (the caller maps ASP_input_conv / ASP_ResNet.j / ASP_output_conv ... onto them). */
-enum ab_generator_kind { AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3 };
+ * "conv_post" (the caller maps ASP_input_conv / ASP_ResNet.j / ASP_output_conv ... onto them).
+ * AB_GEN_MELGAN: MelGAN.forward (models/vocoders/gan/generator/melgan.py:50-101): reflection-padded conv_pre (k = 7),
+ * then per ratio r: leaky_relu(0.2), ConvTranspose1d(k = 2r, stride r, padding r//2 + r%2, output_padding r%2) and
+ * n_residual_layers ResnetBlocks x = shortcut(x) + conv1x1(lrelu(conv3(lrelu(x, 0.2), reflect-padded, dilation 3^j), 0.2));
+ * then leaky_relu(0.2), reflection-padded conv_post (k = 7), tanh.  Config fields: upsample_rates = ratios,
+ * upsample_kernel_sizes = 2 * ratios, upsample_initial_channel = ngf * 2^len(ratios), num_kernels = 1,
+ * resblock_kernel_sizes[0] = 3, num_dilations[0] = n_residual_layers, resblock_dilation_sizes[0][j] = 3^j; anything else
+ * is refused.  Tensors keep the reference's nn.Sequential names: "model.1" (conv_pre), "model.{2+i(2+R)+1}" (ConvTranspose
+ * of stage i), "model.{2+i(2+R)+2+j}.block.2" / ".block.4" / ".shortcut" (block j), "model.{2+n(2+R)+2}" (conv_post),
+ * R = n_residual_layers, n = len(ratios).  A forward whose mel has fewer than 4 frames, or whose stage is not longer
+ * than one of its dilations, fails with AB_ERR_ARG before any launch (the reference's ReflectionPad1d raises). */
+enum ab_generator_kind { AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4 };
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
@@ -68,6 +78,7 @@ int ab_device_is_sm90(void);
  * Generator: HiFiGAN.forward     (models/vocoders/gan/generator/hifigan.py:203-219)
  *            BigVGAN.forward     (models/vocoders/gan/generator/bigvgan.py:313-331)
  *            NSFHiFiGAN.forward  (models/vocoders/gan/generator/nsfhifigan.py:262-283)
+ *            MelGAN.forward      (models/vocoders/gan/generator/melgan.py:100-101)
  * The config mirrors cfg.model.{hifigan,bigvgan}.* + cfg.preprocess.n_mel
  * (hifigan.py:151-201, bigvgan.py:232-311).
  * ---------------------------------------------------------------------- */
