@@ -10,7 +10,7 @@ AB_MAX_STAGES = 8
 AB_MAX_KERNELS = 8
 AB_MAX_DILATIONS = 8
 
-GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN = 0, 1, 2, 3, 4
+GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN, GEN_VOCOS = 0, 1, 2, 3, 4, 5
 ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA = 0, 1, 2
 PRECISIONS = {"fp32": 0, "tc_f16": 1, "tc_bf16": 2}
 
@@ -35,6 +35,10 @@ class GeneratorConfig(C.Structure):
         ("trunk_out_channels", C.c_int32),
         ("trunk_in_kernel", C.c_int32),
         ("trunk_out_kernel", C.c_int32),
+        ("ffn_channels", C.c_int32),
+        ("num_layers", C.c_int32),
+        ("istft_n_fft", C.c_int32),
+        ("istft_hop", C.c_int32),
     ]
 
 

@@ -57,6 +57,7 @@ struct Slot {
   int stride;         // ConvTranspose1d stride (SLOT_CONVT_W)
   int dilation;       // Conv1d dilation (SLOT_CONV_W)
   float gain = 1.0f;  // applied to the fp32 image at load time (NSF-HiFiGAN: 2 on every ups weight / bias)
+  bool head_cols = false;   // Vocos' head.out: the weight image pairs each bin's magnitude and phase rows
 };
 
 struct ConvRef {   // one weight-normed conv of the model
@@ -75,6 +76,18 @@ struct BlockRef {  // one ResBlock / AMPBlock
   std::vector<ConvRef> c1, c2;  // c2 empty for ResBlock2 / AMPBlock2
   std::vector<ActRef> acts;     // 2*nd (type 1) or nd (type 2); empty for HiFi-GAN
   ConvRef sc;                   // MelGAN ResnetBlock: the 1x1 shortcut (c1, c2 then hold one conv each)
+};
+
+// Vocos (AB_GEN_VOCOS): slot indices of the backbone and head; the Linear layers are k = 1 convs
+struct VocosBlockRef {   // one ConvNeXtBlock (vocos.py:469-527)
+  int dw_w = -1, dw_b = -1, ln_w = -1, ln_b = -1, gamma = -1;
+  ConvRef pw1, pw2;
+};
+
+struct VocosRef {
+  int norm_w = -1, norm_b = -1, final_w = -1, final_b = -1, window = -1;
+  std::vector<VocosBlockRef> blocks;
+  ConvRef head;   // head.out: [n_fft + 2, dim]
 };
 
 struct StageRef {
@@ -109,6 +122,8 @@ struct ab_generator {
   int cond_w = -1, cond_b = -1;   // HiFiGAN_vits global conditioning (hifigan.py:424-425)
   ActRef act_post;
   std::vector<StageRef> stages;
+  VocosRef vocos;
+  ab_mel* istft = nullptr;   // Vocos: the iSTFT plan (cuFFT C2R + overlap-add of ab_istft_forward)
 
   // profiling (ab_generator_set_profiling)
   bool profiling = false;
@@ -124,6 +139,7 @@ struct ab_generator {
   ~ab_generator() {
     for (auto& r : prof_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
     for (auto e : event_pool) cudaEventDestroy(e);
+    ab_mel_destroy(istft);
   }
 
   int add_slot(const std::string& name, SlotKind kind, std::initializer_list<int64_t> shape) {
@@ -180,10 +196,32 @@ ActRef make_act(ab_generator* g, const std::string& prefix, int ch, bool has_bet
   return a;
 }
 
+// AB_GEN_VOCOS: only its own fields; the ISTFT needs what ab_istft_forward serves
+int validate_vocos_config(const ab_generator_config& c) {
+  if (c.num_upsamples || c.resblock || c.num_kernels || c.activation || c.snake_logscale || c.gin_channels ||
+      c.conv_post_no_bias || c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel)
+    return fail(AB_ERR_ARG, "config: Vocos uses only n_mel, upsample_initial_channel, ffn_channels, num_layers, istft_n_fft "
+                            "and istft_hop (every other field must be 0)");
+  const int lim = 1 << 16;
+  if (c.n_mel <= 0 || c.n_mel > lim || c.upsample_initial_channel <= 0 || c.upsample_initial_channel > lim ||
+      c.ffn_channels <= 0 || c.ffn_channels > lim || c.num_layers <= 0 || c.num_layers > 4096)
+    return fail(AB_ERR_ARG, "config: Vocos input_channels %d, dim %d, intermediate_dim %d, num_layers %d out of range", c.n_mel,
+                c.upsample_initial_channel, c.ffn_channels, c.num_layers);
+  if (c.istft_n_fft <= 0 || c.istft_hop <= 0 || c.istft_n_fft > lim)
+    return fail(AB_ERR_ARG, "config: Vocos n_fft %d / hop %d out of range", c.istft_n_fft, c.istft_hop);
+  if ((c.istft_n_fft & 1) || c.istft_hop > c.istft_n_fft || ((c.istft_n_fft - c.istft_hop) & 1))
+    return fail(AB_ERR_UNSUPPORTED, "config: Vocos iSTFT needs an even n_fft, hop <= n_fft and n_fft - hop even (n_fft %d, hop %d)",
+                c.istft_n_fft, c.istft_hop);
+  return AB_OK;
+}
+
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
-      c.kind != AB_GEN_MELGAN)
+      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
+  if (c.kind == AB_GEN_VOCOS) return validate_vocos_config(c);
+  if (c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop)
+    return fail(AB_ERR_ARG, "config: ffn_channels / num_layers / istft_* belong to AB_GEN_VOCOS");
   const bool trunk = c.kind == AB_GEN_TRUNK;
   const bool melgan = c.kind == AB_GEN_MELGAN;
   if (trunk) {
@@ -356,6 +394,46 @@ void add_melgan_tensors(ab_generator* g) {
   g->conv_post.reflect = true;
 }
 
+// nn.Linear(cin, cout) as a k = 1 conv: weight [out, in] (state-dict shape), repacked as [in][1][out]
+ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout) {
+  ConvRef c;
+  c.cin = cin;
+  c.cout = cout;
+  c.k = 1;
+  c.w = g->add_slot(name + ".weight", SLOT_CONV_W, {cout, cin});
+  g->slots[c.w].shape[2] = 1;
+  c.b = g->add_slot(name + ".bias", SLOT_VEC, {cout});
+  return c;
+}
+
+// Vocos tensors (AB_GEN_VOCOS), the reference's state-dict names (vocos.py:469-527, :720-783, :314-361, :824-881)
+void add_vocos_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int D = cfg->upsample_initial_channel, F = cfg->ffn_channels;
+  VocosRef& v = g->vocos;
+  g->conv_pre = make_conv(g, "backbone.embed", cfg->n_mel, D, 7, 1, false);
+  v.norm_w = g->add_slot("backbone.norm.weight", SLOT_VEC, {D});
+  v.norm_b = g->add_slot("backbone.norm.bias", SLOT_VEC, {D});
+  for (int i = 0; i < cfg->num_layers; ++i) {
+    const std::string pre = "backbone.convnext." + std::to_string(i);
+    VocosBlockRef b;
+    b.dw_w = g->add_slot(pre + ".dwconv.weight", SLOT_VEC, {D, 1, 7});
+    b.dw_b = g->add_slot(pre + ".dwconv.bias", SLOT_VEC, {D});
+    b.ln_w = g->add_slot(pre + ".norm.weight", SLOT_VEC, {D});
+    b.ln_b = g->add_slot(pre + ".norm.bias", SLOT_VEC, {D});
+    b.pw1 = make_linear(g, pre + ".pwconv1", D, F);
+    b.pw2 = make_linear(g, pre + ".pwconv2", F, D);
+    b.gamma = g->add_slot(pre + ".gamma", SLOT_VEC, {D});
+    v.blocks.push_back(b);
+  }
+  v.final_w = g->add_slot("backbone.final_layer_norm.weight", SLOT_VEC, {D});
+  v.final_b = g->add_slot("backbone.final_layer_norm.bias", SLOT_VEC, {D});
+  v.head = make_linear(g, "head.out", D, cfg->istft_n_fft + 2);
+  g->slots[v.head.w].head_cols = true;
+  v.window = g->add_slot("head.istft.window", SLOT_VEC, {cfg->istft_n_fft});
+  g->hop = cfg->istft_hop;
+}
+
 }  // namespace
 
 extern "C" {
@@ -377,10 +455,19 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
   ab_generator* g = new ab_generator();
   g->cfg = *cfg;
   g->hop = 1;
-  if (cfg->kind == AB_GEN_MELGAN)
+  if (cfg->kind == AB_GEN_MELGAN) {
     add_melgan_tensors(g);
-  else
+  } else if (cfg->kind == AB_GEN_VOCOS) {
+    add_vocos_tensors(g);
+    const ab_mel_config mc = {cfg->istft_n_fft, cfg->istft_hop, cfg->istft_n_fft, 0, 0, 0.0f, 0.0f};
+    rc = ab_mel_create(&mc, &g->istft);
+    if (rc != AB_OK) {
+      delete g;
+      return rc;
+    }
+  } else {
     add_gan_tensors(g);
+  }
 
   // tensor-core weight images live behind the fp32 images
   size_t tc = 0;
@@ -476,6 +563,11 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
       const Slot& s = g->slots[i];
       if (!s.tc_bytes) continue;
       const bool t = s.kind == SLOT_CONVT_W;   // state-dict shape: ConvTranspose1d [C_in, C_out, k], Conv1d [C_out, C_in, k]
+      if (s.head_cols) {
+        int rc = launch_tc_pack_head_weight(g->fptr((int)i), g->tcptr((int)i), (int)s.shape[1], (int)s.shape[0], precision, st);
+        if (rc != AB_OK) return rc;
+        continue;
+      }
       int rc = launch_tc_pack_weight(g->fptr((int)i), g->tcptr((int)i), t ? 1 : 0, (int)s.shape[t ? 0 : 1],
                                      (int)s.shape[t ? 1 : 0], (int)s.shape[2], t ? s.stride : s.dilation, precision, st);
       if (rc != AB_OK) return rc;
@@ -534,6 +626,35 @@ size_t stage_max_elems(const ab_generator* g, int64_t B, int64_t T) {
   }
   return mx;
 }
+// Vocos workspace: the fp32 residual stream X, the embed / final-norm output Y (fp32), the block input H and the
+// intermediate I (fp32 at AB_PREC_FP32, else 16-bit operand images; I also holds the fp32 head output), the spectrum S
+// [B*T][bins] complex and the iSTFT's workspace.  base == nullptr: sizes only.  0 when the iSTFT plan fails.
+struct VocosWs {
+  float *X, *Y, *H, *I, *S;
+  void* ist;
+  size_t ist_bytes;
+};
+
+size_t vocos_layout(const ab_generator* g, int64_t B, int64_t T, char* base, VocosWs* w) {
+  const int D = g->cfg.upsample_initial_channel, F = g->cfg.ffn_channels, bins = g->cfg.istft_n_fft / 2 + 1;
+  const bool fp32 = g->precision == AB_PREC_FP32;
+  const size_t el = (size_t)B * T;
+  const size_t ist = ab_istft_workspace_bytes(g->istft, B, T);
+  if (ist == 0) return 0;
+  const size_t sz[6] = {el * D * 4, el * D * 4, fp32 ? el * D * 4 : tc_act_image_bytes(B, D, T),
+                        fp32 ? el * std::max(F, 2 * bins) * 4 : tc_act_image_bytes(B, F, T), el * bins * 8, ist};
+  char* p[6];
+  size_t off = 0;
+  for (int i = 0; i < 6; ++i) {
+    p[i] = base ? base + off : nullptr;
+    off += align_up(sz[i], 256);
+  }
+  if (w) {
+    w->X = reinterpret_cast<float*>(p[0]); w->Y = reinterpret_cast<float*>(p[1]); w->H = reinterpret_cast<float*>(p[2]);
+    w->I = reinterpret_cast<float*>(p[3]); w->S = reinterpret_cast<float*>(p[4]); w->ist = p[5]; w->ist_bytes = align_up(ist, 256);
+  }
+  return off;
+}
 }  // namespace
 
 // NSF-HiFiGAN: length of stage i's output after `length = min(x.shape[-1], x_source.shape[-1])` (nsfhifigan.py:264-268).
@@ -551,6 +672,7 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
 
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
+  if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
   return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
          NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
 }
@@ -575,6 +697,7 @@ int ab_generator_set_tail_events(ab_generator* g, void* const* events, int32_t n
 
 int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64_t source_frames) {
   if (!g || frames <= 0) return 0;
+  if (g->cfg.kind == AB_GEN_VOCOS) return frames * g->hop;
   int64_t Tn = frames;
   for (int i = 0; i < g->cfg.num_upsamples; ++i) Tn = nsf_stage_length(g, i, Tn * g->cfg.upsample_rates[i], source_frames);
   return Tn;
@@ -582,6 +705,7 @@ int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64
 
 int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
   if (!g || !key) return fail(AB_ERR_ARG, "set_option: null argument");
+  if (g->cfg.kind == AB_GEN_VOCOS) return fail(AB_ERR_ARG, "set_option: Vocos has no execution-plan option ('%s')", key);
   if (strcmp(key, "nsf_source_frames") == 0) {   // one-shot: consumed by the next forward
     if (value < 0) return fail(AB_ERR_ARG, "set_option: nsf_source_frames must be >= 0");
     if (value > 0 && g->cfg.kind != AB_GEN_NSFHIFIGAN) return fail(AB_ERR_ARG, "set_option: nsf_source_frames belongs to NSF-HiFiGAN");
@@ -598,9 +722,11 @@ int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
 
 int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max_entries, int32_t* n_out) {
   if (!g || !out || !n_out) return fail(AB_ERR_ARG, "get_profile: null argument");
-  static const char* kNames[5] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv"};
-  if (max_entries < 5) return fail(AB_ERR_ARG, "get_profile: need room for 5 entries");
-  for (int i = 0; i < 5; ++i) {
+  static const char* kNames[7] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
+                                  "tc_pointwise", "vocos_norm"};
+  const int n = g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;   // the last two classes are Vocos' kernels
+  if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
+  for (int i = 0; i < n; ++i) {
     memset(&out[i], 0, sizeof(out[i]));
     strncpy(out[i].name, kNames[i], sizeof(out[i].name) - 1);
   }
@@ -616,7 +742,7 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
     g->event_pool.push_back(r.e1);
   }
   g->prof_recs.clear();
-  *n_out = 5;
+  *n_out = n;
   return AB_OK;
 }
 
@@ -740,6 +866,105 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   // conv_pre (hifigan.py:204, bigvgan.py:314)
   const int C0 = g->cfg.upsample_initial_channel;
   const ConvRef& cpre = g->conv_pre;
+  if (g->cfg.kind == AB_GEN_VOCOS) {
+    const VocosRef& v = g->vocos;
+    const int Tn = (int)T, bins = g->cfg.istft_n_fft / 2 + 1;
+    VocosWs w;
+    if (vocos_layout(g, B, T, static_cast<char*>(dev_workspace), &w) == 0) return fail(AB_ERR_CUDA, "forward: iSTFT plan: %s", g_err);
+    uint16_t *Himg = reinterpret_cast<uint16_t*>(w.H), *Iimg = reinterpret_cast<uint16_t*>(w.I);
+    const double el = (double)B * T;
+    auto rup16 = [](int c) { return (double)((c + 15) / 16 * 16); };
+    // LayerNorm over channels [after the depthwise conv] -> fp32 y or the operand image yimg
+    auto norm = [&](const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float* y, uint16_t* yimg) -> int {
+      NormParams p;
+      p.x = x; p.dw_w = g->fptr(dw_w); p.dw_b = g->fptr(dw_b); p.ln_w = g->fptr(ln_w); p.ln_b = g->fptr(ln_b);
+      p.y = y; p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
+      p.B = (int)B; p.C = C0; p.T = Tn; p.eps = 1e-6f;
+      ++launches;
+      prof_begin(6, el * C0 * ((dw_w >= 0 ? 14.0 : 0.0) + 8.0), 4.0 * el * C0 + (y ? 4.0 * el * C0 : 2.0 * el * rup16(C0)));
+      const int r = launch_vocos_norm(p, st);
+      prof_end();
+      return r;
+    };
+    // fp32 Linear over channels (k = 1 conv) with the GELU or layer-scale residual epilogue
+    auto linear_fp32 = [&](const ConvRef& c, const float* x, float* y, int epi, const float* gamma) -> int {
+      ConvParams p;
+      p.x = x; p.xsb = (int64_t)c.cin * Tn; p.xsc = Tn; p.xst = 1;
+      p.w_t = g->fptr(c.w); p.bias = g->fptr(c.b);
+      p.residual = epi == CONV_EPI_GAMMA_RESIDUAL ? y : nullptr; p.acc_prev = nullptr; p.y = y;
+      p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = 1; p.d = 1;
+      p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0; p.epi = epi; p.gamma = gamma;
+      ++launches;
+      prof_begin(1, 2.0 * el * c.cin * c.cout,
+                 4.0 * (el * c.cin + el * c.cout * (epi == CONV_EPI_GAMMA_RESIDUAL ? 2 : 1) + (double)c.cin * c.cout));
+      const int r = launch_conv1d_fp32(p, st);
+      prof_end();
+      return r;
+    };
+    // Linear over channels on the pointwise wgmma GEMM, from the operand image ximg
+    auto pointwise = [&](const ConvRef& c, int epi, const uint16_t* ximg, uint16_t* yimg, float* y, const float* gamma,
+                         float* spec) -> int {
+      TcPwParams p;
+      p.epilogue = epi; p.ximg = ximg; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.gamma = gamma;
+      p.yimg = yimg; p.y = y; p.spec = spec;
+      p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.precision = g->precision;
+      ++launches;
+      const double out = epi == AB_PW_GELU ? 2.0 * el * rup16(c.cout) : epi == AB_PW_GAMMA_RESIDUAL ? 8.0 * el * c.cout
+                                                                                                     : 8.0 * el * (c.cout / 2);
+      prof_begin(5, 2.0 * el * c.cin * c.cout, 2.0 * el * rup16(c.cin) + 2.0 * c.cin * c.cout + out);
+      const int r = launch_tc_pointwise(p, st);
+      prof_end();
+      return r;
+    };
+    // x = norm(embed(x)) (vocos.py:764-772)
+    rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, w.Y, nullptr, Tn,
+                               1.0f, nullptr, nullptr, 1.0f, 0, conv_bytes(cpre, Tn, nullptr, nullptr))
+                     : conv(cpre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], w.Y, Tn, 1.0f, nullptr, nullptr, 1.0f, 0);
+    if (rc == AB_OK) rc = norm(w.Y, -1, -1, v.norm_w, v.norm_b, w.X, nullptr);
+    // x = x + gamma * pwconv2(gelu(pwconv1(norm(dwconv(x))))) (vocos.py:509-527)
+    for (size_t i = 0; rc == AB_OK && i < v.blocks.size(); ++i) {
+      const VocosBlockRef& blk = v.blocks[i];
+      if (tc) {
+        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, nullptr, Himg);
+        if (rc == AB_OK) rc = pointwise(blk.pw1, AB_PW_GELU, Himg, Iimg, nullptr, nullptr, nullptr);
+        if (rc == AB_OK) rc = pointwise(blk.pw2, AB_PW_GAMMA_RESIDUAL, Iimg, nullptr, w.X, g->fptr(blk.gamma), nullptr);
+      } else {
+        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, w.H, nullptr);
+        if (rc == AB_OK) rc = linear_fp32(blk.pw1, w.H, w.I, CONV_EPI_GELU, nullptr);
+        if (rc == AB_OK) rc = linear_fp32(blk.pw2, w.I, w.X, CONV_EPI_GAMMA_RESIDUAL, g->fptr(blk.gamma));
+      }
+    }
+    // final_layer_norm (:781), then the head's Linear and S = min(exp(mag), 1e2) (cos p + i sin p) (:343-360)
+    if (rc == AB_OK) rc = norm(w.X, -1, -1, v.final_w, v.final_b, tc ? nullptr : w.Y, tc ? Himg : nullptr);
+    if (rc == AB_OK && tc) rc = pointwise(v.head, AB_PW_SPECTRUM, Himg, nullptr, nullptr, nullptr, w.S);
+    if (rc == AB_OK && !tc) {
+      rc = linear_fp32(v.head, w.Y, w.I, CONV_EPI_NONE, nullptr);
+      // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart
+      for (int64_t b = 0; rc == AB_OK && b < B; ++b) {
+        const float* hb = w.I + b * 2 * bins * T;
+        ++launches;
+        rc = ab_spectral_head_forward(hb, hb + (int64_t)bins * T, nullptr, 1, bins, T, 1e2f, nullptr, nullptr, nullptr,
+                                      w.S + b * T * bins * 2, stream);
+      }
+    }
+    // ISTFT "same" (:142-167) in contiguous batch chunks, an event after each (ab_generator_set_tail_events)
+    const int nchunk = g->tail_events.empty() ? 1 : (int)std::min<int64_t>((int64_t)g->tail_events.size(), B);
+    for (int ci = 0; rc == AB_OK && ci < nchunk; ++ci) {
+      const int64_t b0 = B * ci / nchunk, b1 = B * (ci + 1) / nchunk;
+      launches += 2;
+      rc = ab_istft_forward(g->istft, w.S + b0 * T * bins * 2, b1 - b0, T, g->fptr(v.window), dev_wav + b0 * T * g->hop, w.ist,
+                            w.ist_bytes, stream);
+      if (rc == AB_OK && !g->tail_events.empty()) {
+        const size_t e0 = g->tail_events.size() * (size_t)ci / nchunk, e1 = g->tail_events.size() * (size_t)(ci + 1) / nchunk;
+        for (size_t e = e0; e < e1; ++e) cudaEventRecord(g->tail_events[e], st);
+      }
+    }
+    g->tail_events.clear();
+    g->source_frames = 0;
+    if (rc != AB_OK) return rc;
+    g->launches = launches;
+    return AB_OK;
+  }
   // HiFi-GAN: a tensor-core stage-0 ConvTranspose reads lrelu(x, 0.1) -> conv_pre emits that operand image, unless the
   // conditioning add changes x after it
   const bool pre_img = !big && !melgan && dev_g == nullptr && on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&

@@ -59,7 +59,12 @@ struct ConvParams {
   float out_div;        // 1.0f = none (IEEE division, as the reference's xs / num_kernels)
   int post_tanh;
   int reflect = 0;      // 1: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN, melgan.py:39-40,59-66,90-95)
+  // Vocos' pointwise layers (vocos.py:509-527), replacing residual / acc_prev / out_div / tanh:
+  //   CONV_EPI_GELU: y = gelu(bias + W x) (exact erf);  CONV_EPI_GAMMA_RESIDUAL: y = residual + gamma * (bias + W x)
+  int epi = 0;
+  const float* gamma = nullptr;   // [Cout]
 };
+enum { CONV_EPI_NONE = 0, CONV_EPI_GELU = 1, CONV_EPI_GAMMA_RESIDUAL = 2 };
 
 struct ConvTParams {
   const float* x;       // contiguous [B, Cin, Tin]
@@ -136,7 +141,23 @@ struct SnakeParams {
   int bf16;
 };
 
+// Vocos LayerNorm over the channels of every time step (eps, two-pass mean and biased variance, affine; vocos.py:
+// 493-527, :758-783), optionally after the k = 7 zero-padded depthwise conv with bias (ConvNeXtBlock.dwconv).
+struct NormParams {
+  const float* x = nullptr;       // contiguous [B, C, T] fp32
+  const float* dw_w = nullptr;    // nullable: depthwise weight [C][7]; dw_b its bias [C]
+  const float* dw_b = nullptr;
+  const float* ln_w = nullptr;    // [C]
+  const float* ln_b = nullptr;    // [C]
+  float* y = nullptr;             // fp32 [B, C, T] output, or
+  uint16_t* yimg = nullptr;       // 16-bit operand image [B][ceil16(C)/8][T][8] (padding channels zero)
+  int bf16 = 0;
+  int B = 0, C = 0, T = 0;
+  float eps = 1e-6f;
+};
+
 // launchers (ab_kernels_fp32.cu)
+int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);
 int launch_conv_transpose1d_fp32(const ConvTParams& p, cudaStream_t s);
 int launch_activation1d(const SnakeParams& p, cudaStream_t s);

@@ -24,7 +24,8 @@ constexpr int CI_T = 8;
 constexpr int NT = 256;
 
 // REFLECT: ReflectionPad1d(halo / 2) in place of the zero padding (MelGAN's ResnetBlock conv, melgan.py:39-40)
-template <int REFLECT>
+// EPI: ConvParams::epi (Vocos' pointwise layers); 0 = the generic epilogue below
+template <int REFLECT, int EPI = CONV_EPI_NONE>
 __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
   extern __shared__ float smem[];
   const int halo = (p.k - 1) * p.d;
@@ -96,10 +97,16 @@ __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
       const int t = t0 + tx + 16 * i;
       if (t >= p.T) continue;
       float v = acc[c][i] + bv;
-      if (p.residual) v += __ldg(p.residual + row + t);
-      if (p.acc_prev) v += __ldg(p.acc_prev + row + t);
-      if (p.out_div != 1.0f) v = v / p.out_div;
-      if (p.post_tanh) v = tanhf(v);
+      if constexpr (EPI == CONV_EPI_GELU) {
+        v = 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f));
+      } else if constexpr (EPI == CONV_EPI_GAMMA_RESIDUAL) {
+        v = __fadd_rn(__ldg(p.residual + row + t), __fmul_rn(__ldg(p.gamma + co), v));
+      } else {
+        if (p.residual) v += __ldg(p.residual + row + t);
+        if (p.acc_prev) v += __ldg(p.acc_prev + row + t);
+        if (p.out_div != 1.0f) v = v / p.out_div;
+        if (p.post_tanh) v = tanhf(v);
+      }
       p.y[row + t] = v;
     }
   }
@@ -349,7 +356,10 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
   const int halo = (p.k - 1) * p.d;
   if (p.reflect && halo / 2 >= p.T)
     return fail(AB_ERR_ARG, "conv1d: reflection padding %d needs more than %d samples", halo / 2, p.T);
-  if (p.Cout == 1 && p.k == 7 && p.d == 1 && !p.residual && !p.acc_prev && p.out_div == 1.0f) {
+  if (p.epi != CONV_EPI_NONE) {
+    if (p.reflect || (p.epi == CONV_EPI_GAMMA_RESIDUAL && (!p.residual || !p.gamma)) || p.epi > CONV_EPI_GAMMA_RESIDUAL)
+      return fail(AB_ERR_ARG, "conv1d: epilogue %d needs zero padding (and residual + gamma for the layer scale)", p.epi);
+  } else if (p.Cout == 1 && p.k == 7 && p.d == 1 && !p.residual && !p.acc_prev && p.out_div == 1.0f) {
     dim3 grid((unsigned)ceil_div(p.T, PT), 1, (unsigned)p.B);
     const bool vec = p.xst == 1 && (p.T & 3) == 0 && (p.xsc & 3) == 0 && (p.xsb & 3) == 0 &&
                      (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0;
@@ -363,7 +373,7 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
     AB_LAUNCH_CHECK("conv_post_fp32_kernel");
     return AB_OK;
   }
-  if (p.Cout <= 4) {
+  if (p.Cout <= 4 && p.epi == CONV_EPI_NONE) {
     const size_t smem = sizeof(float) * ((size_t)PCI * (PT + halo) + (size_t)p.Cin * p.k * p.Cout);
     if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "conv1d(few-out): filter too large for smem");
     static DeviceOnce configured[2];
@@ -378,9 +388,11 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
   const size_t smem = sizeof(float) * ((size_t)CI_T * (TT + halo) + (size_t)CI_T * p.k * CO_T);
   if (smem > 200 * 1024)
     return fail(AB_ERR_UNSUPPORTED, "conv1d: k=%d dilation=%d needs %zu B of shared memory", p.k, p.d, smem);
-  static DeviceOnce configured[2];
-  auto kern = p.reflect ? conv1d_fp32_kernel<1> : conv1d_fp32_kernel<0>;
-  if (smem > 48 * 1024 && configured[p.reflect ? 1 : 0].need()) {
+  static DeviceOnce configured[4];
+  auto kern = p.epi == CONV_EPI_GELU ? conv1d_fp32_kernel<0, CONV_EPI_GELU>
+              : p.epi == CONV_EPI_GAMMA_RESIDUAL ? conv1d_fp32_kernel<0, CONV_EPI_GAMMA_RESIDUAL>
+              : p.reflect ? conv1d_fp32_kernel<1> : conv1d_fp32_kernel<0>;
+  if (smem > 48 * 1024 && configured[p.epi ? 1 + p.epi : (p.reflect ? 1 : 0)].need()) {
     AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   if (ceil_div(p.Cout, CO_T) > 65535) return fail(AB_ERR_UNSUPPORTED, "conv1d: too many channels");
@@ -957,6 +969,117 @@ int launch_cond_add(float* x, const float* g, int64_t g_batch_stride, const floa
   if (B <= 0 || C <= 0 || gin <= 0 || T <= 0 || B > 65535) return fail(AB_ERR_ARG, "cond_add: bad shape");
   cond_add_kernel<<<dim3((unsigned)C, (unsigned)B), 128, 0, s>>>(x, g, g_batch_stride, w, bias, C, gin, T);
   AB_LAUNCH_CHECK("cond_add_kernel");
+  return AB_OK;
+}
+
+// ===========================================================================
+// Vocos LayerNorm, optionally after the depthwise conv (vocos.py:493-527, :758-783).  One CTA per (utterance, tile of
+// TT time steps): the values of all C channels of the tile go to shared memory [C][TT] once, then the mean, the
+// biased variance (a second pass over the centred values, as torch.layer_norm) and the affine output per time step.
+// DW: the k = 7 zero-padded depthwise conv with bias first.  OUT: 0 fp32 [B, C, T]; 1 / 2 the fp16 / bf16 operand image.
+// ===========================================================================
+namespace {
+constexpr int LN_THREADS = 256;
+
+template <int DW, int OUT>
+__global__ void __launch_bounds__(LN_THREADS) vocos_norm_kernel(NormParams p, int TT, int tiles) {
+  extern __shared__ float lsm[];   // [C][TT] values, [LN_THREADS] partial sums, [TT] mean, [TT] 1/std
+  float* part = lsm + (size_t)p.C * TT;
+  float* mean_s = part + LN_THREADS;
+  float* rstd_s = mean_s + TT;
+  const int b = blockIdx.x / tiles, t0 = (blockIdx.x - b * tiles) * TT;
+  const int tid = threadIdx.x, tt = tid % TT, grp = tid / TT, ngrp = LN_THREADS / TT;
+  const float* xb = p.x + (int64_t)b * p.C * p.T;
+  const int n = p.C * TT;
+  for (int i = tid; i < n; i += LN_THREADS) {
+    const int c = i / TT, t = t0 + (i - c * TT);
+    float v = 0.f;
+    if (t < p.T) {
+      const float* xr = xb + (int64_t)c * p.T;
+      if (DW) {
+        float a = 0.f;
+#pragma unroll
+        for (int j = 0; j < 7; ++j) {
+          const int s = t + j - 3;
+          if (s >= 0 && s < p.T) a = fmaf(__ldg(p.dw_w + c * 7 + j), __ldg(xr + s), a);
+        }
+        v = a + __ldg(p.dw_b + c);
+      } else {
+        v = __ldg(xr + t);
+      }
+    }
+    lsm[i] = v;
+  }
+  __syncthreads();
+  float a = 0.f;
+  for (int c = grp; c < p.C; c += ngrp) a += lsm[c * TT + tt];
+  part[tid] = a;
+  __syncthreads();
+  if (tid < TT) {
+    float s = 0.f;
+    for (int q = 0; q < ngrp; ++q) s += part[q * TT + tid];
+    mean_s[tid] = s / (float)p.C;
+  }
+  __syncthreads();
+  const float mu = mean_s[tt];
+  a = 0.f;
+  for (int c = grp; c < p.C; c += ngrp) {
+    const float d = lsm[c * TT + tt] - mu;
+    a = fmaf(d, d, a);
+  }
+  part[tid] = a;
+  __syncthreads();
+  if (tid < TT) {
+    float s = 0.f;
+    for (int q = 0; q < ngrp; ++q) s += part[q * TT + tid];
+    rstd_s[tid] = 1.0f / sqrtf(s / (float)p.C + p.eps);
+  }
+  __syncthreads();
+  auto norm = [&](int c, int u) {
+    return (lsm[c * TT + u] - mean_s[u]) * rstd_s[u] * __ldg(p.ln_w + c) + __ldg(p.ln_b + c);
+  };
+  if (OUT == 0) {
+    for (int i = tid; i < n; i += LN_THREADS) {
+      const int c = i / TT, u = i - c * TT, t = t0 + u;
+      if (t < p.T) p.y[((int64_t)b * p.C + c) * p.T + t] = norm(c, u);
+    }
+  } else {
+    const int c8n = (p.C + 15) / 16 * 2;
+    for (int i = tid; i < c8n * TT; i += LN_THREADS) {
+      const int c8 = i / TT, u = i - c8 * TT, t = t0 + u;
+      if (t >= p.T) continue;
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = c8 * 8 + e < p.C ? norm(c8 * 8 + e, u) : 0.f;
+      *reinterpret_cast<uint4*>(p.yimg + (((size_t)b * c8n + c8) * p.T + t) * 8) =
+          make_uint4(cvt_pair<OUT - 1>(v[0], v[1]), cvt_pair<OUT - 1>(v[2], v[3]), cvt_pair<OUT - 1>(v[4], v[5]),
+                     cvt_pair<OUT - 1>(v[6], v[7]));
+    }
+  }
+}
+}  // namespace
+
+int launch_vocos_norm(const NormParams& p, cudaStream_t s) {
+  if (!p.x || !p.ln_w || !p.ln_b || (!p.y) == (!p.yimg) || (!p.dw_w) != (!p.dw_b))
+    return fail(AB_ERR_ARG, "vocos norm: null argument");
+  if (p.B <= 0 || p.C <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "vocos norm: bad shape");
+  // time tile: up to 16 steps, fewer for wide C so that a few CTAs share an SM
+  int TT = 16;
+  auto smem_of = [&](int tt) { return sizeof(float) * ((size_t)p.C * tt + LN_THREADS + 2 * tt); };
+  while (TT > 1 && smem_of(TT) > 64 * 1024) TT >>= 1;
+  const size_t smem = smem_of(TT);
+  if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "vocos norm: %d channels do not fit shared memory", p.C);
+  const int64_t tiles = ceil_div(p.T, TT), grid = (int64_t)p.B * tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "vocos norm: grid too large");
+  const int out = p.y ? 0 : (p.bf16 ? 2 : 1);
+  void (*kerns[2][3])(NormParams, int, int) = {{vocos_norm_kernel<0, 0>, vocos_norm_kernel<0, 1>, vocos_norm_kernel<0, 2>},
+                                                {vocos_norm_kernel<1, 0>, vocos_norm_kernel<1, 1>, vocos_norm_kernel<1, 2>}};
+  const int dw = p.dw_w ? 1 : 0;
+  static DeviceOnce configured[2][3];
+  if (smem > 48 * 1024 && configured[dw][out].need())
+    AB_CUDA_TRY(cudaFuncSetAttribute(kerns[dw][out], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  kerns[dw][out]<<<(unsigned)grid, LN_THREADS, smem, s>>>(p, TT, (int)tiles);
+  AB_LAUNCH_CHECK("vocos_norm_kernel");
   return AB_OK;
 }
 

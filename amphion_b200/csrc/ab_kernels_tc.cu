@@ -18,7 +18,8 @@
 //      streamed with cp.async.bulk (TMA 1-D) through an mbarrier ring; thread 0 refills a stage once every warp
 //      has released it.
 //   D: fp32 in the registers of two consumer warpgroups (MT m64 tiles each); the epilogues run on the fragments.
-// hconv_kernel (conv), hconvt_kernel (conv-transpose), hpair_kernel (conv pair) and hchain_kernel (block mode) share the operand
+// hconv_kernel (conv), hconvt_kernel (conv-transpose), hpair_kernel (conv pair), hchain_kernel (block mode) and hpw_kernel
+// (Vocos' pointwise layers) share the operand
 // loader, the wgmma batch, the intermediate-tile and output epilogues and the shared-memory layout below; they differ in
 // how they schedule them.
 #include <stdlib.h>
@@ -1127,6 +1128,172 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hconvt_kernel(HcArgs p, HcGeom 
   }
 }
 
+// Pointwise (1x1) GEMM of Vocos' ConvNeXt blocks and iSTFT head (launch_tc_pointwise): D[t, n] = sum_ci A[t, ci] W[n, ci]
+// from the operand image of the input, K = C_in and N = C_out unbounded.  Same persistent warp-specialised schedule as
+// hconvt_kernel with a single tap: work items (utterance, time tile, N block), the N block fastest, so the NB items of
+// a tile share its A chunks through L2.  Epilogues (compile time, PwEpi):
+//   PW_GELU:     yimg = cvt(gelu(acc + b))                           (pwconv1 + nn.GELU(), exact erf)
+//   PW_GAMMA:    y = y + gamma * (acc + b), fp32 in place            (pwconv2, layer scale and residual, vocos.py:509-527)
+//   PW_SPECTRUM: columns 2j, 2j + 1 hold bin j's log-magnitude and phase (launch_tc_pack_head_weight):
+//                spec[b T + t][j] = min(exp(m), 1e2) (cos p, sin p)  (ISTFTHead, vocos.py:343-361)
+enum PwEpi : int { PW_GELU = AB_PW_GELU, PW_GAMMA = AB_PW_GAMMA_RESIDUAL, PW_SPECTRUM = AB_PW_SPECTRUM };
+struct PwArgs {
+  const float* gamma;   // PW_GAMMA: [C_out]
+  float2* spec;         // PW_SPECTRUM: [B*T][C_out / 2]
+};
+
+template <int NW, int BF16, int EPI>
+__global__ void __launch_bounds__(HB_THREADS, 1) hpw_kernel(HcArgs p, HcGeom g, PwArgs e) {
+  constexpr int MT = mt_of(NW);
+  constexpr int NACC = NW / 2;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  const uint32_t sA = smem_u32(smem), sW = sA + g.off_w;
+  const uint32_t abytes = (uint32_t)g.rowsA * 64u;   // one A chunk: 4 c8 planes x rowsA rows
+  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
+  const uint32_t bar0 = smem_u32(smem + g.off_bar);
+  auto w_full = [&](int s) { return bar0 + 8u * s; };
+  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
+  auto a_full = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + s); };
+  auto a_empty = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + HP_ABUF_MAX + s); };
+  const int nwork = p.B * g.tiles * g.NB;
+
+  if (tid == 0) {
+    for (int s = 0; s < g.nstages; ++s) {
+      mbar_init(w_full(s), 1);
+      mbar_init(w_empty(s), 8);
+    }
+    for (int s = 0; s < g.nabuf; ++s) {
+      mbar_init(a_full(s), HB_LOADERS);
+      mbar_init(a_empty(s), 8);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  stage_biases(bias_s, p, 1, g.NB * NW, tid, HB_THREADS);
+  __syncthreads();
+
+  // ------------------------------------------------------------------------------------------------ producer
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+    if (tid == 0) {
+      RingPos r;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+        const int i0 = (w % g.NB) * g.nkc;
+        for (int i = 0; i < g.nkc; ++i, r.next(g.nstages)) {
+          if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
+          mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
+          bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, 0, i0 + i), g.stage_bytes, w_full(r.s));
+        }
+      }
+    } else if (tid >= 32) {
+      RingPos r;
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+        const int bt = w / g.NB, b = bt / g.tiles, t0 = (bt - b * g.tiles) * g.V;
+        for (int kc = 0; kc < g.nkc; ++kc, r.next(g.nabuf)) {
+          if (r.wrapped) mbar_wait(a_empty(r.s), r.ph ^ 1u);
+          load_tile<BF16>(p, g, b, smem + r.s * abytes, 4 * kc, 4, g.rowsA, t0, tid - 32, HB_LOADERS);
+          fence_proxy_async();
+          mbar_arrive(a_full(r.s));
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------------------------------------ consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
+  const int cw = wg - 1;
+  float acc[MT][NACC];
+  RingPos wr, ar;
+  // two batches in flight when both rings leave a slot to fill next to the two they hold
+  const bool deep = g.nstages >= 3 && g.nabuf >= 3;
+  int pw1 = -1;   // (W slot << 8) | A buffer of the batch in flight, -1: none
+
+  auto fence_acc = [&]() {
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
+  };
+  auto release = [&](int s) {   // W slot s and the A buffer of the same chunk (one tap: the rings advance together)
+    __syncwarp();
+    if (lane == 0 && s >= 0) {
+      mbar_arrive(w_empty(s >> 8));
+      mbar_arrive(a_empty(s & 255));
+    }
+  };
+
+  for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+    const int bt = w / g.NB, nb = w - bt * g.NB, b = bt / g.tiles, O = (bt - b * g.tiles) * g.V;
+    bool first = true;
+    for (int kc = 0; kc < g.nkc; ++kc) {
+      const int abuf = ar.s, s = wr.s;
+      mbar_wait(a_full(abuf), ar.ph);
+      mbar_wait(w_full(s), wr.ph);
+      ar.next(g.nabuf);
+      wr.next(g.nstages);
+      fence_acc();
+      wg_fence();
+      mma_batch<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64, sW + (uint32_t)s * g.stage_bytes, first);
+      wg_commit();
+      if (deep) {
+        wg_wait<1>();   // the previous batch has completed: its W slot and A buffer can be refilled
+        fence_acc();
+        release(pw1);
+      } else {
+        wg_wait<0>();
+        fence_acc();
+        release((s << 8) | abuf);
+      }
+      pw1 = (s << 8) | abuf;
+      first = false;
+    }
+    wg_wait<0>();
+    fence_acc();
+    if (deep) release(pw1);
+    pw1 = -1;
+
+    const Frag<MT> f(cw);
+    const int co0 = nb * NW;
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = O + f.row(mt, h);
+        if (t >= g.Tout) continue;
+#pragma unroll
+        for (int c = 0; c < NW / 8; ++c) {
+          const int co = co0 + c * 8 + f.col;
+          const float a0 = acc[mt][c * 4 + 2 * h], a1 = acc[mt][c * 4 + 2 * h + 1];
+          if constexpr (EPI == PW_GELU) {
+            if ((co >> 3) >= g.c8n_out) continue;
+            float v[2] = {a0 + bias_s[co], a1 + bias_s[co + 1]};
+#pragma unroll
+            for (int q = 0; q < 2; ++q) v[q] = co + q < p.Cout ? 0.5f * v[q] * (1.0f + erff(v[q] * 0.70710678118654752440f)) : 0.f;
+            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+                pack2t<BF16>(v[0], v[1]);
+          } else if constexpr (EPI == PW_GAMMA) {
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              if (co + q >= p.Cout) continue;
+              const float v = (q ? a1 : a0) + bias_s[co + q];
+              float* y = p.y + ((int64_t)b * p.Cout + co + q) * g.Tout + t;
+              *y = __fadd_rn(*y, __fmul_rn(__ldg(e.gamma + co + q), v));
+            }
+          } else {
+            const int bins = p.Cout >> 1, j = co >> 1;
+            if (j >= bins) continue;
+            float amp = expf(a0 + bias_s[j]);
+            amp = fminf(amp, 1e2f);
+            float sn, cs;
+            sincosf(a1 + bias_s[bins + j], &sn, &cs);
+            e.spec[((int64_t)b * g.Tout + t) * bins + j] = make_float2(amp * cs, amp * sn);
+          }
+        }
+      }
+  }
+}
+
 // ---------------------------------------------------------------------------
 // weight images: stage (nb, kc, tap) = [4 c8][NW rows][8] — the A/B operand layout of ab_tc_ptx.cuh
 // ---------------------------------------------------------------------------
@@ -1192,6 +1359,29 @@ __global__ void hc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* _
       const int cl = n / L.u, phi = n - cl * L.u, co = nb * L.cc + cl, j = phi + L.u * tap;
       if (ci < cin && cl < L.cc && co < cout && j < k) v = w_t[((int64_t)ci * k + j) * cout + co];
     }
+    img[idx] = (uint16_t)(pack2(v, 0.f, bf16) & 0xffffu);
+  }
+}
+
+// Weight image of Vocos' iSTFT head for the PW_SPECTRUM epilogue (k = 1, conv layout): image column 2j holds output
+// row j (log-magnitude of bin j), column 2j + 1 row bins + j (its phase), so one thread's accumulator pair is one bin.
+__global__ void hc_pack_head_weight_kernel(const float* __restrict__ w_t, uint16_t* __restrict__ img, HcLayer L, int cin,
+                                           int cout, int bf16) {
+  const int64_t total = (int64_t)L.NB * L.nkc * 32 * L.NW;
+  const int bins = cout >> 1;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (int64_t)gridDim.x * blockDim.x) {
+    const int e = (int)(idx & 7);
+    int64_t r = idx >> 3;
+    const int n = (int)(r % L.NW);
+    r /= L.NW;
+    const int c8l = (int)(r & 3);
+    r >>= 2;
+    const int kc = (int)(r % L.nkc);
+    const int nb = (int)(r / L.nkc);
+    const int ci = kc * 32 + c8l * 8 + e, col = nb * L.NW + n, j = col >> 1;
+    const int co = (col & 1) ? bins + j : j;
+    const float v = (ci < cin && j < bins) ? w_t[(int64_t)ci * cout + co] : 0.f;
     img[idx] = (uint16_t)(pack2(v, 0.f, bf16) & 0xffffu);
   }
 }
@@ -1495,6 +1685,73 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev; a.post_tanh = p.post_tanh;
   a.yimg = p.yimg; a.img_slope = p.img_slope;
   return launch_hconv(a, g, p.precision, s, p.reflect != 0);
+}
+
+
+// Pointwise GEMM geometry: make_geom's k = 1 conv tiles, laid out for one persistent CTA per SM with as many A chunk
+// buffers as fit next to the W ring.
+static int make_pw_geom(int cin, int cout, int T, HcGeom& g) {
+  int rc = make_geom(0, cin, cout, 1, 1, T, true, g);
+  if (rc != AB_OK) return rc;
+  const uint32_t abytes = (uint32_t)g.rowsA * 64u, nbias = (uint32_t)g.NB * (g.stage_bytes / 64u);
+  bool fits;
+  g.nabuf = HP_ABUF_MAX;
+  while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, 0, nbias, 16u * (HC_STAGES_MAX + HP_ABUF_MAX), HC_SMEM_1CTA)) &&
+         g.nabuf > 1)
+    --g.nabuf;
+  if (!fits) return fail(AB_ERR_UNSUPPORTED, "tc pointwise: C_out=%d does not fit shared memory", cout);
+  return AB_OK;
+}
+
+int launch_tc_pack_head_weight(const float* w_t, void* image, int cin, int cout, int precision, cudaStream_t s) {
+  HcLayer L;
+  int rc = layer_geom(0, cin, cout, 1, 1, L);
+  if (rc != AB_OK) return rc;
+  if (cout & 1) return fail(AB_ERR_ARG, "tc head weight: C_out %d must be even (magnitude and phase halves)", cout);
+  const int64_t total = (int64_t)layer_image_bytes(L) / 2;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 132 * 8);
+  hc_pack_head_weight_kernel<<<blocks, 256, 0, s>>>(w_t, static_cast<uint16_t*>(image), L, cin, cout,
+                                                    precision == AB_PREC_TC_BF16 ? 1 : 0);
+  AB_LAUNCH_CHECK("hc_pack_head_weight_kernel");
+  return AB_OK;
+}
+
+int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s) {
+  if (!p.ximg || !p.w || !p.bias) return fail(AB_ERR_ARG, "tc pointwise: null argument");
+  if (p.B <= 0 || p.T <= 0 || p.Cin <= 0 || p.Cout <= 0) return fail(AB_ERR_ARG, "tc pointwise: bad shape");
+  if (p.precision != AB_PREC_TC_F16 && p.precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc pointwise: bad precision");
+  if ((p.epilogue == AB_PW_GELU && !p.yimg) || (p.epilogue == AB_PW_GAMMA_RESIDUAL && (!p.y || !p.gamma)) ||
+      (p.epilogue == AB_PW_SPECTRUM && (!p.spec || (p.Cout & 1))))
+    return fail(AB_ERR_ARG, "tc pointwise: epilogue %d: missing output or odd C_out", p.epilogue);
+  HcGeom g;
+  int rc = make_pw_geom(p.Cin, p.Cout, p.T, g);
+  if (rc != AB_OK) return rc;
+  HcArgs a = base_args(nullptr, 0, 0, 0, p.ximg, 1.0f, p.B, p.Cin, p.Cout);
+  a.ws[0] = p.w; a.bs[0] = p.bias;
+  a.y = p.y; a.yimg = p.yimg;
+  PwArgs e;
+  e.gamma = p.gamma;
+  e.spec = reinterpret_cast<float2*>(p.spec);
+  unsigned grid = 0;
+  rc = persistent_grid((int64_t)p.B * g.tiles * g.NB, "tc pointwise", grid);
+  if (rc != AB_OK) return rc;
+  return with_nw(g, p.precision, [&](auto nw, auto bf16) -> int {
+    constexpr int NW = decltype(nw)::value, BF = decltype(bf16)::value;
+    auto go = [&](auto kern) -> int {
+      static DeviceOnce configured[3];
+      if (configured[p.epilogue].need())
+        AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
+      kern<<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g, e);
+      AB_LAUNCH_CHECK("hpw_kernel");
+      return AB_OK;
+    };
+    switch (p.epilogue) {
+      case AB_PW_GELU: return go(hpw_kernel<NW, BF, PW_GELU>);
+      case AB_PW_GAMMA_RESIDUAL: return go(hpw_kernel<NW, BF, PW_GAMMA>);
+      case AB_PW_SPECTRUM: return go(hpw_kernel<NW, BF, PW_SPECTRUM>);
+    }
+    return fail(AB_ERR_ARG, "tc pointwise: unknown epilogue %d", p.epilogue);
+  });
 }
 
 }  // namespace ab

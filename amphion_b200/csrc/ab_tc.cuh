@@ -71,6 +71,27 @@ struct TcChainParams {
 double tc_chain_recompute(int C, int k, const int* dil, int npairs, int nconv);
 int launch_tc_chain(const TcChainParams& p, cudaStream_t s);
 
+// Pointwise (1x1, nn.Linear over channels) GEMM of Vocos (hpw_kernel): input the operand image of x, any C_in / C_out.
+//   AB_PW_GELU:            yimg = image of gelu(W x + b)                    (ConvNeXtBlock pwconv1 + nn.GELU())
+//   AB_PW_GAMMA_RESIDUAL:  y = y + gamma * (W x + b), fp32 [B, C_out, T]    (pwconv2, layer scale, residual)
+//   AB_PW_SPECTRUM:        spec [B*T][C_out/2] complex = min(exp(m), 1e2) (cos p + i sin p), m / p the two halves of
+//                          W x + b (ISTFTHead); w from launch_tc_pack_head_weight
+enum { AB_PW_GELU = 0, AB_PW_GAMMA_RESIDUAL = 1, AB_PW_SPECTRUM = 2 };
+struct TcPwParams {
+  int epilogue = AB_PW_GELU;
+  const uint16_t* ximg = nullptr;   // [B][ceil16(Cin)/8][T][8], padding channels zero
+  const void* w = nullptr;          // launch_tc_pack_weight(mode 0, k 1) image, or launch_tc_pack_head_weight
+  const float* bias = nullptr;      // [Cout]
+  const float* gamma = nullptr;     // AB_PW_GAMMA_RESIDUAL
+  uint16_t* yimg = nullptr;         // AB_PW_GELU: [B][ceil16(Cout)/8][T][8] (padding channels written as zero)
+  float* y = nullptr;               // AB_PW_GAMMA_RESIDUAL
+  float* spec = nullptr;            // AB_PW_SPECTRUM: interleaved (re, im)
+  int B = 0, Cin = 0, Cout = 0, T = 0;
+  int precision = AB_PREC_TC_F16;
+};
+int launch_tc_pack_head_weight(const float* w_t, void* image, int cin, int cout, int precision, cudaStream_t s);
+int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s);
+
 // square convs that pair mode and block mode serve (C <= 256, odd k <= 31)
 bool tc_conv_supported(int C, int k);
 size_t tc_act_image_bytes(int64_t B, int C, int64_t T);

@@ -172,7 +172,10 @@ def _side_stream(device):
 
 
 def _hop_of(model):
+    """Samples per mel frame: cfg.preprocess.hop_size, else the model's ``hop_length`` (Vocos, built from
+    cfg.model.vocos), else None."""
     try:
         return int(model.cfg.preprocess.hop_size)
     except AttributeError:
-        return None
+        hop = getattr(model, "hop_length", None)
+        return None if hop is None else int(hop)

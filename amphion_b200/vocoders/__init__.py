@@ -5,6 +5,7 @@ from .bigvgan import BigVGAN
 from .hifigan import HiFiGAN, HiFiGAN_vits
 from .melgan import MelGAN
 from .nsfhifigan import NSFHiFiGAN
+from .vocos import Vocos
 from .gan_vocoder_inference import synthesis_audios, synthesize_to_files
 from .gan_vocoder_inference import vocoder_inference as _gan_vocoder_inference
 
@@ -13,7 +14,8 @@ _vocoders = {"hifigan": HiFiGAN, "bigvgan": BigVGAN, "nsfhifigan": NSFHiFiGAN, "
 _vocoder_forward_funcs = {k: _gan_vocoder_inference for k in _vocoders}
 _vocoder_infer_funcs = {k: synthesis_audios for k in _vocoders}
 
-__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "NSFHiFiGAN", "MelGAN", "APNet", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
+# Vocos is not in the registry: the reference has no entry for it and its constructor takes cfg.model.vocos, not cfg
+__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "NSFHiFiGAN", "MelGAN", "APNet", "Vocos", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
            "_vocoder_forward_funcs", "_vocoder_infer_funcs"]
 
 # `amphion_b200.vocoders.vocoder_inference` is the MODULE (synthesis, load_nnvocoder), as

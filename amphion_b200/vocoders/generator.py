@@ -91,6 +91,15 @@ class NativeGenerator(nn.Module):
         """Upsampling factor of each stage; their product is the hop."""
         return [int(u) for u in self._hp().upsample_rates]
 
+    def _input_channels(self):
+        return int(self.cfg.preprocess.n_mel)
+
+    def _hop(self):
+        hop = 1
+        for u in self._upsample_rates():
+            hop *= u
+        return hop
+
     def _c_config(self):
         hp = self._hp()
         c = _capi.GeneratorConfig()
@@ -181,8 +190,8 @@ class NativeGenerator(nn.Module):
     def _forward_native(self, x, g=None, out=None, tail_events=None, out_samples=None):
         """``g`` [B, gin_channels] (HiFiGAN_vits conditioning) or None."""
         _capi.require_cuda(x, f"{type(self).__name__}.forward")
-        if x.dim() != 3 or x.shape[1] != int(self.cfg.preprocess.n_mel):
-            raise ValueError(f"expected mel of shape [B, {self.cfg.preprocess.n_mel}, T], got {tuple(x.shape)}")
+        if x.dim() != 3 or x.shape[1] != self._input_channels():
+            raise ValueError(f"expected mel of shape [B, {self._input_channels()}, T], got {tuple(x.shape)}")
         if x.dtype != torch.float32:
             x = x.float()
         B, _, T = x.shape
@@ -191,9 +200,7 @@ class NativeGenerator(nn.Module):
         with torch.cuda.device(x.device):
             self._sync_params(x.device)
             lib, h = _capi.lib, self._handle
-            hop = 1
-            for u in self._upsample_rates():
-                hop *= u
+            hop = self._hop()
             need = lib.ab_generator_workspace_bytes(h, B, T)
             if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != x.device:
                 self._workspace = None

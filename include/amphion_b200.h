@@ -59,8 +59,19 @@ extern "C" {
  * is refused.  Tensors keep the reference's nn.Sequential names: "model.1" (conv_pre), "model.{2+i(2+R)+1}" (ConvTranspose
  * of stage i), "model.{2+i(2+R)+2+j}.block.2" / ".block.4" / ".shortcut" (block j), "model.{2+n(2+R)+2}" (conv_post),
  * R = n_residual_layers, n = len(ratios).  A forward whose mel has fewer than 4 frames, or whose stage is not longer
- * than one of its dilations, fails with AB_ERR_ARG before any launch (the reference's ReflectionPad1d raises). */
-enum ab_generator_kind { AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4 };
+ * than one of its dilations, fails with AB_ERR_ARG before any launch (the reference's ReflectionPad1d raises).
+ * AB_GEN_VOCOS: Vocos.forward (models/codec/amphion_codec/vocos.py:824-881, non-conditional backbone, "same" padding):
+ * x = LayerNorm(embed(mel)) [Conv1d k = 7]; num_layers ConvNeXt blocks x = x + gamma * pwconv2(gelu(pwconv1(LayerNorm(
+ * dwconv(x))))) [depthwise k = 7, LayerNorm eps 1e-6, Linear layers over channels] (:469-527); final LayerNorm; ISTFTHead:
+ * Linear(dim, n_fft + 2), S = min(exp(mag), 1e2) (cos p + i sin p), ISTFT "same" with the loaded window (:84-167,
+ * :314-361).  Config fields: n_mel = input_channels, upsample_initial_channel = dim, ffn_channels = intermediate_dim,
+ * num_layers, istft_n_fft (even), istft_hop (<= n_fft, n_fft - hop even); every other field 0.  Tensors keep the
+ * reference's state-dict names ("backbone.embed.weight", "backbone.convnext.3.pwconv1.weight" [out, in], ".gamma",
+ * "backbone.final_layer_norm.bias", "head.out.weight", "head.istft.window", ...).  Output: wav [B, 1, T * istft_hop];
+ * with tail events the iSTFT runs in the batch chunks. */
+enum ab_generator_kind {
+  AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5
+};
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
@@ -79,6 +90,7 @@ int ab_device_is_sm90(void);
  *            BigVGAN.forward     (models/vocoders/gan/generator/bigvgan.py:313-331)
  *            NSFHiFiGAN.forward  (models/vocoders/gan/generator/nsfhifigan.py:262-283)
  *            MelGAN.forward      (models/vocoders/gan/generator/melgan.py:100-101)
+ *            Vocos.forward       (models/codec/amphion_codec/vocos.py:877-881)
  * The config mirrors cfg.model.{hifigan,bigvgan}.* + cfg.preprocess.n_mel
  * (hifigan.py:151-201, bigvgan.py:232-311).
  * ---------------------------------------------------------------------- */
@@ -105,6 +117,11 @@ typedef struct ab_generator_config {
   int32_t trunk_out_channels;                   /* conv_post output channels (n_fft/2+1, or 2*(n_fft/2+1) for R|I) */
   int32_t trunk_in_kernel;                      /* conv_pre kernel size (odd) */
   int32_t trunk_out_kernel;                     /* conv_post kernel size (odd) */
+  /* AB_GEN_VOCOS only (0 elsewhere) */
+  int32_t ffn_channels;                         /* ConvNeXt intermediate_dim */
+  int32_t num_layers;                           /* ConvNeXt blocks */
+  int32_t istft_n_fft;
+  int32_t istft_hop;
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -157,7 +174,8 @@ int ab_generator_last_launches(const ab_generator* g);
  * ab_generator_get_profile synchronises on the recorded events, accumulates
  * (launches, milliseconds, algorithmic FLOPs, algorithmic HBM bytes) per class
  * since the last call, and resets.  Classes: "tc_conv", "conv1d_fp32",
- * "conv_transpose1d_fp32", "activation1d", "tc_gemmconv" (max_entries >= 5). */
+ * "conv_transpose1d_fp32", "activation1d", "tc_gemmconv" (max_entries >= 5), then, when max_entries >= 7,
+ * "tc_pointwise" (Vocos' pointwise GEMMs and head) and "vocos_norm" (its depthwise conv + LayerNorm kernels). */
 typedef struct ab_profile_entry {
   char name[32];
   int32_t launches;
