@@ -1,5 +1,5 @@
-// wgmma implicit-GEMM convolutions (sm_90a): the ResBlock / AMPBlock convs, ConvTranspose1d and the
-// non-square / wide Conv1d layers.
+// wgmma implicit-GEMM convolutions (sm_90a): the ResBlock / AMPBlock convs, ConvTranspose1d, the non-square / wide
+// Conv1d layers and Vocos' pointwise layers.
 //
 // Mapping (DESIGN.md §4):  D[row, n] += sum_{tap} A[row + shift(tap), ci] * W[tap][n, ci]
 //   M = time rows, N = output channels (<= 256 per N block), K = C_in per tap.
@@ -18,10 +18,11 @@
 //      streamed with cp.async.bulk (TMA 1-D) through an mbarrier ring; thread 0 refills a stage once every warp
 //      has released it.
 //   D: fp32 in the registers of two consumer warpgroups (MT m64 tiles each); the epilogues run on the fragments.
-// hconv_kernel (conv), hconvt_kernel (conv-transpose), hpair_kernel (conv pair), hchain_kernel (block mode) and hpw_kernel
-// (Vocos' pointwise layers) share the operand
-// loader, the wgmma batch, the intermediate-tile and output epilogues and the shared-memory layout below; they differ in
-// how they schedule them.
+// Kernels: hconv_kernel (one CTA per tile: conv and conv-transpose from fp32 input), and three persistent,
+// warp-specialised kernels on one pipeline (Rings, Batches): hpair_kernel (conv pair), hchain_kernel (block mode) and
+// hitem_kernel ((utterance, tile, N block) work items: conv-transpose from an operand image, Vocos' pointwise GEMM).
+// They share the operand loader, the wgmma batch, the intermediate-tile and output epilogues and the shared-memory
+// layout below; they differ in how they schedule them.
 #include <stdlib.h>
 #include <string.h>
 
@@ -67,7 +68,7 @@ struct HcArgs {
 };
 
 struct HcGeom {
-  int mode;                // 0 conv, 1 conv-transpose (hconv_kernel; hconvt_kernel from an operand image), 2 conv pair (hpair_kernel)
+  int mode;                // 0 conv, 1 conv-transpose (hconv_kernel; hitem_kernel from an operand image), 2 conv pair (hpair_kernel)
   int NB, cc;              // N blocks; output channels per block
   int R, V, tiles;         // rows per CTA tile, valid output rows per tile, tiles per sequence
   int ntaps, d;            // taps of every conv; the row step between the (first) conv's taps
@@ -242,7 +243,7 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
 // ------------------------------------------------------------------------------------------------ kernels
 
 // modes 0 (conv) and 1 (conv-transpose from fp32 input); launch_hconv runs conv-transpose from an operand image on
-// hconvt_kernel, pair mode (2) on hpair_kernel, and block mode runs on hchain_kernel.  The mode-2 branch below is no longer launched but stays: without it ptxas (nvcc 12.9, build.py's
+// hitem_kernel, pair mode (2) on hpair_kernel, and block mode runs on hchain_kernel.  The mode-2 branch below is no longer launched but stays: without it ptxas (nvcc 12.9, build.py's
 // flags) reports spill stores / loads of 956 / 1220 bytes at N = 256 and 784 / 1020 at N = 128, against 4 / 4 and
 // 16 / 20 with it, which made HiFi-GAN V1's ConvTranspose layers about 5 ms per step slower (H100 80GB HBM3, 400 W
 // power limit).  Re-check those numbers before deleting it.
@@ -385,23 +386,34 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   }
 }
 
-// Block mode (launch_tc_chain): warp-specialised and persistent.  One CTA of three warpgroups per SM walks the
-// (utterance, time tile) work items with a static stride.
-//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams the weight stages of every tile through the W ring;
-//     warps 1-3 load the operand tile X of the next work item as soon as the consumers release it, so that load
-//     overlaps the current tile's output epilogue.
-//   warpgroups 1-2 (consumers, setmaxnreg 232): one wgmma batch per tap with the two previous batches still in flight; a
-//     W slot is released once the batch that read it has completed.  Consumer-only synchronisation is a named
-//     barrier.  The residual stream x_p of the whole ResBlock stays in registers in the accumulator fragment layout.
-// The accumulation order of every output element is that of hconv_kernel's per-pair mode (K chunk -> tap -> k16).
+// ------------------------------------------------------------------------------------------------ persistent pipeline
+// hchain_kernel, hpair_kernel and hitem_kernel are warp-specialised and persistent: one CTA of three warpgroups per SM
+// walks the work items with a static stride, and all three run the pipeline below.
+//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams each item's weight stages through the W ring, running ahead
+//     across items (Rings::stream_weights); warps 1-3 load each item's A operand through the A ring as soon as the
+//     consumers release a buffer (Rings::load_item), so the next item's loads run under this item's epilogue.
+//   warpgroups 1-2 (consumers, setmaxnreg 232): one wgmma batch per tap with up to D batches left in flight; a W slot,
+//     and an A buffer after the last tap that reads it, is released once the batch that read it has completed
+//     (Batches).  Consumer-only synchronisation is a named barrier.
 constexpr int HB_THREADS = 3 * 128;
 constexpr int HB_LOADERS = 96;
 constexpr int HB_PRODUCER_REGS = 40;
 constexpr int HB_CONSUMER_REGS = 232;
 static_assert(128 * HB_PRODUCER_REGS + 256 * HB_CONSUMER_REGS <= 65536, "setmaxnreg split of the register file");
-constexpr int HP_ABUF_MAX = 3;   // hpair_kernel: A chunk buffers, as many as fit (one for very wide tap reach)
+// A chunk buffers of hpair_kernel and hitem_kernel: as many as fit (one for very wide tap reach)
+constexpr int HP_ABUF_MAX = 3;
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Splits the register file between the roles: true in the producer warpgroup, false in the two consumer warpgroups.
+__device__ __forceinline__ bool producer_warpgroup(int wg) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+    return true;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
+  return false;
+}
 
 // Position in a ring of n mbarrier slots: the slot, the parity of its current round, and whether the ring has wrapped
 // (the producer waits for a slot's release from the second round on).  Counters instead of a division per tap.
@@ -418,30 +430,171 @@ struct RingPos {
   }
 };
 
+// The W ring (g.nstages weight stages at sW) and the A ring (nabuf <= AMAX operand buffers from shared-memory offset
+// 0) and their mbarriers at bar0: W full / empty (HC_STAGES_MAX each), then A full / empty (AMAX each).  A full slot
+// takes thread 0's expect_tx (W) or every loader thread's arrival (A); an empty slot one arrival per consumer warp.
+template <int AMAX>
+struct Rings {
+  static constexpr uint32_t BAR_BYTES = 8u * (2 * HC_STAGES_MAX + 2 * AMAX);
+  uint32_t bar0, sW;
+  __device__ __forceinline__ uint32_t w_full(int s) const { return bar0 + 8u * s; }
+  __device__ __forceinline__ uint32_t w_empty(int s) const { return bar0 + 8u * (HC_STAGES_MAX + s); }
+  __device__ __forceinline__ uint32_t a_full(int s) const { return bar0 + 8u * (2 * HC_STAGES_MAX + s); }
+  __device__ __forceinline__ uint32_t a_empty(int s) const { return bar0 + 8u * (2 * HC_STAGES_MAX + AMAX + s); }
+
+  // thread 0, before the __syncthreads that precedes every use
+  __device__ __forceinline__ void init(int nstages, int nabuf) const {
+    for (int s = 0; s < nstages; ++s) {
+      mbar_init(w_full(s), 1);
+      mbar_init(w_empty(s), 8);
+    }
+    for (int s = 0; s < nabuf; ++s) {
+      mbar_init(a_full(s), HB_LOADERS);
+      mbar_init(a_empty(s), 8);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+
+  // thread 0: stages [i0, i0 + n) of conv st's weight image into the next W slots
+  __device__ __forceinline__ void stream_weights(const HcArgs& p, const HcGeom& g, RingPos& r, int st, int i0,
+                                                 int n) const {
+    for (int i = 0; i < n; ++i, r.next(g.nstages)) {
+      if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
+      mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
+      bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, st, i0 + i), g.stage_bytes, w_full(r.s));
+    }
+  }
+
+  // loader warps (producer threads 32-127): one work item's A operand into the next nchunks A buffers, chunk kc holding
+  // c8 planes [planes kc, planes (kc + 1)) x `rows` rows at times t0 + row of utterance b
+  template <int BF16>
+  __device__ __forceinline__ void load_item(const HcArgs& p, const HcGeom& g, RingPos& r, uint8_t* smem, int nabuf,
+                                            int b, int t0, int nchunks, int planes, int rows) const {
+    const uint32_t abytes = (uint32_t)(planes * rows) * 16u;
+    for (int kc = 0; kc < nchunks; ++kc, r.next(nabuf)) {
+      if (r.wrapped) mbar_wait(a_empty(r.s), r.ph ^ 1u);
+      load_tile<BF16>(p, g, b, smem + r.s * abytes, planes * kc, planes, rows, t0, threadIdx.x - 32, HB_LOADERS);
+      fence_proxy_async();
+      mbar_arrive(a_full(r.s));
+    }
+  }
+};
+
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
+template <int MT, int NACC>
+__device__ __forceinline__ void fence_acc(float (&acc)[MT][NACC]) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
+}
+
+// Consumer side of the rings: one wgmma batch per weight stage, in stream order.  After each batch is issued, at most D
+// batches stay in flight, D - 1 when !deep (rings too small to leave a slot to fill next to the ones D batches hold).
+// w[] / a[]: the W slot and the A buffer (-1: none) that the batches in flight read, oldest first; a batch holds its A
+// buffer when it ran the last tap of the buffer's chunk.
+template <int D, int AMAX>
+struct Batches {
+  static_assert(D == 1 || D == 2, "one or two wgmma batches in flight");
+  const Rings<AMAX>& R;
+  const HcGeom& g;
+  const bool deep;
+  RingPos wr;   // W slot of the next weight stage
+  int w[D], a[D];
+
+  __device__ __forceinline__ Batches(const Rings<AMAX>& rings, const HcGeom& geom, bool deep_)
+      : R(rings), g(geom), deep(deep_) {
+#pragma unroll
+    for (int i = 0; i < D; ++i) w[i] = a[i] = -1;
+  }
+
+  __device__ __forceinline__ void release(int ws, int as) const {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) {
+      if (ws >= 0) mbar_arrive(R.w_empty(ws));
+      if (as >= 0) mbar_arrive(R.a_empty(as));
+    }
+  }
+
+  // acc (+)= the next weight stage x the operand at aBase (aRows rows per c8 plane) from row row0; the batch holds A
+  // buffer abuf (-1: none)
+  template <int NW, int BF16, int MT>
+  __device__ __forceinline__ void mma(float (&acc)[MT][NW / 2], uint32_t aBase, int aRows, int row0, int abuf,
+                                      bool& first) {
+    const int s = wr.s;
+    mbar_wait(R.w_full(s), wr.ph);
+    wr.next(g.nstages);
+    fence_acc(acc);
+    wg_fence();
+    mma_batch<NW, BF16>(acc, aBase, aRows, row0, R.sW + (uint32_t)s * g.stage_bytes, first);
+    wg_commit();
+    if constexpr (D == 2) {
+      if (deep) {
+        wg_wait<2>();   // the batch before the previous one has completed: its W slot (and A buffer) can be refilled
+        fence_acc(acc);
+        release(w[0], a[0]);
+        w[0] = w[1];
+        a[0] = a[1];
+      } else {
+        wg_wait<1>();
+        fence_acc(acc);
+        release(w[1], a[1]);
+      }
+      w[1] = s;
+      a[1] = abuf;
+    } else if (deep) {
+      wg_wait<1>();   // the previous batch has completed
+      fence_acc(acc);
+      release(w[0], a[0]);
+      w[0] = s;
+      a[0] = abuf;
+    } else {
+      wg_wait<0>();
+      fence_acc(acc);
+      release(s, abuf);
+    }
+    first = false;
+  }
+
+  // the ntaps taps of one 32-channel K chunk, tap j from row row0 + j tapstep; the last one holds A buffer abuf
+  template <int NW, int BF16, int MT>
+  __device__ __forceinline__ void chunk(float (&acc)[MT][NW / 2], uint32_t aBase, int aRows, int row0, int ntaps,
+                                        int tapstep, int abuf, bool& first) {
+    for (int j = 0; j < ntaps; ++j)
+      mma<NW, BF16>(acc, aBase, aRows, row0 + j * tapstep, j == ntaps - 1 ? abuf : -1, first);
+  }
+
+  // every batch has completed and released its slots
+  template <int MT, int NACC>
+  __device__ __forceinline__ void drain(float (&acc)[MT][NACC]) {
+    wg_wait<0>();
+    fence_acc(acc);
+#pragma unroll
+    for (int i = 0; i < D; ++i) {
+      release(w[i], a[i]);
+      w[i] = a[i] = -1;
+    }
+  }
+};
+
+// Block mode (launch_tc_chain): the work items are (utterance, time tile).  The A ring is a single buffer, the operand
+// tile X of all channels, which the loaders refill for the next tile once the consumers have finished their last MMA
+// on it.  Two wgmma batches in flight where the W ring leaves a slot to fill next to the two they hold.  The residual
+// stream x_p of the whole ResBlock stays in registers in the accumulator fragment layout.
+// The accumulation order of every output element is that of hconv_kernel's per-pair mode (K chunk -> tap -> k16).
 template <int NW, int BF16>
 __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-  const uint32_t sX = smem_u32(smem), sI = sX + g.off_i, sW = sX + g.off_w;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t sX = smem_u32(smem), sI = sX + g.off_i;
   float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
-  const uint32_t bar0 = smem_u32(smem + g.off_bar);
-  auto w_full = [&](int s) { return bar0 + 8u * s; };
-  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
-  const uint32_t x_full = bar0 + 16u * HC_STAGES_MAX, x_empty = x_full + 8u;
+  const Rings<1> R{smem_u32(smem + g.off_bar), sX + g.off_w};
   const int nwork = p.B * g.tiles;
   const int per_step = g.nkc * g.ntaps;
 
-  if (tid == 0) {
-    for (int s = 0; s < g.nstages; ++s) {
-      mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), 8);
-    }
-    mbar_init(x_full, HB_LOADERS);
-    mbar_init(x_empty, 8);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  if (tid == 0) R.init(g.nstages, 1);
   stage_biases(bias_s, p, g.nsteps, NW, tid, HB_THREADS);
   // rows and channels of the intermediate that no step writes stay zero for every tile
   for (int i = tid; i < g.nkc * 4 * g.rowsX; i += HB_THREADS)
@@ -450,86 +603,26 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
   __syncthreads();
 
   // ------------------------------------------------------------------------------------------------ producer
-  if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+  if (producer_warpgroup(wg)) {
+    RingPos r;
     if (tid == 0) {
-      RingPos r;
-      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        for (int st = 0; st < g.nsteps; ++st)
-          for (int i = 0; i < per_step; ++i, r.next(g.nstages)) {
-            if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
-            mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
-            bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(r.s));
-          }
-      }
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x)
+        for (int st = 0; st < g.nsteps; ++st) R.stream_weights(p, g, r, st, 0, per_step);
     } else if (tid >= 32) {
       // X <- lrelu(x, pre_slope) over all channels, rows [0, rowsX) at times O - H - G + row
-      int n = 0;
-      for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
-        const int b = w / g.tiles, t0 = (w - b * g.tiles) * g.V - g.H - g.G;
-        if (n > 0) mbar_wait(x_empty, (uint32_t)(n - 1) & 1u);
-        load_tile<BF16>(p, g, b, smem, 0, 4 * g.nkc, g.rowsX, t0, tid - 32, HB_LOADERS);
-        fence_proxy_async();
-        mbar_arrive(x_full);
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+        const int b = w / g.tiles;
+        R.load_item<BF16>(p, g, r, smem, 1, b, (w - b * g.tiles) * g.V - g.H - g.G, 1, 4 * g.nkc, g.rowsX);
       }
     }
     return;
   }
 
   // ------------------------------------------------------------------------------------------------ consumers
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
   const int cw = wg - 1;
   const Frag<MT> f(cw);
   float acc[MT][NACC];
-  RingPos wr;        // W slot of the next weight stage
-  // W slots read by the batches in flight, oldest first (-1: none).  Two batches stay in flight when the ring leaves a
-  // slot to fill next to the two they hold.
-  const bool deep = g.nstages >= 3;
-  int pw0 = -1, pw1 = -1;
-
-  // keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
-  auto fence_acc = [&]() {
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
-  };
-  auto release_w = [&](int pw) {
-    __syncwarp();
-    if (lane == 0 && pw >= 0) mbar_arrive(w_empty(pw));
-  };
-  // the taps of one 32-channel K chunk over the operand at aBase
-  auto mma_chunk = [&](uint32_t aBase, int ntaps, int tapstep, bool& first) {
-    for (int j = 0; j < ntaps; ++j) {
-      const int s = wr.s;
-      mbar_wait(w_full(s), wr.ph);
-      wr.next(g.nstages);
-      const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
-      fence_acc();
-      wg_fence();
-      mma_batch<NW, BF16>(acc, aBase, g.rowsX, cw * MT * 64 + j * tapstep, wS, first);
-      wg_commit();
-      if (deep) {
-        wg_wait<2>();    // the batch before the previous one has completed: its W slot can be refilled
-        fence_acc();
-        release_w(pw0);
-        pw0 = pw1;
-      } else {
-        wg_wait<1>();
-        fence_acc();
-        release_w(pw1);
-      }
-      pw1 = s;
-      first = false;
-    }
-  };
-  auto drain = [&]() {
-    wg_wait<0>();
-    fence_acc();
-    release_w(pw0);
-    release_w(pw1);
-    pw0 = pw1 = -1;
-  };
+  Batches<2, 1> batches(R, g, g.nstages >= 3);
 
   int n = 0;
   for (int w = blockIdx.x; w < nwork; w += gridDim.x, ++n) {
@@ -549,7 +642,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
             xr[mt][c * 4 + 2 * h + e] = (t >= 0 && t < g.Tin && co < p.Cout) ? __ldg(p.x + ((int64_t)b * p.Cout + co) * g.Tin + t) : 0.f;
           }
       }
-    mbar_wait(x_full, (uint32_t)n & 1u);
+    mbar_wait(R.a_full(0), (uint32_t)n & 1u);
     // lrelu(v [+ bb], mid_slope) of the fragment -> operand tile at off (rows offset by G)
     auto store_tile = [&](uint32_t off, const float (&v)[MT][NACC], const float* bb) {
       consumer_sync();   // both warpgroups have finished the MMAs that read the tile (ResBlock2 overwrites X)
@@ -562,8 +655,10 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
       const int d = cv == 0 ? g.dil[pr] : 1, hh = (g.ntaps - 1) * d / 2;
       const uint32_t aT = cv == 0 ? sX : sI;
       bool first = true;
-      for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.ntaps, d, first);
-      drain();
+      for (int kc = 0; kc < g.nkc; ++kc)
+        batches.chunk<NW, BF16>(acc, aT + (uint32_t)(kc * 4 * g.rowsX + g.G - hh) * 16u, g.rowsX, cw * MT * 64,
+                                g.ntaps, d, -1, first);
+      batches.drain(acc);
       const float* bb = bias_s + st * NW;
       if (g.nconv == 2 && cv == 0) {
         store_tile(g.off_i, acc, bb);
@@ -582,23 +677,19 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
       }
     }
     // every MMA of this tile has completed: the producer may load the next X
-    __syncwarp();
-    if (lane == 0) mbar_arrive(x_empty);
+    batches.release(-1, 0);
     // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V)
     epilogue_out<NW, BF16, EP_ACC_PREV>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
                                         [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
   }
 }
 
-// Pair mode (launch_tc_conv with a second conv; one ResBlock1 step): warp-specialised and persistent like
-// hchain_kernel, with the per-pair tile geometry of make_geom (output row r at time O + r, V = R - (k - 1)).
-//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams both convs' weight stages of every tile through the W
-//     ring; warps 1-3 stream the A operand in 32-channel K chunks through a ring of g.nabuf chunk buffers.  Conv2 reads
-//     only the intermediate tile, so the next tile's chunks load under this tile's conv2 and output epilogue.
-//   warpgroups 1-2 (consumers, setmaxnreg 232): two wgmma batches in flight (one where the rings are too small); a
-//     W slot, and an A buffer after its last tap, is released once the batch that read it has completed.  Below N = 256 each consumer loads the residual
-//     of its fragment into registers at the start of the tile, so that HBM read runs under the MMAs; the branch sum
-//     would need another 64 registers at N = 128 (ptxas spills) and is read in the epilogue.
+// Pair mode (launch_tc_conv with a second conv; one ResBlock1 step): the work items are (utterance, time tile), with
+// the per-pair tile geometry of make_geom (output row r at time O + r, V = R - (k - 1)).  The loaders stream the A
+// operand in 32-channel K chunks through g.nabuf buffers; conv2 reads only the intermediate tile, so the next tile's
+// chunks load under this tile's conv2 and output epilogue.  Below N = 256 each consumer loads the residual of its
+// fragment into registers at the start of the tile, so that HBM read runs under the MMAs; the branch sum would need
+// another 64 registers at N = 128 (ptxas spills) and is read in the epilogue.
 // Accumulation order (K chunk -> tap -> k16, conv1 then conv2) and epilogue association are those of the per-pair
 // arithmetic, so the tile shape does not enter any output element.
 template <int NW, int BF16>
@@ -608,29 +699,15 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
   constexpr bool PREFETCH = MT * NACC <= 64;   // 64 accumulators leave room for 64 prefetched residuals
   constexpr int PM = PREFETCH ? MT : 1, PN = PREFETCH ? NACC : 1;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-  const uint32_t sA = smem_u32(smem), sI = sA + g.off_i, sW = sA + g.off_w;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t sA = smem_u32(smem), sI = sA + g.off_i;
   const uint32_t abytes = (uint32_t)g.rowsA * 64u;   // one A chunk: 4 c8 planes x rowsA rows
   float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
-  const uint32_t bar0 = smem_u32(smem + g.off_bar);
-  auto w_full = [&](int s) { return bar0 + 8u * s; };
-  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
-  auto a_full = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + s); };
-  auto a_empty = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + HP_ABUF_MAX + s); };
+  const Rings<HP_ABUF_MAX> R{smem_u32(smem + g.off_bar), sA + g.off_w};
   const int nwork = p.B * g.tiles;
   const int per_step = g.nkc * g.ntaps;
 
-  if (tid == 0) {
-    for (int s = 0; s < g.nstages; ++s) {
-      mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), 8);
-    }
-    for (int s = 0; s < g.nabuf; ++s) {
-      mbar_init(a_full(s), HB_LOADERS);
-      mbar_init(a_empty(s), 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  if (tid == 0) R.init(g.nstages, g.nabuf);
   stage_biases(bias_s, p, 2, NW, tid, HB_THREADS);
   // rows and channels of the intermediate that store_frag_tile does not write stay zero for every tile
   for (int i = tid; i < g.nkc * 4 * g.rowsI; i += HB_THREADS)
@@ -639,96 +716,29 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
   __syncthreads();
 
   // ------------------------------------------------------------------------------------------------ producer
-  if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+  if (producer_warpgroup(wg)) {
+    RingPos r;
     if (tid == 0) {
-      RingPos r;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x)
-        for (int st = 0; st < 2; ++st)
-          for (int i = 0; i < per_step; ++i, r.next(g.nstages)) {
-            if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
-            mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
-            bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, st, i), g.stage_bytes, w_full(r.s));
-          }
+        for (int st = 0; st < 2; ++st) R.stream_weights(p, g, r, st, 0, per_step);
     } else if (tid >= 32) {
       // A chunk kc of a tile: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
-      int q = 0;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        const int b = w / g.tiles, t0 = (w - b * g.tiles) * g.V - g.a0;
-        for (int kc = 0; kc < g.nkc; ++kc, ++q) {
-          const int s = q % g.nabuf;
-          if (q >= g.nabuf) mbar_wait(a_empty(s), (uint32_t)(q / g.nabuf - 1) & 1u);
-          load_tile<BF16>(p, g, b, smem + s * abytes, 4 * kc, 4, g.rowsA, t0, tid - 32, HB_LOADERS);
-          fence_proxy_async();
-          mbar_arrive(a_full(s));
-        }
+        const int b = w / g.tiles;
+        R.load_item<BF16>(p, g, r, smem, g.nabuf, b, (w - b * g.tiles) * g.V - g.a0, g.nkc, 4, g.rowsA);
       }
     }
     return;
   }
 
   // ------------------------------------------------------------------------------------------------ consumers
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
   const int cw = wg - 1;
   float acc[MT][NACC];
-  RingPos wr;             // W slot of the next weight stage
-  int q = 0;              // A chunks consumed so far
-  // Batches in flight, oldest first: the W slot each read, and the A buffer whose last tap it was (-1: none).  Two
-  // stay in flight when the rings allow it: every W slot held by an in-flight batch must leave one to fill
+  RingPos ar;   // A buffer of the next chunk
+  // Two batches stay in flight when the rings allow it: every W slot held by an in-flight batch must leave one to fill
   // (nstages >= 3), and the loaders must not need the buffer of the last tap of the chunk before the previous one
   // (ntaps >= 2, or three buffers; one buffer is drained after every chunk).
-  const bool deep = g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2);
-  int pw0 = -1, pw1 = -1, pa0 = -1, pa1 = -1;
-
-  auto fence_acc = [&]() {
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
-  };
-  auto release = [&](int w, int a) {
-    __syncwarp();
-    if (lane == 0) {
-      if (w >= 0) mbar_arrive(w_empty(w));
-      if (a >= 0) mbar_arrive(a_empty(a));
-    }
-  };
-  // the taps of one 32-channel K chunk over the operand at aBase (aRows rows per c8 plane); abuf: the A buffer it
-  // reads, or -1 for the intermediate tile
-  auto mma_chunk = [&](uint32_t aBase, int aRows, int tapstep, int abuf, bool& first) {
-    for (int j = 0; j < g.ntaps; ++j) {
-      const int s = wr.s;
-      mbar_wait(w_full(s), wr.ph);
-      wr.next(g.nstages);
-      const uint32_t wS = sW + (uint32_t)s * g.stage_bytes;
-      fence_acc();
-      wg_fence();
-      mma_batch<NW, BF16>(acc, aBase, aRows, cw * MT * 64 + j * tapstep, wS, first);
-      wg_commit();
-      const int a = j == g.ntaps - 1 ? abuf : -1;
-      if (deep) {
-        wg_wait<2>();    // the batch before the previous one has completed: its W slot (and A buffer) can be refilled
-        fence_acc();
-        release(pw0, pa0);
-        pw0 = pw1;
-        pa0 = pa1;
-      } else {
-        wg_wait<1>();
-        fence_acc();
-        release(pw1, pa1);
-      }
-      pw1 = s;
-      pa1 = a;
-      first = false;
-    }
-  };
-  auto drain = [&]() {
-    wg_wait<0>();
-    fence_acc();
-    release(pw0, pa0);
-    release(pw1, pa1);
-    pw0 = pw1 = pa0 = pa1 = -1;
-  };
+  Batches<2, HP_ABUF_MAX> batches(R, g, g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2));
 
   for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
     const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
@@ -754,13 +764,14 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
     }
     // conv1 over the A chunks
     bool first = true;
-    for (int kc = 0; kc < g.nkc; ++kc, ++q) {
-      const int s = q % g.nabuf;
-      mbar_wait(a_full(s), (uint32_t)(q / g.nabuf) & 1u);
-      mma_chunk(sA + (uint32_t)s * abytes, g.rowsA, g.d, s, first);
-      if (g.nabuf == 1) drain();   // the loaders refill the only buffer with the next chunk
+    for (int kc = 0; kc < g.nkc; ++kc) {
+      const int abuf = ar.s;
+      mbar_wait(R.a_full(abuf), ar.ph);
+      ar.next(g.nabuf);
+      batches.chunk<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64, g.ntaps, g.d, abuf, first);
+      if (g.nabuf == 1) batches.drain(acc);   // the loaders refill the only buffer with the next chunk
     }
-    drain();
+    batches.drain(acc);
     // intermediate = lrelu(conv1 + b1, mid_slope) -> operand tile, row 0 at time O - h2, zero outside [0, T)
     consumer_sync();   // both warpgroups have finished the previous tile's conv2, which read the intermediate
     store_frag_tile<NW, BF16>(smem + g.off_i, acc, bias_s, Frag<MT>(cw), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc,
@@ -768,8 +779,9 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
     fence_proxy_async();
     consumer_sync();
     first = true;
-    for (int kc = 0; kc < g.nkc; ++kc) mma_chunk(sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, 1, -1, first);
-    drain();
+    for (int kc = 0; kc < g.nkc; ++kc)
+      batches.chunk<NW, BF16>(acc, sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, cw * MT * 64, g.ntaps, 1, -1, first);
+    batches.drain(acc);
     // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
     const Frag<MT> f(cw);
     const float* b2 = bias_s + NW;
@@ -981,316 +993,134 @@ __device__ __forceinline__ void epilogue_convt(const HcArgs& p, const HcGeom& g,
   }
 }
 
-// ConvTranspose1d from an operand image (launch_tc_conv mode 1 with ximg): warp-specialised and persistent like
-// hpair_kernel.  A work item is
-// (utterance, time tile, N block) with the N block fastest, so the NB items of a tile run at once on different SMs
-// and read their A chunks from L2.
-//   warpgroup 0 (producer, setmaxnreg 40): thread 0 streams the weight stages of every item through the W ring;
-//     warps 1-3 stream the item's A chunks of the operand image through g.nabuf buffers.
-//   warpgroups 1-2 (consumers, setmaxnreg 232): two wgmma batches in flight where the rings allow it; a W slot, and an
-//     A buffer after its last tap, is released once the batch that read it has completed, so the next item's chunks
-//     and stages load under this item's epilogue_convt.
+// Epilogues of Vocos' pointwise (1x1) GEMM D[t, n] = sum_ci A[t, ci] W[n, ci] (launch_tc_pointwise) on hitem_kernel,
+// output channels co0 + column at time O + row:
+//   PW_GELU:     yimg = cvt(gelu(acc + b))                           (pwconv1 + nn.GELU(), exact erf)
+//   PW_GAMMA:    y = y + gamma * (acc + b), fp32 in place            (pwconv2, layer scale and residual, vocos.py:509-527)
+//   PW_SPECTRUM: columns 2j, 2j + 1 hold bin j's log-magnitude and phase (launch_tc_pack_head_weight):
+//                spec[b T + t][j] = min(exp(m), 1e2) (cos p, sin p)  (ISTFTHead, vocos.py:343-361)
+// ITEM_CONVT selects hitem_kernel's ConvTranspose epilogue, epilogue_convt.
+enum ItemEpi : int { PW_GELU = AB_PW_GELU, PW_GAMMA = AB_PW_GAMMA_RESIDUAL, PW_SPECTRUM = AB_PW_SPECTRUM, ITEM_CONVT };
+struct PwArgs {
+  const float* gamma;   // PW_GAMMA: [C_out]
+  float2* spec;         // PW_SPECTRUM: [B*T][C_out / 2]
+};
+
+template <int NW, int BF16, int EPI, int MT>
+__device__ __forceinline__ void epilogue_pw(const HcArgs& p, const HcGeom& g, const PwArgs& e, const Frag<MT>& f,
+                                            const float (&acc)[MT][NW / 2], const float* bias_s, int b, int O, int co0) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int t = O + f.row(mt, h);
+      if (t >= g.Tout) continue;
+#pragma unroll
+      for (int c = 0; c < NW / 8; ++c) {
+        const int co = co0 + c * 8 + f.col;
+        const float a0 = acc[mt][c * 4 + 2 * h], a1 = acc[mt][c * 4 + 2 * h + 1];
+        if constexpr (EPI == PW_GELU) {
+          if ((co >> 3) >= g.c8n_out) continue;
+          float v[2] = {a0 + bias_s[co], a1 + bias_s[co + 1]};
+#pragma unroll
+          for (int q = 0; q < 2; ++q) v[q] = co + q < p.Cout ? 0.5f * v[q] * (1.0f + erff(v[q] * 0.70710678118654752440f)) : 0.f;
+          *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
+              pack2t<BF16>(v[0], v[1]);
+        } else if constexpr (EPI == PW_GAMMA) {
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            if (co + q >= p.Cout) continue;
+            const float v = (q ? a1 : a0) + bias_s[co + q];
+            float* y = p.y + ((int64_t)b * p.Cout + co + q) * g.Tout + t;
+            *y = __fadd_rn(*y, __fmul_rn(__ldg(e.gamma + co + q), v));
+          }
+        } else {
+          static_assert(EPI == PW_SPECTRUM, "pointwise epilogue");
+          const int bins = p.Cout >> 1, j = co >> 1;
+          if (j >= bins) continue;
+          float amp = expf(a0 + bias_s[j]);
+          amp = fminf(amp, 1e2f);
+          float sn, cs;
+          sincosf(a1 + bias_s[bins + j], &sn, &cs);
+          e.spec[((int64_t)b * g.Tout + t) * bins + j] = make_float2(amp * cs, amp * sn);
+        }
+      }
+    }
+}
+
+// The (utterance, time tile, N block) walk over an operand image: ConvTranspose1d from an image (launch_tc_conv mode 1
+// with ximg, EPI = ITEM_CONVT) and Vocos' pointwise GEMM (EPI = PW_*; one tap, K = C_in and N = C_out unbounded).  The
+// N block is fastest, so the NB items of a tile run at once on different SMs and read their A chunks from L2.  An item
+// streams its A chunks through g.nabuf buffers and its N block's (K chunk, tap) weight stages.  The ConvTranspose
+// keeps two wgmma batches in flight where the rings allow it (hpair_kernel's condition); the GEMM keeps one where both
+// rings leave a slot to fill next to it, none otherwise.
 // Accumulation order: K chunk -> tap m in the reversed row shift ntaps - 1 - m -> k16, then the bias.
-template <int NW, int BF16>
-__global__ void __launch_bounds__(HB_THREADS, 1) hconvt_kernel(HcArgs p, HcGeom g) {
+template <int NW, int BF16, int EPI>
+__global__ void __launch_bounds__(HB_THREADS, 1) hitem_kernel(HcArgs p, HcGeom g, PwArgs e) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
+  constexpr bool CONVT = EPI == ITEM_CONVT;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-  const uint32_t sA = smem_u32(smem), sW = sA + g.off_w;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t sA = smem_u32(smem);
   const uint32_t abytes = (uint32_t)g.rowsA * 64u;   // one A chunk: 4 c8 planes x rowsA rows
   float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
-  const uint32_t bar0 = smem_u32(smem + g.off_bar);
-  auto w_full = [&](int s) { return bar0 + 8u * s; };
-  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
-  auto a_full = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + s); };
-  auto a_empty = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + HP_ABUF_MAX + s); };
+  const Rings<HP_ABUF_MAX> R{smem_u32(smem + g.off_bar), sA + g.off_w};
   const int nwork = p.B * g.tiles * g.NB;
-  const int per_nb = g.nkc * g.ntaps;
+  const int ntaps = CONVT ? g.ntaps : 1;   // compile time for the GEMM: no tap loop in its chunk loop
+  const int per_nb = g.nkc * ntaps;
 
-  if (tid == 0) {
-    for (int s = 0; s < g.nstages; ++s) {
-      mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), 8);
-    }
-    for (int s = 0; s < g.nabuf; ++s) {
-      mbar_init(a_full(s), HB_LOADERS);
-      mbar_init(a_empty(s), 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  if (tid == 0) R.init(g.nstages, g.nabuf);
   stage_biases(bias_s, p, 1, g.NB * g.cc, tid, HB_THREADS);
   __syncthreads();
 
   // ------------------------------------------------------------------------------------------------ producer
-  if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
+  if (producer_warpgroup(wg)) {
+    RingPos r;
     if (tid == 0) {
-      RingPos r;
-      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        const int i0 = (w % g.NB) * per_nb;
-        for (int i = 0; i < per_nb; ++i, r.next(g.nstages)) {
-          if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
-          mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
-          bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, 0, i0 + i), g.stage_bytes, w_full(r.s));
-        }
-      }
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x) R.stream_weights(p, g, r, 0, (w % g.NB) * per_nb, per_nb);
     } else if (tid >= 32) {
       // A chunk kc of an item: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
-      RingPos r;
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        const int bt = w / g.NB, b = bt / g.tiles, t0 = (bt - b * g.tiles) * g.V - g.a0;
-        for (int kc = 0; kc < g.nkc; ++kc, r.next(g.nabuf)) {
-          if (r.wrapped) mbar_wait(a_empty(r.s), r.ph ^ 1u);
-          load_tile<BF16>(p, g, b, smem + r.s * abytes, 4 * kc, 4, g.rowsA, t0, tid - 32, HB_LOADERS);
-          fence_proxy_async();
-          mbar_arrive(a_full(r.s));
-        }
+        const int bt = w / g.NB, b = bt / g.tiles;
+        R.load_item<BF16>(p, g, r, smem, g.nabuf, b, (bt - b * g.tiles) * g.V - g.a0, g.nkc, 4, g.rowsA);
       }
     }
     return;
   }
 
   // ------------------------------------------------------------------------------------------------ consumers
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
   const int cw = wg - 1;
   float acc[MT][NACC];
-  RingPos wr, ar;   // W slot of the next weight stage, A buffer of the next chunk
-  // batches in flight, oldest first: the W slot each read and the A buffer whose last tap it was (-1: none); the
-  // condition for two in flight is hpair_kernel's
-  const bool deep = g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2);
-  int pw0 = -1, pw1 = -1, pa0 = -1, pa1 = -1;
-
-  auto fence_acc = [&]() {
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
-  };
-  auto release = [&](int w, int a) {
-    __syncwarp();
-    if (lane == 0) {
-      if (w >= 0) mbar_arrive(w_empty(w));
-      if (a >= 0) mbar_arrive(a_empty(a));
-    }
-  };
-  auto drain = [&]() {
-    wg_wait<0>();
-    fence_acc();
-    release(pw0, pa0);
-    release(pw1, pa1);
-    pw0 = pw1 = pa0 = pa1 = -1;
-  };
+  RingPos ar;   // A buffer of the next chunk
+  Batches<CONVT ? 2 : 1, HP_ABUF_MAX> batches(
+      R, g, CONVT ? g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2) : g.nstages >= 3 && g.nabuf >= 3);
 
   for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
     const int bt = w / g.NB, nb = w - bt * g.NB, b = bt / g.tiles, O = (bt - b * g.tiles) * g.V;
     bool first = true;
     for (int kc = 0; kc < g.nkc; ++kc) {
       const int abuf = ar.s;
-      mbar_wait(a_full(abuf), ar.ph);
+      mbar_wait(R.a_full(abuf), ar.ph);
       ar.next(g.nabuf);
-      const uint32_t aBase = sA + (uint32_t)abuf * abytes;
-      for (int j = 0; j < g.ntaps; ++j) {
-        const int s = wr.s;
-        mbar_wait(w_full(s), wr.ph);
-        wr.next(g.nstages);
-        fence_acc();
-        wg_fence();
-        mma_batch<NW, BF16>(acc, aBase, g.rowsA, cw * MT * 64 + (g.ntaps - 1 - j), sW + (uint32_t)s * g.stage_bytes, first);
-        wg_commit();
-        const int a = j == g.ntaps - 1 ? abuf : -1;
-        if (deep) {
-          wg_wait<2>();   // the batch before the previous one has completed: its W slot (and A buffer) can be refilled
-          fence_acc();
-          release(pw0, pa0);
-          pw0 = pw1;
-          pa0 = pa1;
-        } else {
-          wg_wait<1>();
-          fence_acc();
-          release(pw1, pa1);
-        }
-        pw1 = s;
-        pa1 = a;
-        first = false;
-      }
-      if (g.nabuf == 1) drain();   // the loaders refill the only buffer with the next chunk
+      batches.chunk<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64 + ntaps - 1, ntaps, -1, abuf,
+                              first);
+      // the loaders refill the only buffer with the next chunk; the GEMM, never deep with one buffer, has released it
+      if (CONVT && g.nabuf == 1) batches.drain(acc);
     }
-    drain();
+    batches.drain(acc);
     const Frag<MT> f(cw);
     const int co0 = nb * g.cc;
-    switch (g.pad & 1 ? (g.u == 2 ? 2 : 0) : g.u) {
-      case 8: epilogue_convt<NW, BF16, 8>(p, g, f, acc, bias_s, b, O, co0); break;
-      case 4: epilogue_convt<NW, BF16, 4>(p, g, f, acc, bias_s, b, O, co0); break;
-      case 2: epilogue_convt<NW, BF16, 2>(p, g, f, acc, bias_s, b, O, co0); break;
-      default: epilogue_convt<NW, BF16, 0>(p, g, f, acc, bias_s, b, O, co0); break;
-    }
-  }
-}
-
-// Pointwise (1x1) GEMM of Vocos' ConvNeXt blocks and iSTFT head (launch_tc_pointwise): D[t, n] = sum_ci A[t, ci] W[n, ci]
-// from the operand image of the input, K = C_in and N = C_out unbounded.  Same persistent warp-specialised schedule as
-// hconvt_kernel with a single tap: work items (utterance, time tile, N block), the N block fastest, so the NB items of
-// a tile share its A chunks through L2.  Epilogues (compile time, PwEpi):
-//   PW_GELU:     yimg = cvt(gelu(acc + b))                           (pwconv1 + nn.GELU(), exact erf)
-//   PW_GAMMA:    y = y + gamma * (acc + b), fp32 in place            (pwconv2, layer scale and residual, vocos.py:509-527)
-//   PW_SPECTRUM: columns 2j, 2j + 1 hold bin j's log-magnitude and phase (launch_tc_pack_head_weight):
-//                spec[b T + t][j] = min(exp(m), 1e2) (cos p, sin p)  (ISTFTHead, vocos.py:343-361)
-enum PwEpi : int { PW_GELU = AB_PW_GELU, PW_GAMMA = AB_PW_GAMMA_RESIDUAL, PW_SPECTRUM = AB_PW_SPECTRUM };
-struct PwArgs {
-  const float* gamma;   // PW_GAMMA: [C_out]
-  float2* spec;         // PW_SPECTRUM: [B*T][C_out / 2]
-};
-
-template <int NW, int BF16, int EPI>
-__global__ void __launch_bounds__(HB_THREADS, 1) hpw_kernel(HcArgs p, HcGeom g, PwArgs e) {
-  constexpr int MT = mt_of(NW);
-  constexpr int NACC = NW / 2;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-  const uint32_t sA = smem_u32(smem), sW = sA + g.off_w;
-  const uint32_t abytes = (uint32_t)g.rowsA * 64u;   // one A chunk: 4 c8 planes x rowsA rows
-  float* bias_s = reinterpret_cast<float*>(smem + g.off_bias);
-  const uint32_t bar0 = smem_u32(smem + g.off_bar);
-  auto w_full = [&](int s) { return bar0 + 8u * s; };
-  auto w_empty = [&](int s) { return bar0 + 8u * (HC_STAGES_MAX + s); };
-  auto a_full = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + s); };
-  auto a_empty = [&](int s) { return bar0 + 8u * (2 * HC_STAGES_MAX + HP_ABUF_MAX + s); };
-  const int nwork = p.B * g.tiles * g.NB;
-
-  if (tid == 0) {
-    for (int s = 0; s < g.nstages; ++s) {
-      mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), 8);
-    }
-    for (int s = 0; s < g.nabuf; ++s) {
-      mbar_init(a_full(s), HB_LOADERS);
-      mbar_init(a_empty(s), 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  stage_biases(bias_s, p, 1, g.NB * NW, tid, HB_THREADS);
-  __syncthreads();
-
-  // ------------------------------------------------------------------------------------------------ producer
-  if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HB_PRODUCER_REGS));
-    if (tid == 0) {
-      RingPos r;
-      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        const int i0 = (w % g.NB) * g.nkc;
-        for (int i = 0; i < g.nkc; ++i, r.next(g.nstages)) {
-          if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
-          mbar_arrive_expect_tx(w_full(r.s), g.stage_bytes);
-          bulk_g2s(sW + (uint32_t)r.s * g.stage_bytes, weight_stage(p, g, 0, i0 + i), g.stage_bytes, w_full(r.s));
-        }
+    if constexpr (CONVT) {
+      switch (g.pad & 1 ? (g.u == 2 ? 2 : 0) : g.u) {
+        case 8: epilogue_convt<NW, BF16, 8>(p, g, f, acc, bias_s, b, O, co0); break;
+        case 4: epilogue_convt<NW, BF16, 4>(p, g, f, acc, bias_s, b, O, co0); break;
+        case 2: epilogue_convt<NW, BF16, 2>(p, g, f, acc, bias_s, b, O, co0); break;
+        default: epilogue_convt<NW, BF16, 0>(p, g, f, acc, bias_s, b, O, co0); break;
       }
-    } else if (tid >= 32) {
-      RingPos r;
-      for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-        const int bt = w / g.NB, b = bt / g.tiles, t0 = (bt - b * g.tiles) * g.V;
-        for (int kc = 0; kc < g.nkc; ++kc, r.next(g.nabuf)) {
-          if (r.wrapped) mbar_wait(a_empty(r.s), r.ph ^ 1u);
-          load_tile<BF16>(p, g, b, smem + r.s * abytes, 4 * kc, 4, g.rowsA, t0, tid - 32, HB_LOADERS);
-          fence_proxy_async();
-          mbar_arrive(a_full(r.s));
-        }
-      }
+    } else {
+      epilogue_pw<NW, BF16, EPI>(p, g, e, f, acc, bias_s, b, O, co0);
     }
-    return;
-  }
-
-  // ------------------------------------------------------------------------------------------------ consumers
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HB_CONSUMER_REGS));
-  const int cw = wg - 1;
-  float acc[MT][NACC];
-  RingPos wr, ar;
-  // two batches in flight when both rings leave a slot to fill next to the two they hold
-  const bool deep = g.nstages >= 3 && g.nabuf >= 3;
-  int pw1 = -1;   // (W slot << 8) | A buffer of the batch in flight, -1: none
-
-  auto fence_acc = [&]() {
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
-  };
-  auto release = [&](int s) {   // W slot s and the A buffer of the same chunk (one tap: the rings advance together)
-    __syncwarp();
-    if (lane == 0 && s >= 0) {
-      mbar_arrive(w_empty(s >> 8));
-      mbar_arrive(a_empty(s & 255));
-    }
-  };
-
-  for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-    const int bt = w / g.NB, nb = w - bt * g.NB, b = bt / g.tiles, O = (bt - b * g.tiles) * g.V;
-    bool first = true;
-    for (int kc = 0; kc < g.nkc; ++kc) {
-      const int abuf = ar.s, s = wr.s;
-      mbar_wait(a_full(abuf), ar.ph);
-      mbar_wait(w_full(s), wr.ph);
-      ar.next(g.nabuf);
-      wr.next(g.nstages);
-      fence_acc();
-      wg_fence();
-      mma_batch<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64, sW + (uint32_t)s * g.stage_bytes, first);
-      wg_commit();
-      if (deep) {
-        wg_wait<1>();   // the previous batch has completed: its W slot and A buffer can be refilled
-        fence_acc();
-        release(pw1);
-      } else {
-        wg_wait<0>();
-        fence_acc();
-        release((s << 8) | abuf);
-      }
-      pw1 = (s << 8) | abuf;
-      first = false;
-    }
-    wg_wait<0>();
-    fence_acc();
-    if (deep) release(pw1);
-    pw1 = -1;
-
-    const Frag<MT> f(cw);
-    const int co0 = nb * NW;
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int t = O + f.row(mt, h);
-        if (t >= g.Tout) continue;
-#pragma unroll
-        for (int c = 0; c < NW / 8; ++c) {
-          const int co = co0 + c * 8 + f.col;
-          const float a0 = acc[mt][c * 4 + 2 * h], a1 = acc[mt][c * 4 + 2 * h + 1];
-          if constexpr (EPI == PW_GELU) {
-            if ((co >> 3) >= g.c8n_out) continue;
-            float v[2] = {a0 + bias_s[co], a1 + bias_s[co + 1]};
-#pragma unroll
-            for (int q = 0; q < 2; ++q) v[q] = co + q < p.Cout ? 0.5f * v[q] * (1.0f + erff(v[q] * 0.70710678118654752440f)) : 0.f;
-            *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
-                pack2t<BF16>(v[0], v[1]);
-          } else if constexpr (EPI == PW_GAMMA) {
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-              if (co + q >= p.Cout) continue;
-              const float v = (q ? a1 : a0) + bias_s[co + q];
-              float* y = p.y + ((int64_t)b * p.Cout + co + q) * g.Tout + t;
-              *y = __fadd_rn(*y, __fmul_rn(__ldg(e.gamma + co + q), v));
-            }
-          } else {
-            const int bins = p.Cout >> 1, j = co >> 1;
-            if (j >= bins) continue;
-            float amp = expf(a0 + bias_s[j]);
-            amp = fminf(amp, 1e2f);
-            float sn, cs;
-            sincosf(a1 + bias_s[bins + j], &sn, &cs);
-            e.spec[((int64_t)b * g.Tout + t) * bins + j] = make_float2(amp * cs, amp * sn);
-          }
-        }
-      }
   }
 }
 
@@ -1402,8 +1232,9 @@ bool layout_smem(HcGeom& g, uint32_t abytes, uint32_t ibytes, uint32_t nbias, ui
 }
 
 // Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.  mode 1: padding
-// pad (-1: (k - u) / 2), Tin * u outputs.
-int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg, HcGeom& g, int pad = -1) {
+// pad (-1: (k - u) / 2), Tin * u outputs.  persistent: for hpair_kernel or hitem_kernel (one CTA per SM, as many A
+// chunk buffers as fit next to two W stages) rather than hconv_kernel.
+int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool persistent, HcGeom& g, int pad = -1) {
   HcLayer L;
   int rc = layer_geom(mode == 2 ? 0 : mode, cin, cout, k, d_or_u, L);
   if (rc != AB_OK) return rc;
@@ -1452,12 +1283,11 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg
   g.stage_bytes = 64u * (uint32_t)L.NW;
   const uint32_t abytes = (uint32_t)g.rowsA * 64u, nbias = (uint32_t)(g.nsteps * g.NB * L.NW);
   bool fits;
-  if (mode == 2 || (mode == 1 && ximg)) {   // hpair_kernel, hconvt_kernel: one CTA per SM, as many A chunk buffers as
-                                            // fit next to two W stages
+  if (persistent) {
     const uint32_t ibytes = (uint32_t)g.nkc * 64u * (uint32_t)g.rowsI;
     g.nabuf = HP_ABUF_MAX;
-    while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, ibytes, nbias,
-                                16u * (HC_STAGES_MAX + HP_ABUF_MAX), HC_SMEM_1CTA)) && g.nabuf > 1)
+    while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, ibytes, nbias, Rings<HP_ABUF_MAX>::BAR_BYTES,
+                                HC_SMEM_1CTA)) && g.nabuf > 1)
       --g.nabuf;
   } else {
     g.nabuf = 1;
@@ -1469,13 +1299,14 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool ximg
   return AB_OK;
 }
 
-// Launches K after raising its dynamic shared-memory limit to `limit`, once per device.
-template <void (*K)(HcArgs, HcGeom)>
-int launch_kernel(const char* name, unsigned grid, int threads, uint32_t limit, const HcArgs& a, const HcGeom& g,
-                  cudaStream_t s) {
+// Launches K<<<grid, threads, smem, s>>>(args...) after raising its dynamic shared-memory limit to `limit`, once per
+// device and instantiation.
+template <auto K, class... Args>
+int launch_kernel(const char* name, unsigned grid, int threads, uint32_t limit, uint32_t smem, cudaStream_t s,
+                  const Args&... args) {
   static DeviceOnce configured;
   if (configured.need()) AB_CUDA_TRY(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
-  K<<<grid, threads, g.smem_bytes, s>>>(a, g);
+  K<<<grid, threads, smem, s>>>(args...);
   AB_LAUNCH_CHECK(name);
   return AB_OK;
 }
@@ -1525,8 +1356,8 @@ int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, 
   g.c8n_in = g.c8n_out = rup(C, 16) / 8;
   g.stage_bytes = 64u * (uint32_t)L.NW;
   const uint32_t xbytes = (uint32_t)g.nkc * 64u * (uint32_t)g.rowsX;   // X and the intermediate tile
-  // mbarriers: W ring full / empty, X full / empty
-  if (!layout_smem(g, xbytes, xbytes, (uint32_t)(g.nsteps * L.NW), 16u * HC_STAGES_MAX + 16u, HC_SMEM_1CTA))
+  // X is the A ring's only buffer
+  if (!layout_smem(g, xbytes, xbytes, (uint32_t)(g.nsteps * L.NW), Rings<1>::BAR_BYTES, HC_SMEM_1CTA))
     return fail(AB_ERR_UNSUPPORTED, "tc block: does not fit shared memory");
   g.out_scale = 1.0f;
   g.mid_slope = 1.0f;
@@ -1543,39 +1374,44 @@ int persistent_grid(int64_t work, const char* what, unsigned& grid) {
   return AB_OK;
 }
 
+// One CTA of HB_THREADS per SM over `work` items: kernel(IntC<NW>(), IntC<BF16>()) names the instantiation for g's N
+// width and the precision.
+template <class Kernel, class... Args>
+int launch_persistent(const char* name, const char* what, int64_t work, const HcGeom& g, int precision, cudaStream_t s,
+                      Kernel kernel, const Args&... args) {
+  unsigned grid = 0;
+  const int rc = persistent_grid(work, what, grid);
+  if (rc != AB_OK) return rc;
+  return with_nw(g, precision, [&](auto nw, auto bf16) {
+    constexpr auto K = kernel(nw, bf16);
+    return launch_kernel<K>(name, grid, HB_THREADS, HC_SMEM_1CTA, g.smem_bytes, s, args...);
+  });
+}
+
 // conv and conv-transpose from fp32 input on hconv_kernel (one CTA per tile); conv-transpose from an operand image
-// on the persistent hconvt_kernel, pair mode on the persistent hpair_kernel.  From fp32 input, hconvt_kernel's 96 loader
+// on the persistent hitem_kernel, pair mode on the persistent hpair_kernel.  From fp32 input, hitem_kernel's 96 loader
 // threads (8 scattered loads in flight each) cannot keep up with the MMAs and it is slower than hconv_kernel, whose
 // 256 threads all load.
 int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s, bool reflect = false) {
   if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
   const int64_t work = (int64_t)a.B * g.tiles;
-  if (g.mode == 1 && a.ximg) {
-    unsigned grid = 0;
-    const int rc = persistent_grid(work * g.NB, "tc conv-transpose", grid);
-    if (rc != AB_OK) return rc;
-    return with_nw(g, precision, [&](auto nw, auto bf16) {
-      return launch_kernel<hconvt_kernel<decltype(nw)::value, decltype(bf16)::value>>("hconvt_kernel", grid, HB_THREADS,
-                                                                                      HC_SMEM_1CTA, a, g, s);
-    });
-  }
-  if (g.mode == 2) {
-    unsigned grid = 0;
-    const int rc = persistent_grid(work, "tc conv pair", grid);
-    if (rc != AB_OK) return rc;
-    return with_nw(g, precision, [&](auto nw, auto bf16) {
-      return launch_kernel<hpair_kernel<decltype(nw)::value, decltype(bf16)::value>>("hpair_kernel", grid, HB_THREADS,
-                                                                                     HC_SMEM_1CTA, a, g, s);
-    });
-  }
+  if (g.mode == 1 && a.ximg)
+    return launch_persistent("hitem_kernel", "tc conv-transpose", work * g.NB, g, precision, s, [](auto nw, auto bf16) {
+      return hitem_kernel<decltype(nw)::value, decltype(bf16)::value, ITEM_CONVT>;
+    }, a, g, PwArgs{});
+  if (g.mode == 2)
+    return launch_persistent("hpair_kernel", "tc conv pair", work, g, precision, s, [](auto nw, auto bf16) {
+      return hpair_kernel<decltype(nw)::value, decltype(bf16)::value>;
+    }, a, g);
   if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
   return with_nw(g, precision, [&](auto nw, auto bf16) {
     constexpr int NW = decltype(nw)::value;
+    constexpr uint32_t limit = NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA;
     if (reflect)
-      return launch_kernel<hconv_kernel<NW, decltype(bf16)::value, 1>>("hconv_kernel", (unsigned)work, HC_THREADS,
-                                                                        NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
-    return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)work, HC_THREADS,
-                                                                   NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA, a, g, s);
+      return launch_kernel<hconv_kernel<NW, decltype(bf16)::value, 1>>("hconv_kernel", (unsigned)work, HC_THREADS, limit,
+                                                                        g.smem_bytes, s, a, g);
+    return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)work, HC_THREADS, limit,
+                                                                   g.smem_bytes, s, a, g);
   });
 }
 
@@ -1612,17 +1448,10 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s) {
     a.bs[i] = p.bias[i];
   }
   a.y = p.y; a.acc_prev = p.acc_prev; a.yimg = p.yimg; a.img_slope = p.img_slope;
-  unsigned grid = 0;
-  rc = persistent_grid((int64_t)a.B * g.tiles, "tc block", grid);
-  if (rc != AB_OK) return rc;
-  return with_nw(g, p.precision, [&](auto nw, auto bf16) {
-    constexpr int NW = decltype(nw)::value;
-    if constexpr (NW > AB_TC_CHAIN_MAX_C)   // make_chain_geom rejects wider blocks
-      return fail(AB_ERR_UNSUPPORTED, "tc block: N block %d", NW);
-    else
-      return launch_kernel<hchain_kernel<NW, decltype(bf16)::value>>("hchain_kernel", grid, HB_THREADS, HC_SMEM_1CTA, a,
-                                                                      g, s);
-  });
+  // make_chain_geom rejects N blocks wider than AB_TC_CHAIN_MAX_C: the clamp only keeps them from being compiled
+  return launch_persistent("hchain_kernel", "tc block", (int64_t)a.B * g.tiles, g, p.precision, s, [](auto nw, auto bf16) {
+    return hchain_kernel<std::min(decltype(nw)::value, AB_TC_CHAIN_MAX_C), decltype(bf16)::value>;
+  }, a, g);
 }
 
 bool tc_conv_supported(int C, int k) { return C > 0 && C <= TC_MAX_C && (k & 1) && k <= 31; }
@@ -1673,7 +1502,9 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   if (p.reflect && (p.mode != 0 || pair))
     return fail(AB_ERR_UNSUPPORTED, "tc conv: reflection padding belongs to a single conv (mode 0)");
   HcGeom g;
-  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, p.ximg != nullptr, g, p.pad);
+  // pairs and ConvTranspose layers from an operand image run on the persistent kernels (launch_hconv)
+  const bool persistent = pair || (p.mode == 1 && p.ximg);
+  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, persistent, g, p.pad);
   if (rc != AB_OK) return rc;
   if (p.reflect && g.a0 >= p.T)
     return fail(AB_ERR_ARG, "tc conv: reflection padding %d needs more than %d samples", g.a0, p.T);
@@ -1687,21 +1518,6 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   return launch_hconv(a, g, p.precision, s, p.reflect != 0);
 }
 
-
-// Pointwise GEMM geometry: make_geom's k = 1 conv tiles, laid out for one persistent CTA per SM with as many A chunk
-// buffers as fit next to the W ring.
-static int make_pw_geom(int cin, int cout, int T, HcGeom& g) {
-  int rc = make_geom(0, cin, cout, 1, 1, T, true, g);
-  if (rc != AB_OK) return rc;
-  const uint32_t abytes = (uint32_t)g.rowsA * 64u, nbias = (uint32_t)g.NB * (g.stage_bytes / 64u);
-  bool fits;
-  g.nabuf = HP_ABUF_MAX;
-  while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, 0, nbias, 16u * (HC_STAGES_MAX + HP_ABUF_MAX), HC_SMEM_1CTA)) &&
-         g.nabuf > 1)
-    --g.nabuf;
-  if (!fits) return fail(AB_ERR_UNSUPPORTED, "tc pointwise: C_out=%d does not fit shared memory", cout);
-  return AB_OK;
-}
 
 int launch_tc_pack_head_weight(const float* w_t, void* image, int cin, int cout, int precision, cudaStream_t s) {
   HcLayer L;
@@ -1724,7 +1540,7 @@ int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s) {
       (p.epilogue == AB_PW_SPECTRUM && (!p.spec || (p.Cout & 1))))
     return fail(AB_ERR_ARG, "tc pointwise: epilogue %d: missing output or odd C_out", p.epilogue);
   HcGeom g;
-  int rc = make_pw_geom(p.Cin, p.Cout, p.T, g);
+  int rc = make_geom(0, p.Cin, p.Cout, 1, 1, p.T, true, g);   // k = 1 conv tiles
   if (rc != AB_OK) return rc;
   HcArgs a = base_args(nullptr, 0, 0, 0, p.ximg, 1.0f, p.B, p.Cin, p.Cout);
   a.ws[0] = p.w; a.bs[0] = p.bias;
@@ -1732,26 +1548,18 @@ int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s) {
   PwArgs e;
   e.gamma = p.gamma;
   e.spec = reinterpret_cast<float2*>(p.spec);
-  unsigned grid = 0;
-  rc = persistent_grid((int64_t)p.B * g.tiles * g.NB, "tc pointwise", grid);
-  if (rc != AB_OK) return rc;
-  return with_nw(g, p.precision, [&](auto nw, auto bf16) -> int {
-    constexpr int NW = decltype(nw)::value, BF = decltype(bf16)::value;
-    auto go = [&](auto kern) -> int {
-      static DeviceOnce configured[3];
-      if (configured[p.epilogue].need())
-        AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HC_SMEM_1CTA));
-      kern<<<grid, HB_THREADS, g.smem_bytes, s>>>(a, g, e);
-      AB_LAUNCH_CHECK("hpw_kernel");
-      return AB_OK;
-    };
-    switch (p.epilogue) {
-      case AB_PW_GELU: return go(hpw_kernel<NW, BF, PW_GELU>);
-      case AB_PW_GAMMA_RESIDUAL: return go(hpw_kernel<NW, BF, PW_GAMMA>);
-      case AB_PW_SPECTRUM: return go(hpw_kernel<NW, BF, PW_SPECTRUM>);
-    }
-    return fail(AB_ERR_ARG, "tc pointwise: unknown epilogue %d", p.epilogue);
-  });
+  auto run = [&](auto epi) {
+    return launch_persistent("hitem_kernel", "tc pointwise", (int64_t)p.B * g.tiles * g.NB, g, p.precision, s,
+                             [](auto nw, auto bf16) {
+                               return hitem_kernel<decltype(nw)::value, decltype(bf16)::value, decltype(epi)::value>;
+                             }, a, g, e);
+  };
+  switch (p.epilogue) {
+    case AB_PW_GELU: return run(IntC<PW_GELU>());
+    case AB_PW_GAMMA_RESIDUAL: return run(IntC<PW_GAMMA>());
+    case AB_PW_SPECTRUM: return run(IntC<PW_SPECTRUM>());
+  }
+  return fail(AB_ERR_ARG, "tc pointwise: unknown epilogue %d", p.epilogue);
 }
 
 }  // namespace ab

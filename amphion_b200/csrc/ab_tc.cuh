@@ -1,12 +1,14 @@
-// Tensor-core (wgmma / bulk-TMA) convolution path — interface.  hconv_kernel (ab_kernels_tc.cu) runs every
-// tensor-core Conv1d and ConvTranspose1d through launch_tc_conv; block mode (launch_tc_chain) has a kernel of its own.
-// The weight image of a layer depends only on (mode, C_in, C_out, k, dilation | stride).
+// Tensor-core (wgmma / bulk-TMA) convolution path — interface.  launch_tc_conv runs every tensor-core Conv1d and
+// ConvTranspose1d (ab_kernels_tc.cu: hconv_kernel, or the persistent hpair_kernel for a conv pair and hitem_kernel for
+// a ConvTranspose1d from an operand image); block mode (launch_tc_chain) runs on hchain_kernel and Vocos' pointwise
+// layers (launch_tc_pointwise) on hitem_kernel.  The weight image of a layer depends only on (mode, C_in, C_out, k,
+// dilation | stride).
 #pragma once
 #include "ab_common.cuh"
 
 namespace ab {
 
-// One launch of hconv_kernel, act(x) = lrelu(x, pre_slope) or the operand image ximg:
+// One launch of launch_tc_conv, act(x) = lrelu(x, pre_slope) or the operand image ximg:
 //   conv (mode 0, "same", dilation d_or_u):  y = ((conv(act(x), d) + bias) + residual + acc_prev) / out_div  [tanh]
 //   pair (mode 0 with w2):  y = ((conv2(lrelu(conv(act(x), d) + bias, mid_slope), 1) + b2) + residual + acc_prev) / out_div
 //     i.e. one (c1, c2) step of ResBlock1.forward (hifigan.py:93-100); a single conv is one step of ResBlock2
@@ -35,7 +37,7 @@ struct TcConvParams {
   int reflect = 0;                   // conv only, no w2: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN)
   int pad = -1;                      // conv-transpose padding, 0 <= pad < k; -1 = (k-u)/2 (HiFi-GAN; MelGAN: u//2 + u%2)
 };
-// 16-bit weight image of a layer, 0 when hconv_kernel cannot run it
+// 16-bit weight image of a layer, 0 when launch_tc_conv cannot run it
 size_t tc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u);
 // w_t: fp32 [Cin][k][Cout] (the repacked fp32 image) -> the layer's weight image
 int launch_tc_pack_weight(const float* w_t, void* image, int mode, int cin, int cout, int k, int d_or_u, int precision,
@@ -71,7 +73,7 @@ struct TcChainParams {
 double tc_chain_recompute(int C, int k, const int* dil, int npairs, int nconv);
 int launch_tc_chain(const TcChainParams& p, cudaStream_t s);
 
-// Pointwise (1x1, nn.Linear over channels) GEMM of Vocos (hpw_kernel): input the operand image of x, any C_in / C_out.
+// Pointwise (1x1, nn.Linear over channels) GEMM of Vocos (hitem_kernel): input the operand image of x, any C_in / C_out.
 //   AB_PW_GELU:            yimg = image of gelu(W x + b)                    (ConvNeXtBlock pwconv1 + nn.GELU())
 //   AB_PW_GAMMA_RESIDUAL:  y = y + gamma * (W x + b), fp32 [B, C_out, T]    (pwconv2, layer scale, residual)
 //   AB_PW_SPECTRUM:        spec [B*T][C_out/2] complex = min(exp(m), 1e2) (cos p + i sin p), m / p the two halves of

@@ -6,7 +6,7 @@ trace with CUDA activities.
 
 The tensor-core launches of `forward_impl` come in a fixed order: conv_pre, then per stage one ConvTranspose and per
 ResBlock either one block-mode launch (`hchain_kernel`) or one `hpair_kernel` launch per dilation pair; conv_pre runs
-on `hconv_kernel` and the ConvTranspose layers on `hconvt_kernel`.  The script
+on `hconv_kernel` and the ConvTranspose layers on `hitem_kernel`.  The script
 walks that order, attributes each tensor-core launch to (stage, plan) and prints time, share of the step, achieved
 TFLOP/s and algorithmic GB/s per row.  Algorithmic bytes per ResBlock launch: the 16-bit operand image and the fp32
 residual read, the fp32 output and its operand image written, the running branch sum read when it is accumulated, and
@@ -104,7 +104,7 @@ def main():
     kern = sorted((e for e in prof.events() if e.device_type.name == "CUDA" and "memcpy" not in e.name.lower()
                    and "memset" not in e.name.lower()), key=lambda e: e.time_range.start)
     step_us = kern[-1].time_range.end - kern[0].time_range.start
-    tc = ("hconv_kernel", "hconvt_kernel", "hchain_kernel", "hpair_kernel")
+    tc = ("hconv_kernel", "hitem_kernel", "hchain_kernel", "hpair_kernel")
     hc = [e for e in kern if any(n in e.name for n in tc)]
     other_us = sum(e.time_range.elapsed_us() for e in kern if not any(n in e.name for n in tc))
 
