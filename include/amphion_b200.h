@@ -189,6 +189,10 @@ int ab_generator_set_profiling(ab_generator* g, int32_t enable);
  *   whole ResBlock per launch (residual stream in registers, halo recomputed in the tile) where served (C <= 64) and
  *   the recompute is small, else per pair; 3, 4 = a whole ResBlock per launch wherever served.  All plans run the same
  *   arithmetic in the same order: their outputs are bit-equal.
+ *   "pair_schedule": how a per-pair launch at 64 and 128 channels (N block 64 or 128) shares its CTA's two consumer
+ *   warpgroups: 0 (default) = both on one time tile; 1 = ping-pong, each on its own tile with their MMA phases
+ *   alternating, where shared memory allows it and the launch has more tiles than SMs (slower on H100 today, see
+ *   DESIGN.md §6).  Outputs are bit-equal.
  *   "nsf_source_frames" (NSF-HiFiGAN, one-shot, consumed by the next forward): frames of the f0 track when it does
  *   not cover the mel; every stage is then truncated to the harmonic source's length as the reference does
  *   (nsfhifigan.py:264-268) and the output holds ab_generator_output_samples() samples per utterance.

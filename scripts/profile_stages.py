@@ -3,6 +3,8 @@
 trace with CUDA activities.
 
     python scripts/profile_stages.py [--batch 64] [--frames 1024] [--fusion 2] [--out DIR]
+    python scripts/profile_stages.py --time-fusions 0,2,3      # ms per step of each resblock_fusion, profiler off
+    python scripts/profile_stages.py --time-schedules 0,1      # per-stage table of each pair_schedule, then ms per step
 
 The tensor-core launches of `forward_impl` come in a fixed order: conv_pre, then per stage one ConvTranspose and per
 ResBlock either one block-mode launch (`hchain_kernel`) or one `hpair_kernel` launch per dilation pair; conv_pre runs
@@ -60,10 +62,11 @@ def main():
     ap.add_argument("--out", default="", help="directory for the JSON table (and nothing else)")
     ap.add_argument("--time-fusions", default="", metavar="M,M,...",
                     help="instead of profiling, time these resblock_fusion settings alternately")
+    ap.add_argument("--time-schedules", default="", metavar="S,S,...",
+                    help="profile one step at each of these pair_schedule settings, then time them alternately")
     args = ap.parse_args()
 
     import torch
-    from torch.profiler import ProfilerActivity, profile
     from amphion_b200.vocoders import _vocoders
 
     w = WORKLOADS["hifigan_v1"]
@@ -74,14 +77,14 @@ def main():
     model.set_option("resblock_fusion", args.fusion)
     B, T = args.batch, args.frames
     mel = torch.randn(B, w["n_mel"], T, generator=torch.Generator().manual_seed(0)).to(dev)
-    if args.time_fusions:
-        # profiler off: ms per step of each resblock_fusion setting, alternated over three rounds
-        modes = [int(m) for m in args.time_fusions.split(",")]
-        res = {m: [] for m in modes}
+
+    def time_alternately(key, values):
+        # profiler off: ms per step of each setting of option `key`, alternated over three rounds
+        res = {m: [] for m in values}
         with torch.no_grad():
             for _ in range(3):
-                for m in modes:
-                    model.set_option("resblock_fusion", m)
+                for m in values:
+                    model.set_option(key, m)
                     model(mel)
                     torch.cuda.synchronize()
                     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -91,9 +94,30 @@ def main():
                     e1.record()
                     torch.cuda.synchronize()
                     res[m].append(e0.elapsed_time(e1) / 5)
-        for m in modes:
-            print(f"resblock_fusion {m}: ms per step " + " ".join(f"{v:.1f}" for v in res[m]))
+        for m in values:
+            print(f"{key} {m}: ms per step " + " ".join(f"{v:.1f}" for v in res[m]))
+
+    if args.time_fusions:
+        time_alternately("resblock_fusion", [int(m) for m in args.time_fusions.split(",")])
         return
+    if args.time_schedules:
+        schedules = [int(s) for s in args.time_schedules.split(",")]
+        for s in schedules:
+            model.set_option("pair_schedule", s)
+            profile_step(model, mel, args, w, f"pair_schedule {s}", f"_schedule{s}")
+        time_alternately("pair_schedule", schedules)
+        return
+    profile_step(model, mel, args, w, "", "")
+
+
+def profile_step(model, mel, args, w, label, suffix):
+    """One profiled step after args.warmup warm-ups: prints the per-row and per-stage tables, and writes them to
+    args.out when given."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    B, T = mel.shape[0], mel.shape[2]
+    dev = mel.device
     with torch.no_grad():
         for _ in range(args.warmup):
             model(mel)
@@ -135,8 +159,9 @@ def main():
         raise SystemExit(f"launch walk matched {pos} of {len(hc)} tensor-core launches: plan and trace disagree")
 
     props = torch.cuda.get_device_properties(dev)
-    print(f"# {props.name}, HiFi-GAN V1 B={B} 80x{T} {args.precision}, resblock_fusion {args.fusion}: "
-          f"step {step_us / 1e3:.1f} ms (first kernel start to last kernel end, profiler on)")
+    print(f"# {props.name}, HiFi-GAN V1 B={B} 80x{T} {args.precision}, resblock_fusion {args.fusion}"
+          f"{', ' + label if label else ''}: step {step_us / 1e3:.1f} ms (first kernel start to last kernel end, "
+          f"profiler on)")
     print(f"{'stage':<9} {'plan':<13} {'n':>3} {'ms':>8} {'share':>6} {'TFLOP/s':>8} {'GB/s':>7}")
     out = []
     by_stage = OrderedDict()
@@ -155,7 +180,7 @@ def main():
         print(f"{stage:<9} {us / 1e3:>8.2f} ms {us / step_us:>6.1%} {fl / us / 1e6:>8.1f} TFLOP/s {nb / us / 1e3:>7.0f} GB/s")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, f"profile_fusion{args.fusion}.json"), "w") as f:
+        with open(os.path.join(args.out, f"profile_fusion{args.fusion}{suffix}.json"), "w") as f:
             json.dump(dict(gpu=props.name, batch=B, frames=T, fusion=args.fusion, step_ms=step_us / 1e3,
                            other_ms=other_us / 1e3, rows=out), f, indent=1)
 
