@@ -10,7 +10,7 @@ AB_MAX_STAGES = 8
 AB_MAX_KERNELS = 8
 AB_MAX_DILATIONS = 8
 
-GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN, GEN_VOCOS = 0, 1, 2, 3, 4, 5
+GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN, GEN_VOCOS, GEN_DIFFWAVE = 0, 1, 2, 3, 4, 5, 6
 ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA = 0, 1, 2
 PRECISIONS = {"fp32": 0, "tc_f16": 1, "tc_bf16": 2}
 
@@ -39,6 +39,8 @@ class GeneratorConfig(C.Structure):
         ("num_layers", C.c_int32),
         ("istft_n_fft", C.c_int32),
         ("istft_hop", C.c_int32),
+        ("dilation_cycle", C.c_int32),
+        ("embedding_rows", C.c_int32),
     ]
 
 
@@ -84,6 +86,13 @@ SIGNATURES = {
     "ab_generator_output_samples": (C.c_int64, [_P, C.c_int64, C.c_int64]),
     "ab_generator_set_tail_events": (C.c_int, [_P, C.POINTER(C.c_void_p), C.c_int32]),
     "ab_generator_get_profile": (C.c_int, [_P, C.POINTER(ProfileEntry), C.c_int32, C.POINTER(C.c_int32)]),
+    "ab_diffwave_workspace_bytes": (C.c_size_t, [_P, C.c_int64, C.c_int64, C.c_int32]),
+    "ab_diffwave_condition": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _I64P, C.POINTER(C.c_float), C.c_int32, _P,
+                                        C.c_size_t, _P]),
+    "ab_diffwave_step": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_float, C.c_float, _P, _P, _P,
+                                   C.c_size_t, _P]),
+    "ab_diffwave_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _P, _I64P, C.POINTER(C.c_float), C.c_int32, _P, _P,
+                                      C.c_size_t, _P]),
     "ab_activation1d_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P, C.c_int32, _P, _P, _P]),
     "ab_conv1d_forward": (C.c_int, [_P, _P, _P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                     C.c_int32, C.c_float, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),

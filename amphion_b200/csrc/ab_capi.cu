@@ -90,6 +90,23 @@ struct VocosRef {
   ConvRef head;   // head.out: [n_fft + 2, dim]
 };
 
+// DiffWave (AB_GEN_DIFFWAVE): slot indices; every tensor is a SLOT_VEC copied as is, the layer weights are repacked
+// into the arena's packed region at finalize (launch_dw_pack)
+struct DiffWaveLayerRef {   // one ResidualBlock (diffwave.py:90-122)
+  int dil = 1;
+  int wdil = -1, bdil = -1, wdp = -1, bdp = -1, wcond = -1, bcond = -1, wout = -1, bout = -1;
+};
+
+struct DiffWaveRef {
+  int win = -1, bin = -1, table = -1, wp1 = -1, bp1 = -1, wp2 = -1, bp2 = -1;
+  int wup[2] = {-1, -1}, bup[2] = {-1, -1};
+  int wsk = -1, bsk = -1, wo = -1, bo = -1;
+  std::vector<DiffWaveLayerRef> layers;
+  size_t packed_offset = 0;   // arena offset of the packed region (diffwave_packed_floats)
+  int64_t cond_B = 0, cond_T = 0;   // shapes of the last ab_diffwave_condition (0: none yet)
+  int cond_rows = 0;
+};
+
 struct StageRef {
   ConvRef up;   // cin/cout/k, d unused; stride in `u`
   int u = 1;
@@ -124,6 +141,7 @@ struct ab_generator {
   ActRef act_post;
   std::vector<StageRef> stages;
   VocosRef vocos;
+  DiffWaveRef dw;
   ab_mel* istft = nullptr;   // Vocos: the iSTFT plan (cuFFT C2R + overlap-add of ab_istft_forward)
 
   // profiling (ab_generator_set_profiling)
@@ -216,10 +234,32 @@ int validate_vocos_config(const ab_generator_config& c) {
   return AB_OK;
 }
 
+// AB_GEN_DIFFWAVE: only its own fields
+int validate_diffwave_config(const ab_generator_config& c) {
+  if (c.resblock || c.num_kernels || c.activation || c.snake_logscale || c.gin_channels || c.conv_post_no_bias ||
+      c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel || c.ffn_channels || c.istft_n_fft || c.istft_hop)
+    return fail(AB_ERR_ARG, "config: DiffWave uses only n_mel, upsample_initial_channel, num_layers, num_upsamples, "
+                            "upsample_rates, dilation_cycle and embedding_rows (every other field must be 0)");
+  if (c.n_mel <= 0 || c.n_mel > 512 || c.num_layers <= 0 || c.num_layers > 256 || c.dilation_cycle <= 0 ||
+      c.dilation_cycle > 20 || c.embedding_rows <= 0 || c.embedding_rows > (1 << 20) || c.num_upsamples != 2)
+    return fail(AB_ERR_ARG, "config: DiffWave n_mel %d (1..512), residual_layers %d (1..256), dilation_cycle %d (1..20), "
+                "embedding rows %d or upsample factors (%d, need 2) out of range", c.n_mel, c.num_layers, c.dilation_cycle,
+                c.embedding_rows, c.num_upsamples);
+  if (c.upsample_initial_channel != DW_CHANNELS)
+    return fail(AB_ERR_UNSUPPORTED, "config: DiffWave runs residual_channels = %d only (got %d)", DW_CHANNELS,
+                c.upsample_initial_channel);
+  for (int i = 0; i < 2; ++i)   // an odd factor makes the upsampled mel one sample longer than the audio
+    if (c.upsample_rates[i] <= 0 || (c.upsample_rates[i] & 1) || c.upsample_rates[i] > 4096)
+      return fail(AB_ERR_UNSUPPORTED, "config: DiffWave upsample factor %d must be even and positive", c.upsample_rates[i]);
+  return AB_OK;
+}
+
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
-      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS)
+      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
+  if (c.kind == AB_GEN_DIFFWAVE) return validate_diffwave_config(c);
+  if (c.dilation_cycle || c.embedding_rows) return fail(AB_ERR_ARG, "config: dilation_cycle / embedding_rows belong to AB_GEN_DIFFWAVE");
   if (c.kind == AB_GEN_VOCOS) return validate_vocos_config(c);
   if (c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop)
     return fail(AB_ERR_ARG, "config: ffn_channels / num_layers / istft_* belong to AB_GEN_VOCOS");
@@ -435,6 +475,73 @@ void add_vocos_tensors(ab_generator* g) {
   g->hop = cfg->istft_hop;
 }
 
+// DiffWave tensors (AB_GEN_DIFFWAVE), the reference's names (diffwave.py:28-66, :90-110, :127-162)
+void add_diffwave_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int C = cfg->upsample_initial_channel, nm = cfg->n_mel;
+  DiffWaveRef& d = g->dw;
+  d.win = g->add_slot("input_projection.weight", SLOT_VEC, {C, 1, 1});
+  d.bin = g->add_slot("input_projection.bias", SLOT_VEC, {C});
+  d.table = g->add_slot("diffusion_embedding.embedding", SLOT_VEC, {cfg->embedding_rows, 128});
+  d.wp1 = g->add_slot("diffusion_embedding.projection1.weight", SLOT_VEC, {512, 128});
+  d.bp1 = g->add_slot("diffusion_embedding.projection1.bias", SLOT_VEC, {512});
+  d.wp2 = g->add_slot("diffusion_embedding.projection2.weight", SLOT_VEC, {512, 512});
+  d.bp2 = g->add_slot("diffusion_embedding.projection2.bias", SLOT_VEC, {512});
+  for (int i = 0; i < 2; ++i) {   // ConvTranspose2d weight [1, 1, 3, 2f]: any shape of 6f elements loads
+    const std::string pre = "spectrogram_upsampler.conv" + std::to_string(i + 1);
+    d.wup[i] = g->add_slot(pre + ".weight", SLOT_VEC, {1, 3, 2 * cfg->upsample_rates[i]});
+    d.bup[i] = g->add_slot(pre + ".bias", SLOT_VEC, {1});
+    g->hop *= cfg->upsample_rates[i];
+  }
+  for (int i = 0; i < cfg->num_layers; ++i) {
+    const std::string pre = "residual_layers." + std::to_string(i);
+    DiffWaveLayerRef l;
+    l.dil = 1 << (i % cfg->dilation_cycle);
+    l.wdil = g->add_slot(pre + ".dilated_conv.weight", SLOT_VEC, {2 * C, C, 3});
+    l.bdil = g->add_slot(pre + ".dilated_conv.bias", SLOT_VEC, {2 * C});
+    l.wdp = g->add_slot(pre + ".diffusion_projection.weight", SLOT_VEC, {C, 512});
+    l.bdp = g->add_slot(pre + ".diffusion_projection.bias", SLOT_VEC, {C});
+    l.wcond = g->add_slot(pre + ".conditioner_projection.weight", SLOT_VEC, {2 * C, nm, 1});
+    l.bcond = g->add_slot(pre + ".conditioner_projection.bias", SLOT_VEC, {2 * C});
+    l.wout = g->add_slot(pre + ".output_projection.weight", SLOT_VEC, {2 * C, C, 1});
+    l.bout = g->add_slot(pre + ".output_projection.bias", SLOT_VEC, {2 * C});
+    d.layers.push_back(l);
+  }
+  d.wsk = g->add_slot("skip_projection.weight", SLOT_VEC, {C, C, 1});
+  d.bsk = g->add_slot("skip_projection.bias", SLOT_VEC, {C});
+  d.wo = g->add_slot("output_projection.weight", SLOT_VEC, {1, C, 1});
+  d.bo = g->add_slot("output_projection.bias", SLOT_VEC, {1});
+}
+
+// Packed region of a DiffWave handle, in floats: per layer w1p [3C + n_mel][2C], b1p [2C], w2p [C][2C], b2p [2C], then
+// the 16-bit images of the tensor-core kernel w1h [2C][dw_k1p] and w2h [2C][C] (each part 64-float aligned; the images
+// are written only at tensor-core precision), then every layer's diffusion_projection [layers][C][512] and bias
+// [layers][C] back to back.
+size_t dw_layer_packed_floats(int n_mel) {
+  const size_t C = DW_CHANNELS;
+  return align_up((3 * C + n_mel) * 2 * C, 64) + align_up(2 * C, 64) + align_up(C * 2 * C, 64) + align_up(2 * C, 64) +
+         align_up(C * dw_k1p(n_mel), 64) + align_up(C * C, 64);
+}
+// layer l's parts of the packed region
+struct DwLayerPack {
+  float *w1, *b1, *w2, *b2;
+  uint16_t *w1h, *w2h;
+};
+DwLayerPack dw_layer_pack(char* packed, int n_mel, int l) {
+  const size_t C = DW_CHANNELS;
+  DwLayerPack r;
+  r.w1 = reinterpret_cast<float*>(packed) + l * dw_layer_packed_floats(n_mel);
+  r.b1 = r.w1 + align_up((3 * C + n_mel) * 2 * C, 64);
+  r.w2 = r.b1 + align_up(2 * C, 64);
+  r.b2 = r.w2 + align_up(C * 2 * C, 64);
+  r.w1h = reinterpret_cast<uint16_t*>(r.b2 + align_up(2 * C, 64));
+  r.w2h = reinterpret_cast<uint16_t*>(r.b2 + align_up(2 * C, 64) + align_up(C * dw_k1p(n_mel), 64));
+  return r;
+}
+size_t diffwave_packed_floats(const ab_generator_config& c) {
+  return c.num_layers * (dw_layer_packed_floats(c.n_mel) + (size_t)DW_CHANNELS * 513);
+}
+
 }  // namespace
 
 extern "C" {
@@ -466,6 +573,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
       delete g;
       return rc;
     }
+  } else if (cfg->kind == AB_GEN_DIFFWAVE) {
+    add_diffwave_tensors(g);
   } else {
     add_gan_tensors(g);
   }
@@ -479,6 +588,10 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     tc += align_up(s.tc_bytes, 256);
   }
   g->arena_need = g->fp32_bytes + tc;
+  if (cfg->kind == AB_GEN_DIFFWAVE) {
+    g->dw.packed_offset = g->arena_need;
+    g->arena_need += align_up(diffwave_packed_floats(*cfg) * sizeof(float), 256);
+  }
   *out = g;
   return AB_OK;
 }
@@ -558,6 +671,32 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
   if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
     return fail(AB_ERR_ARG, "finalize: unknown precision %d", precision);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (g->cfg.kind == AB_GEN_DIFFWAVE) {
+    if (precision != AB_PREC_FP32 && !ab_device_is_sm90())
+      return fail(AB_ERR_UNSUPPORTED, "finalize: tensor-core precision needs an sm_90 (Hopper) device");
+    const int nl = g->cfg.num_layers, nm = g->cfg.n_mel, C = DW_CHANNELS;
+    float* pk = reinterpret_cast<float*>(g->arena + g->dw.packed_offset);
+    float* proj = pk + nl * dw_layer_packed_floats(nm);
+    for (int l = 0; l < nl; ++l) {
+      const DiffWaveLayerRef& L = g->dw.layers[l];
+      DwPackParams p;
+      p.wdil = g->fptr(L.wdil); p.bdil = g->fptr(L.bdil); p.wcond = g->fptr(L.wcond); p.bcond = g->fptr(L.bcond);
+      p.wout = g->fptr(L.wout); p.bout = g->fptr(L.bout);
+      const DwLayerPack lp = dw_layer_pack(g->arena + g->dw.packed_offset, nm, l);
+      p.w1p = lp.w1; p.b1p = lp.b1; p.w2p = lp.w2; p.b2p = lp.b2;
+      p.w1h = precision != AB_PREC_FP32 ? lp.w1h : nullptr; p.w2h = lp.w2h;
+      p.bf16 = precision == AB_PREC_TC_BF16;
+      p.n_mel = nm;
+      const int rc = launch_dw_pack(p, st);
+      if (rc != AB_OK) return rc;
+      AB_CUDA_TRY(cudaMemcpyAsync(proj + (size_t)l * C * 512, g->fptr(L.wdp), (size_t)C * 512 * 4, cudaMemcpyDeviceToDevice, st));
+      AB_CUDA_TRY(cudaMemcpyAsync(proj + (size_t)nl * C * 512 + l * C, g->fptr(L.bdp), C * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    g->dw.cond_B = g->dw.cond_T = 0;
+    g->precision = precision;
+    g->finalized = true;
+    return AB_OK;
+  }
   if (precision != AB_PREC_FP32) {
     if (!ab_device_is_sm90()) return fail(AB_ERR_UNSUPPORTED, "finalize: tensor-core precision needs an sm_90 (Hopper) device");
     for (size_t i = 0; i < g->slots.size(); ++i) {
@@ -674,6 +813,7 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
   if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
+  if (g->cfg.kind == AB_GEN_DIFFWAVE) return 0;
   return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
          NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
 }
@@ -698,7 +838,7 @@ int ab_generator_set_tail_events(ab_generator* g, void* const* events, int32_t n
 
 int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64_t source_frames) {
   if (!g || frames <= 0) return 0;
-  if (g->cfg.kind == AB_GEN_VOCOS) return frames * g->hop;
+  if (g->cfg.kind == AB_GEN_VOCOS || g->cfg.kind == AB_GEN_DIFFWAVE) return frames * g->hop;
   int64_t Tn = frames;
   for (int i = 0; i < g->cfg.num_upsamples; ++i) Tn = nsf_stage_length(g, i, Tn * g->cfg.upsample_rates[i], source_frames);
   return Tn;
@@ -707,6 +847,7 @@ int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64
 int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
   if (!g || !key) return fail(AB_ERR_ARG, "set_option: null argument");
   if (g->cfg.kind == AB_GEN_VOCOS) return fail(AB_ERR_ARG, "set_option: Vocos has no execution-plan option ('%s')", key);
+  if (g->cfg.kind == AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "set_option: DiffWave has no execution-plan option ('%s')", key);
   if (strcmp(key, "nsf_source_frames") == 0) {   // one-shot: consumed by the next forward
     if (value < 0) return fail(AB_ERR_ARG, "set_option: nsf_source_frames must be >= 0");
     if (value > 0 && g->cfg.kind != AB_GEN_NSFHIFIGAN) return fail(AB_ERR_ARG, "set_option: nsf_source_frames belongs to NSF-HiFiGAN");
@@ -728,9 +869,11 @@ int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
 
 int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max_entries, int32_t* n_out) {
   if (!g || !out || !n_out) return fail(AB_ERR_ARG, "get_profile: null argument");
-  static const char* kNames[7] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
-                                  "tc_pointwise", "vocos_norm"};
-  const int n = g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;   // the last two classes are Vocos' kernels
+  static const char* kNames[11] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
+                                   "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
+                                   "diffwave_tail"};
+  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's
+  const int n = g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
   for (int i = 0; i < n; ++i) {
     memset(&out[i], 0, sizeof(out[i]));
@@ -763,6 +906,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   if (dev_g != nullptr && g->cond_w < 0) return fail(AB_ERR_STATE, "forward: conditioning given but the generator has gin_channels == 0");
   if (dev_g != nullptr && g_batch_stride < g->cfg.gin_channels) return fail(AB_ERR_ARG, "forward: g row stride < gin_channels");
   if (!g->finalized) return fail(AB_ERR_STATE, "forward: finalize() the generator first");
+  if (g->cfg.kind == AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "forward: a DiffWave handle runs through ab_diffwave_forward");
   if (B <= 0 || T <= 0) return fail(AB_ERR_ARG, "forward: batch and frames must be positive (got %lld, %lld)", (long long)B, (long long)T);
   if (B > 65535) return fail(AB_ERR_UNSUPPORTED, "forward: batch %lld > 65535", (long long)B);
   if ((int64_t)T * g->hop > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "forward: sequence too long");
@@ -1218,6 +1362,178 @@ int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, in
                               const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
                               size_t workspace_bytes, void* stream) {
   return forward_impl(g, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes, stream);
+}
+
+// ---------------------------------------------------------------------------
+// DiffWave
+// ---------------------------------------------------------------------------
+namespace {
+// Workspace: the fp32 residual stream in two buffers X0 / X1 (layer l reads one and writes the other), the skip sum,
+// the upsampled mel [B, n_mel, L], then the diffusion projections [n_steps][layers][C] and the step values.
+struct DiffWaveWs {
+  float *X[2], *S, *M, *D, *steps;
+};
+
+size_t diffwave_layout(const ab_generator* g, int64_t B, int64_t T, int n_steps, char* base, DiffWaveWs* w) {
+  const size_t L = (size_t)T * g->hop;
+  const size_t sz[6] = {B * DW_CHANNELS * L * 4, B * DW_CHANNELS * L * 4, B * DW_CHANNELS * L * 4,
+                        B * (size_t)g->cfg.n_mel * L * 4, (size_t)n_steps * g->cfg.num_layers * DW_CHANNELS * 4,
+                        (size_t)n_steps * 4};
+  float* p[6];
+  size_t off = 0;
+  for (int i = 0; i < 6; ++i) {
+    p[i] = base ? reinterpret_cast<float*>(base + off) : nullptr;
+    off += align_up(sz[i], 256);
+  }
+  if (w) *w = {{p[0], p[1]}, p[2], p[3], p[4], p[5]};
+  return off;
+}
+
+int diffwave_check(const ab_generator* g, int64_t B, int64_t T, int n_steps, void* ws, size_t ws_bytes, const char* what) {
+  if (!g) return fail(AB_ERR_ARG, "%s: null handle", what);
+  if (g->cfg.kind != AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "%s: not a DiffWave handle", what);
+  if (!g->finalized) return fail(AB_ERR_STATE, "%s: finalize() the generator first", what);
+  if (B <= 0 || T <= 0 || B > 65535) return fail(AB_ERR_ARG, "%s: batch %lld / frames %lld out of range", what, (long long)B, (long long)T);
+  if (T * g->hop > (1ll << 30) || B * (int64_t)std::max(DW_CHANNELS, g->cfg.n_mel) * T * g->hop > (1ll << 40))
+    return fail(AB_ERR_UNSUPPORTED, "%s: sequence too long", what);
+  const size_t need = diffwave_layout(g, B, T, n_steps, nullptr, nullptr);
+  if (!ws || ws_bytes < need) return fail(AB_ERR_WORKSPACE, "%s: workspace %zu B < required %zu B", what, ws_bytes, need);
+  if (reinterpret_cast<uintptr_t>(ws) & 255) return fail(AB_ERR_ARG, "%s: workspace must be 256-byte aligned", what);
+  return AB_OK;
+}
+
+// per-launch device timing (ab_generator_set_profiling), classes 7-10
+struct DwProf {
+  ab_generator* g;
+  cudaStream_t st;
+  void begin(int cls, double flops, double bytes) {
+    if (!g->profiling) return;
+    ab_generator::ProfRec r;
+    r.cls = cls; r.flops = flops; r.bytes = bytes;
+    r.e0 = g->get_event(); r.e1 = g->get_event();
+    cudaEventRecord(r.e0, st);
+    g->prof_recs.push_back(r);
+  }
+  void end() {
+    if (g->profiling) cudaEventRecord(g->prof_recs.back().e1, st);
+  }
+};
+}  // namespace
+
+size_t ab_diffwave_workspace_bytes(const ab_generator* g, int64_t B, int64_t T, int32_t n_steps) {
+  if (!g || g->cfg.kind != AB_GEN_DIFFWAVE || B <= 0 || T <= 0 || n_steps <= 0) return 0;
+  return diffwave_layout(g, B, T, n_steps, nullptr, nullptr);
+}
+
+int ab_diffwave_condition(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
+                          const float* host_steps, int32_t n_steps, void* ws, size_t ws_bytes, void* stream) {
+  if (!dev_mel || !mel_strides || !host_steps) return fail(AB_ERR_ARG, "diffwave_condition: null argument");
+  if (n_steps <= 0 || n_steps > 65535) return fail(AB_ERR_ARG, "diffwave_condition: n_steps %d out of range", n_steps);
+  int rc = diffwave_check(g, B, T, n_steps, ws, ws_bytes, "diffwave_condition");
+  if (rc != AB_OK) return rc;
+  for (int i = 0; i < n_steps; ++i)   // the reference indexes the table at floor(t) and ceil(t)
+    if (!(host_steps[i] >= 0.f) || !(ceilf(host_steps[i]) < (float)g->cfg.embedding_rows))
+      return fail(AB_ERR_ARG, "diffwave_condition: diffusion step %g outside the embedding table [0, %d)", host_steps[i],
+                  g->cfg.embedding_rows);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DiffWaveWs w;
+  diffwave_layout(g, B, T, n_steps, static_cast<char*>(ws), &w);
+  const DiffWaveRef& d = g->dw;
+  const int nm = g->cfg.n_mel, nl = g->cfg.num_layers, C = DW_CHANNELS;
+  DwProf prof{g, st};
+  g->dw.cond_B = 0;
+  AB_CUDA_TRY(cudaMemcpyAsync(w.steps, host_steps, (size_t)n_steps * 4, cudaMemcpyHostToDevice, st));
+  DwUpsampleParams up;
+  up.mel = dev_mel; up.msb = mel_strides[0]; up.msc = mel_strides[1]; up.mst = mel_strides[2];
+  up.w1 = g->fptr(d.wup[0]); up.b1 = g->fptr(d.bup[0]); up.w2 = g->fptr(d.wup[1]); up.b2 = g->fptr(d.bup[1]);
+  up.out = w.M; up.B = (int)B; up.n_mel = nm; up.F = (int)T; up.f1 = g->cfg.upsample_rates[0]; up.f2 = g->cfg.upsample_rates[1];
+  const double L = (double)T * g->hop;
+  prof.begin(7, 2.0 * B * nm * L * 36.0, 4.0 * B * nm * (T + L));
+  rc = launch_dw_upsample(up, st);
+  prof.end();
+  if (rc != AB_OK) return rc;
+  DwEmbedParams e;
+  const float* proj = reinterpret_cast<const float*>(g->arena + d.packed_offset) + nl * dw_layer_packed_floats(nm);
+  e.steps = w.steps; e.table = g->fptr(d.table); e.w1 = g->fptr(d.wp1); e.b1 = g->fptr(d.bp1);
+  e.w2 = g->fptr(d.wp2); e.b2 = g->fptr(d.bp2); e.wd = proj; e.bd = proj + (size_t)nl * C * 512; e.d = w.D; e.layers = nl;
+  prof.begin(7, 2.0 * n_steps * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512),
+             4.0 * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512 + (double)n_steps * nl * C));
+  rc = launch_dw_embed(e, n_steps, st);
+  prof.end();
+  if (rc != AB_OK) return rc;
+  g->dw.cond_B = B; g->dw.cond_T = T; g->dw.cond_rows = n_steps;
+  g->launches = 2;
+  return AB_OK;
+}
+
+int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t B, int64_t T, int32_t step_row, float c1, float c2,
+                     float sigma, const float* dev_noise, float* dev_eps, void* ws, size_t ws_bytes, void* stream) {
+  if (!dev_audio) return fail(AB_ERR_ARG, "diffwave_step: null audio");
+  if (!g || g->cfg.kind != AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "diffwave_step: not a DiffWave handle");
+  if (g->dw.cond_B != B || g->dw.cond_T != T)
+    return fail(AB_ERR_STATE, "diffwave_step: run ab_diffwave_condition for this batch (%lld x %lld frames) first", (long long)B,
+                (long long)T);
+  const int rows = g->dw.cond_rows;
+  int rc = diffwave_check(g, B, T, rows, ws, ws_bytes, "diffwave_step");
+  if (rc != AB_OK) return rc;
+  if (step_row < -1 || step_row >= rows || (step_row == -1 && rows != B))
+    return fail(AB_ERR_ARG, "diffwave_step: step row %d with %d conditioned steps and batch %lld", step_row, rows, (long long)B);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DiffWaveWs w;
+  diffwave_layout(g, B, T, rows, static_cast<char*>(ws), &w);
+  const DiffWaveRef& d = g->dw;
+  const int nm = g->cfg.n_mel, nl = g->cfg.num_layers, C = DW_CHANNELS;
+  const int64_t L = T * g->hop;
+  const double el = (double)B * L;
+  DwProf prof{g, st};
+  int launches = 0;
+  ++launches;
+  prof.begin(8, 2.0 * el * C, 4.0 * el * (1 + C));
+  rc = launch_dw_input(dev_audio, g->fptr(d.win), g->fptr(d.bin), w.X[0], (int)B, L, st);
+  prof.end();
+  for (int l = 0; rc == AB_OK && l < nl; ++l) {
+    DwLayerParams p;
+    p.x_in = w.X[l & 1]; p.x_out = w.X[(l + 1) & 1]; p.skip = w.S; p.cond = w.M;
+    p.d = w.D + ((size_t)(step_row < 0 ? 0 : step_row) * nl + l) * C;
+    p.d_bstride = step_row < 0 ? (int64_t)nl * C : 0;
+    const DwLayerPack lp = dw_layer_pack(g->arena + d.packed_offset, nm, l);
+    p.w1 = lp.w1; p.b1 = lp.b1; p.w2 = lp.w2; p.b2 = lp.b2; p.w1h = lp.w1h; p.w2h = lp.w2h; p.precision = g->precision;
+    p.B = (int)B; p.n_mel = nm; p.dil = d.layers[l].dil; p.first = l == 0; p.L = L;
+    ++launches;
+    // x read (3 taps, once from HBM), x written, skip read + written (stored by the first layer), mel read
+    prof.begin(9, 2.0 * el * 2 * C * (3 * C + nm + C), 4.0 * el * (C * (l == 0 ? 3 : 4) + nm));
+    rc = launch_dw_layer(p, st);
+    prof.end();
+  }
+  if (rc != AB_OK) return rc;
+  DwTailParams t;
+  t.skip = w.S; t.wsk = g->fptr(d.wsk); t.bsk = g->fptr(d.bsk); t.wo = g->fptr(d.wo); t.bo = g->fptr(d.bo);
+  t.skip_div = (float)sqrt((double)nl);
+  t.B = (int)B; t.L = L; t.eps = dev_eps; t.audio = dev_audio; t.noise = dev_noise; t.c1 = c1; t.c2 = c2; t.sigma = sigma;
+  ++launches;
+  prof.begin(10, 2.0 * el * (C * C + C), 4.0 * el * (C + (dev_eps ? 1 : 2) + (dev_noise ? 1 : 0)));
+  rc = launch_dw_tail(t, st);
+  prof.end();
+  if (rc != AB_OK) return rc;
+  g->launches = launches;
+  return AB_OK;
+}
+
+int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t B, int64_t T, const float* dev_mel,
+                        const int64_t mel_strides[3], const float* host_steps, int32_t n_steps, float* dev_eps, void* ws,
+                        size_t ws_bytes, void* stream) {
+  if (!dev_eps || !dev_audio) return fail(AB_ERR_ARG, "diffwave_forward: null argument");
+  if (n_steps != 1 && n_steps != B)
+    return fail(AB_ERR_ARG, "diffwave_forward: %d diffusion steps for a batch of %lld (need 1 or the batch)", n_steps, (long long)B);
+  int rc = ab_diffwave_condition(g, dev_mel, B, T, mel_strides, host_steps, n_steps, ws, ws_bytes, stream);
+  if (rc != AB_OK) return rc;
+  const int cond_launches = g->launches;
+  // the audio is only read when eps is given
+  rc = ab_diffwave_step(g, const_cast<float*>(dev_audio), B, T, n_steps == 1 ? 0 : -1, 1.f, 0.f, 0.f, nullptr, dev_eps, ws,
+                        ws_bytes, stream);
+  if (rc != AB_OK) return rc;
+  g->launches += cond_launches;
+  return AB_OK;
 }
 
 // ---------------------------------------------------------------------------

@@ -156,6 +156,65 @@ struct NormParams {
   float eps = 1e-6f;
 };
 
+// ---- DiffWave (ab_diffwave.cu) -------------------------------------------
+constexpr int DW_CHANNELS = 64;   // residual_channels the DiffWave kernels are compiled for
+
+struct DwUpsampleParams {   // SpectrogramUpsampler: mel [B, n_mel, F] (element strides) -> out [B, n_mel, F f1 f2]
+  const float* mel;
+  int64_t msb, msc, mst;
+  const float *w1, *b1, *w2, *b2;   // ConvTranspose2d weights [3][2 f] and biases [1]
+  float* out;
+  int B, n_mel, F, f1, f2;
+};
+struct DwEmbedParams {      // d [steps][layers][C] from the step values (host-checked to index the table)
+  const float* steps;
+  const float* table;               // [rows][128]
+  const float *w1, *b1, *w2, *b2;   // projection1 [512][128], projection2 [512][512]
+  const float *wd, *bd;             // every layer's diffusion_projection, [layers][C][512] and [layers][C]
+  float* d;
+  int layers;
+};
+struct DwLayerParams {      // one ResidualBlock
+  const float* x_in;      // [B, C, L]
+  float* x_out;           // [B, C, L], not x_in (neighbouring tiles read x_in's halo)
+  float* skip;            // [B, C, L] running skip sum
+  const float* cond;      // upsampled mel [B, n_mel, L]
+  const float* d;         // this layer's diffusion projection [C] of utterance 0
+  int64_t d_bstride;      // 0: one step for the batch
+  const float *w1, *b1, *w2, *b2;   // packed by launch_dw_pack (b1 / b2 serve both paths)
+  const uint16_t *w1h, *w2h;        // 16-bit images for the tensor-core layer kernel (precision != AB_PREC_FP32)
+  int precision;
+  int B, n_mel, dil, first;
+  int64_t L;
+};
+struct DwTailParams {
+  const float* skip;
+  const float *wsk, *bsk, *wo, *bo;   // skip_projection [C][C], output_projection [C]
+  float skip_div;                      // sqrt(residual_layers)
+  int B;
+  int64_t L;
+  float* eps;                          // [B, L], or nullptr: sampler update of audio
+  float* audio;
+  const float* noise;                  // nullable
+  float c1, c2, sigma;
+};
+struct DwPackParams {
+  const float *wdil, *bdil, *wcond, *bcond, *wout, *bout;   // state-dict layouts
+  float *w1p, *b1p, *w2p, *b2p;   // [3C + n_mel][2C], [2C], [C][2C], [2C]
+  uint16_t *w1h, *w2h;            // nullptr, or the 16-bit images [2C][dw_k1p(n_mel)] and [2C][C] (column-major in K)
+  int bf16;
+  int n_mel;
+};
+// K of the tensor-core conv1: three dilated taps of C channels, then n_mel rounded up to 16
+inline int dw_k1p(int n_mel) { return 3 * DW_CHANNELS + (n_mel + 15) / 16 * 16; }
+size_t dw_layer_smem_bytes(int n_mel, int precision);
+int launch_dw_upsample(const DwUpsampleParams& p, cudaStream_t s);
+int launch_dw_embed(const DwEmbedParams& p, int steps, cudaStream_t s);
+int launch_dw_input(const float* audio, const float* w, const float* bias, float* x, int B, int64_t L, cudaStream_t s);
+int launch_dw_layer(const DwLayerParams& p, cudaStream_t s);
+int launch_dw_tail(const DwTailParams& p, cudaStream_t s);
+int launch_dw_pack(const DwPackParams& p, cudaStream_t s);
+
 // launchers (ab_kernels_fp32.cu)
 int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);

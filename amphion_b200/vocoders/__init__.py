@@ -1,7 +1,9 @@
-"""Native GAN vocoders behind the reference's registry/dispatch surface
+"""Native vocoders behind the reference's registry/dispatch surface
 (models/vocoders/vocoder_inference.py:39-75)."""
 from .apnet import APNet, ISTFT, ISTFTHead
 from .bigvgan import BigVGAN
+from .diffwave import DiffWave
+from . import diffusion_vocoder_inference
 from .hifigan import HiFiGAN, HiFiGAN_vits
 from .melgan import MelGAN
 from .nsfhifigan import NSFHiFiGAN
@@ -13,9 +15,12 @@ from .gan_vocoder_inference import vocoder_inference as _gan_vocoder_inference
 _vocoders = {"hifigan": HiFiGAN, "bigvgan": BigVGAN, "nsfhifigan": NSFHiFiGAN, "melgan": MelGAN, "apnet": APNet}
 _vocoder_forward_funcs = {k: _gan_vocoder_inference for k in _vocoders}
 _vocoder_infer_funcs = {k: synthesis_audios for k in _vocoders}
+_vocoders["diffwave"] = DiffWave
+_vocoder_forward_funcs["diffwave"] = diffusion_vocoder_inference.vocoder_inference
+_vocoder_infer_funcs["diffwave"] = diffusion_vocoder_inference.synthesis_audios
 
 # Vocos is not in the registry: the reference has no entry for it and its constructor takes cfg.model.vocos, not cfg
-__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "NSFHiFiGAN", "MelGAN", "APNet", "Vocos", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
+__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "DiffWave", "NSFHiFiGAN", "MelGAN", "APNet", "Vocos", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
            "_vocoder_forward_funcs", "_vocoder_infer_funcs"]
 
 # `amphion_b200.vocoders.vocoder_inference` is the MODULE (synthesis, load_nnvocoder), as

@@ -240,9 +240,9 @@ class NativeGenerator(nn.Module):
 
     def get_profile(self):
         """{class: dict(launches, ms, flops, bytes)} accumulated since the last call (synchronises)."""
-        arr = (_capi.ProfileEntry * 8)()
+        arr = (_capi.ProfileEntry * 16)()
         n = C.c_int32(0)
-        _capi.check(_capi.lib.ab_generator_get_profile(self._ensure_handle(), arr, 8, C.byref(n)), "get_profile")
+        _capi.check(_capi.lib.ab_generator_get_profile(self._ensure_handle(), arr, 16, C.byref(n)), "get_profile")
         return {arr[i].name.decode(): dict(launches=arr[i].launches, ms=arr[i].ms, flops=arr[i].flops,
                                            bytes=arr[i].bytes) for i in range(n.value)}
 

@@ -68,9 +68,22 @@ extern "C" {
  * num_layers, istft_n_fft (even), istft_hop (<= n_fft, n_fft - hop even); every other field 0.  Tensors keep the
  * reference's state-dict names ("backbone.embed.weight", "backbone.convnext.3.pwconv1.weight" [out, in], ".gamma",
  * "backbone.final_layer_norm.bias", "head.out.weight", "head.istft.window", ...).  Output: wav [B, 1, T * istft_hop];
- * with tail events the iSTFT runs in the batch chunks. */
+ * with tail events the iSTFT runs in the batch chunks.
+ * AB_GEN_DIFFWAVE: DiffWave.forward (models/vocoders/diffusion/diffwave/diffwave.py:130-183): x = relu(input_projection(
+ * audio)); per residual layer i (dilation 2^(i % dilation_cycle)): y = dilated_conv(x + diffusion_projection(emb)) +
+ * conditioner_projection(up(mel)), z = sigmoid(y[:C]) tanh(y[C:]), (r, s) = output_projection(z), x = (x + r) / sqrt(2),
+ * skip += s; eps = output_projection(relu(skip_projection(skip / sqrt(layers)))).  emb = silu(projection2(silu(
+ * projection1(lerp of the embedding table at the step))))); up = two ConvTranspose2d(1, 1, [3, 2f], stride [1, f],
+ * padding [1, f/2]) each followed by leaky_relu(0.4).  Config fields: n_mel, upsample_initial_channel = residual_channels
+ * (64), num_layers = residual_layers, num_upsamples = 2, upsample_rates = upsample_factors (even), dilation_cycle,
+ * embedding_rows = len(noise_schedule); every other field 0.  Tensors keep the reference's names, including the
+ * non-persistent "diffusion_embedding.embedding" [embedding_rows, 128].  At AB_PREC_TC_F16 / TC_BF16 the residual
+ * layers' convolutions take 16-bit operands (x + d, the upsampled mel, the gate, the weights) with fp32 accumulation;
+ * the x and skip streams, the upsampler, the step embeddings and the tail stay fp32 at every precision.  It runs
+ * through the ab_diffwave_* entry points below, not ab_generator_forward. */
 enum ab_generator_kind {
-  AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5
+  AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
+  AB_GEN_DIFFWAVE = 6
 };
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
 /* arithmetic of the k-tap channel-mixing convolutions */
@@ -91,6 +104,7 @@ int ab_device_is_sm90(void);
  *            NSFHiFiGAN.forward  (models/vocoders/gan/generator/nsfhifigan.py:262-283)
  *            MelGAN.forward      (models/vocoders/gan/generator/melgan.py:100-101)
  *            Vocos.forward       (models/codec/amphion_codec/vocos.py:877-881)
+ *            DiffWave.forward    (models/vocoders/diffusion/diffwave/diffwave.py:164-183), see ab_diffwave_*
  * The config mirrors cfg.model.{hifigan,bigvgan}.* + cfg.preprocess.n_mel
  * (hifigan.py:151-201, bigvgan.py:232-311).
  * ---------------------------------------------------------------------- */
@@ -122,6 +136,9 @@ typedef struct ab_generator_config {
   int32_t num_layers;                           /* ConvNeXt blocks */
   int32_t istft_n_fft;
   int32_t istft_hop;
+  /* AB_GEN_DIFFWAVE only (0 elsewhere) */
+  int32_t dilation_cycle;                       /* dilation_cycle_length */
+  int32_t embedding_rows;                       /* rows of the diffusion-step table, len(noise_schedule) */
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -153,6 +170,7 @@ int ab_generator_load_weight_norm(ab_generator* g, const char* name, const float
  * operand images it needs.  Fails with AB_ERR_STATE if a tensor is missing. */
 int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream);
 
+/* 0 for AB_GEN_DIFFWAVE (see ab_diffwave_workspace_bytes) */
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t batch, int64_t frames);
 /* mel [B, n_mel, T] fp32 with arbitrary element strides (the reference feeds
  * transposed views: models/vocoders/vocoder_inference.py:349,505)
@@ -175,7 +193,10 @@ int ab_generator_last_launches(const ab_generator* g);
  * (launches, milliseconds, algorithmic FLOPs, algorithmic HBM bytes) per class
  * since the last call, and resets.  Classes: "tc_conv", "conv1d_fp32",
  * "conv_transpose1d_fp32", "activation1d", "tc_gemmconv" (max_entries >= 5), then, when max_entries >= 7,
- * "tc_pointwise" (Vocos' pointwise GEMMs and head) and "vocos_norm" (its depthwise conv + LayerNorm kernels). */
+ * "tc_pointwise" (Vocos' pointwise GEMMs and head) and "vocos_norm" (its depthwise conv + LayerNorm kernels); a DiffWave
+ * handle lists, when max_entries >= 11, also "diffwave_cond" (spectrogram upsampler and step embeddings, once per
+ * call), "diffwave_input" (input projection), "diffwave_layer" (residual layers) and "diffwave_tail" (skip/output
+ * projections and the sampler update). */
 typedef struct ab_profile_entry {
   char name[32];
   int32_t launches;
@@ -207,6 +228,33 @@ int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64
  * can start sending chunk i while chunk i+1 is computed.  One-shot: cleared by that forward.  n = 0 clears. */
 int ab_generator_set_tail_events(ab_generator* g, void* const* events, int32_t n);
 int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max_entries, int32_t* n_out);
+
+/* ------------------------------------------------------------------------
+ * DiffWave (AB_GEN_DIFFWAVE): DiffWave.forward and the denoising step of vocoder_inference
+ * (models/vocoders/diffusion/diffusion_vocoder_inference.py:13-73).  The conditioning (upsampled mel and the diffusion
+ * projections of every step the call will use) is computed once into the workspace by ab_diffwave_condition; each
+ * ab_diffwave_step is one network pass over the audio that reads it.  The audio of `frames` mel frames has
+ * frames * prod(upsample_rates) samples.  Workspace: ab_diffwave_workspace_bytes(g, batch, frames, n_steps), 256-byte
+ * aligned; the same workspace and shapes for the condition call and the steps that follow it.
+ * ---------------------------------------------------------------------- */
+size_t ab_diffwave_workspace_bytes(const ab_generator* g, int64_t batch, int64_t frames, int32_t n_steps);
+/* mel [B, n_mel, frames] fp32, any element strides; host_steps [n_steps] diffusion steps (an integer step as its float
+ * value, which the lerp reproduces exactly), each with 0 <= floor and ceil < embedding_rows. */
+int ab_diffwave_condition(ab_generator* g, const float* dev_mel, int64_t batch, int64_t frames, const int64_t mel_strides[3],
+                          const float* host_steps, int32_t n_steps, void* dev_workspace, size_t workspace_bytes,
+                          void* stream);
+/* One network pass over dev_audio [B, frames * hop] (contiguous) with the step of conditioning row step_row for every
+ * utterance, or row b for utterance b when step_row = -1 (n_steps == B).  dev_eps != NULL: eps [B, 1, frames * hop]
+ * is written and the audio is left alone.  dev_eps == NULL: the sampler update in place, audio = clamp(c1 (audio -
+ * c2 eps) + sigma noise, -1, 1), the noise term only when dev_noise [B, frames * hop] is given. */
+int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t batch, int64_t frames, int32_t step_row, float c1,
+                     float c2, float sigma, const float* dev_noise, float* dev_eps, void* dev_workspace,
+                     size_t workspace_bytes, void* stream);
+/* DiffWave.forward(audio, diffusion_step, spectrogram): ab_diffwave_condition with n_steps = 1 (one step for the batch)
+ * or B (one per utterance), then ab_diffwave_step writing eps. */
+int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t batch, int64_t frames, const float* dev_mel,
+                        const int64_t mel_strides[3], const float* host_steps, int32_t n_steps, float* dev_eps,
+                        void* dev_workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Activation1d(Snake|SnakeBeta).forward  (modules/anti_aliasing/act.py:31-36,
