@@ -896,7 +896,10 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
 }
 
 
-// block mode (resblock_fusion 2) is chosen when it computes at most this many tile rows per output row
+// block mode (resblock_fusion 2) is chosen when it computes at most this many tile rows per output row.  On HiFi-GAN
+// V1 that is the k = 3 blocks at 128, 64 and 32 channels (1.23, 1.10, 1.05), the k = 7 blocks at 64 and 32 (1.39,
+// 1.16) and the k = 11 block at 32 (1.31); the 64-channel k = 11 (1.88) and 128-channel k = 7 (2.29) blocks were
+// slower in block mode than as pairs on an H100 (DESIGN.md §6).
 static constexpr double kChainMaxRecompute = 1.5;
 
 static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],

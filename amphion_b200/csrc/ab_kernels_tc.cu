@@ -199,7 +199,8 @@ __device__ __forceinline__ void store_frag_tile(uint8_t* tile, const float (&v)[
 }
 
 // What epilogue_out reads from HBM and applies; a term that is not compiled in is either never set by the kernel's
-// launches (block mode: residual, tanh) or already part of val (hpair_kernel's prefetched residual and branch sum).
+// launches (block mode: residual, tanh) or already part of val (the residual and branch sum that hpair_kernel and
+// hchain_kernel fold in with add_terms).
 enum : int { EP_RESIDUAL = 1, EP_ACC_PREV = 2, EP_TANH = 4, EP_ALL = 7 };
 
 // Output epilogue on fragment rows [r0, r1) at times t0 + row < Tout, output channels co0 + column < C_out:
@@ -243,21 +244,23 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
 
 // The additive terms of epilogue_out folded into the accumulators first, in its association:
 //   acc = ((acc [+ bias]) [+ residual]) [+ acc_prev]     (each term when its pointer is non-null)
-// on fragment rows < V at time O + row.  The loads of both terms go out G fragment columns at a time, so that a group
-// waits for one HBM round trip: read inside epilogue_out, between its fp32 stores (which may alias acc_prev), every
-// element would wait for its own.  epilogue_out then runs without EP_RESIDUAL / EP_ACC_PREV on the accumulators.
+// on the valid fragment rows [r0, r1) at time t0 + row (pair mode: [0, V) at O + row; block mode: [H, H + V) at
+// O - H + row).  The loads of both terms go out G fragment columns at a time, so that a group waits for one HBM round
+// trip: read inside epilogue_out, between its fp32 stores (which may alias acc_prev), every element would wait for its
+// own.  epilogue_out then runs without EP_RESIDUAL / EP_ACC_PREV on the accumulators.
 template <int NW, int MT>
 __device__ __forceinline__ void add_terms(float (&acc)[MT][NW / 2], const Frag<MT>& f, const float* bias,
                                           const float* residual, const float* acc_prev, const HcArgs& p,
-                                          const HcGeom& g, int b, int O) {
+                                          const HcGeom& g, int b, int t0, int r0, int r1) {
   // columns per group: 8 below 128 accumulators per thread; 2 at 128, where ptxas (168 registers) spills more
   constexpr int G = MT * NW / 2 > 64 ? 2 : (NW / 8 < 8 ? NW / 8 : 8);
 #pragma unroll
   for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int row = f.row(mt, h), t = O + row;
-      const bool ok = row < g.V && t < g.Tout;
+      const int row = f.row(mt, h), t = t0 + row;
+      // one comparison for the row window: a second one makes ptxas spill more at N = 256
+      const bool ok = (unsigned)(row - r0) < (unsigned)(r1 - r0) && t < g.Tout;
       const int64_t base = ((int64_t)b * p.Cout + f.col) * g.Tout + t;   // element of column f.col
 #pragma unroll
       for (int c0 = 0; c0 < NW / 8; c0 += G) {
@@ -737,9 +740,10 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     }
     // every MMA of this tile has completed: the producer may load the next X
     batches.release(-1, 0);
-    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V)
-    epilogue_out<NW, BF16, EP_ACC_PREV>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
-                                        [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
+    // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); acc_prev (which may alias y) is read in batches
+    add_terms<NW>(xr, f, nullptr, nullptr, p.acc_prev, p, g, b, O - g.H, g.H, g.H + g.V);
+    epilogue_out<NW, BF16, 0>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
+                              [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
   }
 }
 
@@ -862,7 +866,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
       batches.wr.skip((n - 1 - cw) * per_step, g.nstages);
       // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
       const Frag<MT> f(0);
-      add_terms<NW>(acc, f, bias_s + NW, p.residual, p.acc_prev, p, g, b, O);
+      add_terms<NW>(acc, f, bias_s + NW, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
       epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
                                       [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
     }
@@ -920,9 +924,9 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
             acc[mt][i] += b2[(i >> 2) * 8 + f.col + (i & 1)];
             if (p.residual) acc[mt][i] += xres[mt][i];
           }
-        add_terms<NW>(acc, f, nullptr, nullptr, p.acc_prev, p, g, b, O);
+        add_terms<NW>(acc, f, nullptr, nullptr, p.acc_prev, p, g, b, O, 0, g.V);
       } else {
-        add_terms<NW>(acc, f, b2, p.residual, p.acc_prev, p, g, b, O);
+        add_terms<NW>(acc, f, b2, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
       }
       epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
                                       [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
@@ -1465,7 +1469,7 @@ int with_nw(const HcGeom& g, int precision, F f) {
   return fail(AB_ERR_UNSUPPORTED, "tc conv: N block %u", g.stage_bytes / 64u);
 }
 
-// Block-mode geometry: npairs x nconv convs of one ResBlock (C <= 64) with the halo recomputed inside the tile.
+// Block-mode geometry: npairs x nconv convs of one ResBlock (C <= 128) with the halo recomputed inside the tile.
 int make_chain_geom(int C, int k, const int* dil, int npairs, int nconv, int T, HcGeom& g) {
   if (npairs < 1 || npairs > AB_TC_CHAIN_MAX_PAIRS || (nconv != 1 && nconv != 2) || !tc_conv_supported(C, k))
     return fail(AB_ERR_UNSUPPORTED, "tc block: unsupported block");

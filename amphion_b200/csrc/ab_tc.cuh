@@ -48,14 +48,16 @@ bool tc_can_emit_image(int mode, int cin, int cout, int k, int d_or_u);
 int launch_tc_conv(const TcConvParams& p, cudaStream_t s);
 
 
-// One whole ResBlock per launch ("block mode", C <= 64): npairs x nconv k-tap convs with the residual stream x_p in
+// One whole ResBlock per launch ("block mode", C <= 128): npairs x nconv k-tap convs with the residual stream x_p in
 // registers and the halo recomputed inside the time tile, so the block reads its input once and writes its output once.
+// The residual stream takes as many registers per thread as the accumulators (64 up to N = 128, one m64 tile per
+// consumer warpgroup at 128); at N = 256 the two would need 128 + 128.
 //   for q < npairs:  x <- x + conv[q][1](lrelu(conv[q][0](lrelu(x, slope), dil[q]) + b, slope), 1) + b   (nconv == 2)
 //                    x <- x + conv[q][0](lrelu(x, slope), dil[q]) + b                                      (nconv == 1)
 //   y = (x + acc_prev) / out_div ; yimg = cvt(lrelu(y, img_slope))
 // Same arithmetic in the same order as npairs launches of launch_tc_conv: the results are bit-equal.
 constexpr int AB_TC_CHAIN_MAX_PAIRS = 3;
-constexpr int AB_TC_CHAIN_MAX_C = 64;
+constexpr int AB_TC_CHAIN_MAX_C = 128;
 struct TcChainParams {
   const float* x;          // contiguous [B, C, T] fp32 (block input = first residual)
   const uint16_t* ximg;    // nullable: operand image of lrelu(x, slope), [B][ceil16(C)/8][T][8]

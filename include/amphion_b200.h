@@ -207,7 +207,7 @@ typedef struct ab_profile_entry {
 int ab_generator_set_profiling(ab_generator* g, int32_t enable);
 /* Execution-plan options (no reference counterpart; tuning / test knobs, results stay within the stated tolerance):
  *   "resblock_fusion": 0, 1 = one launch per (c1, c2) pair (the intermediate stays in shared memory); 2 (default) = a
- *   whole ResBlock per launch (residual stream in registers, halo recomputed in the tile) where served (C <= 64) and
+ *   whole ResBlock per launch (residual stream in registers, halo recomputed in the tile) where served (C <= 128) and
  *   the recompute is small, else per pair; 3, 4 = a whole ResBlock per launch wherever served.  All plans run the same
  *   arithmetic in the same order: their outputs are bit-equal.
  *   "pair_schedule": how a per-pair launch at 64 and 128 channels (N block 64 or 128) shares its CTA's two consumer
