@@ -1,7 +1,7 @@
 """Block mode (`hchain_kernel`, one launch per ResBlock: `resblock_fusion` 3) at 128 channels against the per-pair
-launches (`hpair_kernel`, `resblock_fusion` 1).  Both run the same arithmetic in the same order, so the 128-channel
-pairs, which have no second kernel of their own, are checked bit for bit here as the 64- and 32-channel ones are in
-test_pair_kernel.py."""
+launches (`hpair_kernel`, `resblock_fusion` 1).  Both run the same arithmetic in the same order, so the outputs must
+be bit-equal, as the 64- and 32-channel ones are in test_pair_kernel.py.  Agreement of the two routes does not show
+that either is right: test_resblock_exact.py checks each of them against the operand-rounded oracle bit for bit."""
 import pytest
 import torch
 

@@ -1,9 +1,9 @@
 """ResBlock pair launches (`hpair_kernel`, one launch per dilation pair: `resblock_fusion` 1) on small HiFi-GAN
 generators.  Each case is checked against whole-block launches (`resblock_fusion` 3) bit for bit where block mode
-serves the stage (C <= 64), and against the CPU oracle where it does not.  At N = 128 and 256 there is no second
-kernel to compare with bit for bit, so a change of accumulation order or epilogue association there would pass the
-oracle bars; the bit-equality of those stages rests on comparing `bench.py --dump-outputs` with the previous
-version.  Every generator has at least two stages
+serves the stage (C <= 64), and against the CPU oracle where it does not.  The bars here are whole-generator ones;
+the bit-level check of every route at every width (N = 128 and 256 included) is test_resblock_exact.py, which
+compares single stages with one-hot weights against the operand-rounded oracle exactly.  A change of the fp32
+accumulation order alone passes both.  Every generator has at least two stages
 and two ResBlock kernel sizes, so the branch sum (`acc_prev` aliasing `y`) and the operand image a stage emits for
 the next one are exercised."""
 import numpy as np
