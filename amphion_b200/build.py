@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libamphion_b200.so")
-SOURCES = ["ab_capi.cu", "ab_kernels_fp32.cu", "ab_kernels_tc.cu", "ab_mel.cu", "ab_pcm.cu", "ab_diffwave.cu"]
+SOURCES = ["ab_capi.cu", "ab_kernels_fp32.cu", "ab_kernels_tc.cu", "ab_mel.cu", "ab_pcm.cu", "ab_diffwave.cu", "ab_facodec.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

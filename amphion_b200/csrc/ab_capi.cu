@@ -58,6 +58,7 @@ struct Slot {
   int dilation;       // Conv1d dilation (SLOT_CONV_W)
   float gain = 1.0f;  // applied to the fp32 image at load time (NSF-HiFiGAN: 2 on every ups weight / bias)
   bool head_cols = false;   // Vocos' head.out: the weight image pairs each bin's magnitude and phase rows
+  bool no_tc = false;       // never runs on the wgmma kernel (FACodec's out_proj, read by the vq2emb kernel)
 };
 
 struct ConvRef {   // one weight-normed conv of the model
@@ -112,7 +113,19 @@ struct StageRef {
   int u = 1;
   int ch = 0;
   bool has_up = true;   // false: AB_GEN_TRUNK's single stage (no transposed conv in front of the blocks)
+  ActRef act;           // AB_GEN_FACODEC: the DecoderBlock's Activation1d in front of the transposed conv
   std::vector<BlockRef> blocks;
+};
+
+// FACodec (AB_GEN_FACODEC): timbre_linear and the codebook layers of the three ResidualVQs, in code-row order
+struct FacodecLayerRef {
+  int cb = -1;
+  ConvRef out_proj;
+  int64_t rows = 0;
+};
+struct FacodecRef {
+  int style_w = -1, style_b = -1;
+  std::vector<FacodecLayerRef> layers;
 };
 
 }  // namespace
@@ -142,6 +155,7 @@ struct ab_generator {
   std::vector<StageRef> stages;
   VocosRef vocos;
   DiffWaveRef dw;
+  FacodecRef fac;
   ab_mel* istft = nullptr;   // Vocos: the iSTFT plan (cuFFT C2R + overlap-add of ab_istft_forward)
 
   // profiling (ab_generator_set_profiling)
@@ -254,10 +268,48 @@ int validate_diffwave_config(const ab_generator_config& c) {
   return AB_OK;
 }
 
+// AB_GEN_FACODEC: the decoder's fixed block structure (facodec.py:121-133, :220-240) and the ResidualVQ geometry
+int validate_facodec_config(const ab_generator_config& c) {
+  if (c.gin_channels || c.conv_post_no_bias || c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel ||
+      c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop || c.dilation_cycle || c.embedding_rows)
+    return fail(AB_ERR_ARG, "config: FACodec uses only the generator fields and vq_* (gin / trunk / Vocos / DiffWave fields must be 0)");
+  const int lim = 1 << 16;
+  if (c.n_mel <= 0 || c.n_mel > lim || c.upsample_initial_channel <= 0 || c.upsample_initial_channel > lim)
+    return fail(AB_ERR_ARG, "config: FACodec in_channels %d / upsample_initial_channel %d out of range", c.n_mel,
+                c.upsample_initial_channel);
+  if (c.num_upsamples <= 0 || c.num_upsamples > AB_MAX_STAGES || (c.upsample_initial_channel >> c.num_upsamples) <= 0)
+    return fail(AB_ERR_ARG, "config: FACodec up_ratios: %d stages for %d channels", c.num_upsamples, c.upsample_initial_channel);
+  for (int i = 0; i < c.num_upsamples; ++i)
+    if (c.upsample_rates[i] <= 0 || c.upsample_rates[i] > 64 || c.upsample_kernel_sizes[i] != 2 * c.upsample_rates[i])
+      return fail(AB_ERR_ARG, "config: FACodec stage %d: ratio %d (1..64) with kernel %d (must be 2 x ratio)", i,
+                  c.upsample_rates[i], c.upsample_kernel_sizes[i]);
+  if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
+      c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
+    return fail(AB_ERR_ARG, "config: FACodec DecoderBlocks hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, "
+                            "num_kernels 1, kernel 7, 3 dilations");
+  if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
+    return fail(AB_ERR_ARG, "config: FACodec uses SnakeBeta with alpha_logscale = True");
+  if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
+      c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
+    return fail(AB_ERR_ARG, "config: FACodec vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, at most %d in all",
+                c.vq_num_q[0], c.vq_num_q[1], c.vq_num_q[2], AB_FACODEC_MAX_Q);
+  for (int i = 0; i < 3; ++i)
+    if (c.vq_codebook_bits[i] <= 0 || c.vq_codebook_bits[i] > 24)
+      return fail(AB_ERR_ARG, "config: FACodec codebook size 2^%d out of range (bits 1..24)", c.vq_codebook_bits[i]);
+  if (c.vq_codebook_dim <= 0 || c.vq_codebook_dim > FAC_MAX_CODEBOOK_DIM || c.vq_codebook_dim == c.n_mel)
+    return fail(AB_ERR_UNSUPPORTED, "config: FACodec codebook_dim %d (1..%d, != vq_dim: out_proj must be a Linear)",
+                c.vq_codebook_dim, FAC_MAX_CODEBOOK_DIM);
+  return AB_OK;
+}
+
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
-      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE)
+      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
+  if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
+  for (int i = 0; i < 3; ++i)
+    if (c.vq_num_q[i] || c.vq_codebook_bits[i]) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
+  if (c.vq_codebook_dim) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
   if (c.kind == AB_GEN_DIFFWAVE) return validate_diffwave_config(c);
   if (c.dilation_cycle || c.embedding_rows) return fail(AB_ERR_ARG, "config: dilation_cycle / embedding_rows belong to AB_GEN_DIFFWAVE");
   if (c.kind == AB_GEN_VOCOS) return validate_vocos_config(c);
@@ -435,6 +487,57 @@ void add_melgan_tensors(ab_generator* g) {
   g->conv_post.reflect = true;
 }
 
+ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout);   // below
+
+// FACodec decoder tensors (AB_GEN_FACODEC), the reference's names (facodec.py:121-133, :220-240, :286-369, fvq.py:23-29)
+void add_facodec_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int c0 = cfg->upsample_initial_channel, n = cfg->num_upsamples;
+  auto mod = [](int i) { return "model." + std::to_string(i); };
+  g->conv_pre = make_conv(g, mod(0), cfg->n_mel, c0, 7, 1, false);
+  int ch = c0;
+  for (int i = 0; i < n; ++i) {
+    StageRef st;
+    const std::string base = mod(1 + i) + ".block.";
+    const int cin = c0 >> i;
+    ch = st.ch = c0 >> (i + 1);
+    st.u = cfg->upsample_rates[i];
+    g->hop *= st.u;
+    st.act = make_act(g, base + "0", cin, true);
+    st.up = make_conv(g, base + "1", cin, ch, 2 * st.u, 1, true);
+    g->slots[st.up.w].stride = st.u;
+    BlockRef blk;   // the three ResidualUnits as one AMPBlock1-like block: act, k = 7 conv, act, k = 1 conv per unit
+    blk.k = 7;
+    for (int p = 0; p < 3; ++p) {
+      const int d = cfg->resblock_dilation_sizes[0][p];
+      const std::string pre = base + std::to_string(2 + p) + ".block.";
+      blk.dil.push_back(d);
+      blk.acts.push_back(make_act(g, pre + "0", ch, true));
+      blk.c1.push_back(make_conv(g, pre + "1", ch, ch, 7, d, false));
+      blk.acts.push_back(make_act(g, pre + "2", ch, true));
+      blk.c2.push_back(make_conv(g, pre + "3", ch, ch, 1, 1, false));
+    }
+    st.blocks.push_back(blk);
+    g->stages.push_back(st);
+  }
+  g->act_post = make_act(g, mod(1 + n), ch, true);
+  g->conv_post = make_conv(g, mod(2 + n), ch, 1, 7, 1, false);
+  FacodecRef& f = g->fac;
+  const int C = cfg->n_mel, D = cfg->vq_codebook_dim;
+  f.style_w = g->add_slot("timbre_linear.weight", SLOT_VEC, {2 * C, C});
+  f.style_b = g->add_slot("timbre_linear.bias", SLOT_VEC, {2 * C});
+  for (int q = 0; q < 3; ++q)
+    for (int j = 0; j < cfg->vq_num_q[q]; ++j) {
+      const std::string pre = "quantizer." + std::to_string(q) + ".layers." + std::to_string(j) + ".";
+      FacodecLayerRef l;
+      l.rows = (int64_t)1 << cfg->vq_codebook_bits[q];
+      l.cb = g->add_slot(pre + "_codebook.weight", SLOT_VEC, {l.rows, D});
+      l.out_proj = make_linear(g, pre + "out_proj", D, C);
+      g->slots[l.out_proj.w].no_tc = true;
+      f.layers.push_back(l);
+    }
+}
+
 // nn.Linear(cin, cout) as a k = 1 conv: weight [out, in] (state-dict shape), repacked as [in][1][out]
 ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout) {
   ConvRef c;
@@ -575,6 +678,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     }
   } else if (cfg->kind == AB_GEN_DIFFWAVE) {
     add_diffwave_tensors(g);
+  } else if (cfg->kind == AB_GEN_FACODEC) {
+    add_facodec_tensors(g);
   } else {
     add_gan_tensors(g);
   }
@@ -583,7 +688,7 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
   size_t tc = 0;
   for (size_t i = 0; i < g->slots.size(); ++i) {
     Slot& s = g->slots[i];
-    s.tc_bytes = tc_image_bytes(s, (int)i == g->conv_pre.w || (int)i == g->conv_post.w);
+    s.tc_bytes = s.no_tc ? 0 : tc_image_bytes(s, (int)i == g->conv_pre.w || (int)i == g->conv_post.w);
     s.tc_offset = g->fp32_bytes + tc;
     tc += align_up(s.tc_bytes, 256);
   }
@@ -810,12 +915,25 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
   return std::max<int64_t>(std::min(Tn, xs), 0);
 }
 
+// bytes of forward_impl's buffers (the stage buffers and operand images)
+static size_t gan_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
+  return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
+         NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
+}
+
+// FACodec: forward_impl's buffers, then the FiLM output (fp32, or conv_pre's operand image) and the style [B][2C]
+static size_t facodec_film_bytes(const ab_generator* g, int64_t B, int64_t T) {
+  const int C = g->cfg.n_mel;
+  return align_up(std::max((size_t)B * C * T * sizeof(float), tc_act_image_bytes(B, C, T)), 256);
+}
+
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
   if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return 0;
-  return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
-         NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
+  if (g->cfg.kind == AB_GEN_FACODEC)
+    return gan_workspace_bytes(g, B, T) + facodec_film_bytes(g, B, T) + align_up((size_t)B * 2 * g->cfg.n_mel * sizeof(float), 256);
+  return gan_workspace_bytes(g, B, T);
 }
 
 int ab_generator_last_launches(const ab_generator* g) { return g ? g->launches : 0; }
@@ -869,11 +987,11 @@ int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
 
 int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max_entries, int32_t* n_out) {
   if (!g || !out || !n_out) return fail(AB_ERR_ARG, "get_profile: null argument");
-  static const char* kNames[11] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
+  static const char* kNames[12] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
                                    "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
-                                   "diffwave_tail"};
-  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's
-  const int n = g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
+                                   "diffwave_tail", "facodec_prologue"};
+  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's
+  const int n = g->cfg.kind == AB_GEN_FACODEC ? 12 : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
   for (int i = 0; i < n; ++i) {
     memset(&out[i], 0, sizeof(out[i]));
@@ -902,9 +1020,10 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
 // slower in block mode than as pairs on an H100 (DESIGN.md §6).
 static constexpr double kChainMaxRecompute = 1.5;
 
+// x_img (FACodec at tensor-core precision): conv_pre's input as an operand image, in place of dev_mel
 static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
                         const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
-                        size_t workspace_bytes, void* stream) {
+                        size_t workspace_bytes, void* stream, const uint16_t* x_img = nullptr) {
   if (!g || !dev_mel || !dev_wav || !mel_strides) return fail(AB_ERR_ARG, "forward: null argument");
   if (dev_g != nullptr && g->cond_w < 0) return fail(AB_ERR_STATE, "forward: conditioning given but the generator has gin_channels == 0");
   if (dev_g != nullptr && g_batch_stride < g->cfg.gin_channels) return fail(AB_ERR_ARG, "forward: g row stride < gin_channels");
@@ -939,7 +1058,9 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   uint16_t *U16 = img[0], *P16[2] = {img[1], img[2]}, *R16 = img[3];
   const uint16_t* r_img = nullptr;   // operand image of lrelu(stage input, 0.1) when the previous stage emitted it
   float *R[2] = {buf[0], buf[1]}, *U = buf[2], *P[2] = {buf[3], buf[4]}, *TMP = buf[5], *ACT = buf[6];
-  const bool big = g->cfg.kind == AB_GEN_BIGVGAN;
+  // FACodec's generator is BigVGAN's pipeline with an activation in front of each transposed conv
+  const bool fac = g->cfg.kind == AB_GEN_FACODEC;
+  const bool big = g->cfg.kind == AB_GEN_BIGVGAN || fac;
   const bool tc = g->precision != AB_PREC_FP32;
   const int nk = g->cfg.num_kernels;
   int launches = 0;
@@ -1123,7 +1244,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   const bool pre_img = !big && !melgan && dev_g == nullptr && on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&
                        on_tc(g->stages[0].up) && (C0 % 16) == 0 &&
                        tc_can_emit_image(0, cpre.cin, cpre.cout, cpre.k, cpre.d);
-  rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, R[0],
+  rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], x_img, R[0],
                              pre_img ? R16 : nullptr, (int)T, 1.0f, nullptr, nullptr, 1.0f, 0,
                              conv_bytes(cpre, (int)T, nullptr, nullptr) + (pre_img ? 2.0 * B * T * C0 : 0.0))
                    : conv(cpre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], R[0], (int)T, 1.0f,
@@ -1147,6 +1268,16 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       std::swap(U, R[cur_r]);   // AB_GEN_TRUNK: the blocks read conv_pre's output in place
     } else {
       const bool up_tc = on_tc(sg.up);
+      // FACodec: x = Activation1d(SnakeBeta)(x) in front of the transposed conv (facodec.py:224-232), as the operand
+      // image the tensor-core ConvTranspose reads or as fp32
+      const float* up_x = R[cur_r];
+      if (fac) {
+        const bool img = up_tc && (cin % 16) == 0;
+        rc = img ? snake(sg.act, R[cur_r], nullptr, cin, Tn, P16[0]) : snake(sg.act, R[cur_r], ACT, cin, Tn);
+        if (rc != AB_OK) return rc;
+        r_img = img ? P16[0] : nullptr;
+        up_x = ACT;
+      }
       // x = leaky_relu(x, 0.2) ; x = ConvTranspose1d(k = 2u, padding u//2 + u%2, output_padding u%2) (melgan.py:72-80)
       const float pre_slope = big ? 1.0f : melgan ? 0.2f : 0.1f;
       ++launches;
@@ -1156,20 +1287,20 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       if (up_tc) {
         TcConvParams p;
         p.mode = 1;
-        p.x = R[cur_r]; p.xsb = (int64_t)cin * Tn; p.xsc = Tn; p.xst = 1; p.pre_slope = pre_slope;
+        p.x = up_x; p.xsb = (int64_t)cin * Tn; p.xsc = Tn; p.xst = 1; p.pre_slope = pre_slope;
         p.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr;
         p.w = g->tcptr(sg.up.w); p.bias = g->fptr(sg.up.b); p.y = U;
         // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
         u_img = (!big && !melgan && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
         p.yimg = u_img; p.img_slope = 0.1f;
         p.B = (int)B; p.Cin = cin; p.Cout = sg.ch; p.T = Tn; p.k = sg.up.k; p.d_or_u = sg.u; p.precision = g->precision;
-        p.pad = melgan ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
+        p.pad = melgan || fac ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
         rc = launch_tc_conv(p, st);
       } else {
         ConvTParams tp;
-        tp.x = R[cur_r]; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
+        tp.x = up_x; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
         tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u; tp.pre_slope = pre_slope;
-        tp.pad = melgan ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
+        tp.pad = melgan || fac ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
         rc = launch_conv_transpose1d_fp32(tp, st);
       }
       prof_end();
@@ -1358,12 +1489,14 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
 int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64_t T,
                          const int64_t mel_strides[3], float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream) {
+  if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   return forward_impl(g, dev_mel, B, T, mel_strides, nullptr, 0, dev_wav, dev_workspace, workspace_bytes, stream);
 }
 
 int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
                               const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
                               size_t workspace_bytes, void* stream) {
+  if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   return forward_impl(g, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes, stream);
 }
 
@@ -1536,6 +1669,101 @@ int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t B, int6
                         ws_bytes, stream);
   if (rc != AB_OK) return rc;
   g->launches += cond_launches;
+  return AB_OK;
+}
+
+// ---------------------------------------------------------------------------
+// FACodec decoder
+// ---------------------------------------------------------------------------
+static int facodec_check(const ab_generator* g, int64_t B, int64_t T, const char* what) {
+  if (!g) return fail(AB_ERR_ARG, "%s: null handle", what);
+  if (g->cfg.kind != AB_GEN_FACODEC) return fail(AB_ERR_ARG, "%s: not a FACodec handle", what);
+  if (!g->finalized) return fail(AB_ERR_STATE, "%s: finalize() the generator first", what);
+  if (B <= 0 || T <= 0 || B > 65535) return fail(AB_ERR_ARG, "%s: batch %lld / frames %lld out of range", what, (long long)B, (long long)T);
+  if (T * g->hop > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "%s: sequence too long", what);
+  return AB_OK;
+}
+
+int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q, int64_t B,
+                      int64_t T, int32_t use_residual, float* dev_out, void* stream) {
+  int rc = facodec_check(g, B, T, "facodec_vq2emb");
+  if (rc != AB_OK) return rc;
+  if (!dev_codes || !codes_strides || !dev_out) return fail(AB_ERR_ARG, "facodec_vq2emb: null argument");
+  const int* nq = g->cfg.vq_num_q;
+  const int n_all = nq[0] + nq[1] + nq[2], n_pc = nq[0] + nq[1];
+  // facodec.py:564: the residual group joins when the decoder has one and use_residual_code is set
+  const bool resid = use_residual && nq[2] > 0;
+  if (n_q != n_all && !(!use_residual && n_q == n_pc))
+    return fail(AB_ERR_ARG, "facodec_vq2emb: %d code rows; the decoder has %d (%d prosody, %d content, %d residual)", n_q,
+                n_all, nq[0], nq[1], nq[2]);
+  FacVqParams p;
+  memset(&p, 0, sizeof(p));
+  p.codes = dev_codes; p.cs0 = codes_strides[0]; p.cs1 = codes_strides[1]; p.cs2 = codes_strides[2];
+  p.nq = resid ? n_all : n_pc;
+  for (int q = 0; q < p.nq; ++q) {
+    const FacodecLayerRef& l = g->fac.layers[q];
+    p.cb[q] = g->fptr(l.cb); p.w[q] = g->fptr(l.out_proj.w); p.bias[q] = g->fptr(l.out_proj.b); p.rows[q] = l.rows;
+  }
+  p.group_end[0] = nq[0]; p.group_end[1] = n_pc; p.group_end[2] = n_all;
+  p.ngroups = resid ? 3 : 2;
+  p.B = (int)B; p.C = g->cfg.n_mel; p.T = (int)T; p.D = g->cfg.vq_codebook_dim; p.out = dev_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DwProf prof{g, st};
+  const double el = (double)B * T;
+  prof.begin(11, 2.0 * el * p.nq * p.C * p.D, 8.0 * el * p.nq + 4.0 * el * p.C + 4.0 * p.nq * (double)p.C * (p.D + 1));
+  rc = launch_facodec_vq2emb(p, st);
+  prof.end();
+  if (rc != AB_OK) return rc;
+  g->launches = 1;
+  return AB_OK;
+}
+
+int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
+                         const float* dev_spk, int64_t spk_row_stride, float* dev_wav, void* dev_workspace,
+                         size_t workspace_bytes, void* stream) {
+  int rc = facodec_check(g, B, T, "facodec_inference");
+  if (rc == AB_OK && (!dev_x || !x_strides || !dev_spk || !dev_wav))
+    rc = fail(AB_ERR_ARG, "facodec_inference: null argument");
+  const int C = g ? g->cfg.n_mel : 0;
+  if (rc == AB_OK && spk_row_stride < C) rc = fail(AB_ERR_ARG, "facodec_inference: speaker-embedding row stride < %d", C);
+  const size_t need = ab_generator_workspace_bytes(g, B, T);
+  if (rc == AB_OK && (!dev_workspace || workspace_bytes < need))
+    rc = fail(AB_ERR_WORKSPACE, "facodec_inference: workspace %zu B < required %zu B", workspace_bytes, need);
+  if (rc == AB_OK && (reinterpret_cast<uintptr_t>(dev_workspace) & 255))
+    rc = fail(AB_ERR_ARG, "facodec_inference: workspace must be 256-byte aligned");
+  if (rc != AB_OK) {
+    if (g) g->tail_events.clear();
+    return rc;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  char* film = static_cast<char*>(dev_workspace) + gan_workspace_bytes(g, B, T);
+  float* style = reinterpret_cast<float*>(film + facodec_film_bytes(g, B, T));
+  // conv_pre reads the FiLM output as its operand image when it runs on the wgmma kernel
+  const bool img = g->precision != AB_PREC_FP32 && g->slots[g->conv_pre.w].tc_bytes > 0;
+  DwProf prof{g, st};
+  const double el = (double)B * T;
+  prof.begin(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C));
+  rc = launch_facodec_style(dev_spk, spk_row_stride, g->fptr(g->fac.style_w), g->fptr(g->fac.style_b), style, (int)B, C, st);
+  prof.end();
+  if (rc == AB_OK) {
+    FacFilmParams p;
+    p.x = dev_x; p.xsb = x_strides[0]; p.xsc = x_strides[1]; p.xst = x_strides[2];
+    p.style = style; p.y = img ? nullptr : reinterpret_cast<float*>(film);
+    p.yimg = img ? reinterpret_cast<uint16_t*>(film) : nullptr; p.bf16 = g->precision == AB_PREC_TC_BF16;
+    p.B = (int)B; p.C = C; p.T = (int)T;
+    prof.begin(11, 10.0 * el * C, 4.0 * el * C + (img ? 2.0 * el * ((C + 15) / 16 * 16) : 4.0 * el * C));
+    rc = launch_facodec_film(p, st);
+    prof.end();
+  }
+  if (rc != AB_OK) {
+    g->tail_events.clear();
+    return rc;
+  }
+  const int64_t strides[3] = {(int64_t)C * T, T, 1};
+  rc = forward_impl(g, reinterpret_cast<const float*>(film), B, T, strides, nullptr, 0, dev_wav, dev_workspace,
+                    workspace_bytes, stream, img ? reinterpret_cast<const uint16_t*>(film) : nullptr);
+  if (rc != AB_OK) return rc;
+  g->launches += 2;
   return AB_OK;
 }
 

@@ -215,6 +215,34 @@ int launch_dw_layer(const DwLayerParams& p, cudaStream_t s);
 int launch_dw_tail(const DwTailParams& p, cudaStream_t s);
 int launch_dw_pack(const DwPackParams& p, cudaStream_t s);
 
+// ---- FACodec decoder prologue (ab_facodec.cu) ----------------------------
+constexpr int FAC_MAX_CODEBOOK_DIM = 16;
+struct FacFilmParams {      // y = LayerNorm(x over channels, eps 1e-5, no affine) * gamma + beta
+  const float* x;           // [B, C, T] with element strides xsb / xsc / xst
+  int64_t xsb, xsc, xst;
+  const float* style;       // [B][2C]: gamma then beta (timbre_linear's output)
+  float* y;                 // fp32 [B, C, T], or
+  uint16_t* yimg;           // 16-bit operand image [B][ceil16(C)/8][T][8] (padding channels zero)
+  int bf16;
+  int B, C, T;
+};
+struct FacVqParams {        // out [B, C, T] = sum over the groups of (sum over the group's layers of out_proj(codebook[code]))
+  const int64_t* codes;     // [nq, B, T] with element strides cs0 / cs1 / cs2
+  int64_t cs0, cs1, cs2;
+  const float* cb[AB_FACODEC_MAX_Q];     // codebook [rows][D]
+  const float* w[AB_FACODEC_MAX_Q];      // out_proj, repacked [D][C] (weight norm folded)
+  const float* bias[AB_FACODEC_MAX_Q];   // [C]
+  int64_t rows[AB_FACODEC_MAX_Q];
+  int group_end[3];         // layer q belongs to the first group g with q < group_end[g]
+  int ngroups, nq;
+  int B, C, T, D;
+  float* out;
+};
+int launch_facodec_style(const float* spk, int64_t spk_stride, const float* w, const float* bias, float* style, int B,
+                         int C, cudaStream_t s);
+int launch_facodec_film(const FacFilmParams& p, cudaStream_t s);
+int launch_facodec_vq2emb(const FacVqParams& p, cudaStream_t s);
+
 // launchers (ab_kernels_fp32.cu)
 int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);

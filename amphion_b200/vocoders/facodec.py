@@ -1,0 +1,350 @@
+"""FACodecDecoder — drop-in for the decoder of NaturalSpeech 3's FACodec (``models/codec/ns3_codec/facodec.py:242``):
+the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_proj,out_proj,_codebook}``, ``model.*``,
+``timbre_encoder.*``, ``timbre_linear``, the ``CNNLSTM`` predictors and the ``use_gr_*`` heads), so the released
+``ns3_facodec_decoder.bin`` loads strictly.  The waveform path runs natively (``AB_GEN_FACODEC``):
+
+- ``vq2emb(vq, use_residual_code=True)``: codes ``[n_q, B, T]`` -> ``[B, in_channels, T]`` (:556-566);
+- ``inference(x, speaker_embedding)``: the timbre FiLM (LayerNorm over channels, ``x * gamma + beta``) and the
+  BigVGAN-family generator -> ``[B, 1, T * prod(up_ratios)]`` (:568-576).
+
+The encoder-side ``forward`` (quantization, the timbre transformer) and the training branch are not served; the modules
+only ``forward`` evaluates are kept as parameters."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+from torch import nn
+from torch.nn.utils import remove_weight_norm, weight_norm
+
+from .. import _capi
+from .activations import Activation1d, SnakeBeta
+from .generator import NativeGenerator
+
+_SERVED = "amphion_b200 serves FACodecDecoder.vq2emb() and FACodecDecoder.inference()"
+
+
+def _native_only(name):
+    raise RuntimeError(f"amphion_b200: FACodec's {name} executes inside the decoder's CUDA pipeline; {_SERVED}")
+
+
+def _act(ch):
+    return Activation1d(activation=SnakeBeta(ch, alpha_logscale=True))
+
+
+class ResidualUnit(nn.Module):
+    """Parameter holder for facodec.py:121-133: act, WNConv1d(k = 7, dilation), act, WNConv1d(k = 1)."""
+
+    def __init__(self, dim: int = 16, dilation: int = 1):
+        super().__init__()
+        pad = ((7 - 1) * dilation) // 2
+        self.block = nn.Sequential(
+            _act(dim), weight_norm(nn.Conv1d(dim, dim, kernel_size=7, dilation=dilation, padding=pad)),
+            _act(dim), weight_norm(nn.Conv1d(dim, dim, kernel_size=1)))
+
+    def forward(self, x):
+        _native_only("ResidualUnit")
+
+
+class DecoderBlock(nn.Module):
+    """Parameter holder for facodec.py:220-239."""
+
+    def __init__(self, input_dim: int = 16, output_dim: int = 8, stride: int = 1):
+        super().__init__()
+        self.block = nn.Sequential(
+            _act(input_dim),
+            weight_norm(nn.ConvTranspose1d(input_dim, output_dim, kernel_size=2 * stride, stride=stride,
+                                           padding=stride // 2 + stride % 2, output_padding=stride % 2)),
+            ResidualUnit(output_dim, dilation=1), ResidualUnit(output_dim, dilation=3), ResidualUnit(output_dim, dilation=9))
+
+    def forward(self, x):
+        _native_only("DecoderBlock")
+
+
+class FactorizedVectorQuantize(nn.Module):
+    """Parameter holder for quantize/fvq.py:16-29 (dim != codebook_dim: weight-normed in_proj / out_proj)."""
+
+    def __init__(self, dim, codebook_size, codebook_dim, commitment=0.005, **kwargs):
+        super().__init__()
+        self.codebook_size, self.codebook_dim, self.commitment = codebook_size, codebook_dim, commitment
+        self.in_proj = weight_norm(nn.Linear(dim, codebook_dim))
+        self.out_proj = weight_norm(nn.Linear(codebook_dim, dim))
+        self._codebook = nn.Embedding(codebook_size, codebook_dim)
+
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError(f"FACodec quantization is not served; {_SERVED}")
+
+
+class ResidualVQ(nn.Module):
+    """Parameter holder for quantize/rvq.py:12-25."""
+
+    def __init__(self, *, num_quantizers, codebook_size, **kwargs):
+        super().__init__()
+        if isinstance(codebook_size, int):
+            codebook_size = [codebook_size] * num_quantizers
+        self.layers = nn.ModuleList([FactorizedVectorQuantize(codebook_size=2 ** s, **kwargs) for s in codebook_size])
+        self.num_quantizers = num_quantizers
+
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError(f"FACodec quantization is not served; {_SERVED}")
+
+
+class _Holder(nn.Module):
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError(f"amphion_b200: {type(self).__name__} is not served; {_SERVED}")
+
+
+class GradientReversal(_Holder):
+    """gradient_reversal.py:29-35 (no state-dict entries)."""
+
+    def __init__(self, alpha):
+        super().__init__()
+        self.alpha = torch.tensor(alpha, requires_grad=False)
+
+
+class CNNLSTM(_Holder):
+    """Parameter holder for facodec.py:35-54 (the f0 / phone predictors)."""
+
+    def __init__(self, indim, outdim, head, global_pred=False):
+        super().__init__()
+        self.global_pred = global_pred
+        self.model = nn.Sequential(ResidualUnit(indim, dilation=1), ResidualUnit(indim, dilation=2),
+                                   ResidualUnit(indim, dilation=3), _act(indim))
+        self.heads = nn.ModuleList([nn.Linear(indim, outdim) for _ in range(head)])
+
+
+class _PositionalEncoding(_Holder):
+    """transformer.py:35-47: the persistent ``pe`` buffer [max_len, 1, d_model]."""
+
+    def __init__(self, d_model, max_len=5000):
+        super().__init__()
+        self.register_buffer("pe", torch.zeros(max_len, 1, d_model))
+
+
+class _FFN(_Holder):
+    def __init__(self, hidden, filt, k):
+        super().__init__()
+        self.ffn_1 = nn.Conv1d(hidden, filt, k, padding=k // 2)
+        self.ffn_2 = nn.Linear(filt, hidden)
+
+
+class _EncoderLayer(_Holder):
+    def __init__(self, hidden, heads, filt, k):
+        super().__init__()
+        self.ln_1 = nn.LayerNorm(hidden)
+        self.ln_2 = nn.LayerNorm(hidden)
+        self.self_attn = nn.MultiheadAttention(hidden, heads, batch_first=True)
+        self.ffn = _FFN(hidden, filt, k)
+
+
+class TransformerEncoder(_Holder):
+    """Parameter holder for transformer.py:154-217 (the timbre encoder, use_cln=False)."""
+
+    def __init__(self, encoder_layer=4, encoder_hidden=256, encoder_head=4, conv_filter_size=1024, conv_kernel_size=5):
+        super().__init__()
+        self.position_emb = _PositionalEncoding(encoder_hidden)
+        self.layers = nn.ModuleList([_EncoderLayer(encoder_hidden, encoder_head, conv_filter_size, conv_kernel_size)
+                                     for _ in range(encoder_layer)])
+        self.last_ln = nn.LayerNorm(encoder_hidden)
+
+
+class FACodecDecoder(NativeGenerator):
+    kind = "facodec"
+
+    def __init__(self, in_channels=256, upsample_initial_channel=1536, ngf=32, up_ratios=(5, 5, 4, 2), vq_num_q_c=2,
+                 vq_num_q_p=1, vq_num_q_r=3, vq_dim=1024, vq_commit_weight=0.005, vq_weight_init=False,
+                 vq_full_commit_loss=False, codebook_dim=8, codebook_size_prosody=10, codebook_size_content=10,
+                 codebook_size_residual=10, quantizer_dropout=0.0, dropout_type="linear", use_gr_content_f0=False,
+                 use_gr_prosody_phone=False, use_gr_residual_f0=False, use_gr_residual_phone=False,
+                 use_gr_x_timbre=False, use_random_mask_residual=True, prob_random_mask_residual=0.75):
+        super().__init__()
+        if in_channels != vq_dim:
+            # vq2emb's output is inference's input (README flow): the two widths must agree
+            raise ValueError(f"amphion_b200: FACodecDecoder needs in_channels == vq_dim (got {in_channels}, {vq_dim})")
+        if codebook_dim == vq_dim:
+            raise ValueError("amphion_b200: FACodecDecoder with codebook_dim == vq_dim (identity projections) is not served")
+        self.hop_length = int(np.prod(up_ratios))
+        self.ngf = ngf
+        self.up_ratios = [int(u) for u in up_ratios]
+        self.in_channels, self.upsample_initial_channel = int(in_channels), int(upsample_initial_channel)
+        self.use_random_mask_residual = use_random_mask_residual
+        self.prob_random_mask_residual = prob_random_mask_residual
+        self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r = int(vq_num_q_p), int(vq_num_q_c), int(vq_num_q_r)
+        self.codebook_size_prosody = codebook_size_prosody
+        self.codebook_size_content = codebook_size_content
+        self.codebook_size_residual = codebook_size_residual
+        self.codebook_dim = int(codebook_dim)
+
+        def rvq(n, size):
+            return ResidualVQ(num_quantizers=n, dim=vq_dim, codebook_size=size, codebook_dim=codebook_dim,
+                              commitment=vq_commit_weight)
+
+        self.quantizer = nn.ModuleList([rvq(vq_num_q_p, codebook_size_prosody), rvq(vq_num_q_c, codebook_size_content)])
+        if self.vq_num_q_r > 0:
+            self.quantizer.append(rvq(vq_num_q_r, codebook_size_residual))
+
+        channels = upsample_initial_channel
+        layers = [weight_norm(nn.Conv1d(in_channels, channels, kernel_size=7, padding=3))]
+        for i, stride in enumerate(up_ratios):
+            layers.append(DecoderBlock(channels // 2 ** i, channels // 2 ** (i + 1), stride))
+        output_dim = channels // 2 ** len(up_ratios)
+        layers += [_act(output_dim), weight_norm(nn.Conv1d(output_dim, 1, kernel_size=7, padding=3)), nn.Tanh()]
+        self.model = nn.Sequential(*layers)
+
+        self.timbre_encoder = TransformerEncoder()
+        self.timbre_linear = nn.Linear(in_channels, in_channels * 2)
+        self.timbre_linear.bias.data[:in_channels] = 1
+        self.timbre_linear.bias.data[in_channels:] = 0
+        self.timbre_norm = nn.LayerNorm(in_channels, elementwise_affine=False)
+        self.f0_predictor = CNNLSTM(in_channels, 1, 2)
+        self.phone_predictor = CNNLSTM(in_channels, 5003, 1)
+        self.use_gr_content_f0 = use_gr_content_f0
+        self.use_gr_prosody_phone = use_gr_prosody_phone
+        self.use_gr_residual_f0 = use_gr_residual_f0
+        self.use_gr_residual_phone = use_gr_residual_phone
+        self.use_gr_x_timbre = use_gr_x_timbre
+        if self.vq_num_q_r > 0 and use_gr_residual_f0:
+            self.res_f0_predictor = nn.Sequential(GradientReversal(alpha=1.0), CNNLSTM(in_channels, 1, 2))
+        if self.vq_num_q_r > 0 and use_gr_residual_phone > 0:
+            self.res_phone_predictor = nn.Sequential(GradientReversal(alpha=1.0), CNNLSTM(in_channels, 5003, 1))
+        if use_gr_content_f0:
+            self.content_f0_predictor = nn.Sequential(GradientReversal(alpha=1.0), CNNLSTM(in_channels, 1, 2))
+        if use_gr_prosody_phone:
+            self.prosody_phone_predictor = nn.Sequential(GradientReversal(alpha=1.0), CNNLSTM(in_channels, 5003, 1))
+        if use_gr_x_timbre:
+            self.x_timbre_predictor = nn.Sequential(GradientReversal(alpha=1),
+                                                    CNNLSTM(in_channels, 245200, 1, global_pred=True))
+
+    # ---- NativeGenerator hooks -------------------------------------------------------
+    def _input_channels(self):
+        return self.in_channels
+
+    def _hop(self):
+        return self.hop_length
+
+    def _upsample_rates(self):
+        return list(self.up_ratios)
+
+    def _c_config(self):
+        if len(self.up_ratios) > _capi.AB_MAX_STAGES:
+            raise ValueError("amphion_b200: too many up_ratios for the native decoder")
+        c = _capi.GeneratorConfig()
+        c.kind = _capi.GEN_FACODEC
+        c.n_mel = self.in_channels
+        c.upsample_initial_channel = self.upsample_initial_channel
+        c.num_upsamples = len(self.up_ratios)
+        for i, u in enumerate(self.up_ratios):
+            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
+        c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
+        for p, d in enumerate((1, 3, 9)):
+            c.resblock_dilation_sizes[0][p] = d
+        c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
+        for i, (n, bits) in enumerate(((self.vq_num_q_p, self.codebook_size_prosody),
+                                       (self.vq_num_q_c, self.codebook_size_content),
+                                       (self.vq_num_q_r, self.codebook_size_residual))):
+            c.vq_num_q[i], c.vq_codebook_bits[i] = n, int(bits)
+        c.vq_codebook_dim = self.codebook_dim
+        return c
+
+    def _workspace_for(self, device, need):
+        if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != device:
+            self._workspace = None
+            self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
+        return (self._workspace.data_ptr() + 255) // 256 * 256
+
+    # ---- served methods --------------------------------------------------------------
+    def vq2emb(self, vq, use_residual_code=True):
+        """codes [n_q, B, T] (integer, any strides) -> [B, in_channels, T] fp32 on the codes' device."""
+        n_pc = self.vq_num_q_p + self.vq_num_q_c
+        n_all = n_pc + self.vq_num_q_r
+        if vq.dim() != 3 or vq.is_floating_point() or vq.is_complex():
+            raise ValueError(f"FACodecDecoder.vq2emb expects integer codes [n_q, B, T], got {vq.dtype} {tuple(vq.shape)}")
+        n_q, B, T = vq.shape
+        if n_q != n_all and not (not use_residual_code and n_q == n_pc):
+            raise ValueError(f"FACodecDecoder.vq2emb: {n_q} code rows, the decoder has {n_all} "
+                             f"({self.vq_num_q_p} prosody, {self.vq_num_q_c} content, {self.vq_num_q_r} residual)")
+        if B == 0 or T == 0:
+            raise ValueError("amphion_b200: empty code batch")
+        _capi.require_cuda(vq, "FACodecDecoder.vq2emb")
+        vq = vq.long()
+        # codes the kernel would not read (it writes NaN there): refuse them before the launch, as F.embedding does
+        groups = [(0, self.vq_num_q_p, self.codebook_size_prosody), (self.vq_num_q_p, n_pc, self.codebook_size_content)]
+        if use_residual_code and self.vq_num_q_r > 0:
+            groups.append((n_pc, n_all, self.codebook_size_residual))
+        for q0, q1, bits in groups:
+            part = vq[q0:q1]
+            lo, hi = int(part.min()), int(part.max())
+            if lo < 0 or hi >= 2 ** int(bits):
+                raise ValueError(f"FACodecDecoder.vq2emb: code rows {q0}..{q1 - 1} hold {lo}..{hi}, outside the "
+                                 f"codebook [0, {2 ** int(bits)})")
+        with torch.cuda.device(vq.device):
+            self._sync_params(vq.device)
+            out = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=vq.device)
+            _capi.check(_capi.lib.ab_facodec_vq2emb(self._handle, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B, T,
+                                                    int(bool(use_residual_code)), _capi.ptr(out), _capi.stream_ptr()),
+                        "ab_facodec_vq2emb")
+            self.last_launches = _capi.lib.ab_generator_last_launches(self._handle)
+        return out
+
+    def inference(self, x, speaker_embedding, out=None, tail_events=None):
+        """x [B, in_channels, T] (any strides), speaker_embedding [B, in_channels] -> wav [B, 1, T * hop] fp32.
+
+        ``out`` / ``tail_events`` (beyond the reference signature) behave as in the other generators' forward."""
+        if x.dim() != 3 or x.shape[1] != self.in_channels:
+            raise ValueError(f"FACodecDecoder.inference expects x of shape [B, {self.in_channels}, T], got {tuple(x.shape)}")
+        spk = speaker_embedding
+        if spk.dim() != 2 or spk.shape[1] != self.in_channels or spk.shape[0] != x.shape[0]:
+            raise ValueError(f"FACodecDecoder.inference expects a speaker embedding of shape [{x.shape[0]}, "
+                             f"{self.in_channels}], got {tuple(spk.shape)}")
+        if spk.device != x.device:
+            raise ValueError("FACodecDecoder.inference: x and the speaker embedding are on different devices")
+        B, _, T = x.shape
+        if B == 0 or T == 0:
+            raise ValueError("amphion_b200: empty latent batch")
+        _capi.require_cuda(x, "FACodecDecoder.inference")
+        if x.dtype != torch.float32:
+            x = x.float()
+        spk = spk.float()
+        if spk.stride(1) != 1:
+            spk = spk.contiguous()
+        with torch.cuda.device(x.device):
+            self._sync_params(x.device)
+            lib, h = _capi.lib, self._handle
+            need = lib.ab_generator_workspace_bytes(h, B, T)
+            wbase = self._workspace_for(x.device, need)
+            n_out = T * self.hop_length
+            if out is None:
+                wav = torch.empty(B, 1, n_out, dtype=torch.float32, device=x.device)
+            else:
+                if (tuple(out.shape) != (B, 1, n_out) or out.dtype != torch.float32 or out.device != x.device
+                        or not out.is_contiguous()):
+                    raise ValueError(f"out must be a contiguous fp32 [{B}, 1, {n_out}] tensor on {x.device}")
+                wav = out
+            if tail_events:
+                for ev in tail_events:
+                    ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded below
+                arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
+                _capi.check(lib.ab_generator_set_tail_events(h, arr, len(tail_events)), "ab_generator_set_tail_events")
+            _capi.check(lib.ab_facodec_inference(h, _capi.ptr(x), B, T, _capi.shape_array(x.stride()), _capi.ptr(spk),
+                                                 spk.stride(0), _capi.ptr(wav), C.c_void_p(wbase), need,
+                                                 _capi.stream_ptr()), "ab_facodec_inference")
+            self.last_launches = lib.ab_generator_last_launches(h)
+        return wav
+
+    def forward(self, x=None, vq=True, get_vq=False, eval_vq=True, speaker_embedding=None, n_quantizers=None,
+                quantized=None):
+        if vq is True:
+            raise NotImplementedError(f"amphion_b200: FACodecDecoder.forward(vq=True) (quantization and the timbre "
+                                      f"transformer) is not served; {_SERVED}")
+        raise NotImplementedError(f"amphion_b200: the training branch of FACodecDecoder.forward (the predictors, "
+                                  f"random residual masking) is not served; {_SERVED}")
+
+    def remove_weight_norm(self):
+        def _remove(m):
+            try:
+                remove_weight_norm(m)
+            except ValueError:   # this module has no weight norm
+                return
+        self.apply(_remove)
+        self.invalidate()

@@ -80,11 +80,25 @@ extern "C" {
  * non-persistent "diffusion_embedding.embedding" [embedding_rows, 128].  At AB_PREC_TC_F16 / TC_BF16 the residual
  * layers' convolutions take 16-bit operands (x + d, the upsampled mel, the gate, the weights) with fp32 accumulation;
  * the x and skip streams, the upsampler, the step embeddings and the tail stay fp32 at every precision.  It runs
- * through the ab_diffwave_* entry points below, not ab_generator_forward. */
+ * through the ab_diffwave_* entry points below, not ab_generator_forward.
+ * AB_GEN_FACODEC: the waveform path of NaturalSpeech 3's FACodecDecoder (models/codec/ns3_codec/facodec.py:220-240,
+ * :556-576): vq2emb (codebook rows through each layer's weight-normed out_proj, summed per ResidualVQ) and inference:
+ * x = LayerNorm(x over channels, no affine, eps 1e-5) * gamma + beta, (gamma, beta) = timbre_linear(speaker embedding);
+ * conv_pre (k = 7); per stage i: Activation1d(SnakeBeta), ConvTranspose1d(k = 2u, stride u, padding u//2 + u%2,
+ * output_padding u%2) and three ResidualUnits x = x + conv_k1(act(conv_k7(act(x), dilation d))); final act, conv_post
+ * (C -> 1, k = 7), tanh.  Config fields: n_mel = in_channels (= vq_dim), upsample_initial_channel, num_upsamples and
+ * upsample_rates = up_ratios, upsample_kernel_sizes = 2 u, resblock = 1, num_kernels = 1, resblock_kernel_sizes[0] = 7,
+ * num_dilations[0] = 3 with dilations (1, 3, 9), activation = AB_ACT_SNAKEBETA, snake_logscale = 1, and the vq_* fields;
+ * every other field 0.  Tensors keep the reference's names: "model.0" (conv_pre), "model.{1+i}.block.0" (the stage's
+ * activation), "model.{1+i}.block.1" (ConvTranspose), "model.{1+i}.block.{2,3,4}.block.{0,1,2,3}" (a ResidualUnit's
+ * act, k = 7 conv, act, k = 1 conv), "model.{1+n}" (final act), "model.{2+n}" (conv_post), "timbre_linear.{weight,bias}",
+ * "quantizer.{q}.layers.{j}._codebook.weight" and ".out_proj.weight" (weight-normed nn.Linear: load_weight_norm with
+ * weight_g [out, 1]) / ".out_proj.bias".  Runs through the ab_facodec_* entry points, not ab_generator_forward. */
 enum ab_generator_kind {
   AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
-  AB_GEN_DIFFWAVE = 6
+  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7
 };
+#define AB_FACODEC_MAX_Q 32   /* most codebook layers over the three ResidualVQs */
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
@@ -139,6 +153,10 @@ typedef struct ab_generator_config {
   /* AB_GEN_DIFFWAVE only (0 elsewhere) */
   int32_t dilation_cycle;                       /* dilation_cycle_length */
   int32_t embedding_rows;                       /* rows of the diffusion-step table, len(noise_schedule) */
+  /* AB_GEN_FACODEC only (0 elsewhere): the prosody, content and residual ResidualVQs (facodec.py:286-334) */
+  int32_t vq_num_q[3];                          /* vq_num_q_p, vq_num_q_c, vq_num_q_r (the residual group may be 0) */
+  int32_t vq_codebook_bits[3];                  /* codebook_size_{prosody,content,residual}: 2^bits rows */
+  int32_t vq_codebook_dim;                      /* codebook_dim */
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -196,7 +214,8 @@ int ab_generator_last_launches(const ab_generator* g);
  * "tc_pointwise" (Vocos' pointwise GEMMs and head) and "vocos_norm" (its depthwise conv + LayerNorm kernels); a DiffWave
  * handle lists, when max_entries >= 11, also "diffwave_cond" (spectrogram upsampler and step embeddings, once per
  * call), "diffwave_input" (input projection), "diffwave_layer" (residual layers) and "diffwave_tail" (skip/output
- * projections and the sampler update). */
+ * projections and the sampler update).  A FACodec handle lists the first five and "facodec_prologue" (timbre_linear, the
+ * LayerNorm and the FiLM, and vq2emb) when max_entries >= 12, the six unused classes with zero launches. */
 typedef struct ab_profile_entry {
   char name[32];
   int32_t launches;
@@ -255,6 +274,23 @@ int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t batch, int64_t f
 int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t batch, int64_t frames, const float* dev_mel,
                         const int64_t mel_strides[3], const float* host_steps, int32_t n_steps, float* dev_eps,
                         void* dev_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * FACodec decoder (AB_GEN_FACODEC): FACodecDecoder.vq2emb and .inference (models/codec/ns3_codec/facodec.py:556-576).
+ * ---------------------------------------------------------------------- */
+/* codes int64 [n_q, B, T] with element strides codes_strides (prosody layers, then content, then residual) ->
+ * out [B, in_channels, T] fp32 contiguous.  Each ResidualVQ sums its layers in layer order (quantize/rvq.py:75-81), then
+ * out = prosody + content [+ residual].  n_q is the total number of layers, or the prosody + content layers when
+ * use_residual == 0.  A code outside [0, 2^bits) is never read: its time step of `out` is written as NaN. */
+int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q, int64_t batch,
+                      int64_t frames, int32_t use_residual, float* dev_out, void* stream);
+/* x [B, in_channels, T] fp32 with any element strides, spk [B, in_channels] fp32 with row stride spk_row_stride ->
+ * wav [B, 1, T * prod(up_ratios)].  Workspace: ab_generator_workspace_bytes.  Tail events (ab_generator_set_tail_events)
+ * split conv_post into batch chunks as for the other generators.  set_option's "resblock_fusion" and "pair_schedule"
+ * are accepted and change nothing: every FACodec conv runs as a single conv. */
+int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t batch, int64_t frames, const int64_t x_strides[3],
+                         const float* dev_spk, int64_t spk_row_stride, float* dev_wav, void* dev_workspace,
+                         size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Activation1d(Snake|SnakeBeta).forward  (modules/anti_aliasing/act.py:31-36,
