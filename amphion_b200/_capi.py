@@ -106,6 +106,10 @@ SIGNATURES = {
     "ab_conv_transpose1d_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "ab_conv_transpose1d_forward": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                                               C.c_int32, C.c_int32, C.c_float, C.c_int32, _P, C.c_size_t, _P]),
+    "ab_tc_conv_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    "ab_tc_conv_forward": (C.c_int, [C.c_int32, _P, _I64P, C.c_float, _P, _P, _P, _P, _P, C.c_float, C.c_int32, _P, _P,
+                                     C.c_float, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_int32, _P, C.c_size_t, _P]),
     "ab_mel_create": (C.c_int, [C.POINTER(MelConfig), C.POINTER(_P)]),
     "ab_mel_destroy": (None, [_P]),
     "ab_mel_num_frames": (C.c_int64, [_P, C.c_int64]),

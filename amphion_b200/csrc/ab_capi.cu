@@ -1856,4 +1856,37 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
   return launch_conv_transpose1d_fp32(p, st);
 }
 
+size_t ab_tc_conv_workspace_bytes(int32_t mode, int64_t cin, int64_t cout, int32_t k, int32_t d_or_u) {
+  return align_up((size_t)cin * cout * k * sizeof(float), 256) +
+         align_up(tc_weight_image_bytes(mode, (int)cin, (int)cout, k, d_or_u), 256);
+}
+
+int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides[3], float pre_slope,
+                       const uint16_t* dev_ximg, const float* dev_w, const float* dev_bias, const float* dev_residual,
+                       const float* dev_acc_prev, float out_div, int32_t reflect, float* dev_y, uint16_t* dev_yimg,
+                       float img_slope, int64_t B, int64_t cin, int64_t cout, int64_t T, int32_t k, int32_t d_or_u,
+                       int32_t pad, int32_t precision, void* ws, size_t ws_bytes, void* stream) {
+  if (!dev_w || !ws || (dev_x && !dev_ximg && !x_strides)) return fail(AB_ERR_ARG, "tc conv: null argument");
+  if (ws_bytes < ab_tc_conv_workspace_bytes(mode, cin, cout, k, d_or_u)) return fail(AB_ERR_WORKSPACE, "tc conv: workspace too small");
+  if (B > INT32_MAX || cin > INT32_MAX || cout > INT32_MAX || T * (mode == 1 ? d_or_u : 1) > (1ll << 30))
+    return fail(AB_ERR_UNSUPPORTED, "tc conv: shape too large");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* w_t = static_cast<float*>(ws);
+  void* img = static_cast<char*>(ws) + align_up((size_t)cin * cout * k * sizeof(float), 256);
+  int rc = mode == 1 ? launch_repack_weight(dev_w, nullptr, w_t, (int)cin, (int)cout, k, 1, st)
+                     : launch_repack_weight(dev_w, nullptr, w_t, (int)cout, (int)cin, k, 0, st);
+  if (rc != AB_OK) return rc;
+  rc = launch_tc_pack_weight(w_t, img, mode, (int)cin, (int)cout, k, d_or_u, precision, st);
+  if (rc != AB_OK) return rc;
+  TcConvParams p;
+  p.mode = mode;
+  p.x = dev_x; p.ximg = dev_ximg; p.pre_slope = pre_slope;
+  if (dev_x && !dev_ximg) { p.xsb = x_strides[0]; p.xsc = x_strides[1]; p.xst = x_strides[2]; }
+  p.w = img; p.bias = dev_bias; p.residual = dev_residual; p.acc_prev = dev_acc_prev; p.out_div = out_div;
+  p.reflect = reflect; p.pad = pad;
+  p.y = dev_y; p.yimg = dev_yimg; p.img_slope = img_slope;
+  p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)T; p.k = k; p.d_or_u = d_or_u; p.precision = precision;
+  return launch_tc_conv(p, st);
+}
+
 }  // extern "C"

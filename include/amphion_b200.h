@@ -324,6 +324,25 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
                                 int64_t length_in, int32_t ksize, int32_t stride, float pre_slope,
                                 int32_t precision, void* dev_workspace, size_t workspace_bytes,
                                 void* stream);
+/* tc_conv: one launch of the tensor-core convolution that the generators' wgmma layers run on (hconv_kernel from fp32
+ * input; a ConvTranspose1d from an operand image on hitem_kernel).  act(x) = rnd(lrelu(x, pre_slope)) of x [B, Cin, T]
+ * with element strides x_strides, or, when dev_ximg is given, the 16-bit operand image [B][ceil16(Cin)/8][T][8] of the
+ * already activated input (mode 1: Cin % 16 == 0); rnd = round to nearest, saturating, to `precision`
+ * (AB_PREC_TC_F16 | AB_PREC_TC_BF16).  The weight is repacked and packed into the workspace as ab_conv1d_forward does.
+ *   mode 0, Conv1d "same", dilation d_or_u, odd k, w [Cout, Cin, k]:
+ *     y = (((conv(act(x)) + bias) + residual) + acc_prev) * (1.0f / out_div); reflect = 1: ReflectionPad1d((k-1)d/2)
+ *     in place of the zero padding (AB_ERR_ARG, nothing launched, when the reflection needs more than T samples)
+ *   mode 1, ConvTranspose1d stride u = d_or_u, padding pad (-1: (k-u)/2), T*u outputs, w [Cin, Cout, k]:
+ *     y = conv_transpose(act(x)) + bias; residual, acc_prev and out_div != 1 are refused
+ *   y fp32 [B, Cout, T_out]; dev_yimg (nullable): the operand image [B][ceil16(Cout)/8][T_out][8] of
+ *   rnd(lrelu(y, img_slope)), padding channels zero (mode 1: Cout % 16 == 0).  bias, residual, acc_prev nullable. */
+size_t ab_tc_conv_workspace_bytes(int32_t mode, int64_t cin, int64_t cout, int32_t ksize, int32_t d_or_u);
+int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides[3], float pre_slope,
+                       const uint16_t* dev_ximg, const float* dev_w, const float* dev_bias, const float* dev_residual,
+                       const float* dev_acc_prev, float out_div, int32_t reflect, float* dev_y, uint16_t* dev_yimg,
+                       float img_slope, int64_t batch, int64_t cin, int64_t cout, int64_t length, int32_t ksize,
+                       int32_t d_or_u, int32_t pad, int32_t precision, void* dev_workspace, size_t workspace_bytes,
+                       void* stream);
 
 /* ------------------------------------------------------------------------
  * Mel front end:

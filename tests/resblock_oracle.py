@@ -19,7 +19,8 @@ these epilogues, so there is no fused multiply-add to mirror.
          the H100's wgmma accumulation: on a single dense conv it matches the measured error to 1.1-1.3x, with the
          same 84 % of errors toward zero, where IEEE float32 sits 3-15x closer to the exact sum (DESIGN.md §5).
 With one-hot weights (`OneHot`) every output is one exact product, so every order gives the same bits and the
-convolution is a gather."""
+convolution is a gather.  `conv_transpose` and `OneHotT` are the same for the ConvTranspose layers (`hconv_kernel`
+from fp32 input, `hitem_kernel` from an operand image), and `image_bits` / `to_image` give the operand images."""
 from __future__ import annotations
 
 import numpy as np
@@ -79,15 +80,22 @@ def _round_w(w, prec):
     return w.rounded(prec) if isinstance(w, OneHot) else rnd(w, prec)
 
 
-def conv(a, w, d, acc="f64"):
-    """'same' Conv1d without bias of the operand a [B, C_in, T] with w (dense [C_out, C_in, k] or OneHot), dilation d,
-    summed as `acc` says and rounded to fp32 once: [B, C_out, T] float32."""
+def conv(a, w, d, acc="f64", reflect=False):
+    """'same' Conv1d without bias of the operand a [B, C_in, T] (any strides) with w (dense [C_out, C_in, k] or
+    OneHot), dilation d, summed as `acc` says and rounded to fp32 once: [B, C_out, T] float32.  reflect: ReflectionPad1d
+    ((k-1) d / 2) in place of the zero padding, zero where the reflected time is outside [0, T) too."""
     a = np.asarray(a, np.float32)
     B, cin, T = a.shape
     k = w.shape[2]
     h = (k - 1) * d // 2
     ap = np.zeros((B, cin, T + 2 * h), np.float32)
-    ap[:, :, h:h + T] = a
+    if reflect:
+        t = np.arange(-h, T + h)
+        t = np.where(t < 0, -t, np.where(t >= T, 2 * (T - 1) - t, t))
+        ok = (t >= 0) & (t < T)
+        ap[:, :, ok] = a[:, :, t[ok]]
+    else:
+        ap[:, :, h:h + T] = a
     if isinstance(w, OneHot):
         idx = w.tap[:, None] * d + np.arange(T)[None, :]                 # [C_out, T]
         return (ap[:, w.perm[:, None], idx].astype(np.float64) * w.scale[None, :, None]).astype(np.float32)
@@ -117,21 +125,101 @@ def _to_f32_rz(v):
     return r
 
 
+class OneHotT:
+    """A ConvTranspose weight [C_in, C_out, k] of stride u with one non-zero per (output channel co, phase phi):
+    W[ci[co, phi], co, phi + u m[co, phi]] = scale[co, phi].  Output t = s u - pad + phi is then one product,
+    act(x)[ci, s - m] * scale (zero where s - m is outside [0, T))."""
+
+    def __init__(self, ci, m, scale, cin, u, k):
+        self.ci, self.m = np.asarray(ci, np.int64), np.asarray(m, np.int64)
+        self.scale, self.cin, self.u, self.k = np.asarray(scale, np.float32), int(cin), int(u), int(k)
+
+    @property
+    def shape(self):
+        return (self.cin, self.ci.shape[0], self.k)
+
+    def dense(self):
+        w = np.zeros(self.shape, np.float32)
+        co, phi = np.meshgrid(np.arange(self.ci.shape[0]), np.arange(self.u), indexing="ij")
+        w[self.ci, co, phi + self.u * self.m] = self.scale
+        return w
+
+    def rounded(self, prec):
+        return OneHotT(self.ci, self.m, rnd(self.scale, prec), self.cin, self.u, self.k)
+
+
+def random_one_hot_t(rng, cin, cout, k, u, exps):
+    """ci: random channels; m: a random tap of the phase (phi + u m < k); scale: +-2^e, e drawn from exps."""
+    taps = (k - np.arange(u) + u - 1) // u                             # taps m of phase phi
+    m = np.minimum((rng.random((cout, u)) * taps[None, :]).astype(np.int64), taps[None, :] - 1)
+    scale = rng.choice([-1.0, 1.0], (cout, u)) * np.exp2(rng.choice(np.asarray(exps, np.float64), (cout, u)))
+    return OneHotT(rng.integers(0, cin, (cout, u)), m, scale, cin, u, k)
+
+
 def conv_transpose(a, w, u, pad, acc="f64"):
-    """ConvTranspose1d without bias, w [C_in, C_out, k], stride u, padding pad, T_out = T * u (k - u even)."""
+    """ConvTranspose1d without bias of a [B, C_in, T] with w (dense [C_in, C_out, k] or OneHotT), stride u, padding pad
+    in [0, k), T_out = T * u: torch's conv_transpose1d with output_padding u + 2 pad - k where that is in [0, u).
+    Output t = s u - pad + phi sums the taps m of phase phi (k index phi + u m) over input time s - m; "mma" and "f32"
+    in the kernels' order, 32-channel K chunk -> tap m -> 16-channel half."""
     a = np.asarray(a, np.float32)
     B, cin, T = a.shape
-    _, cout, k = w.shape
-    dt = np.float32 if acc == "f32" else np.float64
-    full = np.zeros((B, cout, (T - 1) * u + k), dt)
-    step = 16 if acc == "mma" else cin   # "mma": each 16-channel partial sum, then truncation to fp32
-    for c1 in range(0, cin, step):
+    k, Tout = w.shape[2], T * u
+    if isinstance(w, OneHotT):
+        q = np.arange(Tout) + pad
+        s, phi = q // u, q % u
+        src = s[None, :] - w.m[:, phi]                                   # [C_out, T_out]
+        ok = (src >= 0) & (src < T)
+        g = a[:, w.ci[:, phi], np.clip(src, 0, T - 1)].astype(np.float64) * w.scale[None, :, phi]
+        return np.where(ok[None], g, 0.0).astype(np.float32)
+    w = np.asarray(w, np.float32)
+    cout = w.shape[1]
+    full_len = max((T - 1) * u + k, pad + Tout)     # position s u + j of input time s and k index j
+    if acc == "f64":
+        w64, a64 = w.astype(np.float64), a.astype(np.float64)
+        full = np.zeros((B, cout, full_len))
         for j in range(k):
-            s = slice(j, j + (T - 1) * u + 1, u)
-            full[:, :, s] += np.matmul(np.asarray(w[c1:c1 + step, :, j], dt).T, a[:, c1:c1 + step].astype(dt))
-            if acc == "mma":
-                full[:, :, s] = _to_f32_rz(full[:, :, s])
-    return full[:, :, pad:pad + T * u].astype(np.float32)
+            full[:, :, j:j + (T - 1) * u + 1:u] += np.matmul(w64[:, :, j].T, a64)
+        return full[:, :, pad:pad + Tout].astype(np.float32)
+    assert acc in ("f32", "mma"), acc
+    dt = np.float32 if acc == "f32" else np.float64
+    full = np.zeros((B, cout, full_len), np.float32)
+    for c0 in range(0, cin, 32):                                         # K chunk
+        for m in range((k + u - 1) // u):                                # tap
+            for c1 in range(c0, min(c0 + 32, cin), 16):                  # k16 half
+                for phi in range(u):                                     # disjoint outputs
+                    j = phi + u * m
+                    if j >= k:
+                        continue
+                    s = slice(j, j + (T - 1) * u + 1, u)
+                    part = np.matmul(np.asarray(w[c1:c1 + 16, :, j], dt).T, np.asarray(a[:, c1:c1 + 16], dt))
+                    full[:, :, s] = (full[:, :, s] + part if acc == "f32"
+                                     else _to_f32_rz(full[:, :, s].astype(np.float64) + part))
+    return full[:, :, pad:pad + Tout]
+
+
+def image_bits(v, slope, prec):
+    """The 16-bit patterns (uint16) of rnd(lrelu(v, slope), prec): the values an operand image holds."""
+    r = rnd(lrelu(v, slope), prec)
+    if prec == "f16":
+        return r.astype(np.float16).view(np.uint16)
+    assert prec == "bf16", prec
+    return (r.view(np.uint32) >> 16).astype(np.uint16)
+
+
+def to_image(bits):
+    """[B, C, T] uint16 -> the operand-image layout [B][ceil16(C)/8][T][8], padding channels zero."""
+    B, C, T = bits.shape
+    c16 = (C + 15) // 16 * 16
+    img = np.zeros((B, c16, T), np.uint16)
+    img[:, :C] = bits
+    return np.ascontiguousarray(img.reshape(B, c16 // 8, 8, T).transpose(0, 1, 3, 2))
+
+
+def from_image(img, C):
+    """The inverse of to_image: [B][c8][T][8] -> [B, C, T] (and the padding channels as [B, c16 - C, T])."""
+    B, c8n, T, _ = img.shape
+    full = np.asarray(img).transpose(0, 1, 3, 2).reshape(B, c8n * 8, T)
+    return full[:, :C], full[:, C:]
 
 
 def block(k, dils, c1, c2=None):

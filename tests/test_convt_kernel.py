@@ -1,7 +1,8 @@
 """ConvTranspose1d launches.  From an operand image they run on `hitem_kernel`: persistent CTAs over (utterance, time
 tile, N block) work items and the polyphase epilogue with 16-byte operand-image stores.  The single-layer cases go
 through `ab_conv_transpose1d_forward`, whose fp32 input runs on `hconv_kernel`; the generators exercise conv_pre's
-operand image and the image-in, image-out ConvTranspose layers of HiFi-GAN at strides 8 and 2."""
+operand image and the image-in, image-out ConvTranspose layers of HiFi-GAN at strides 8 and 2.  test_tc_conv_exact.py
+launches both kernels directly and checks every epilogue specialisation and the operand images bit for bit."""
 import numpy as np
 import pytest
 import torch

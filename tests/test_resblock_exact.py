@@ -17,7 +17,9 @@ ResBlock convs are plain tensors (no weight-norm fold), so the only rounding is 
 * Whole HiFi-GAN generators (ResBlock1 and ResBlock2) under the same floor rule.
 
 Not covered: a change of the fp32 accumulation order alone.  One-hot weights make every order give the same bits, and
-with dense weights such a change moves the output by about the floor, which the floor rule admits."""
+with dense weights such a change moves the output by about the floor, which the floor rule admits.  (For the
+ConvTranspose layers, test_tc_conv_exact.py compares `hitem_kernel` with `hconv_kernel` bit for bit on dense weights,
+which catches such a change in either kernel.)"""
 import numpy as np
 import pytest
 import torch
