@@ -110,6 +110,13 @@ SIGNATURES = {
     "ab_tc_conv_forward": (C.c_int, [C.c_int32, _P, _I64P, C.c_float, _P, _P, _P, _P, _P, C.c_float, C.c_int32, _P, _P,
                                      C.c_float, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, _P, C.c_size_t, _P]),
+    "ab_diffwave_layer_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "ab_diffwave_layer_forward": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_int64,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),
+    "ab_diffwave_tail_forward": (C.c_int, [_P, _P, _P, _P, _P, C.c_float, C.c_int64, C.c_int64, _P, _P, _P, C.c_float,
+                                           C.c_float, C.c_float, _P]),
+    "ab_diffwave_upsample_forward": (C.c_int, [_P, _I64P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int64, C.c_int32,
+                                               C.c_int64, _P, _P]),
     "ab_mel_create": (C.c_int, [C.POINTER(MelConfig), C.POINTER(_P)]),
     "ab_mel_destroy": (None, [_P]),
     "ab_mel_num_frames": (C.c_int64, [_P, C.c_int64]),

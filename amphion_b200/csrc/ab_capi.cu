@@ -1889,4 +1889,74 @@ int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides
   return launch_tc_conv(p, st);
 }
 
+size_t ab_diffwave_layer_workspace_bytes(int32_t n_mel) {
+  return n_mel < 1 ? 0 : dw_layer_packed_floats(n_mel) * sizeof(float);
+}
+
+int ab_diffwave_layer_forward(const float* dev_x_in, const float* dev_d, int64_t d_batch_stride, const float* dev_cond,
+                              const float* dev_wdil, const float* dev_bdil, const float* dev_wcond, const float* dev_bcond,
+                              const float* dev_wout, const float* dev_bout, float* dev_x_out, float* dev_skip, int64_t B,
+                              int64_t L, int32_t n_mel, int32_t dilation, int32_t first, int32_t precision, void* ws,
+                              size_t ws_bytes, void* stream) {
+  if (!dev_x_in || !dev_d || !dev_cond || !dev_wdil || !dev_bdil || !dev_wcond || !dev_bcond || !dev_wout || !dev_bout ||
+      !dev_x_out || !dev_skip || !ws)
+    return fail(AB_ERR_ARG, "diffwave_layer: null argument");
+  if (dev_x_out == dev_x_in) return fail(AB_ERR_ARG, "diffwave_layer: x_out must not be x_in (tiles read x_in's halo)");
+  if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
+    return fail(AB_ERR_ARG, "diffwave_layer: unknown precision %d", precision);
+  if (B < 1 || B > 65535 || L < 1 || L > (1ll << 30) || n_mel < 1 || dilation < 1 || d_batch_stride < 0)
+    return fail(AB_ERR_ARG, "diffwave_layer: batch %lld, length %lld, %d mels, dilation %d, d stride %lld", (long long)B,
+                (long long)L, n_mel, dilation, (long long)d_batch_stride);
+  if (dw_layer_smem_bytes(n_mel, precision) > 227 * 1024)
+    return fail(AB_ERR_UNSUPPORTED, "diffwave_layer: %d mels do not fit the layer tile", n_mel);
+  if (ws_bytes < ab_diffwave_layer_workspace_bytes(n_mel) || reinterpret_cast<uintptr_t>(ws) % 256)
+    return fail(AB_ERR_WORKSPACE, "diffwave_layer: workspace %zu B (256-byte aligned) < required %zu B", ws_bytes,
+                ab_diffwave_layer_workspace_bytes(n_mel));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const DwLayerPack lp = dw_layer_pack(static_cast<char*>(ws), n_mel, 0);
+  DwPackParams pk;
+  pk.wdil = dev_wdil; pk.bdil = dev_bdil; pk.wcond = dev_wcond; pk.bcond = dev_bcond; pk.wout = dev_wout; pk.bout = dev_bout;
+  pk.w1p = lp.w1; pk.b1p = lp.b1; pk.w2p = lp.w2; pk.b2p = lp.b2;
+  pk.w1h = precision != AB_PREC_FP32 ? lp.w1h : nullptr; pk.w2h = lp.w2h;
+  pk.bf16 = precision == AB_PREC_TC_BF16;
+  pk.n_mel = n_mel;
+  int rc = launch_dw_pack(pk, st);
+  if (rc != AB_OK) return rc;
+  DwLayerParams p;
+  p.x_in = dev_x_in; p.x_out = dev_x_out; p.skip = dev_skip; p.cond = dev_cond; p.d = dev_d; p.d_bstride = d_batch_stride;
+  p.w1 = lp.w1; p.b1 = lp.b1; p.w2 = lp.w2; p.b2 = lp.b2; p.w1h = lp.w1h; p.w2h = lp.w2h; p.precision = precision;
+  p.B = (int)B; p.n_mel = n_mel; p.dil = dilation; p.first = first != 0; p.L = L;
+  return launch_dw_layer(p, st);
+}
+
+int ab_diffwave_tail_forward(const float* dev_skip, const float* dev_wsk, const float* dev_bsk, const float* dev_wo,
+                             const float* dev_bo, float skip_div, int64_t B, int64_t L, float* dev_eps, float* dev_audio,
+                             const float* dev_noise, float c1, float c2, float sigma, void* stream) {
+  if (!dev_skip || !dev_wsk || !dev_bsk || !dev_wo || !dev_bo || (!dev_eps && !dev_audio))
+    return fail(AB_ERR_ARG, "diffwave_tail: null argument");
+  if (B < 1 || L < 1 || B > INT32_MAX || B * L > (1ll << 40))
+    return fail(AB_ERR_ARG, "diffwave_tail: batch %lld, length %lld", (long long)B, (long long)L);
+  DwTailParams t;
+  t.skip = dev_skip; t.wsk = dev_wsk; t.bsk = dev_bsk; t.wo = dev_wo; t.bo = dev_bo; t.skip_div = skip_div;
+  t.B = (int)B; t.L = L; t.eps = dev_eps; t.audio = dev_audio; t.noise = dev_noise;
+  t.c1 = c1; t.c2 = c2; t.sigma = sigma;
+  return launch_dw_tail(t, static_cast<cudaStream_t>(stream));
+}
+
+int ab_diffwave_upsample_forward(const float* dev_mel, const int64_t mel_strides[3], const float* dev_w1, const float* dev_b1,
+                                 const float* dev_w2, const float* dev_b2, int32_t f1, int32_t f2, int64_t B, int32_t n_mel,
+                                 int64_t frames, float* dev_out, void* stream) {
+  if (!dev_mel || !mel_strides || !dev_w1 || !dev_b1 || !dev_w2 || !dev_b2 || !dev_out)
+    return fail(AB_ERR_ARG, "diffwave_upsample: null argument");
+  if (f1 < 2 || f2 < 2 || (f1 & 1) || (f2 & 1))
+    return fail(AB_ERR_UNSUPPORTED, "diffwave_upsample: factors %d, %d (need even factors >= 2)", f1, f2);
+  if (B < 1 || n_mel < 1 || frames < 1 || B > INT32_MAX || frames * f1 * f2 > (1ll << 30))
+    return fail(AB_ERR_ARG, "diffwave_upsample: batch %lld, %d mels, %lld frames", (long long)B, n_mel, (long long)frames);
+  DwUpsampleParams up;
+  up.mel = dev_mel; up.msb = mel_strides[0]; up.msc = mel_strides[1]; up.mst = mel_strides[2];
+  up.w1 = dev_w1; up.b1 = dev_b1; up.w2 = dev_w2; up.b2 = dev_b2; up.out = dev_out;
+  up.B = (int)B; up.n_mel = n_mel; up.F = (int)frames; up.f1 = f1; up.f2 = f2;
+  return launch_dw_upsample(up, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -17,6 +17,7 @@
 #include <algorithm>
 
 #include "ab_common.cuh"
+#include "ab_tc_ptx.cuh"
 
 namespace ab {
 
@@ -253,10 +254,11 @@ __global__ void dw_pack_kernel(const DwPackParams p) {
 
 
 // ---- tensor-core layer ------------------------------------------------------------------------------------------
+// fp32 -> 16-bit operand, round to nearest and saturating (cvt.rn.satfinite): an operand never becomes inf, whose
+// products with the zero weights of its k16 block would be NaN (DESIGN.md §5)
 template <bool BF16>
 __device__ __forceinline__ uint16_t to16(float v) {
-  if constexpr (BF16) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
-  else return __half_as_ushort(__float2half_rn(v));
+  return (uint16_t)(tcx::pack2t<BF16>(v, 0.f) & 0xffffu);
 }
 
 template <bool BF16>
@@ -377,7 +379,7 @@ __global__ void dw_pack_tc_kernel(const DwPackParams p) {
       const int n = (i - n1) / C, k = (i - n1) % C;
       v = p.wout[src(n) * C + k];
     }
-    const uint16_t h = p.bf16 ? __bfloat16_as_ushort(__float2bfloat16_rn(v)) : __half_as_ushort(__float2half_rn(v));
+    const uint16_t h = p.bf16 ? to16<true>(v) : to16<false>(v);
     (i < n1 ? p.w1h[i] : p.w2h[i - n1]) = h;
   }
 }

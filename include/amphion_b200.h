@@ -343,6 +343,33 @@ int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides
                        float img_slope, int64_t batch, int64_t cin, int64_t cout, int64_t length, int32_t ksize,
                        int32_t d_or_u, int32_t pad, int32_t precision, void* dev_workspace, size_t workspace_bytes,
                        void* stream);
+/* DiffWave building blocks: one launch each of the kernels ab_diffwave_step / ab_diffwave_condition run (no reference
+ * counterpart; exposed for the bit-exact tests).  Every tensor fp32, contiguous unless strides are given; C = 64.
+ * diffwave_layer: one ResidualBlock (diffwave.py:96-124) from the state-dict layouts dilated_conv [2C, C, 3] + [2C],
+ *   conditioner_projection [2C, n_mel(, 1)] + [2C], output_projection [2C, C(, 1)] + [2C]; the weights are packed into
+ *   the workspace (ab_diffwave_layer_workspace_bytes(n_mel), 256-byte aligned) as ab_generator_finalize packs them,
+ *   then the layer kernel of `precision` runs once.  x_in [B, C, L]; d: utterance b's diffusion projection [C] at
+ *   d + b d_batch_stride (0: one for the batch); cond: the upsampled mel [B, n_mel, L]; any L >= 1, dilation >= 1.
+ *   y = dilated_conv(x + d) + conditioner_projection(cond) (the two biases summed first), z = sigmoid(gate) tanh(filter),
+ *   (res, s) = output_projection(z); x_out = (x_in + res) / sqrt(2) (x_out != x_in), skip = s (first != 0) or skip + s.
+ * diffwave_tail: skip [B, C, L] -> s = skip / skip_div, h = relu(skip_projection(s)), e = output_projection(h); dev_eps
+ *   != NULL: eps [B, L] = e; otherwise audio [B, L] = clamp(c1 (audio - c2 e) + sigma noise, -1, 1) in place, the noise
+ *   term only when dev_noise [B, L] is given.  wsk [C, C(, 1)], bsk [C], wo [1, C(, 1)], bo [1].
+ * diffwave_upsample: SpectrogramUpsampler (diffwave.py:68-93) of mel [B, n_mel, frames] with element strides mel_strides:
+ *   two ConvTranspose2d(1, 1, [3, 2f], stride [1, f], padding [1, f / 2]) (weights [3, 2f], biases [1]), each followed by
+ *   leaky_relu(0.4), even f1, f2 -> out [B, n_mel, frames f1 f2]. */
+size_t ab_diffwave_layer_workspace_bytes(int32_t n_mel);
+int ab_diffwave_layer_forward(const float* dev_x_in, const float* dev_d, int64_t d_batch_stride, const float* dev_cond,
+                              const float* dev_wdil, const float* dev_bdil, const float* dev_wcond, const float* dev_bcond,
+                              const float* dev_wout, const float* dev_bout, float* dev_x_out, float* dev_skip, int64_t batch,
+                              int64_t length, int32_t n_mel, int32_t dilation, int32_t first, int32_t precision,
+                              void* dev_workspace, size_t workspace_bytes, void* stream);
+int ab_diffwave_tail_forward(const float* dev_skip, const float* dev_wsk, const float* dev_bsk, const float* dev_wo,
+                             const float* dev_bo, float skip_div, int64_t batch, int64_t length, float* dev_eps,
+                             float* dev_audio, const float* dev_noise, float c1, float c2, float sigma, void* stream);
+int ab_diffwave_upsample_forward(const float* dev_mel, const int64_t mel_strides[3], const float* dev_w1, const float* dev_b1,
+                                 const float* dev_w2, const float* dev_b2, int32_t f1, int32_t f2, int64_t batch,
+                                 int32_t n_mel, int64_t frames, float* dev_out, void* stream);
 
 /* ------------------------------------------------------------------------
  * Mel front end:
