@@ -59,6 +59,7 @@ struct Slot {
   float gain = 1.0f;  // applied to the fp32 image at load time (NSF-HiFiGAN: 2 on every ups weight / bias)
   bool head_cols = false;   // Vocos' head.out: the weight image pairs each bin's magnitude and phase rows
   bool no_tc = false;       // never runs on the wgmma kernel (FACodec's out_proj, read by the vq2emb kernel)
+  bool strided = false;     // Conv1d of stride `stride` (the FACodec encoder's downsampling convs)
 };
 
 struct ConvRef {   // one weight-normed conv of the model
@@ -113,7 +114,9 @@ struct StageRef {
   int u = 1;
   int ch = 0;
   bool has_up = true;   // false: AB_GEN_TRUNK's single stage (no transposed conv in front of the blocks)
-  ActRef act;           // AB_GEN_FACODEC: the DecoderBlock's Activation1d in front of the transposed conv
+  ActRef act;           // AB_GEN_FACODEC: the DecoderBlock's Activation1d in front of the transposed conv;
+                        // AB_GEN_FACODEC_ENCODER: the EncoderBlock's Activation1d in front of the strided conv
+  int down = 0;         // AB_GEN_FACODEC_ENCODER: `up` is the strided Conv1d (stride down) that closes the stage
   std::vector<BlockRef> blocks;
 };
 
@@ -302,9 +305,38 @@ int validate_facodec_config(const ab_generator_config& c) {
   return AB_OK;
 }
 
+// AB_GEN_FACODEC_ENCODER: the encoder's fixed block structure (facodec.py:121-194)
+int validate_facodec_encoder_config(const ab_generator_config& c) {
+  if (c.gin_channels || c.conv_post_no_bias || c.trunk_in_kernel || c.trunk_out_kernel || c.ffn_channels || c.num_layers ||
+      c.istft_n_fft || c.istft_hop)
+    return fail(AB_ERR_ARG, "config: the FACodec encoder uses only the generator fields and trunk_out_channels "
+                            "(gin / trunk kernels / Vocos fields must be 0)");
+  if (c.n_mel != 1) return fail(AB_ERR_ARG, "config: the FACodec encoder reads one waveform channel (n_mel must be 1, got %d)", c.n_mel);
+  const int lim = 1 << 16;
+  if (c.upsample_initial_channel <= 0 || c.trunk_out_channels <= 0 || c.trunk_out_channels > lim)
+    return fail(AB_ERR_ARG, "config: FACodec encoder ngf %d / out_channels %d out of range", c.upsample_initial_channel,
+                c.trunk_out_channels);
+  if (c.num_upsamples <= 0 || c.num_upsamples > AB_MAX_STAGES || ((int64_t)c.upsample_initial_channel << c.num_upsamples) > lim)
+    return fail(AB_ERR_ARG, "config: FACodec encoder up_ratios: %d stages from ngf %d", c.num_upsamples, c.upsample_initial_channel);
+  // strides beyond the tensor-core strided conv's (AB_TC_MAX_STRIDE) are refused rather than served at fp32
+  for (int i = 0; i < c.num_upsamples; ++i)
+    if (c.upsample_rates[i] <= 0 || c.upsample_rates[i] > AB_TC_MAX_STRIDE ||
+        c.upsample_kernel_sizes[i] != 2 * c.upsample_rates[i])
+      return fail(AB_ERR_UNSUPPORTED, "config: FACodec encoder stage %d: stride %d (1..%d) with kernel %d (must be 2 x stride)",
+                  i, c.upsample_rates[i], AB_TC_MAX_STRIDE, c.upsample_kernel_sizes[i]);
+  if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
+      c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
+    return fail(AB_ERR_ARG, "config: FACodec EncoderBlocks hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, "
+                            "num_kernels 1, kernel 7, 3 dilations");
+  if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
+    return fail(AB_ERR_ARG, "config: the FACodec encoder uses SnakeBeta with alpha_logscale = True");
+  return AB_OK;
+}
+
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
-      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC)
+      c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC &&
+      c.kind != AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
   for (int i = 0; i < 3; ++i)
@@ -312,6 +344,7 @@ int validate_config(const ab_generator_config& c) {
   if (c.vq_codebook_dim) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
   if (c.kind == AB_GEN_DIFFWAVE) return validate_diffwave_config(c);
   if (c.dilation_cycle || c.embedding_rows) return fail(AB_ERR_ARG, "config: dilation_cycle / embedding_rows belong to AB_GEN_DIFFWAVE");
+  if (c.kind == AB_GEN_FACODEC_ENCODER) return validate_facodec_encoder_config(c);
   if (c.kind == AB_GEN_VOCOS) return validate_vocos_config(c);
   if (c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop)
     return fail(AB_ERR_ARG, "config: ffn_channels / num_layers / istft_* belong to AB_GEN_VOCOS");
@@ -375,6 +408,7 @@ size_t tc_image_bytes(const Slot& s, bool pre_or_post) {
   if (s.kind == SLOT_CONVT_W) return tc_weight_image_bytes(1, (int)s.shape[0], (int)s.shape[1], (int)s.shape[2], s.stride);
   if (s.kind != SLOT_CONV_W) return 0;
   const int cout = (int)s.shape[0], cin = (int)s.shape[1], k = (int)s.shape[2];
+  if (s.strided) return tc_weight_image_bytes(2, cin, cout, k, s.stride);
   if (pre_or_post && (cin == cout || cin > 512 || cout <= 4)) return 0;
   return tc_weight_image_bytes(0, cin, cout, k, s.dilation);
 }
@@ -538,6 +572,48 @@ void add_facodec_tensors(ab_generator* g) {
     }
 }
 
+// FACodec encoder tensors (AB_GEN_FACODEC_ENCODER), the reference's names (facodec.py:121-194): "block.0" (conv_pre,
+// 1 -> ngf, k = 7), per stride i "block.{1+i}.block.{0,1,2}.block.{0..3}" (three ResidualUnits at C = ngf 2^i),
+// ".block.3" (Activation1d) and ".block.4" (the strided conv C -> 2C, k = 2s), "block.{1+n}" (final Activation1d),
+// "block.{2+n}" (conv_post, k = 3)
+void add_facodec_encoder_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int n = cfg->num_upsamples;
+  auto mod = [](int i) { return "block." + std::to_string(i); };
+  g->conv_pre = make_conv(g, mod(0), 1, cfg->upsample_initial_channel, 7, 1, false);
+  g->slots[g->conv_pre.w].no_tc = true;   // one input channel: 31 of the wgmma kernel's 32 K lanes would be zero
+  int ch = cfg->upsample_initial_channel;
+  for (int i = 0; i < n; ++i) {
+    StageRef st;
+    const std::string base = mod(1 + i) + ".block.";
+    st.ch = ch;
+    st.u = 1;
+    st.has_up = false;
+    st.down = cfg->upsample_rates[i];
+    g->hop *= st.down;
+    BlockRef blk;   // the three ResidualUnits, as FACodec's decoder holds them
+    blk.k = 7;
+    for (int p = 0; p < 3; ++p) {
+      const int d = cfg->resblock_dilation_sizes[0][p];
+      const std::string pre = base + std::to_string(p) + ".block.";
+      blk.dil.push_back(d);
+      blk.acts.push_back(make_act(g, pre + "0", ch, true));
+      blk.c1.push_back(make_conv(g, pre + "1", ch, ch, 7, d, false));
+      blk.acts.push_back(make_act(g, pre + "2", ch, true));
+      blk.c2.push_back(make_conv(g, pre + "3", ch, ch, 1, 1, false));
+    }
+    st.blocks.push_back(blk);
+    st.act = make_act(g, base + "3", ch, true);
+    st.up = make_conv(g, base + "4", ch, 2 * ch, 2 * st.down, 1, false);
+    g->slots[st.up.w].stride = st.down;
+    g->slots[st.up.w].strided = true;
+    g->stages.push_back(st);
+    ch *= 2;
+  }
+  g->act_post = make_act(g, mod(1 + n), ch, true);
+  g->conv_post = make_conv(g, mod(2 + n), ch, cfg->trunk_out_channels, 3, 1, false);
+}
+
 // nn.Linear(cin, cout) as a k = 1 conv: weight [out, in] (state-dict shape), repacked as [in][1][out]
 ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout) {
   ConvRef c;
@@ -680,6 +756,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     add_diffwave_tensors(g);
   } else if (cfg->kind == AB_GEN_FACODEC) {
     add_facodec_tensors(g);
+  } else if (cfg->kind == AB_GEN_FACODEC_ENCODER) {
+    add_facodec_encoder_tensors(g);
   } else {
     add_gan_tensors(g);
   }
@@ -813,8 +891,9 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
         if (rc != AB_OK) return rc;
         continue;
       }
-      int rc = launch_tc_pack_weight(g->fptr((int)i), g->tcptr((int)i), t ? 1 : 0, (int)s.shape[t ? 0 : 1],
-                                     (int)s.shape[t ? 1 : 0], (int)s.shape[2], t ? s.stride : s.dilation, precision, st);
+      int rc = launch_tc_pack_weight(g->fptr((int)i), g->tcptr((int)i), t ? 1 : s.strided ? 2 : 0, (int)s.shape[t ? 0 : 1],
+                                     (int)s.shape[t ? 1 : 0], (int)s.shape[2], t || s.strided ? s.stride : s.dilation,
+                                     precision, st);
       if (rc != AB_OK) return rc;
     }
   }
@@ -852,25 +931,34 @@ namespace {
 constexpr int NBUF = 7;  // fp32: R0 R1 U P0 P1 TMP ACT
 constexpr int NIMG = 4;  // 16-bit operand images: U P0 P1 R (stage output, HiFi-GAN)
 
-size_t stage_max_image_bytes(const ab_generator* g, int64_t B, int64_t T) {
-  size_t mx = tc_act_image_bytes(B, g->cfg.upsample_initial_channel, T);   // conv_pre's output (stage 0's input)
+// Output length of the FACodec encoder's strided conv (k = 2s, padding s//2 + s%2) over t samples; 0 when the input is
+// empty or the padded input is shorter than the kernel (Conv1d raises), so an emptied stage stays empty
+int64_t encoder_stage_length(int64_t t, int s) {
+  if (t <= 0) return 0;
+  const int64_t padded = t + 2 * (s / 2 + s % 2);
+  return padded < 2 * s ? 0 : (padded - 2 * s) / s + 1;
+}
+
+// Largest stage tensor of a forward of T frames (T samples for the encoder), in elements (image = false) or as a
+// 16-bit operand image in bytes: conv_pre's output, each stage's blocks and, for the encoder, its strided conv's output
+size_t stage_max(const ab_generator* g, int64_t B, int64_t T, bool image) {
+  auto size = [&](int c, int64_t t) { return image ? tc_act_image_bytes(B, c, t) : (size_t)B * c * t; };
+  size_t mx = size(g->cfg.upsample_initial_channel, T);
   int64_t t = T;
   for (auto& st : g->stages) {
     t *= st.u;
-    mx = std::max(mx, tc_act_image_bytes(B, st.ch, t));
+    mx = std::max(mx, size(st.ch, t));
+    if (st.down) {
+      t = encoder_stage_length(t, st.down);
+      mx = std::max(mx, size(st.up.cout, t));
+    }
   }
   return mx;
 }
 
-size_t stage_max_elems(const ab_generator* g, int64_t B, int64_t T) {
-  size_t mx = (size_t)B * g->cfg.upsample_initial_channel * T;
-  int64_t t = T;
-  for (auto& st : g->stages) {
-    t *= st.u;
-    mx = std::max(mx, (size_t)B * st.ch * t);
-  }
-  return mx;
-}
+size_t stage_max_image_bytes(const ab_generator* g, int64_t B, int64_t T) { return stage_max(g, B, T, true); }
+
+size_t stage_max_elems(const ab_generator* g, int64_t B, int64_t T) { return stage_max(g, B, T, false); }
 // Vocos workspace: the fp32 residual stream X, the embed / final-norm output Y (fp32), the block input H and the
 // intermediate I (fp32 at AB_PREC_FP32, else 16-bit operand images; I also holds the fp32 head output), the spectrum S
 // [B*T][bins] complex and the iSTFT's workspace.  base == nullptr: sizes only.  0 when the iSTFT plan fails.
@@ -956,6 +1044,7 @@ int ab_generator_set_tail_events(ab_generator* g, void* const* events, int32_t n
 
 int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64_t source_frames) {
   if (!g || frames <= 0) return 0;
+  if (g->cfg.kind == AB_GEN_FACODEC_ENCODER) return ab_facodec_encoder_frames(g, frames);
   if (g->cfg.kind == AB_GEN_VOCOS || g->cfg.kind == AB_GEN_DIFFWAVE) return frames * g->hop;
   int64_t Tn = frames;
   for (int i = 0; i < g->cfg.num_upsamples; ++i) Tn = nsf_stage_length(g, i, Tn * g->cfg.upsample_rates[i], source_frames);
@@ -1031,7 +1120,9 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "forward: a DiffWave handle runs through ab_diffwave_forward");
   if (B <= 0 || T <= 0) return fail(AB_ERR_ARG, "forward: batch and frames must be positive (got %lld, %lld)", (long long)B, (long long)T);
   if (B > 65535) return fail(AB_ERR_UNSUPPORTED, "forward: batch %lld > 65535", (long long)B);
-  if ((int64_t)T * g->hop > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "forward: sequence too long");
+  // FACodec's encoder: T counts input samples, and the stages shorten the sequence
+  const bool enc = g->cfg.kind == AB_GEN_FACODEC_ENCODER;
+  if ((int64_t)T * (enc ? 1 : g->hop) > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "forward: sequence too long");
   const size_t need = ab_generator_workspace_bytes(g, B, T);
   if (!dev_workspace || workspace_bytes < need) return fail(AB_ERR_WORKSPACE, "forward: workspace %zu B < required %zu B", workspace_bytes, need);
   if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "forward: workspace must be 256-byte aligned");
@@ -1058,9 +1149,10 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   uint16_t *U16 = img[0], *P16[2] = {img[1], img[2]}, *R16 = img[3];
   const uint16_t* r_img = nullptr;   // operand image of lrelu(stage input, 0.1) when the previous stage emitted it
   float *R[2] = {buf[0], buf[1]}, *U = buf[2], *P[2] = {buf[3], buf[4]}, *TMP = buf[5], *ACT = buf[6];
-  // FACodec's generator is BigVGAN's pipeline with an activation in front of each transposed conv
+  // FACodec's generator is BigVGAN's pipeline with an activation in front of each transposed conv; its encoder the same
+  // ResidualUnits with an activation and a strided conv closing each stage
   const bool fac = g->cfg.kind == AB_GEN_FACODEC;
-  const bool big = g->cfg.kind == AB_GEN_BIGVGAN || fac;
+  const bool big = g->cfg.kind == AB_GEN_BIGVGAN || fac || enc;
   const bool tc = g->precision != AB_PREC_FP32;
   const int nk = g->cfg.num_kernels;
   int launches = 0;
@@ -1446,6 +1538,41 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     cur_r ^= 1;
     cin = C;
     r_img = stage_img_written ? R16 : nullptr;
+    if (sg.down) {
+      // FACodec encoder: x = Conv1d(C, 2C, k = 2s, stride s, padding s//2 + s%2)(Activation1d(SnakeBeta)(x))
+      // (facodec.py:136-154); the activation writes the operand image the tensor-core conv reads, or fp32
+      const ConvRef& dc = sg.up;
+      const int sd = sg.down, pad = sd / 2 + sd % 2;
+      const bool dtc = on_tc(dc), img = dtc && (C % 16) == 0;
+      rc = img ? snake(sg.act, R[cur_r], nullptr, C, Tn, P16[0]) : snake(sg.act, R[cur_r], ACT, C, Tn);
+      if (rc != AB_OK) return rc;
+      const int To = (int)encoder_stage_length(Tn, sd);
+      float* dst = R[cur_r ^ 1];
+      ++launches;
+      prof_begin(dtc ? 4 : 1, 2.0 * B * To * dc.cout * dc.cin * dc.k,
+                 4.0 * ((double)B * C * Tn + (double)B * dc.cout * To + (double)dc.cin * dc.cout * dc.k));
+      if (dtc) {
+        TcConvParams p;
+        p.mode = 2;
+        p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1; p.ximg = img ? P16[0] : nullptr;
+        p.w = g->tcptr(dc.w); p.bias = g->fptr(dc.b); p.y = dst;
+        p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d_or_u = sd; p.pad = pad;
+        p.precision = g->precision;
+        rc = launch_tc_conv(p, st);
+      } else {
+        ConvParams p;
+        p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1;
+        p.w_t = g->fptr(dc.w); p.bias = g->fptr(dc.b); p.residual = nullptr; p.acc_prev = nullptr; p.y = dst;
+        p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d = 1;
+        p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0;
+        rc = launch_conv1d_strided_fp32(p, sd, pad, st);
+      }
+      prof_end();
+      if (rc != AB_OK) return rc;
+      cur_r ^= 1;
+      Tn = To;
+      cin = dc.cout;
+    }
   }
   // post: leaky_relu(x) with the DEFAULT slope 0.01 (hifigan.py:215) or
   // activation_post (bigvgan.py:327); conv_post; tanh
@@ -1462,7 +1589,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   const int64_t Bfull = B;
   const ConvRef& cpost = g->conv_post;
   const float post_slope = big ? 1.0f : melgan ? 0.2f : 0.01f;
-  const int post_tanh = g->cfg.kind == AB_GEN_TRUNK ? 0 : 1;
+  const int post_tanh = g->cfg.kind == AB_GEN_TRUNK || enc ? 0 : 1;
   for (int ci = 0; ci < nchunk; ++ci) {
     const int64_t b0 = Bfull * ci / nchunk, b1 = Bfull * (ci + 1) / nchunk;
     B = b1 - b0;
@@ -1490,6 +1617,8 @@ int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64
                          const int64_t mel_strides[3], float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream) {
   if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
+  if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
+    return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
   return forward_impl(g, dev_mel, B, T, mel_strides, nullptr, 0, dev_wav, dev_workspace, workspace_bytes, stream);
 }
 
@@ -1497,6 +1626,8 @@ int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, in
                               const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
                               size_t workspace_bytes, void* stream) {
   if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
+  if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
+    return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
   return forward_impl(g, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes, stream);
 }
 
@@ -1765,6 +1896,28 @@ int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t
   if (rc != AB_OK) return rc;
   g->launches += 2;
   return AB_OK;
+}
+
+// ---------------------------------------------------------------------------
+// FACodec encoder
+// ---------------------------------------------------------------------------
+int64_t ab_facodec_encoder_frames(const ab_generator* g, int64_t samples) {
+  if (!g || g->cfg.kind != AB_GEN_FACODEC_ENCODER || samples <= 0) return 0;
+  int64_t t = samples;
+  for (auto& st : g->stages) t = encoder_stage_length(t, st.down);
+  return t;
+}
+
+int ab_facodec_encode(ab_generator* g, const float* dev_wav, int64_t B, int64_t N, const int64_t wav_strides[3],
+                      float* dev_out, void* dev_workspace, size_t workspace_bytes, void* stream) {
+  if (!g) return fail(AB_ERR_ARG, "facodec_encode: null handle");
+  if (g->cfg.kind != AB_GEN_FACODEC_ENCODER) return fail(AB_ERR_ARG, "facodec_encode: not a FACodec encoder handle");
+  if (!dev_wav || !wav_strides || !dev_out) return fail(AB_ERR_ARG, "facodec_encode: null argument");
+  if (B <= 0 || N <= 0) return fail(AB_ERR_ARG, "facodec_encode: batch %lld / samples %lld out of range", (long long)B, (long long)N);
+  if (ab_facodec_encoder_frames(g, N) <= 0)
+    return fail(AB_ERR_ARG, "facodec_encode: %lld samples leave a stage with no output (a strided conv's padded input is "
+                "shorter than its kernel)", (long long)N);
+  return forward_impl(g, dev_wav, B, N, wav_strides, nullptr, 0, dev_out, dev_workspace, workspace_bytes, stream);
 }
 
 // ---------------------------------------------------------------------------

@@ -246,6 +246,9 @@ int launch_facodec_vq2emb(const FacVqParams& p, cudaStream_t s);
 // launchers (ab_kernels_fp32.cu)
 int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);
+// strided conv1d (zero padding pad, (T + 2 pad - k) / stride + 1 outputs; p.d = 1, no epilogue terms): p.T is the input
+// length and p.y holds [B, Cout, T_out]
+int launch_conv1d_strided_fp32(const ConvParams& p, int stride, int pad, cudaStream_t s);
 int launch_conv_transpose1d_fp32(const ConvTParams& p, cudaStream_t s);
 int launch_activation1d(const SnakeParams& p, cudaStream_t s);
 // Repack a conv weight into [Cin][k][Cout] fp32, folding weight norm if g != nullptr.

@@ -403,6 +403,111 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
 }
 
 // ===========================================================================
+// Strided conv1d, y[co, t] = bias[co] + sum_ci sum_j W[co, ci, j] act(x)[ci, s t + j - pad] with zero padding,
+// (T + 2 pad - k) / s + 1 outputs (the downsampling conv of FACodec's EncoderBlock, facodec.py:136-154: k = 2s,
+// pad = s//2 + s%2).  The conv1d_fp32_kernel tile: 64 output channels x 128 outputs per CTA, 4 x 8 per thread; the
+// staged input row of a tile spans s (TT - 1) + k samples, stored by phase (sample n at [n % s][n / s], L per phase) so
+// that output t's tap j = s q + r reads [r][t + q]: consecutive lanes read consecutive words, free of bank conflicts.
+// ===========================================================================
+namespace {
+__global__ void __launch_bounds__(NT) conv1d_strided_fp32_kernel(ConvParams p, int stride, int pad, int Tout) {
+  extern __shared__ float smem[];
+  const int XW = stride * (TT - 1) + p.k, L = TT - 1 + (p.k + stride - 1) / stride;
+  float* xs = smem;                        // [CI_T][stride][L]
+  float* ws = smem + CI_T * stride * L;    // [CI_T][k][CO_T]
+  const int t0 = blockIdx.x * TT, co0 = blockIdx.y * CO_T, b = blockIdx.z;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const float slope = p.pre_slope;
+  const float* xb = p.x + (int64_t)b * p.xsb;
+  const int64_t tin0 = (int64_t)t0 * stride - pad;
+
+  float acc[4][8];
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+
+  for (int ci0 = 0; ci0 < p.Cin; ci0 += CI_T) {
+    for (int idx = threadIdx.x; idx < CI_T * XW; idx += NT) {
+      const int ci = idx / XW, n = idx - ci * XW, c = ci0 + ci, q = n / stride;
+      const int64_t t = tin0 + n;
+      float v = 0.f;
+      if (c < p.Cin && t >= 0 && t < p.T) {
+        v = __ldg(xb + (int64_t)c * p.xsc + t * p.xst);
+        v = v >= 0.f ? v : v * slope;
+      }
+      xs[(ci * stride + (n - q * stride)) * L + q] = v;
+    }
+    const int wn = CI_T * p.k * CO_T;
+    for (int idx = threadIdx.x; idx < wn; idx += NT) {
+      const int co = idx & (CO_T - 1);
+      const int r = idx / CO_T;  // ci * k + j
+      const int ci = r / p.k;
+      float v = 0.f;
+      if (ci0 + ci < p.Cin && co0 + co < p.Cout)
+        v = __ldg(p.w_t + ((int64_t)ci0 * p.k + r) * p.Cout + co0 + co);
+      ws[idx] = v;
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int ci = 0; ci < CI_T; ++ci) {
+      const float* xr = xs + ci * stride * L + tx;
+      const float* wr = ws + ci * p.k * CO_T + ty * 4;
+      for (int j = 0; j < p.k; ++j) {
+        const float4 w = *reinterpret_cast<const float4*>(wr + j * CO_T);
+        const int q = j / stride;
+        const float* xj = xr + (j - q * stride) * L + q;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float xv = xj[16 * i];
+          acc[0][i] = fmaf(w.x, xv, acc[0][i]);
+          acc[1][i] = fmaf(w.y, xv, acc[1][i]);
+          acc[2][i] = fmaf(w.z, xv, acc[2][i]);
+          acc[3][i] = fmaf(w.w, xv, acc[3][i]);
+        }
+      }
+    }
+    __syncthreads();
+  }
+
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const int co = co0 + ty * 4 + c;
+    if (co >= p.Cout) continue;
+    const float bv = p.bias ? __ldg(p.bias + co) : 0.f;
+    const int64_t row = ((int64_t)b * p.Cout + co) * Tout;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int t = t0 + tx + 16 * i;
+      if (t < Tout) p.y[row + t] = acc[c][i] + bv;
+    }
+  }
+}
+}  // namespace
+
+int launch_conv1d_strided_fp32(const ConvParams& p, int stride, int pad, cudaStream_t s) {
+  if (p.B <= 0 || p.Cin <= 0 || p.Cout <= 0 || p.T <= 0 || p.k <= 0 || stride <= 0 || stride > 64 || pad < 0 || pad >= p.k)
+    return fail(AB_ERR_ARG, "conv1d strided: bad shape B=%d Cin=%d Cout=%d T=%d k=%d stride=%d pad=%d", p.B, p.Cin, p.Cout,
+                p.T, p.k, stride, pad);
+  if (p.residual || p.acc_prev || p.out_div != 1.0f || p.post_tanh || p.reflect || p.epi != CONV_EPI_NONE || p.d != 1)
+    return fail(AB_ERR_ARG, "conv1d strided: no dilation, residual, acc_prev, out_div, tanh, reflection or epilogue");
+  if ((int64_t)p.T + 2 * pad < p.k) return fail(AB_ERR_ARG, "conv1d strided: %d samples are shorter than the kernel %d", p.T, p.k);
+  if (p.B > 65535) return fail(AB_ERR_UNSUPPORTED, "conv1d strided: batch %d > 65535", p.B);
+  const int Tout = (p.T + 2 * pad - p.k) / stride + 1;
+  const size_t smem = sizeof(float) * ((size_t)CI_T * stride * (TT - 1 + (p.k + stride - 1) / stride) +
+                                      (size_t)CI_T * p.k * CO_T);
+  if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "conv1d strided: k=%d stride=%d needs %zu B of shared memory", p.k, stride, smem);
+  static DeviceOnce configured;
+  if (smem > 48 * 1024 && configured.need())
+    AB_CUDA_TRY(cudaFuncSetAttribute(conv1d_strided_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  if (ceil_div(p.Cout, CO_T) > 65535) return fail(AB_ERR_UNSUPPORTED, "conv1d strided: too many channels");
+  dim3 grid((unsigned)ceil_div(Tout, TT), (unsigned)ceil_div(p.Cout, CO_T), (unsigned)p.B);
+  conv1d_strided_fp32_kernel<<<grid, NT, smem, s>>>(p, stride, pad, Tout);
+  AB_LAUNCH_CHECK("conv1d_strided_fp32_kernel");
+  return AB_OK;
+}
+
+// ===========================================================================
 // ConvTranspose1d(stride=u, padding=p) fused with the leaky_relu in front of it (hifigan.py:206-207, p = (k-u)/2;
 // bigvgan.py:316-318 has no activation; melgan.py:73-80, p = u//2 + u%2 with output_padding u%2), Tin*u outputs:
 //   y[co,t] = b[co] + sum_ci sum_{j = (t+p) mod u, +u, ... < k} x[ci,(t+p-j)/u] * W[ci,co,j]

@@ -118,15 +118,30 @@ __device__ __forceinline__ void stage_biases(float* bias_s, const HcArgs& p, int
 // image or from lrelu(x, pre_slope); zero outside [0, Tin) and C_in.  Thread lt of nthreads cooperating threads.
 // REFLECT: time t outside [0, Tin) reads row -t or 2 (Tin - 1) - t instead (ReflectionPad1d, MelGAN), zero where that
 // row does not exist either (rows no valid output reads).
-template <int BF16, int REFLECT = 0>
+// STRIDED: the polyphase operand of a stride-s conv (make_geom mode 3): K chunk kc = c8_0 / 4 holds phase
+// r = kc / ceil(C_in / 32) of the input channels [32 (kc mod ceil(C_in / 32)), + 32), and row tau is input time
+// s tau + r - pad (s = g.u, pad = g.pad), so each row is gathered from its own input time.
+template <int BF16, int REFLECT = 0, int STRIDED = 0>
 __device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int b, uint8_t* tile, int c8_0, int nplanes,
                                           int rows, int t0, int lt, int nthreads) {
   const int items = nplanes * rows;
+  int tmul = 1, toff = 0;
+  if constexpr (STRIDED) {
+    const int nkc_in = (p.Cin + 31) >> 5, r = (c8_0 >> 2) / nkc_in;
+    c8_0 -= 4 * r * nkc_in;
+    tmul = g.u;
+    toff = r - g.pad;
+  }
+  auto time_of = [&](int row) {
+    if constexpr (REFLECT) return reflect_time(t0 + row, g.Tin);
+    else if constexpr (STRIDED) return tmul * (t0 + row) + toff;
+    else return t0 + row;
+  };
   if (p.ximg != nullptr) {
     const uint16_t* xb = p.ximg + (size_t)b * g.c8n_in * g.Tin * 8;
     for (int idx = lt; idx < items; idx += nthreads) {
       const int c = idx / rows, row = idx - c * rows;
-      const int c8 = c8_0 + c, t = REFLECT ? reflect_time(t0 + row, g.Tin) : t0 + row;
+      const int c8 = c8_0 + c, t = time_of(row);
       const bool ok = c8 < g.c8n_in && t >= 0 && t < g.Tin;
       cp_async16(smem_u32(tile) + unit_offset(rows, c, row),
                  ok ? (const void*)(xb + ((size_t)c8 * g.Tin + t) * 8) : (const void*)xb, ok ? 16u : 0u);
@@ -136,7 +151,7 @@ __device__ __forceinline__ void load_tile(const HcArgs& p, const HcGeom& g, int 
     const float* xb = p.x + (int64_t)b * p.xsb;
     for (int idx = lt; idx < items; idx += nthreads) {
       const int c = idx / rows, row = idx - c * rows;
-      const int t = REFLECT ? reflect_time(t0 + row, g.Tin) : t0 + row;
+      const int t = time_of(row);
       const bool ok = t >= 0 && t < g.Tin;
       float v[8];
 #pragma unroll
@@ -296,7 +311,8 @@ __device__ __forceinline__ void add_terms(float (&acc)[MT][NW / 2], const Frag<M
 // 16 / 20 with it, which made HiFi-GAN V1's ConvTranspose layers about 5 ms per step slower (H100 80GB HBM3, 400 W
 // power limit).  Re-check those numbers before deleting it.
 // REFLECT (mode 0 only): ReflectionPad1d in place of the zero "same" padding (MelGAN's conv_pre and ResnetBlock conv).
-template <int NW, int BF16, int REFLECT = 0>
+// STRIDED (mode 0 only): the stride-s conv as a stride-1 conv over the polyphase operand (load_tile, make_geom mode 3).
+template <int NW, int BF16, int REFLECT = 0, int STRIDED = 0>
 __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
@@ -367,7 +383,7 @@ __global__ void __launch_bounds__(HC_THREADS, NW >= 256 ? 1 : 2) hconv_kernel(Hc
   // A chunk kc: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
   auto load_chunk = [&](int kc) {
     __syncthreads();   // every warp has finished the MMAs that read the previous chunk
-    load_tile<BF16, REFLECT>(p, g, b, smem, 4 * kc, 4, g.rowsA, O - g.a0, tid, HC_THREADS);
+    load_tile<BF16, REFLECT, STRIDED>(p, g, b, smem, 4 * kc, 4, g.rowsA, O - g.a0, tid, HC_THREADS);
     fence_proxy_async();
     __syncthreads();
   };
@@ -1273,12 +1289,23 @@ int pow2_at_least(int x) {
   return n;
 }
 
-// mode 0 conv (d_or_u = dilation), 1 conv-transpose (d_or_u = stride)
+// mode 0 conv (d_or_u = dilation), 1 conv-transpose (d_or_u = stride), 2 strided conv (d_or_u = stride s): a stride-1
+// conv over s phases of the input, K chunk r * ceil(C_in / 32) + kc holding phase r, tap m holding kernel tap s m + r
 int layer_geom(int mode, int cin, int cout, int k, int d_or_u, HcLayer& L) {
   if (cin <= 0 || cout <= 0 || k <= 0 || d_or_u <= 0) return fail(AB_ERR_ARG, "tc conv: bad layer shape");
   L.mode = mode;
   L.nkc = (cin + 31) / 32;
-  if (mode == 0) {
+  if (mode == 2) {
+    const int s = d_or_u;
+    if (s > AB_TC_MAX_STRIDE) return fail(AB_ERR_UNSUPPORTED, "tc conv: stride %d > %d", s, AB_TC_MAX_STRIDE);
+    if (k < s) return fail(AB_ERR_UNSUPPORTED, "tc conv: strided conv needs k >= stride (k %d, stride %d)", k, s);
+    L.NW = std::min(256, pow2_at_least(rup(cout, 16)));
+    L.NB = (cout + L.NW - 1) / L.NW;
+    L.cc = L.NW;
+    L.ntaps = (k + s - 1) / s;
+    L.nkc *= s;
+    L.u = s;
+  } else if (mode == 0) {
     if (!(k & 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv: conv kernel size must be odd");
     L.NW = std::min(256, pow2_at_least(rup(cout, 16)));
     L.NB = (cout + L.NW - 1) / L.NW;
@@ -1320,9 +1347,12 @@ __global__ void hc_pack_weight_kernel(const float* __restrict__ w_t, uint16_t* _
     if (L.mode == 0) {
       const int co = nb * L.NW + n;
       if (ci < cin && co < cout) v = w_t[((int64_t)ci * k + tap) * cout + co];
-    } else {
+    } else if (L.mode == 1) {
       const int cl = n / L.u, phi = n - cl * L.u, co = nb * L.cc + cl, j = phi + L.u * tap;
       if (ci < cin && cl < L.cc && co < cout && j < k) v = w_t[((int64_t)ci * k + j) * cout + co];
+    } else {
+      const int nkc_in = L.nkc / L.u, r = kc / nkc_in, cr = ci - 32 * r * nkc_in, co = nb * L.NW + n, j = L.u * tap + r;
+      if (cr < cin && co < cout && j < k) v = w_t[((int64_t)cr * k + j) * cout + co];
     }
     img[idx] = (uint16_t)(pack2(v, 0.f, bf16) & 0xffffu);
   }
@@ -1367,16 +1397,17 @@ bool layout_smem(HcGeom& g, uint32_t abytes, uint32_t ibytes, uint32_t nbias, ui
 }
 
 // Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.  mode 1: padding
-// pad (-1: (k - u) / 2), Tin * u outputs.  persistent: for hpair_kernel or hitem_kernel (one CTA per SM, as many A
+// pad (-1: (k - u) / 2), Tin * u outputs.  mode 3 (strided conv, stride d_or_u, padding pad): runs as mode 0 over the
+// polyphase operand, output row t reading operand rows t .. t + ceil(k / s) - 1, (Tin + 2 pad - k) / s + 1 outputs.  persistent: for hpair_kernel or hitem_kernel (one CTA per SM, as many A
 // chunk buffers as fit next to two W stages) rather than hconv_kernel.  pingpong: pair mode at N = 64 and 128 lays
 // out hpair_kernel's ping-pong schedule (two intermediate tiles) where it fits, else the cooperative one.
 int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool persistent, HcGeom& g, int pad = -1,
               bool pingpong = false) {
   HcLayer L;
-  int rc = layer_geom(mode == 2 ? 0 : mode, cin, cout, k, d_or_u, L);
+  int rc = layer_geom(mode == 2 ? 0 : mode == 3 ? 2 : mode, cin, cout, k, d_or_u, L);
   if (rc != AB_OK) return rc;
   if (mode == 2 && (cin != cout || L.NB != 1)) return fail(AB_ERR_UNSUPPORTED, "tc conv pair: C=%d not in [1,%d]", cin, TC_MAX_C);
-  g.mode = mode;
+  g.mode = mode == 3 ? 0 : mode;
   g.nsteps = mode == 2 ? 2 : 1;
   g.NB = L.NB;
   g.cc = L.cc;
@@ -1398,6 +1429,14 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool pers
     g.a0 = maxshift;
     g.V = g.R;
     rows_total = (g.Tout - 1 + g.pad) / L.u + 1;
+  } else if (mode == 3) {
+    g.d = 1;
+    g.pad = pad;
+    g.Tout = (Tin + 2 * pad - k) / L.u + 1;
+    maxshift = g.ntaps - 1;
+    g.a0 = 0;
+    g.V = g.R;
+    rows_total = g.Tout;
   } else {
     g.d = d_or_u;
     g.pad = 0;
@@ -1533,7 +1572,8 @@ int launch_persistent(const char* name, const char* what, int64_t work, const Hc
 // on the persistent hitem_kernel, pair mode on the persistent hpair_kernel.  From fp32 input, hitem_kernel's 96 loader
 // threads (8 scattered loads in flight each) cannot keep up with the MMAs and it is slower than hconv_kernel, whose
 // 256 threads all load.
-int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s, bool reflect = false) {
+int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s, bool reflect = false,
+                 bool strided = false) {
   if (precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc conv: bad precision");
   const int64_t work = (int64_t)a.B * g.tiles;
   if (g.mode == 1 && a.ximg)
@@ -1563,6 +1603,9 @@ int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s
     if (reflect)
       return launch_kernel<hconv_kernel<NW, decltype(bf16)::value, 1>>("hconv_kernel", (unsigned)work, HC_THREADS, limit,
                                                                         g.smem_bytes, s, a, g);
+    if (strided)
+      return launch_kernel<hconv_kernel<NW, decltype(bf16)::value, 0, 1>>("hconv_kernel", (unsigned)work, HC_THREADS,
+                                                                           limit, g.smem_bytes, s, a, g);
     return launch_kernel<hconv_kernel<NW, decltype(bf16)::value>>("hconv_kernel", (unsigned)work, HC_THREADS, limit,
                                                                    g.smem_bytes, s, a, g);
   });
@@ -1634,16 +1677,25 @@ int launch_tc_pack_weight(const float* w_t, void* image, int mode, int cin, int 
 // channels as zero; the conv-transpose epilogue writes only c_out < C_out.
 bool tc_can_emit_image(int mode, int cin, int cout, int k, int d_or_u) {
   HcLayer L;
-  return layer_geom(mode, cin, cout, k, d_or_u, L) == AB_OK && (mode == 0 || (cout % 16) == 0);
+  return layer_geom(mode, cin, cout, k, d_or_u, L) == AB_OK && (mode == 0 || (mode == 1 && (cout % 16) == 0));
 }
 
 int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   const bool pair = p.w2 != nullptr;
   if ((!p.x && !p.ximg) || !p.y || !p.w) return fail(AB_ERR_ARG, "tc conv: null argument");
   if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "tc conv: bad shape");
-  if (p.mode != 0 && p.mode != 1) return fail(AB_ERR_ARG, "tc conv: mode must be 0 (conv) or 1 (conv-transpose)");
-  if (p.mode == 1 && (p.residual || p.acc_prev || p.out_div != 1.0f || p.post_tanh))
-    return fail(AB_ERR_ARG, "tc conv-transpose: residual, acc_prev, out_div and tanh belong to conv");
+  if (p.mode < 0 || p.mode > 2) return fail(AB_ERR_ARG, "tc conv: mode must be 0 (conv), 1 (conv-transpose) or 2 (strided conv)");
+  if (p.mode != 0 && (p.residual || p.acc_prev || p.out_div != 1.0f || p.post_tanh))
+    return fail(AB_ERR_ARG, "tc conv: residual, acc_prev, out_div and tanh belong to mode 0");
+  if (p.mode == 2) {
+    if (pair || p.reflect || p.yimg) return fail(AB_ERR_ARG, "tc strided conv: no second conv, reflection or output image");
+    if (p.d_or_u < 1 || p.d_or_u > AB_TC_MAX_STRIDE || p.k < p.d_or_u)
+      return fail(AB_ERR_UNSUPPORTED, "tc strided conv: stride %d needs 1 <= stride <= %d and k = %d >= stride", p.d_or_u,
+                  AB_TC_MAX_STRIDE, p.k);
+    if (p.pad < 0 || p.pad >= p.k) return fail(AB_ERR_ARG, "tc strided conv: padding %d outside [0, k = %d)", p.pad, p.k);
+    if ((int64_t)p.T + 2 * p.pad < p.k)
+      return fail(AB_ERR_ARG, "tc strided conv: %d samples with padding %d are shorter than the kernel %d", p.T, p.pad, p.k);
+  }
   if (pair && !(p.mode == 0 && p.Cin == p.Cout && tc_conv_supported(p.Cin, p.k)))
     return fail(AB_ERR_UNSUPPORTED, "tc conv pair: C_in=%d C_out=%d k=%d", p.Cin, p.Cout, p.k);
   if (p.mode == 1 && p.ximg && (p.Cin % 16) != 0)
@@ -1657,7 +1709,8 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   HcGeom g;
   // pairs and ConvTranspose layers from an operand image run on the persistent kernels (launch_hconv)
   const bool persistent = pair || (p.mode == 1 && p.ximg);
-  int rc = make_geom(pair ? 2 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, persistent, g, p.pad, p.pair_schedule != 0);
+  int rc = make_geom(pair ? 2 : p.mode == 2 ? 3 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, persistent, g, p.pad,
+                     p.pair_schedule != 0);
   if (rc != AB_OK) return rc;
   if (p.reflect && g.a0 >= p.T)
     return fail(AB_ERR_ARG, "tc conv: reflection padding %d needs more than %d samples", g.a0, p.T);
@@ -1668,7 +1721,7 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   a.ws[1] = p.w2; a.bs[1] = p.b2;
   a.y = p.y; a.residual = p.residual; a.acc_prev = p.acc_prev; a.post_tanh = p.post_tanh;
   a.yimg = p.yimg; a.img_slope = p.img_slope;
-  return launch_hconv(a, g, p.precision, s, p.reflect != 0);
+  return launch_hconv(a, g, p.precision, s, p.reflect != 0, p.mode == 2);
 }
 
 

@@ -15,7 +15,7 @@ namespace ab {
 //     (:139-144); residual, acc_prev and out_div are the branch mix of hifigan.py:208-214
 //   conv-transpose (mode 1, stride u = d_or_u, padding `pad`, T*u outputs):  y = conv_transpose(act(x), u) + bias
 struct TcConvParams {
-  int mode = 0;                      // 0 conv, 1 conv-transpose
+  int mode = 0;                      // 0 conv, 1 conv-transpose, 2 strided conv (stride d_or_u, padding pad)
   const float* x = nullptr;          // fp32 [B, Cin, T] with element strides xsb / xsc / xst (unused when ximg is given)
   int64_t xsb = 0, xsc = 0, xst = 0;
   const uint16_t* ximg = nullptr;    // nullable: operand image [B][ceil16(Cin)/8][T][8] of the activated input
@@ -29,13 +29,14 @@ struct TcConvParams {
   const float* acc_prev = nullptr;   // conv only, nullable (may alias y)
   float out_div = 1.0f;              // conv only
   int post_tanh = 0;                 // conv only
-  float* y = nullptr;                // conv: [B, Cout, T]; conv-transpose: [B, Cout, T*u]
+  float* y = nullptr;                // conv: [B, Cout, T]; conv-transpose: [B, Cout, T*u]; strided: [B, Cout, (T+2pad-k)/s+1]
   uint16_t* yimg = nullptr;          // nullable (tc_can_emit_image): operand image of lrelu(y, img_slope) for the next kernel
   float img_slope = 1.0f;
   int B = 0, Cin = 0, Cout = 0, T = 0, k = 0, d_or_u = 1;
   int precision = AB_PREC_FP32;      // set to AB_PREC_TC_F16 | AB_PREC_TC_BF16 (fp32 is rejected)
   int reflect = 0;                   // conv only, no w2: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN)
-  int pad = -1;                      // conv-transpose padding, 0 <= pad < k; -1 = (k-u)/2 (HiFi-GAN; MelGAN: u//2 + u%2)
+  int pad = -1;                      // conv-transpose padding, 0 <= pad < k; -1 = (k-u)/2 (HiFi-GAN; MelGAN: u//2 + u%2);
+                                     // strided conv: zero padding on both sides, 0 <= pad < k
   int pair_schedule = 0;             // pair mode: 0 cooperative, 1 ping-pong where served (N = 64, 128); bit-equal outputs
 };
 // 16-bit weight image of a layer, 0 when launch_tc_conv cannot run it
@@ -58,6 +59,8 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s);
 // Same arithmetic in the same order as npairs launches of launch_tc_conv: the results are bit-equal.
 constexpr int AB_TC_CHAIN_MAX_PAIRS = 3;
 constexpr int AB_TC_CHAIN_MAX_C = 128;
+// largest stride of launch_tc_conv's strided conv (mode 2)
+constexpr int AB_TC_MAX_STRIDE = 8;
 struct TcChainParams {
   const float* x;          // contiguous [B, C, T] fp32 (block input = first residual)
   const uint16_t* ximg;    // nullable: operand image of lrelu(x, slope), [B][ceil16(C)/8][T][8]

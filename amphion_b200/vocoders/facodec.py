@@ -7,8 +7,11 @@ the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_pr
 - ``inference(x, speaker_embedding)``: the timbre FiLM (LayerNorm over channels, ``x * gamma + beta``) and the
   BigVGAN-family generator -> ``[B, 1, T * prod(up_ratios)]`` (:568-576).
 
-The encoder-side ``forward`` (quantization, the timbre transformer) and the training branch are not served; the modules
-only ``forward`` evaluates are kept as parameters."""
+``FACodecEncoder`` (:157-194) serves the waveform -> latent side natively (``AB_GEN_FACODEC_ENCODER``): ``forward`` /
+``inference`` map ``[B, 1, N]`` to ``[B, out_channels, F]`` through the same ResidualUnits and strided convolutions.
+
+The decoder's encoder-side ``forward`` (quantization, the timbre transformer) and the training branch are not served;
+the modules only ``forward`` evaluates are kept as parameters."""
 from __future__ import annotations
 
 import ctypes as C
@@ -22,7 +25,8 @@ from .. import _capi
 from .activations import Activation1d, SnakeBeta
 from .generator import NativeGenerator
 
-_SERVED = "amphion_b200 serves FACodecDecoder.vq2emb() and FACodecDecoder.inference()"
+_SERVED = ("amphion_b200 serves FACodecEncoder.forward() / .inference(), FACodecDecoder.vq2emb() and "
+           "FACodecDecoder.inference()")
 
 
 def _native_only(name):
@@ -339,6 +343,136 @@ class FACodecDecoder(NativeGenerator):
                                       f"transformer) is not served; {_SERVED}")
         raise NotImplementedError(f"amphion_b200: the training branch of FACodecDecoder.forward (the predictors, "
                                   f"random residual masking) is not served; {_SERVED}")
+
+    def remove_weight_norm(self):
+        def _remove(m):
+            try:
+                remove_weight_norm(m)
+            except ValueError:   # this module has no weight norm
+                return
+        self.apply(_remove)
+        self.invalidate()
+
+
+class EncoderBlock(nn.Module):
+    """Parameter holder for facodec.py:136-154: three ResidualUnits at dim // 2, act, WNConv1d(dim // 2, dim, k = 2s,
+    stride s, padding s//2 + s%2)."""
+
+    def __init__(self, dim: int = 16, stride: int = 1):
+        super().__init__()
+        self.block = nn.Sequential(
+            ResidualUnit(dim // 2, dilation=1), ResidualUnit(dim // 2, dilation=3), ResidualUnit(dim // 2, dilation=9),
+            _act(dim // 2),
+            weight_norm(nn.Conv1d(dim // 2, dim, kernel_size=2 * stride, stride=stride, padding=stride // 2 + stride % 2)))
+
+    def forward(self, x):
+        _native_only("EncoderBlock")
+
+
+def _init_weights(m):
+    """facodec.py:21-24, as FACodecEncoder.reset_parameters applies it."""
+    if isinstance(m, nn.Conv1d):
+        nn.init.trunc_normal_(m.weight, std=0.02)
+        nn.init.constant_(m.bias, 0)
+
+
+class FACodecEncoder(NativeGenerator):
+    """Drop-in for FACodecEncoder (facodec.py:157-194): the same constructor and parameter tree (``block.*``), so the
+    released ``ns3_facodec_encoder.bin`` loads strictly.  ``forward(x)`` / ``inference(x)``: wav ``[B, 1, N]`` (any
+    strides) -> ``[B, out_channels, F]`` fp32, F = ``frames(N)``."""
+
+    kind = "facodec_encoder"
+
+    def __init__(self, ngf=32, up_ratios=(2, 4, 5, 5), out_channels=1024):
+        super().__init__()
+        self.hop_length = int(np.prod(up_ratios))
+        self.up_ratios = [int(u) for u in up_ratios]
+        self.ngf, self.out_channels = int(ngf), int(out_channels)
+        d_model = ngf
+        block = [weight_norm(nn.Conv1d(1, d_model, kernel_size=7, padding=3))]
+        for stride in up_ratios:
+            d_model *= 2
+            block.append(EncoderBlock(d_model, stride=stride))
+        block += [_act(d_model), weight_norm(nn.Conv1d(d_model, out_channels, kernel_size=3, padding=1))]
+        self.block = nn.Sequential(*block)
+        self.enc_dim = d_model
+        self.apply(_init_weights)
+
+    # ---- NativeGenerator hooks -------------------------------------------------------
+    def _input_channels(self):
+        return 1
+
+    def _hop(self):
+        return self.hop_length
+
+    def _upsample_rates(self):
+        return list(self.up_ratios)
+
+    def _c_config(self):
+        if len(self.up_ratios) > _capi.AB_MAX_STAGES:
+            raise ValueError("amphion_b200: too many up_ratios for the native encoder")
+        c = _capi.GeneratorConfig()
+        c.kind = _capi.GEN_FACODEC_ENCODER
+        c.n_mel = 1
+        c.upsample_initial_channel = self.ngf
+        c.num_upsamples = len(self.up_ratios)
+        for i, u in enumerate(self.up_ratios):
+            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
+        c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
+        for p, d in enumerate((1, 3, 9)):
+            c.resblock_dilation_sizes[0][p] = d
+        c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
+        c.trunk_out_channels = self.out_channels
+        return c
+
+    def frames(self, n_samples):
+        """Output frames for n_samples input samples (0: a strided conv would have no output)."""
+        t = int(n_samples)
+        for s in self.up_ratios:
+            pad = s // 2 + s % 2
+            if t <= 0 or t + 2 * pad < 2 * s:
+                return 0
+            t = (t + 2 * pad - 2 * s) // s + 1
+        return t
+
+    # ---- served methods --------------------------------------------------------------
+    def forward(self, x, out=None):
+        """wav [B, 1, N] (any strides) -> [B, out_channels, F] fp32 on the wav's device.  ``out`` (beyond the reference
+        signature): a contiguous fp32 [B, out_channels, F] tensor to write into."""
+        if x.dim() != 3 or x.shape[1] != 1:
+            raise ValueError(f"FACodecEncoder expects a waveform of shape [B, 1, N], got {tuple(x.shape)}")
+        B, _, N = x.shape
+        if B == 0 or N == 0:
+            raise ValueError("amphion_b200: empty waveform batch")
+        F = self.frames(N)
+        if F <= 0:
+            raise ValueError(f"FACodecEncoder: {N} samples are too short for up_ratios {self.up_ratios} (a strided "
+                             f"conv's padded input would be shorter than its kernel)")
+        _capi.require_cuda(x, "FACodecEncoder.forward")
+        if x.dtype != torch.float32:
+            x = x.float()
+        with torch.cuda.device(x.device):
+            self._sync_params(x.device)
+            lib, h = _capi.lib, self._handle
+            need = lib.ab_generator_workspace_bytes(h, B, N)
+            if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != x.device:
+                self._workspace = None
+                self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=x.device)
+            wbase = (self._workspace.data_ptr() + 255) // 256 * 256
+            if out is None:
+                y = torch.empty(B, self.out_channels, F, dtype=torch.float32, device=x.device)
+            else:
+                if (tuple(out.shape) != (B, self.out_channels, F) or out.dtype != torch.float32 or out.device != x.device
+                        or not out.is_contiguous()):
+                    raise ValueError(f"out must be a contiguous fp32 [{B}, {self.out_channels}, {F}] tensor on {x.device}")
+                y = out
+            _capi.check(lib.ab_facodec_encode(h, _capi.ptr(x), B, N, _capi.shape_array(x.stride()), _capi.ptr(y),
+                                              C.c_void_p(wbase), need, _capi.stream_ptr()), "ab_facodec_encode")
+            self.last_launches = lib.ab_generator_last_launches(h)
+        return y
+
+    def inference(self, x):
+        return self.forward(x)
 
     def remove_weight_norm(self):
         def _remove(m):

@@ -93,10 +93,23 @@ extern "C" {
  * activation), "model.{1+i}.block.1" (ConvTranspose), "model.{1+i}.block.{2,3,4}.block.{0,1,2,3}" (a ResidualUnit's
  * act, k = 7 conv, act, k = 1 conv), "model.{1+n}" (final act), "model.{2+n}" (conv_post), "timbre_linear.{weight,bias}",
  * "quantizer.{q}.layers.{j}._codebook.weight" and ".out_proj.weight" (weight-normed nn.Linear: load_weight_norm with
- * weight_g [out, 1]) / ".out_proj.bias".  Runs through the ab_facodec_* entry points, not ab_generator_forward. */
+ * weight_g [out, 1]) / ".out_proj.bias".  Runs through the ab_facodec_* entry points, not ab_generator_forward.
+ * AB_GEN_FACODEC_ENCODER: NaturalSpeech 3's FACodecEncoder.forward / .inference (models/codec/ns3_codec/facodec.py:121-194):
+ * wav [B, 1, N] -> conv_pre (1 -> ngf, k = 7, padding 3); per stride s (C = ngf 2^i): three ResidualUnits
+ * x = x + conv_k1(act(conv_k7(act(x), dilation d))) with d = 1, 3, 9, then Activation1d(SnakeBeta) and Conv1d(C, 2C,
+ * k = 2s, stride s, padding s//2 + s%2); final act, conv_post (k = 3, padding 1) -> [B, out_channels, F], no tanh.  Each
+ * strided conv leaves (t + 2 (s//2 + s%2) - 2s) / s + 1 of its t samples (ab_facodec_encoder_frames).  Config fields, in
+ * the decoder's conventions: n_mel = 1 (the waveform channel), upsample_initial_channel = ngf, num_upsamples and
+ * upsample_rates = up_ratios in encoder order (first stride first, each 1..8), upsample_kernel_sizes = 2 s, resblock = 1,
+ * num_kernels = 1, resblock_kernel_sizes[0] = 7, num_dilations[0] = 3 with dilations (1, 3, 9), activation =
+ * AB_ACT_SNAKEBETA, snake_logscale = 1, trunk_out_channels = out_channels; every other field 0.  Tensors keep the
+ * reference's nn.Sequential names: "block.0" (conv_pre), "block.{1+i}.block.{0,1,2}.block.{0,1,2,3}" (a ResidualUnit's
+ * act, k = 7 conv, act, k = 1 conv), "block.{1+i}.block.3" (the stage's activation), "block.{1+i}.block.4" (the strided
+ * conv), "block.{1+n}" (final act), "block.{2+n}" (conv_post).  conv_pre (one input channel) runs on the fp32 CUDA cores
+ * at every precision.  Runs through ab_facodec_encode, not ab_generator_forward. */
 enum ab_generator_kind {
   AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
-  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7
+  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8
 };
 #define AB_FACODEC_MAX_Q 32   /* most codebook layers over the three ResidualVQs */
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
@@ -141,7 +154,7 @@ typedef struct ab_generator_config {
   /* HiFiGAN_vits (hifigan.py:376-449, the decoder inside VITS): kind AB_GEN_HIFIGAN plus */
   int32_t gin_channels;                         /* > 0: tensors "cond.weight" [C0, gin, 1], "cond.bias" [C0] (:424-425) */
   int32_t conv_post_no_bias;                    /* 1: conv_post = Conv1d(ch, 1, 7, bias=False) (:421), no "conv_post.bias" */
-  /* AB_GEN_TRUNK only (0 elsewhere) */
+  /* AB_GEN_TRUNK only (0 elsewhere), and trunk_out_channels for AB_GEN_FACODEC_ENCODER (its out_channels) */
   int32_t trunk_out_channels;                   /* conv_post output channels (n_fft/2+1, or 2*(n_fft/2+1) for R|I) */
   int32_t trunk_in_kernel;                      /* conv_pre kernel size (odd) */
   int32_t trunk_out_kernel;                     /* conv_post kernel size (odd) */
@@ -293,6 +306,16 @@ int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t batch, int
                          size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
+ * FACodec encoder (AB_GEN_FACODEC_ENCODER): FACodecEncoder.forward / .inference (models/codec/ns3_codec/facodec.py:157-194).
+ * ---------------------------------------------------------------------- */
+/* frames F of the encoder's output for `samples` input samples; 0 when a stage would be empty (or g is not an encoder) */
+int64_t ab_facodec_encoder_frames(const ab_generator* g, int64_t samples);
+/* wav [B, 1, N] fp32 with any element strides -> out [B, out_channels, F] fp32 contiguous, F = ab_facodec_encoder_frames.
+ * Workspace: ab_generator_workspace_bytes(g, B, N), 256-byte aligned.  AB_ERR_ARG before any launch when F == 0. */
+int ab_facodec_encode(ab_generator* g, const float* dev_wav, int64_t batch, int64_t samples, const int64_t wav_strides[3],
+                      float* dev_out, void* dev_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
  * Activation1d(Snake|SnakeBeta).forward  (modules/anti_aliasing/act.py:31-36,
  * resample.py:36-45,62-65, filter.py:92-99, activation_functions/snake.py:51-61,110-122)
  * standalone: x [B,C,T] -> y [B,C,T], both contiguous fp32.  beta may alias alpha (Snake).
@@ -334,6 +357,9 @@ int ab_conv_transpose1d_forward(const float* dev_x, const float* dev_w, const fl
  *     in place of the zero padding (AB_ERR_ARG, nothing launched, when the reflection needs more than T samples)
  *   mode 1, ConvTranspose1d stride u = d_or_u, padding pad (-1: (k-u)/2), T*u outputs, w [Cin, Cout, k]:
  *     y = conv_transpose(act(x)) + bias; residual, acc_prev and out_div != 1 are refused
+ *   mode 2, strided Conv1d, stride s = d_or_u (1..8), any k >= s, zero padding 0 <= pad < k, w [Cout, Cin, k]:
+ *     y[t] = bias + sum_j W_j act(x)[s t + j - pad], T_out = (T + 2 pad - k) / s + 1 (AB_ERR_ARG when T + 2 pad < k);
+ *     residual, acc_prev, out_div != 1, reflect and yimg are refused
  *   y fp32 [B, Cout, T_out]; dev_yimg (nullable): the operand image [B][ceil16(Cout)/8][T_out][8] of
  *   rnd(lrelu(y, img_slope)), padding channels zero (mode 1: Cout % 16 == 0).  bias, residual, acc_prev nullable. */
 size_t ab_tc_conv_workspace_bytes(int32_t mode, int64_t cin, int64_t cout, int32_t ksize, int32_t d_or_u);
