@@ -146,7 +146,6 @@ struct ab_generator {
   int hop = 1;
   int launches = 0;
   int rb_mode = 2;          // "resblock_fusion" option
-  int pair_schedule = 0;    // "pair_schedule" option
   std::vector<cudaEvent_t> tail_events;   // ab_generator_set_tail_events: consumed by the next forward
   int64_t source_frames = 0;              // NSF-HiFiGAN: frames of the f0 track of the next forward (0 = covers the mel)
 
@@ -1066,11 +1065,6 @@ int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
     g->rb_mode = value;
     return AB_OK;
   }
-  if (strcmp(key, "pair_schedule") == 0) {
-    if (value < 0 || value > 1) return fail(AB_ERR_ARG, "set_option: pair_schedule must be 0 or 1 (got %d)", value);
-    g->pair_schedule = value;
-    return AB_OK;
-  }
   return fail(AB_ERR_ARG, "set_option: unknown key '%s'", key);
 }
 
@@ -1206,7 +1200,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
     p.residual = residual; p.acc_prev = acc_prev; p.out_div = out_div; p.post_tanh = post_tanh;
     p.y = y; p.yimg = yimg; p.img_slope = 0.1f;
     p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d_or_u = c.d;
-    p.precision = g->precision; p.reflect = c.reflect; p.pair_schedule = g->pair_schedule;
+    p.precision = g->precision; p.reflect = c.reflect;
     ++launches;
     const bool rb = c.cin == c.cout && tc_conv_supported(c.cin, c.k);   // pair / block-mode capable ResBlock conv
     prof_begin(rb ? 0 : 4, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes);

@@ -85,7 +85,6 @@ struct HcGeom {
   int nconv, H, G, rowsX;
   int dil[AB_TC_CHAIN_MAX_PAIRS];
   int nabuf;               // pair mode: A chunk buffers
-  int pingpong;            // pair mode: one intermediate tile per consumer warpgroup (hpair_kernel's ping-pong schedule)
 };
 
 // ------------------------------------------------------------------------------------------------ shared device code
@@ -468,11 +467,6 @@ static_assert(128 * HB_PRODUCER_REGS + 256 * HB_CONSUMER_REGS <= 65536, "setmaxn
 constexpr int HP_ABUF_MAX = 3;
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-// hpair_kernel's ping-pong schedule: named barrier 2 + cw gates consumer warpgroup cw's next MMA phase, which the other
-// warpgroup opens once it has issued its own; barrier 4 + cw syncs warpgroup cw alone.
-__device__ __forceinline__ void turn_wait(int cw) { asm volatile("bar.sync %0, 256;" ::"r"(2 + cw) : "memory"); }
-__device__ __forceinline__ void turn_pass(int cw) { asm volatile("bar.arrive %0, 256;" ::"r"(3 - cw) : "memory"); }
-__device__ __forceinline__ void warpgroup_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(4 + cw) : "memory"); }
 
 // Splits the register file between the roles: true in the producer warpgroup, false in the two consumer warpgroups.
 __device__ __forceinline__ bool producer_warpgroup(int wg) {
@@ -497,20 +491,12 @@ struct RingPos {
       wrapped = true;
     }
   }
-  // k slots further on (the slots another consumer warpgroup takes)
-  __device__ __forceinline__ void skip(int k, int n) {
-    s += k;
-    const int q = s / n;
-    s -= q * n;
-    ph ^= (uint32_t)q & 1u;
-    wrapped = wrapped || q > 0;
-  }
 };
 
 // The W ring (g.nstages weight stages at sW) and the A ring (nabuf <= AMAX operand buffers from shared-memory offset
 // 0) and their mbarriers at bar0: W full / empty (HC_STAGES_MAX each), then A full / empty (AMAX each).  A full slot
-// takes thread 0's expect_tx (W) or every loader thread's arrival (A); an empty slot one arrival per warp of the
-// consumer warpgroups that read it (readers: 8 when both read every slot, 4 when each slot has one reader).
+// takes thread 0's expect_tx (W) or every loader thread's arrival (A); an empty slot one arrival per consumer warp (8:
+// both consumer warpgroups read every slot).
 template <int AMAX>
 struct Rings {
   static constexpr uint32_t BAR_BYTES = 8u * (2 * HC_STAGES_MAX + 2 * AMAX);
@@ -521,14 +507,14 @@ struct Rings {
   __device__ __forceinline__ uint32_t a_empty(int s) const { return bar0 + 8u * (2 * HC_STAGES_MAX + AMAX + s); }
 
   // thread 0, before the __syncthreads that precedes every use
-  __device__ __forceinline__ void init(int nstages, int nabuf, int readers = 8) const {
+  __device__ __forceinline__ void init(int nstages, int nabuf) const {
     for (int s = 0; s < nstages; ++s) {
       mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), readers);
+      mbar_init(w_empty(s), 8);
     }
     for (int s = 0; s < nabuf; ++s) {
       mbar_init(a_full(s), HB_LOADERS);
-      mbar_init(a_empty(s), readers);
+      mbar_init(a_empty(s), 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -771,16 +757,11 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
 // another 64 registers at N = 128 (ptxas spills) and is read after the MMAs by add_terms, as is the residual at N = 256.
 // Accumulation order (K chunk -> tap -> k16, conv1 then conv2) and epilogue association are those of the per-pair
 // arithmetic, so the tile shape does not enter any output element.
-// PING (N = 64, 128; launch_hconv): the ping-pong schedule.  Consumer warpgroup cw takes items cw, cw + 2, ... of the
-// CTA's stride, each as the whole R-row tile (2 mt_of(N) m64 tiles, 128 accumulators per thread), and the two
-// warpgroups' MMA phases alternate conv1(a), conv1(b), conv2(a), conv2(b), conv1(c), ... so that one warpgroup's
-// intermediate store and output epilogue run under the other's MMAs.  The producer streams the weight stages in that
-// phase order, each once per warpgroup tile; every ring slot has one reader, and each warpgroup steps its ring
-// positions over the other's slots.  Each warpgroup has its own intermediate tile; the epilogue reads residual and
-// branch sum after the MMAs (no registers left for the prefetch), under the other warpgroup's MMAs.
-template <int NW, int BF16, bool PING = false>
+// Both consumer warpgroups work on every tile, warpgroup cw on its mt_of(N) m64 row tiles from row 64 mt_of(N) cw, and
+// they meet at a named barrier on either side of the intermediate tile's store.
+template <int NW, int BF16>
 __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g) {
-  constexpr int MT = PING ? 2 * mt_of(NW) : mt_of(NW);
+  constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
   constexpr bool PREFETCH = MT * NACC <= 64;   // 64 accumulators leave room for 64 prefetched residuals
   constexpr int PM = PREFETCH ? MT : 1, PN = PREFETCH ? NACC : 1;
@@ -793,10 +774,10 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
   const int nwork = p.B * g.tiles;
   const int per_step = g.nkc * g.ntaps;
 
-  if (tid == 0) R.init(g.nstages, g.nabuf, PING ? 4 : 8);
+  if (tid == 0) R.init(g.nstages, g.nabuf);
   stage_biases(bias_s, p, 2, NW, tid, HB_THREADS);
-  // rows and channels of the intermediate tile(s) that store_frag_tile does not write stay zero for every tile
-  for (int i = tid; i < (PING ? 2 : 1) * g.nkc * 4 * g.rowsI; i += HB_THREADS)
+  // rows and channels of the intermediate that store_frag_tile does not write stay zero for every tile
+  for (int i = tid; i < g.nkc * 4 * g.rowsI; i += HB_THREADS)
     *reinterpret_cast<uint4*>(smem + g.off_i + (size_t)i * 16) = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
   __syncthreads();
@@ -805,16 +786,8 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
   if (producer_warpgroup(wg)) {
     RingPos r;
     if (tid == 0) {
-      if constexpr (PING) {
-        for (int w0 = blockIdx.x; w0 < nwork; w0 += 2 * gridDim.x) {
-          const int n = w0 + (int)gridDim.x < nwork ? 2 : 1;   // items of this round
-          for (int st = 0; st < 2; ++st)
-            for (int j = 0; j < n; ++j) R.stream_weights(p, g, r, st, 0, per_step);
-        }
-      } else {
-        for (int w = blockIdx.x; w < nwork; w += gridDim.x)
-          for (int st = 0; st < 2; ++st) R.stream_weights(p, g, r, st, 0, per_step);
-      }
+      for (int w = blockIdx.x; w < nwork; w += gridDim.x)
+        for (int st = 0; st < 2; ++st) R.stream_weights(p, g, r, st, 0, per_step);
     } else if (tid >= 32) {
       // A chunk kc of a tile: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
@@ -834,119 +807,65 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
   // (ntaps >= 2, or three buffers; one buffer is drained after every chunk).
   Batches<2, HP_ABUF_MAX> batches(R, g, g.nstages >= 3 && (g.ntaps >= 2 || g.nabuf != 2));
 
-  if constexpr (PING) {
-    uint8_t* itile = smem + g.off_i + (size_t)cw * g.nkc * 64 * g.rowsI;
-    for (int w0 = blockIdx.x; w0 < nwork; w0 += 2 * gridDim.x) {
-      const int n = w0 + (int)gridDim.x < nwork ? 2 : 1;   // items of this round
-      const bool last = w0 + 2 * (int)gridDim.x >= nwork;
-      // Every round has four turns, conv1 and conv2 of each warpgroup, so that the two barriers stay balanced: a
-      // warpgroup with no item in the last round still takes and passes its turns, and the last turn of the CTA
-      // (warpgroup 1's conv2 of the last round) opens none.
-      if (cw >= n) {
-        turn_wait(cw);
-        turn_pass(cw);
-        turn_wait(cw);
-        break;
-      }
-      const int w = w0 + cw * (int)gridDim.x, b = w / g.tiles, O = (w - b * g.tiles) * g.V;
-      // conv1 over the A chunks, after warpgroup 0's conv1 of this round (cw = 1) or warpgroup 1's conv2 of the previous
-      // round (cw = 0)
-      ar.skip(cw * g.nkc, g.nabuf);
-      batches.wr.skip(cw * per_step, g.nstages);
-      if (cw == 1 || w0 != (int)blockIdx.x) turn_wait(cw);
-      bool first = true;
-      for (int kc = 0; kc < g.nkc; ++kc) {
-        const int abuf = ar.s;
-        mbar_wait(R.a_full(abuf), ar.ph);
-        ar.next(g.nabuf);
-        batches.chunk<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, 0, g.ntaps, g.d, abuf, first);
-        if (g.nabuf == 1) batches.drain(acc);
-      }
-      turn_pass(cw);
-      batches.drain(acc);
-      ar.skip((n - 1 - cw) * g.nkc, g.nabuf);
-      // intermediate = lrelu(conv1 + b1, mid_slope) -> this warpgroup's operand tile
-      warpgroup_sync(cw);   // every warp has finished the previous tile's conv2, which read the tile
-      store_frag_tile<NW, BF16>(itile, acc, bias_s, Frag<MT>(0), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc, g.mid_slope);
-      fence_proxy_async();
-      warpgroup_sync(cw);
-      // conv2, after the other warpgroup's conv1 of this round
-      batches.wr.skip((n - 1) * per_step, g.nstages);
-      turn_wait(cw);
-      first = true;
-      for (int kc = 0; kc < g.nkc; ++kc)
-        batches.chunk<NW, BF16>(acc, smem_u32(itile) + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, 0, g.ntaps, 1, -1,
-                                first);
-      if (cw == 0 || !last) turn_pass(cw);
-      batches.drain(acc);
-      batches.wr.skip((n - 1 - cw) * per_step, g.nstages);
-      // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
-      const Frag<MT> f(0);
-      add_terms<NW>(acc, f, bias_s + NW, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
-      epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
-                                      [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
-    }
-  } else {
-    for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
-      const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
-      // residual of this thread's output elements, in flight under the MMAs
-      float xres[PM][PN];
-      if constexpr (PREFETCH) {
-        const Frag<MT> f(cw);
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = f.row(mt, h), t = O + row;
-            const bool ok = row < g.V && t < g.Tout;
-#pragma unroll
-            for (int c = 0; c < NW / 8; ++c)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int co = c * 8 + f.col + e;
-                const bool in = ok && co < p.Cout && p.residual;
-                xres[mt][c * 4 + 2 * h + e] = in ? __ldg(p.residual + ((int64_t)b * p.Cout + co) * g.Tout + t) : 0.f;
-              }
-          }
-      }
-      // conv1 over the A chunks
-      bool first = true;
-      for (int kc = 0; kc < g.nkc; ++kc) {
-        const int abuf = ar.s;
-        mbar_wait(R.a_full(abuf), ar.ph);
-        ar.next(g.nabuf);
-        batches.chunk<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64, g.ntaps, g.d, abuf, first);
-        if (g.nabuf == 1) batches.drain(acc);   // the loaders refill the only buffer with the next chunk
-      }
-      batches.drain(acc);
-      // intermediate = lrelu(conv1 + b1, mid_slope) -> operand tile, row 0 at time O - h2, zero outside [0, T)
-      consumer_sync();   // both warpgroups have finished the previous tile's conv2, which read the intermediate
-      store_frag_tile<NW, BF16>(smem + g.off_i, acc, bias_s, Frag<MT>(cw), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc,
-                                g.mid_slope);
-      fence_proxy_async();
-      consumer_sync();
-      first = true;
-      for (int kc = 0; kc < g.nkc; ++kc)
-        batches.chunk<NW, BF16>(acc, sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, cw * MT * 64, g.ntaps, 1, -1, first);
-      batches.drain(acc);
-      // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
+  for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+    const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
+    // residual of this thread's output elements, in flight under the MMAs
+    float xres[PM][PN];
+    if constexpr (PREFETCH) {
       const Frag<MT> f(cw);
-      const float* b2 = bias_s + NW;
-      if constexpr (PREFETCH) {
 #pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
+      for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-          for (int i = 0; i < NACC; ++i) {
-            acc[mt][i] += b2[(i >> 2) * 8 + f.col + (i & 1)];
-            if (p.residual) acc[mt][i] += xres[mt][i];
-          }
-        add_terms<NW>(acc, f, nullptr, nullptr, p.acc_prev, p, g, b, O, 0, g.V);
-      } else {
-        add_terms<NW>(acc, f, b2, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
-      }
-      epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
-                                      [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
+        for (int h = 0; h < 2; ++h) {
+          const int row = f.row(mt, h), t = O + row;
+          const bool ok = row < g.V && t < g.Tout;
+#pragma unroll
+          for (int c = 0; c < NW / 8; ++c)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int co = c * 8 + f.col + e;
+              const bool in = ok && co < p.Cout && p.residual;
+              xres[mt][c * 4 + 2 * h + e] = in ? __ldg(p.residual + ((int64_t)b * p.Cout + co) * g.Tout + t) : 0.f;
+            }
+        }
     }
+    // conv1 over the A chunks
+    bool first = true;
+    for (int kc = 0; kc < g.nkc; ++kc) {
+      const int abuf = ar.s;
+      mbar_wait(R.a_full(abuf), ar.ph);
+      ar.next(g.nabuf);
+      batches.chunk<NW, BF16>(acc, sA + (uint32_t)abuf * abytes, g.rowsA, cw * MT * 64, g.ntaps, g.d, abuf, first);
+      if (g.nabuf == 1) batches.drain(acc);   // the loaders refill the only buffer with the next chunk
+    }
+    batches.drain(acc);
+    // intermediate = lrelu(conv1 + b1, mid_slope) -> operand tile, row 0 at time O - h2, zero outside [0, T)
+    consumer_sync();   // both warpgroups have finished the previous tile's conv2, which read the intermediate
+    store_frag_tile<NW, BF16>(smem + g.off_i, acc, bias_s, Frag<MT>(cw), g.rowsI, 0, O - g.h2, g.Tin, 4 * g.nkc,
+                              g.mid_slope);
+    fence_proxy_async();
+    consumer_sync();
+    first = true;
+    for (int kc = 0; kc < g.nkc; ++kc)
+      batches.chunk<NW, BF16>(acc, sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, cw * MT * 64, g.ntaps, 1, -1, first);
+    batches.drain(acc);
+    // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
+    const Frag<MT> f(cw);
+    const float* b2 = bias_s + NW;
+    if constexpr (PREFETCH) {
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) {
+          acc[mt][i] += b2[(i >> 2) * 8 + f.col + (i & 1)];
+          if (p.residual) acc[mt][i] += xres[mt][i];
+        }
+      add_terms<NW>(acc, f, nullptr, nullptr, p.acc_prev, p, g, b, O, 0, g.V);
+    } else {
+      add_terms<NW>(acc, f, b2, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
+    }
+    epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
+                                    [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
   }
 }
 
@@ -1399,10 +1318,8 @@ bool layout_smem(HcGeom& g, uint32_t abytes, uint32_t ibytes, uint32_t nbias, ui
 // Launch geometry.  mode 2 (pair): C_in = C_out = C <= 256, conv1 dilation d_or_u, conv2 dilation 1.  mode 1: padding
 // pad (-1: (k - u) / 2), Tin * u outputs.  mode 3 (strided conv, stride d_or_u, padding pad): runs as mode 0 over the
 // polyphase operand, output row t reading operand rows t .. t + ceil(k / s) - 1, (Tin + 2 pad - k) / s + 1 outputs.  persistent: for hpair_kernel or hitem_kernel (one CTA per SM, as many A
-// chunk buffers as fit next to two W stages) rather than hconv_kernel.  pingpong: pair mode at N = 64 and 128 lays
-// out hpair_kernel's ping-pong schedule (two intermediate tiles) where it fits, else the cooperative one.
-int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool persistent, HcGeom& g, int pad = -1,
-              bool pingpong = false) {
+// chunk buffers as fit next to two W stages) rather than hconv_kernel.
+int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool persistent, HcGeom& g, int pad = -1) {
   HcLayer L;
   int rc = layer_geom(mode == 2 ? 0 : mode == 3 ? 2 : mode, cin, cout, k, d_or_u, L);
   if (rc != AB_OK) return rc;
@@ -1459,16 +1376,12 @@ int make_geom(int mode, int cin, int cout, int k, int d_or_u, int Tin, bool pers
   g.stage_bytes = 64u * (uint32_t)L.NW;
   const uint32_t abytes = (uint32_t)g.rowsA * 64u, nbias = (uint32_t)(g.nsteps * g.NB * L.NW);
   bool fits;
-  g.pingpong = mode == 2 && pingpong && (L.NW == 64 || L.NW == 128);
   if (persistent) {
     const uint32_t ibytes = (uint32_t)g.nkc * 64u * (uint32_t)g.rowsI;
-    for (;; g.pingpong = 0) {
-      g.nabuf = HP_ABUF_MAX;
-      while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, (g.pingpong ? 2u : 1u) * ibytes, nbias,
-                                  Rings<HP_ABUF_MAX>::BAR_BYTES, HC_SMEM_1CTA)) && g.nabuf > 1)
-        --g.nabuf;
-      if (fits || !g.pingpong) break;
-    }
+    g.nabuf = HP_ABUF_MAX;
+    while (!(fits = layout_smem(g, (uint32_t)g.nabuf * abytes, ibytes, nbias, Rings<HP_ABUF_MAX>::BAR_BYTES,
+                                HC_SMEM_1CTA)) && g.nabuf > 1)
+      --g.nabuf;
   } else {
     g.nabuf = 1;
     fits = layout_smem(g, abytes, 0, nbias, 16u * HC_STAGES_MAX, L.NW >= 256 ? HC_SMEM_1CTA : HC_SMEM_2CTA);
@@ -1580,22 +1493,10 @@ int launch_hconv(const HcArgs& a, const HcGeom& g, int precision, cudaStream_t s
     return launch_persistent("hitem_kernel", "tc conv-transpose", work * g.NB, g, precision, s, [](auto nw, auto bf16) {
       return hitem_kernel<decltype(nw)::value, decltype(bf16)::value, ITEM_CONVT>;
     }, a, g, PwArgs{});
-  if (g.mode == 2) {
-    // the ping-pong schedule (pair_schedule 1; slower than the cooperative one on an H100, DESIGN.md §6) where its
-    // geometry fits and some CTA walks two items: with one item per CTA the second consumer warpgroup would idle,
-    // while the cooperative schedule splits the tile between both
-    unsigned grid = 0;
-    const int rc = g.pingpong ? persistent_grid(work, "tc conv pair", grid) : AB_OK;
-    if (rc != AB_OK) return rc;
-    if (g.pingpong && work > (int64_t)grid)
-      return launch_persistent("hpair_kernel", "tc conv pair", work, g, precision, s, [](auto nw, auto bf16) {
-        constexpr int NW = decltype(nw)::value;
-        return hpair_kernel<NW, decltype(bf16)::value, NW == 64 || NW == 128>;
-      }, a, g);
+  if (g.mode == 2)
     return launch_persistent("hpair_kernel", "tc conv pair", work, g, precision, s, [](auto nw, auto bf16) {
       return hpair_kernel<decltype(nw)::value, decltype(bf16)::value>;
     }, a, g);
-  }
   if (work > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "tc conv: grid too large");
   return with_nw(g, precision, [&](auto nw, auto bf16) {
     constexpr int NW = decltype(nw)::value;
@@ -1709,8 +1610,7 @@ int launch_tc_conv(const TcConvParams& p, cudaStream_t s) {
   HcGeom g;
   // pairs and ConvTranspose layers from an operand image run on the persistent kernels (launch_hconv)
   const bool persistent = pair || (p.mode == 1 && p.ximg);
-  int rc = make_geom(pair ? 2 : p.mode == 2 ? 3 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, persistent, g, p.pad,
-                     p.pair_schedule != 0);
+  int rc = make_geom(pair ? 2 : p.mode == 2 ? 3 : p.mode, p.Cin, p.Cout, p.k, p.d_or_u, p.T, persistent, g, p.pad);
   if (rc != AB_OK) return rc;
   if (p.reflect && g.a0 >= p.T)
     return fail(AB_ERR_ARG, "tc conv: reflection padding %d needs more than %d samples", g.a0, p.T);

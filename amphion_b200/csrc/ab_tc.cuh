@@ -37,7 +37,6 @@ struct TcConvParams {
   int reflect = 0;                   // conv only, no w2: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN)
   int pad = -1;                      // conv-transpose padding, 0 <= pad < k; -1 = (k-u)/2 (HiFi-GAN; MelGAN: u//2 + u%2);
                                      // strided conv: zero padding on both sides, 0 <= pad < k
-  int pair_schedule = 0;             // pair mode: 0 cooperative, 1 ping-pong where served (N = 64, 128); bit-equal outputs
 };
 // 16-bit weight image of a layer, 0 when launch_tc_conv cannot run it
 size_t tc_weight_image_bytes(int mode, int cin, int cout, int k, int d_or_u);

@@ -242,10 +242,6 @@ int ab_generator_set_profiling(ab_generator* g, int32_t enable);
  *   whole ResBlock per launch (residual stream in registers, halo recomputed in the tile) where served (C <= 128) and
  *   the recompute is small, else per pair; 3, 4 = a whole ResBlock per launch wherever served.  All plans run the same
  *   arithmetic in the same order: their outputs are bit-equal.
- *   "pair_schedule": how a per-pair launch at 64 and 128 channels (N block 64 or 128) shares its CTA's two consumer
- *   warpgroups: 0 (default) = both on one time tile; 1 = ping-pong, each on its own tile with their MMA phases
- *   alternating, where shared memory allows it and the launch has more tiles than SMs (slower on H100 today, see
- *   DESIGN.md §6).  Outputs are bit-equal.
  *   "nsf_source_frames" (NSF-HiFiGAN, one-shot, consumed by the next forward): frames of the f0 track when it does
  *   not cover the mel; every stage is then truncated to the harmonic source's length as the reference does
  *   (nsfhifigan.py:264-268) and the output holds ab_generator_output_samples() samples per utterance.
@@ -299,8 +295,8 @@ int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t c
                       int64_t frames, int32_t use_residual, float* dev_out, void* stream);
 /* x [B, in_channels, T] fp32 with any element strides, spk [B, in_channels] fp32 with row stride spk_row_stride ->
  * wav [B, 1, T * prod(up_ratios)].  Workspace: ab_generator_workspace_bytes.  Tail events (ab_generator_set_tail_events)
- * split conv_post into batch chunks as for the other generators.  set_option's "resblock_fusion" and "pair_schedule"
- * are accepted and change nothing: every FACodec conv runs as a single conv. */
+ * split conv_post into batch chunks as for the other generators.  set_option's "resblock_fusion" is accepted and
+ * changes nothing: every FACodec conv runs as a single conv. */
 int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t batch, int64_t frames, const int64_t x_strides[3],
                          const float* dev_spk, int64_t spk_row_stride, float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream);

@@ -4,7 +4,6 @@ trace with CUDA activities.
 
     python scripts/profile_stages.py [--batch 64] [--frames 1024] [--fusion 2] [--out DIR]
     python scripts/profile_stages.py --time-fusions 0,2,3      # ms per step of each resblock_fusion, profiler off
-    python scripts/profile_stages.py --time-schedules 0,1      # per-stage table of each pair_schedule, then ms per step
 
 The tensor-core launches of `forward_impl` come in a fixed order: conv_pre, then per stage one ConvTranspose and per
 ResBlock either one block-mode launch (`hchain_kernel`) or one `hpair_kernel` launch per dilation pair; conv_pre runs
@@ -62,8 +61,6 @@ def main():
     ap.add_argument("--out", default="", help="directory for the JSON table (and nothing else)")
     ap.add_argument("--time-fusions", default="", metavar="M,M,...",
                     help="instead of profiling, time these resblock_fusion settings alternately")
-    ap.add_argument("--time-schedules", default="", metavar="S,S,...",
-                    help="profile one step at each of these pair_schedule settings, then time them alternately")
     args = ap.parse_args()
 
     import torch
@@ -100,17 +97,10 @@ def main():
     if args.time_fusions:
         time_alternately("resblock_fusion", [int(m) for m in args.time_fusions.split(",")])
         return
-    if args.time_schedules:
-        schedules = [int(s) for s in args.time_schedules.split(",")]
-        for s in schedules:
-            model.set_option("pair_schedule", s)
-            profile_step(model, mel, args, w, f"pair_schedule {s}", f"_schedule{s}")
-        time_alternately("pair_schedule", schedules)
-        return
-    profile_step(model, mel, args, w, "", "")
+    profile_step(model, mel, args, w)
 
 
-def profile_step(model, mel, args, w, label, suffix):
+def profile_step(model, mel, args, w):
     """One profiled step after args.warmup warm-ups: prints the per-row and per-stage tables, and writes them to
     args.out when given."""
     import torch
@@ -159,9 +149,8 @@ def profile_step(model, mel, args, w, label, suffix):
         raise SystemExit(f"launch walk matched {pos} of {len(hc)} tensor-core launches: plan and trace disagree")
 
     props = torch.cuda.get_device_properties(dev)
-    print(f"# {props.name}, HiFi-GAN V1 B={B} 80x{T} {args.precision}, resblock_fusion {args.fusion}"
-          f"{', ' + label if label else ''}: step {step_us / 1e3:.1f} ms (first kernel start to last kernel end, "
-          f"profiler on)")
+    print(f"# {props.name}, HiFi-GAN V1 B={B} 80x{T} {args.precision}, resblock_fusion {args.fusion}: "
+          f"step {step_us / 1e3:.1f} ms (first kernel start to last kernel end, profiler on)")
     print(f"{'stage':<9} {'plan':<13} {'n':>3} {'ms':>8} {'share':>6} {'TFLOP/s':>8} {'GB/s':>7}")
     out = []
     by_stage = OrderedDict()
@@ -180,7 +169,7 @@ def profile_step(model, mel, args, w, label, suffix):
         print(f"{stage:<9} {us / 1e3:>8.2f} ms {us / step_us:>6.1%} {fl / us / 1e6:>8.1f} TFLOP/s {nb / us / 1e3:>7.0f} GB/s")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, f"profile_fusion{args.fusion}{suffix}.json"), "w") as f:
+        with open(os.path.join(args.out, f"profile_fusion{args.fusion}.json"), "w") as f:
             json.dump(dict(gpu=props.name, batch=B, frames=T, fusion=args.fusion, step_ms=step_us / 1e3,
                            other_ms=other_us / 1e3, rows=out), f, indent=1)
 

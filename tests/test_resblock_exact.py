@@ -6,10 +6,10 @@ bias, the stage sees the test's fp32 input exactly and the handle returns lrelu(
 ResBlock convs are plain tensors (no weight-norm fold), so the only rounding is the tensor path's own.
 
 * One-hot weights (output channel co reads input channel perm(co) at tap tap(co), scale +-2^e): every accumulator
-  holds one exact product, so the whole stage is deterministic and every route — pairs (`resblock_fusion` 1,
-  cooperative and ping-pong `pair_schedule`), block mode (2, 3) and the single-conv route (C = 320, k = 33) — must
-  equal the oracle bit for bit.  That pins tap shifts and dilations, halos, ragged tiles, K-chunk / N-block mapping,
-  padded channels, zeroing outside [0, T), bias placement, epilogue association, RN rounding and saturation.
+  holds one exact product, so the whole stage is deterministic and every route — pairs (`resblock_fusion` 1), block
+  mode (2, 3) and the single-conv route (C = 320, k = 33) — must equal the oracle bit for bit.  That pins tap shifts
+  and dilations, halos, ragged tiles, K-chunk / N-block mapping, padded channels, zeroing outside [0, T), bias
+  placement, epilogue association, RN rounding and saturation.
 * Dense weights: the kernels' distance from the float64-accumulation oracle against the floor, the distance from it
   of the oracle with the H100 MMA's truncating fp32 accumulation ("mma" in resblock_oracle.py; IEEE float32 sits
   3-15x closer to the exact sum than the tensor cores do, so it would understate the floor).  This covers
@@ -28,7 +28,7 @@ import resblock_oracle as ro
 
 DEV = "cuda:0"
 PRECS = {"tc_f16": "f16", "tc_bf16": "bf16"}
-ROUTES = [(1, 0), (1, 1), (2, 0), (2, 1), (3, 0), (3, 1)]   # (resblock_fusion, pair_schedule)
+ROUTES = (1, 2, 3)   # resblock_fusion
 # floor rule: the kernel's distance from the float64 oracle within these multiples of the floor's mean and maximum
 FLOOR_MEAN, FLOOR_MAX = 2.0, 3.0
 
@@ -109,12 +109,11 @@ def _stage_class():
         def buffers(self, *a, **k):
             return iter(())
 
-        def run(self, x, prec, fusion, schedule):
+        def run(self, x, prec, fusion):
             """x [B, C, T] -> (lrelu(stage(x), 0.01) [B, C, T] on the host, launches)"""
             import ctypes as C
             self.precision = prec
             self.set_option("resblock_fusion", fusion)
-            self.set_option("pair_schedule", schedule)
             x = torch.from_numpy(x).to(DEV)
             B, _, T = x.shape
             with torch.cuda.device(x.device):
@@ -221,18 +220,34 @@ def test_unrounded_oracle_matches_the_generator_oracle(resblock):
     assert np.abs(got - want).max() <= 1e-5 * max(np.abs(want).max(), 1e-3)
 
 
+def test_plan_options():
+    """set_option takes `resblock_fusion` 0..4 and no pair-schedule key."""
+    from amphion_b200 import _capi
+    from helpers import build_model
+    hp = dict(resblock="1", upsample_rates=[2, 2], upsample_kernel_sizes=[4, 4], upsample_initial_channel=64,
+              resblock_kernel_sizes=[3], resblock_dilation_sizes=[[1]])
+    h = build_model("hifigan", hp, 20, seed=1)._ensure_handle()
+    assert _capi.lib.ab_generator_set_option(h, b"pair_schedule", 0) == -1
+    assert "pair_schedule" in _capi.last_error()
+    for v in range(5):
+        assert _capi.lib.ab_generator_set_option(h, b"resblock_fusion", v) == 0
+    for v in (-1, 5):
+        assert _capi.lib.ab_generator_set_option(h, b"resblock_fusion", v) == -1
+        assert "resblock_fusion" in _capi.last_error()
+
+
 # ------------------------------------------------------------------------------------------------ GPU: one-hot, exact
 # (id, C, [(k, dilations)], B, T, values)
 ONE_HOT = [
     ("c16-T1", 16, [(3, (1, 3, 5))], 2, 1, "ordinary"),
     ("c48-padded-below-halo", 48, [(7, (1, 3, 5)), (3, (1, 3, 5))], 2, 30, "ordinary"),
     ("c64-ragged", 64, [(3, (1, 3, 5)), (7, (1, 3, 5)), (11, (1, 3, 5))], 2, 700, "ordinary"),
-    # more than 2 x 132 items with a partial last stride: ping-pong at 64 channels, block mode's walk
+    # more than 2 x 132 items with a partial last stride: the persistent walks of the pair and block-mode kernels
     ("c64-walk", 64, [(3, (1, 3, 5)), (11, (1, 3, 5))], 6, 6000, "ordinary"),
     ("c96-k13-k1", 96, [(13, (1, 3, 5)), (1, (1, 3, 5))], 2, 300, "ordinary"),
     ("c128-walk", 128, [(3, (1, 3, 5)), (7, (1, 3, 5)), (11, (1, 3, 5))], 7, 5000, "ordinary"),
-    # k = 31 at dilation 70: two intermediate tiles do not fit, ping-pong falls back to the cooperative schedule
-    ("c128-pingpong-fallback", 128, [(31, (70, 1)), (3, (1, 3))], 20, 800, "ordinary"),
+    # k = 31 at dilation 70, tap reach 2100: one A chunk buffer and two W stages next to the intermediate tile
+    ("c128-k31-d70", 128, [(31, (70, 1)), (3, (1, 3))], 20, 800, "ordinary"),
     ("c200-partial-chunk", 200, [(7, (1, 4)), (31, (5, 1))], 2, 333, "ordinary"),
     ("c256", 256, [(3, (1, 3, 5)), (11, (1, 3, 5))], 3, 600, "ordinary"),
     ("c256-k31-d26", 256, [(31, (26, 1))], 2, 240, "ordinary"),   # tap reach 780: one A chunk buffer
@@ -252,7 +267,7 @@ VALUES = {   # input scale, weight exponents, bias std
 @pytest.mark.gpu
 @pytest.mark.parametrize("prec", list(PRECS))
 @pytest.mark.parametrize("case", ONE_HOT, ids=[c[0] for c in ONE_HOT])
-def test_one_hot_stage_is_exact(case, prec):
+def test_one_hot_stage_is_exact_on_every_route(case, prec):
     _, C, shape, B, T, values = case
     scale, exps, bias_std = VALUES[values]
     rng = np.random.default_rng(C * 1000 + T)
@@ -261,11 +276,11 @@ def test_one_hot_stage_is_exact(case, prec):
     want = _post(ro.stage(x, blocks, PRECS[prec]))
     assert np.isfinite(want).all()
     stage = _make_stage(C, blocks)
-    for fusion, schedule in ROUTES:
-        got, launches = stage.run(x, prec, fusion, schedule)
+    for fusion in ROUTES:
+        got, launches = stage.run(x, prec, fusion)
         assert launches == _launches(C, shape, fusion), (fusion, launches)
         bad = got != want
-        assert not bad.any(), (f"fusion {fusion} schedule {schedule}: {int(bad.sum())} of {bad.size} differ, first at "
+        assert not bad.any(), (f"fusion {fusion}: {int(bad.sum())} of {bad.size} differ, first at "
                                f"{np.argwhere(bad)[0].tolist()}: {got[bad][0]!r} vs {want[bad][0]!r}")
 
 
@@ -289,17 +304,17 @@ def _floor_check(what, got, o64, o32):
 @pytest.mark.gpu
 @pytest.mark.parametrize("prec", list(PRECS))
 @pytest.mark.parametrize("case", DENSE, ids=[c[0] for c in DENSE])
-def test_dense_stage_within_the_floor(case, prec):
+def test_dense_stage_within_the_floor_on_every_route(case, prec):
     _, C, shape, B, T = case
     rng = np.random.default_rng(C + T)
     blocks = _blocks(rng, C, shape, "dense", bias_std=0.1)
     x = rng.normal(0, 1, (B, C, T)).astype(np.float32)
     o64, o32 = (_post(ro.stage(x, blocks, PRECS[prec], acc)) for acc in ("f64", "mma"))
     stage = _make_stage(C, blocks)
-    for fusion, schedule in ROUTES:
-        got, launches = stage.run(x, prec, fusion, schedule)
+    for fusion in ROUTES:
+        got, launches = stage.run(x, prec, fusion)
         assert launches == _launches(C, shape, fusion)
-        _floor_check(f"{case[0]} {prec} fusion {fusion} schedule {schedule}", got, o64, o32)
+        _floor_check(f"{case[0]} {prec} fusion {fusion}", got, o64, o32)
 
 
 # ------------------------------------------------------------------------------------------------ GPU: generators
