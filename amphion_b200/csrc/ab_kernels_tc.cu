@@ -259,23 +259,22 @@ __device__ __forceinline__ void epilogue_out(const HcArgs& p, const HcGeom& g, c
 // The additive terms of epilogue_out folded into the accumulators first, in its association:
 //   acc = ((acc [+ bias]) [+ residual]) [+ acc_prev]     (each term when its pointer is non-null)
 // on the valid fragment rows [r0, r1) at time t0 + row (pair mode: [0, V) at O + row; block mode: [H, H + V) at
-// O - H + row).  The loads of both terms go out G fragment columns at a time, so that a group waits for one HBM round
-// trip: read inside epilogue_out, between its fp32 stores (which may alias acc_prev), every element would wait for its
-// own.  epilogue_out then runs without EP_RESIDUAL / EP_ACC_PREV on the accumulators.
+// O - H + row) and output channels co0 + column.  The loads of both terms go out G fragment columns at a time, so that
+// a group waits for one HBM round trip: read inside epilogue_out, between its fp32 stores (which may alias acc_prev),
+// every element would wait for its own.  epilogue_out then runs without EP_RESIDUAL / EP_ACC_PREV on the accumulators.
 template <int NW, int MT>
 __device__ __forceinline__ void add_terms(float (&acc)[MT][NW / 2], const Frag<MT>& f, const float* bias,
                                           const float* residual, const float* acc_prev, const HcArgs& p,
-                                          const HcGeom& g, int b, int t0, int r0, int r1) {
-  // columns per group: 8 below 128 accumulators per thread; 2 at 128, where ptxas (168 registers) spills more
-  constexpr int G = MT * NW / 2 > 64 ? 2 : (NW / 8 < 8 ? NW / 8 : 8);
+                                          const HcGeom& g, int b, int t0, int r0, int r1, int co0) {
+  static_assert(MT * NW / 2 <= 64, "add_terms: 64 accumulators per thread at most");
+  constexpr int G = NW / 8 < 8 ? NW / 8 : 8;   // columns per group
 #pragma unroll
   for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = f.row(mt, h), t = t0 + row;
-      // one comparison for the row window: a second one makes ptxas spill more at N = 256
       const bool ok = (unsigned)(row - r0) < (unsigned)(r1 - r0) && t < g.Tout;
-      const int64_t base = ((int64_t)b * p.Cout + f.col) * g.Tout + t;   // element of column f.col
+      const int64_t base = ((int64_t)b * p.Cout + co0 + f.col) * g.Tout + t;   // element of column f.col
 #pragma unroll
       for (int c0 = 0; c0 < NW / 8; c0 += G) {
         float r[G][2], a[G][2];
@@ -283,7 +282,7 @@ __device__ __forceinline__ void add_terms(float (&acc)[MT][NW / 2], const Frag<M
         for (int c = 0; c < G; ++c)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int co = (c0 + c) * 8 + f.col + e;
+            const int co = co0 + (c0 + c) * 8 + f.col + e;
             const bool in = ok && co < p.Cout;
             const int64_t idx = base + (int64_t)((c0 + c) * 8 + e) * g.Tout;
             r[c][e] = in && residual ? __ldg(residual + idx) : 0.f;
@@ -529,6 +528,27 @@ struct Rings {
     }
   }
 
+  // thread 0: columns [HW n, HW n + HW) of stages [0, nst) of conv st's weight image (HW = half its width) into the
+  // next W slots, one copy per c8 plane, so that a half stage is the [4 c8][HW rows][8] stage of an N = HW wgmma.  Two
+  // consecutive half stages share a slot (the last one alone when nst is odd), so the ring holds as many bytes and as
+  // much MMA work ahead of the consumers as with whole stages.
+  template <int HW>
+  __device__ __forceinline__ void stream_weight_half(const HcArgs& p, const HcGeom& g, RingPos& r, int st, int n,
+                                                     int nst) const {
+    const uint32_t plane = g.stage_bytes / 4u, hbytes = HW * 16u;   // a c8 plane of the image's stage; HW of its rows
+    for (int i = 0; i < nst; i += 2, r.next(g.nstages)) {
+      const int m = min(2, nst - i);
+      if (r.wrapped) mbar_wait(w_empty(r.s), r.ph ^ 1u);
+      mbar_arrive_expect_tx(w_full(r.s), (uint32_t)m * 4u * hbytes);
+      for (int j = 0; j < m; ++j) {
+        const uint8_t* src = weight_stage(p, g, st, i + j) + n * hbytes;
+        const uint32_t dst = sW + (uint32_t)r.s * g.stage_bytes + (uint32_t)j * 4u * hbytes;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) bulk_g2s(dst + c * hbytes, src + c * plane, hbytes, w_full(r.s));
+      }
+    }
+  }
+
   // loader warps (producer threads 32-127): one work item's A operand into the next nchunks A buffers, chunk kc holding
   // c8 planes [planes kc, planes (kc + 1)) x `rows` rows at times t0 + row of utterance b
   template <int BF16>
@@ -551,6 +571,14 @@ __device__ __forceinline__ void fence_acc(float (&acc)[MT][NACC]) {
   for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
     for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(acc[mt][i])::"memory");
+}
+
+template <int MT, int NACC>
+__device__ __forceinline__ void zero_acc(float (&acc)[MT][NACC]) {
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[mt][i] = 0.f;
 }
 
 // Consumer side of the rings: one wgmma batch per weight stage, in stream order.  After each batch is issued, at most D
@@ -581,16 +609,18 @@ struct Batches {
   }
 
   // acc (+)= the next weight stage x the operand at aBase (aRows rows per c8 plane) from row row0; the batch holds A
-  // buffer abuf (-1: none)
+  // buffer abuf (-1: none).  A slot may hold several stages (Rings::stream_weight_half): the stage at byte wofs of the
+  // current slot, whose full barrier the batch at wofs = 0 waits for; the batch with slot_end moves to the next slot
+  // and holds this one, so that it is released when the slot's last batch has completed.
   template <int NW, int BF16, int MT>
   __device__ __forceinline__ void mma(float (&acc)[MT][NW / 2], uint32_t aBase, int aRows, int row0, int abuf,
-                                      bool& first) {
+                                      bool& first, uint32_t wofs = 0, bool slot_end = true) {
     const int s = wr.s;
-    mbar_wait(R.w_full(s), wr.ph);
-    wr.next(g.nstages);
+    if (wofs == 0) mbar_wait(R.w_full(s), wr.ph);
+    if (slot_end) wr.next(g.nstages);
     fence_acc(acc);
     wg_fence();
-    mma_batch<NW, BF16>(acc, aBase, aRows, row0, R.sW + (uint32_t)s * g.stage_bytes, first);
+    mma_batch<NW, BF16>(acc, aBase, aRows, row0, R.sW + (uint32_t)s * g.stage_bytes + wofs, first);
     wg_commit();
     if constexpr (D == 2) {
       if (deep) {
@@ -604,18 +634,18 @@ struct Batches {
         fence_acc(acc);
         release(w[1], a[1]);
       }
-      w[1] = s;
+      w[1] = slot_end ? s : -1;
       a[1] = abuf;
     } else if (deep) {
       wg_wait<1>();   // the previous batch has completed
       fence_acc(acc);
       release(w[0], a[0]);
-      w[0] = s;
+      w[0] = slot_end ? s : -1;
       a[0] = abuf;
     } else {
       wg_wait<0>();
       fence_acc(acc);
-      release(s, abuf);
+      release(slot_end ? s : -1, abuf);
     }
     first = false;
   }
@@ -743,7 +773,7 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
     // every MMA of this tile has completed: the producer may load the next X
     batches.release(-1, 0);
     // y = (x_L + acc_prev) * out_scale on the valid rows [H, H + V); acc_prev (which may alias y) is read in batches
-    add_terms<NW>(xr, f, nullptr, nullptr, p.acc_prev, p, g, b, O - g.H, g.H, g.H + g.V);
+    add_terms<NW>(xr, f, nullptr, nullptr, p.acc_prev, p, g, b, O - g.H, g.H, g.H + g.V, 0);
     epilogue_out<NW, BF16, 0>(p, g, f, b, O - g.H, g.H, g.H + g.V, 0,
                               [&](int mt, int c, int h, int e) { return xr[mt][c * 4 + 2 * h + e]; });
   }
@@ -752,19 +782,25 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hchain_kernel(HcArgs p, HcGeom 
 // Pair mode (launch_tc_conv with a second conv; one ResBlock1 step): the work items are (utterance, time tile), with
 // the per-pair tile geometry of make_geom (output row r at time O + r, V = R - (k - 1)).  The loaders stream the A
 // operand in 32-channel K chunks through g.nabuf buffers; conv2 reads only the intermediate tile, so the next tile's
-// chunks load under this tile's conv2 and output epilogue.  Below N = 256 each consumer loads the residual of its
-// fragment into registers at the start of the tile, so that HBM read runs under the MMAs; the branch sum would need
-// another 64 registers at N = 128 (ptxas spills) and is read after the MMAs by add_terms, as is the residual at N = 256.
+// chunks load under this tile's conv2 and output epilogue.
+// conv2 runs in NH column halves of HW columns, one after the other: one half below N = 256, two of 128 at N = 256
+// (C in (128, 256], so both hold output channels).  Each half holds at most 64 accumulators per thread, which leaves
+// room for the residual of its fragment: each consumer loads it into registers before the half's MMAs (below N = 256
+// at the start of the tile), so that HBM read runs under them.  The branch sum would need another 64 registers (ptxas
+// spills) and is read after the MMAs by add_terms.  At N = 256 conv1 keeps its 128 accumulators, which are dead once
+// the intermediate tile is stored, and a half's wgmmas are m64n128k16 on weight stages of the half's columns only
+// (Rings::stream_weight_half).  Two of those 8 KB stages share a 16 KB slot of the W ring, so the ring, its layout and
+// the bytes and MMA work it holds ahead of the consumers stay those of conv1 and of the other kernels.
 // Accumulation order (K chunk -> tap -> k16, conv1 then conv2) and epilogue association are those of the per-pair
-// arithmetic, so the tile shape does not enter any output element.
+// arithmetic, so neither the tile shape nor the column halves enter any output element.
 // Both consumer warpgroups work on every tile, warpgroup cw on its mt_of(N) m64 row tiles from row 64 mt_of(N) cw, and
 // they meet at a named barrier on either side of the intermediate tile's store.
 template <int NW, int BF16>
 __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g) {
   constexpr int MT = mt_of(NW);
   constexpr int NACC = NW / 2;
-  constexpr bool PREFETCH = MT * NACC <= 64;   // 64 accumulators leave room for 64 prefetched residuals
-  constexpr int PM = PREFETCH ? MT : 1, PN = PREFETCH ? NACC : 1;
+  constexpr int NH = NW > 128 ? 2 : 1, HW = NW / NH;   // conv2's column halves and their width
+  static_assert(MT * HW / 2 <= 64, "a conv2 half leaves room for its prefetched residual");
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, wg = tid >> 7;
   const uint32_t sA = smem_u32(smem), sI = sA + g.off_i;
@@ -787,7 +823,11 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
     RingPos r;
     if (tid == 0) {
       for (int w = blockIdx.x; w < nwork; w += gridDim.x)
-        for (int st = 0; st < 2; ++st) R.stream_weights(p, g, r, st, 0, per_step);
+        for (int st = 0; st < 2; ++st) {
+          if (NH == 1 || st == 0) R.stream_weights(p, g, r, st, 0, per_step);
+          else
+            for (int n = 0; n < NH; ++n) R.stream_weight_half<HW>(p, g, r, st, n, per_step);
+        }
     } else if (tid >= 32) {
       // A chunk kc of a tile: rows [0, rowsA) at times O - a0 + row, channels [32 kc, 32 kc + 32)
       for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
@@ -800,7 +840,6 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
 
   // ------------------------------------------------------------------------------------------------ consumers
   const int cw = wg - 1;
-  float acc[MT][NACC];
   RingPos ar;   // A buffer of the next chunk
   // Two batches stay in flight when the rings allow it: every W slot held by an in-flight batch must leave one to fill
   // (nstages >= 3), and the loaders must not need the buffer of the last tap of the chunk before the previous one
@@ -809,9 +848,14 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
 
   for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
     const int b = w / g.tiles, O = (w - b * g.tiles) * g.V;
-    // residual of this thread's output elements, in flight under the MMAs
-    float xres[PM][PN];
-    if constexpr (PREFETCH) {
+    // conv1's and each conv2 half's accumulators start at zero, although their first batch does not read them: the
+    // wgmma operands are read-write, so without a value here ptxas keeps the registers live from the kernel's entry,
+    // next to the other array
+    float acc[MT][NACC];
+    zero_acc(acc);
+    // residual of this thread's output elements in conv2's half n, in flight under the MMAs that follow
+    float xres[MT][HW / 2];
+    auto prefetch_residual = [&](int n) {
       const Frag<MT> f(cw);
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt)
@@ -820,15 +864,16 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
           const int row = f.row(mt, h), t = O + row;
           const bool ok = row < g.V && t < g.Tout;
 #pragma unroll
-          for (int c = 0; c < NW / 8; ++c)
+          for (int c = 0; c < HW / 8; ++c)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const int co = c * 8 + f.col + e;
+              const int co = n * HW + c * 8 + f.col + e;
               const bool in = ok && co < p.Cout && p.residual;
               xres[mt][c * 4 + 2 * h + e] = in ? __ldg(p.residual + ((int64_t)b * p.Cout + co) * g.Tout + t) : 0.f;
             }
         }
-    }
+    };
+    if constexpr (NH == 1) prefetch_residual(0);
     // conv1 over the A chunks
     bool first = true;
     for (int kc = 0; kc < g.nkc; ++kc) {
@@ -845,27 +890,34 @@ __global__ void __launch_bounds__(HB_THREADS, 1) hpair_kernel(HcArgs p, HcGeom g
                               g.mid_slope);
     fence_proxy_async();
     consumer_sync();
-    first = true;
-    for (int kc = 0; kc < g.nkc; ++kc)
-      batches.chunk<NW, BF16>(acc, sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, cw * MT * 64, g.ntaps, 1, -1, first);
-    batches.drain(acc);
-    // y = ((acc + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
-    const Frag<MT> f(cw);
-    const float* b2 = bias_s + NW;
-    if constexpr (PREFETCH) {
+    // conv2, columns [HW n, HW n + HW) at a time
+    for (int n = 0; n < NH; ++n) {
+      if constexpr (NH > 1) prefetch_residual(n);
+      float acc2[MT][HW / 2];
+      zero_acc(acc2);
+      first = true;
+      // stage i = kc ntaps + tap; two half stages per W slot (Rings::stream_weight_half)
+      for (int kc = 0; kc < g.nkc; ++kc)
+        for (int j = 0; j < g.ntaps; ++j) {
+          const int i = kc * g.ntaps + j, sub = NH > 1 ? i & 1 : 0;
+          batches.mma<HW, BF16>(acc2, sI + (uint32_t)(kc * 4 * g.rowsI) * 16u, g.rowsI, cw * MT * 64 + j, -1, first,
+                                (uint32_t)sub * HW * 64u, NH == 1 || sub == 1 || i == per_step - 1);
+        }
+      batches.drain(acc2);
+      // y = ((acc2 + b2) + residual) + acc_prev) * out_scale [tanh] on the valid rows [0, V)
+      const Frag<MT> f(cw);
+      const float* b2 = bias_s + NW + n * HW;
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-        for (int i = 0; i < NACC; ++i) {
-          acc[mt][i] += b2[(i >> 2) * 8 + f.col + (i & 1)];
-          if (p.residual) acc[mt][i] += xres[mt][i];
+        for (int i = 0; i < HW / 2; ++i) {
+          acc2[mt][i] += b2[(i >> 2) * 8 + f.col + (i & 1)];
+          if (p.residual) acc2[mt][i] += xres[mt][i];
         }
-      add_terms<NW>(acc, f, nullptr, nullptr, p.acc_prev, p, g, b, O, 0, g.V);
-    } else {
-      add_terms<NW>(acc, f, b2, p.residual, p.acc_prev, p, g, b, O, 0, g.V);
+      add_terms<HW>(acc2, f, nullptr, nullptr, p.acc_prev, p, g, b, O, 0, g.V, n * HW);
+      epilogue_out<HW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, n * HW,
+                                      [&](int mt, int c, int h, int e) { return acc2[mt][c * 4 + 2 * h + e]; });
     }
-    epilogue_out<NW, BF16, EP_TANH>(p, g, f, b, O, 0, g.V, 0,
-                                    [&](int mt, int c, int h, int e) { return acc[mt][c * 4 + 2 * h + e]; });
   }
 }
 
