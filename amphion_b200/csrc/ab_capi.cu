@@ -125,10 +125,19 @@ struct FacodecLayerRef {
   int cb = -1;
   ConvRef out_proj;
   int64_t rows = 0;
+  ConvRef in_proj;          // facodec_quantize only
+  size_t cbn_offset = 0;    // facodec_quantize: arena offset of the normalised rows [rows][16], then their squared norms
+};
+struct TimbreLayerRef {     // one TransformerEncoderLayer (transformer.py:84-151), use_cln = False
+  int ln1_w = -1, ln1_b = -1, ln2_w = -1, ln2_b = -1;
+  ConvRef qkv, out_proj, ffn_1, ffn_2;
 };
 struct FacodecRef {
   int style_w = -1, style_b = -1;
   std::vector<FacodecLayerRef> layers;
+  // facodec_quantize: the timbre encoder (transformer.py:154-217)
+  int pe = -1, last_w = -1, last_b = -1;
+  std::vector<TimbreLayerRef> timbre;
 };
 
 }  // namespace
@@ -301,6 +310,12 @@ int validate_facodec_config(const ab_generator_config& c) {
   if (c.vq_codebook_dim <= 0 || c.vq_codebook_dim > FAC_MAX_CODEBOOK_DIM || c.vq_codebook_dim == c.n_mel)
     return fail(AB_ERR_UNSUPPORTED, "config: FACodec codebook_dim %d (1..%d, != vq_dim: out_proj must be a Linear)",
                 c.vq_codebook_dim, FAC_MAX_CODEBOOK_DIM);
+  if (c.facodec_quantize != 0 && c.facodec_quantize != 1)
+    return fail(AB_ERR_ARG, "config: facodec_quantize must be 0 or 1 (got %d)", c.facodec_quantize);
+  // the timbre encoder is always 256 wide (facodec.py:363) and reads x directly
+  if (c.facodec_quantize && c.n_mel != FAC_TIMBRE_C)
+    return fail(AB_ERR_UNSUPPORTED, "config: FACodec quantization needs in_channels == %d (the timbre encoder's width; "
+                "got %d)", FAC_TIMBRE_C, c.n_mel);
   return AB_OK;
 }
 
@@ -338,6 +353,7 @@ int validate_config(const ab_generator_config& c) {
       c.kind != AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
+  if (c.facodec_quantize) return fail(AB_ERR_ARG, "config: facodec_quantize belongs to AB_GEN_FACODEC");
   for (int i = 0; i < 3; ++i)
     if (c.vq_num_q[i] || c.vq_codebook_bits[i]) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
   if (c.vq_codebook_dim) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
@@ -569,6 +585,36 @@ void add_facodec_tensors(ab_generator* g) {
       g->slots[l.out_proj.w].no_tc = true;
       f.layers.push_back(l);
     }
+  if (!cfg->facodec_quantize) return;
+  // FACodecDecoder.forward(vq=True): the quantizers' in_proj (read by the RVQ kernel) and the timbre encoder
+  size_t li = 0;
+  for (int q = 0; q < 3; ++q)
+    for (int j = 0; j < cfg->vq_num_q[q]; ++j, ++li) {
+      FacodecLayerRef& l = f.layers[li];
+      l.in_proj = make_linear(g, "quantizer." + std::to_string(q) + ".layers." + std::to_string(j) + ".in_proj", C, D);
+      g->slots[l.in_proj.w].no_tc = true;
+    }
+  f.pe = g->add_slot("timbre_encoder.position_emb.pe", SLOT_VEC, {FAC_PE_ROWS, 1, FAC_TIMBRE_C});
+  const int H = FAC_TIMBRE_C;
+  for (int i = 0; i < 4; ++i) {
+    const std::string pre = "timbre_encoder.layers." + std::to_string(i) + ".";
+    TimbreLayerRef t;
+    t.ln1_w = g->add_slot(pre + "ln_1.weight", SLOT_VEC, {H});
+    t.ln1_b = g->add_slot(pre + "ln_1.bias", SLOT_VEC, {H});
+    t.ln2_w = g->add_slot(pre + "ln_2.weight", SLOT_VEC, {H});
+    t.ln2_b = g->add_slot(pre + "ln_2.bias", SLOT_VEC, {H});
+    // nn.MultiheadAttention packs q, k and v into in_proj_weight [3H, H] / in_proj_bias [3H]
+    t.qkv.cin = H; t.qkv.cout = 3 * H; t.qkv.k = 1;
+    t.qkv.w = g->add_slot(pre + "self_attn.in_proj_weight", SLOT_CONV_W, {3 * H, H});
+    g->slots[t.qkv.w].shape[2] = 1;
+    t.qkv.b = g->add_slot(pre + "self_attn.in_proj_bias", SLOT_VEC, {3 * H});
+    t.out_proj = make_linear(g, pre + "self_attn.out_proj", H, H);
+    t.ffn_1 = make_conv(g, pre + "ffn.ffn_1", H, 4 * H, 5, 1, false);
+    t.ffn_2 = make_linear(g, pre + "ffn.ffn_2", 4 * H, H);
+    f.timbre.push_back(t);
+  }
+  f.last_w = g->add_slot("timbre_encoder.last_ln.weight", SLOT_VEC, {H});
+  f.last_b = g->add_slot("timbre_encoder.last_ln.bias", SLOT_VEC, {H});
 }
 
 // FACodec encoder tensors (AB_GEN_FACODEC_ENCODER), the reference's names (facodec.py:121-194): "block.0" (conv_pre,
@@ -774,6 +820,13 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     g->dw.packed_offset = g->arena_need;
     g->arena_need += align_up(diffwave_packed_floats(*cfg) * sizeof(float), 256);
   }
+  if (cfg->kind == AB_GEN_FACODEC && cfg->facodec_quantize) {   // normalised codebooks, built at finalize
+    for (auto& l : g->fac.layers) {
+      l.cbn_offset = g->arena_need;
+      g->arena_need += align_up((size_t)l.rows * FAC_MAX_CODEBOOK_DIM * sizeof(float), 256) +
+                       align_up((size_t)l.rows * sizeof(float), 256);
+    }
+  }
   *out = g;
   return AB_OK;
 }
@@ -916,6 +969,19 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
       if (cudaStreamSynchronize(st) != cudaSuccess)
         return fail(AB_ERR_CUDA, "finalize: %s", cudaGetErrorString(cudaGetLastError()));
       for (size_t j = 0; j < ups.size(); ++j) pack_snake_coef(&host[j * 24], &host[j * 24 + 12], &g->act_coef[ups[j]]);
+    }
+  }
+  if (g->cfg.kind == AB_GEN_FACODEC && g->cfg.facodec_quantize) {
+    for (const auto& t : g->fac.timbre)   // the timbre encoder's GEMMs all run on the wgmma kernel at 16 bits
+      for (const ConvRef* c : {&t.qkv, &t.out_proj, &t.ffn_1, &t.ffn_2})
+        if (precision != AB_PREC_FP32 && g->slots[c->w].tc_bytes == 0)
+          return fail(AB_ERR_UNSUPPORTED, "finalize: '%s' has no tensor-core image", g->slots[c->w].name.c_str());
+    for (const auto& l : g->fac.layers) {
+      float* cbn = reinterpret_cast<float*>(g->arena + l.cbn_offset);
+      float* cbn2 = reinterpret_cast<float*>(g->arena + l.cbn_offset +
+                                             align_up((size_t)l.rows * FAC_MAX_CODEBOOK_DIM * sizeof(float), 256));
+      const int rc = launch_facodec_cbnorm(g->fptr(l.cb), cbn, cbn2, l.rows, g->cfg.vq_codebook_dim, st);
+      if (rc != AB_OK) return rc;
     }
   }
   g->precision = precision;
@@ -1070,11 +1136,12 @@ int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
 
 int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max_entries, int32_t* n_out) {
   if (!g || !out || !n_out) return fail(AB_ERR_ARG, "get_profile: null argument");
-  static const char* kNames[12] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
+  static const char* kNames[14] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
                                    "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
-                                   "diffwave_tail", "facodec_prologue"};
-  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's
-  const int n = g->cfg.kind == AB_GEN_FACODEC ? 12 : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
+                                   "diffwave_tail", "facodec_prologue", "facodec_quantize", "timbre_attention"};
+  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder
+  const int n = g->cfg.kind == AB_GEN_FACODEC ? (g->cfg.facodec_quantize ? 14 : 12)
+                : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
   for (int i = 0; i < n; ++i) {
     memset(&out[i], 0, sizeof(out[i]));
@@ -1889,6 +1956,164 @@ int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t
                     workspace_bytes, stream, img ? reinterpret_cast<const uint16_t*>(film) : nullptr);
   if (rc != AB_OK) return rc;
   g->launches += 2;
+  return AB_OK;
+}
+
+// FACodecDecoder.forward(vq=True): workspace of the timbre encoder.  S the fp32 stream [B, 256, T]; H a LayerNorm's
+// output (fp32, or the operand image at 16 bits) and last_ln's output; QKV [B, 768, T]; A the attention output (fp32 or
+// image); F ffn_1's fp32 output [B, 1024, T] and FI the image of its ReLU.
+struct TimbreWs {
+  float *S, *H, *QKV, *A, *F;
+  uint16_t* FI;
+};
+static size_t timbre_layout(int64_t B, int64_t T, char* base, TimbreWs* w) {
+  const size_t el = (size_t)B * T, C = FAC_TIMBRE_C;
+  const size_t sz[6] = {el * C * 4, el * C * 4, el * 3 * C * 4, el * C * 4, el * 4 * C * 4, tc_act_image_bytes(B, 4 * C, T)};
+  char* p[6];
+  size_t off = 0;
+  for (int i = 0; i < 6; ++i) {
+    p[i] = base ? base + off : nullptr;
+    off += align_up(sz[i], 256);
+  }
+  if (w) {
+    w->S = reinterpret_cast<float*>(p[0]); w->H = reinterpret_cast<float*>(p[1]); w->QKV = reinterpret_cast<float*>(p[2]);
+    w->A = reinterpret_cast<float*>(p[3]); w->F = reinterpret_cast<float*>(p[4]); w->FI = reinterpret_cast<uint16_t*>(p[5]);
+  }
+  return off;
+}
+
+size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
+  if (!g || g->cfg.kind != AB_GEN_FACODEC || !g->cfg.facodec_quantize || B <= 0 || T <= 0) return 0;
+  return timbre_layout(B, T, nullptr, nullptr);
+}
+
+int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t B, int64_t T,
+                        int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
+                        float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream) {
+  int rc = facodec_check(g, B, T, "facodec_quantize");
+  if (rc != AB_OK) return rc;
+  if (!g->cfg.facodec_quantize)
+    return fail(AB_ERR_STATE, "facodec_quantize: the handle was created without facodec_quantize");
+  if (!dev_x || !x_strides || !dev_emb_out || !dev_codes_out || !dev_quantized_out || !dev_spk_out)
+    return fail(AB_ERR_ARG, "facodec_quantize: null argument");
+  if (n_quantizers < 1) return fail(AB_ERR_ARG, "facodec_quantize: n_quantizers %d < 1 (no layer would run)", n_quantizers);
+  if (B > FAC_PE_ROWS)   // PositionalEncoding adds pe[:B] (transformer.py:43-45)
+    return fail(AB_ERR_ARG, "facodec_quantize: batch %lld > %d, the rows of the positional encoding", (long long)B, FAC_PE_ROWS);
+  const size_t need = ab_facodec_quantize_workspace_bytes(g, B, T);
+  if (!dev_workspace || workspace_bytes < need)
+    return fail(AB_ERR_WORKSPACE, "facodec_quantize: workspace %zu B < required %zu B", workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "facodec_quantize: workspace must be 256-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  TimbreWs w;
+  timbre_layout(B, T, static_cast<char*>(dev_workspace), &w);
+  const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim, Tn = (int)T;
+  const bool tc = g->precision != AB_PREC_FP32;
+  const double el = (double)B * T;
+  int launches = 0;
+  DwProf prof{g, st};
+
+  // the quantizers (all groups, one launch) and the positional add into S
+  FacRvqParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = dev_x; p.xsb = x_strides[0]; p.xsc = x_strides[1]; p.xst = x_strides[2];
+  int n_used = 0, nq_run = 0;
+  for (int gi = 0, l0 = 0; gi < 3; l0 += g->cfg.vq_num_q[gi], ++gi) {
+    p.layer0[gi] = l0;
+    p.nused[gi] = std::min(n_quantizers, g->cfg.vq_num_q[gi]);   // rvq.py:50-52
+    p.code_row0[gi] = n_used;
+    n_used += p.nused[gi];
+    for (int j = 0; j < p.nused[gi]; ++j) {
+      const FacodecLayerRef& l = g->fac.layers[l0 + j];
+      const int q = l0 + j;
+      p.w_in[q] = g->fptr(l.in_proj.w); p.b_in[q] = g->fptr(l.in_proj.b);
+      p.w_out[q] = g->fptr(l.out_proj.w); p.b_out[q] = g->fptr(l.out_proj.b);
+      p.cb[q] = g->fptr(l.cb);
+      p.cbn[q] = reinterpret_cast<const float*>(g->arena + l.cbn_offset);
+      p.cbn2[q] = reinterpret_cast<const float*>(g->arena + l.cbn_offset +
+                                                 align_up((size_t)l.rows * FAC_MAX_CODEBOOK_DIM * sizeof(float), 256));
+      p.rows[q] = l.rows;
+      nq_run += 1;
+    }
+  }
+  p.ngroups = g->cfg.vq_num_q[2] > 0 ? 3 : 2;
+  p.B = (int)B; p.C = C; p.T = Tn; p.D = D;
+  p.emb = dev_emb_out; p.codes = dev_codes_out; p.quantized = dev_quantized_out;
+  p.pe = g->fptr(g->fac.pe); p.stream = w.S;
+  {
+    double cb_flops = 0.0, cb_bytes = 0.0;
+    for (int q = 0; q < AB_FACODEC_MAX_Q; ++q)
+      if (p.cb[q]) { cb_flops += 2.0 * el * p.rows[q] * D; cb_bytes += 4.0 * p.rows[q] * (FAC_MAX_CODEBOOK_DIM + 1); }
+    ++launches;
+    prof.begin(12, 4.0 * el * nq_run * C * D + cb_flops,
+               4.0 * el * C * (2 + p.ngroups + 1) + 8.0 * el * n_used + cb_bytes + 8.0 * nq_run * (double)C * D);
+    rc = launch_facodec_rvq(p, st);
+    prof.end();
+    if (rc != AB_OK) return rc;
+  }
+
+  // the timbre encoder on S (transformer.py:206-217)
+  const uint16_t* Himg = reinterpret_cast<const uint16_t*>(w.H);
+  auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) -> int {
+    NormParams n;
+    n.x = w.S; n.ln_w = g->fptr(lw); n.ln_b = g->fptr(lb);
+    n.y = y; n.yimg = yimg; n.bf16 = g->precision == AB_PREC_TC_BF16;
+    n.B = (int)B; n.C = C; n.T = Tn; n.eps = 1e-5f;
+    ++launches;
+    prof.begin(6, 8.0 * el * C, 4.0 * el * C + (y ? 4.0 : 2.0) * el * C);
+    const int r = launch_vocos_norm(n, st);
+    prof.end();
+    return r;
+  };
+  // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual / acc_prev = y]
+  auto gemm = [&](const ConvRef& c, const float* x, const uint16_t* ximg, float* y, bool residual, float pre_slope,
+                  uint16_t* yimg) -> int {
+    ++launches;
+    prof.begin(tc ? 0 : 1, 2.0 * el * c.cin * c.cout * c.k,
+               el * c.cin * (tc ? 2.0 : 4.0) + 4.0 * el * c.cout * (residual ? 2 : 1) + (yimg ? 2.0 * el * c.cout : 0.0) +
+                   (tc ? 2.0 : 4.0) * c.cin * c.cout * c.k);
+    int r;
+    if (tc) {
+      TcConvParams t;
+      t.ximg = ximg; t.w = g->tcptr(c.w); t.bias = g->fptr(c.b);
+      t.acc_prev = residual ? y : nullptr; t.y = y; t.yimg = yimg; t.img_slope = 0.0f;
+      t.B = (int)B; t.Cin = c.cin; t.Cout = c.cout; t.T = Tn; t.k = c.k; t.d_or_u = 1; t.precision = g->precision;
+      r = launch_tc_conv(t, st);
+    } else {
+      // residual in place: each output element is read and then written by the same thread
+      ConvParams f;
+      f.x = x; f.xsb = (int64_t)c.cin * Tn; f.xsc = Tn; f.xst = 1;
+      f.w_t = g->fptr(c.w); f.bias = g->fptr(c.b);
+      f.residual = residual ? y : nullptr; f.acc_prev = nullptr; f.y = y;
+      f.B = (int)B; f.Cin = c.cin; f.Cout = c.cout; f.T = Tn; f.k = c.k; f.d = 1;
+      f.pre_slope = pre_slope; f.out_div = 1.0f; f.post_tanh = 0;
+      r = launch_conv1d_fp32(f, st);
+    }
+    prof.end();
+    return r;
+  };
+  for (const TimbreLayerRef& t : g->fac.timbre) {
+    // x = x + out_proj(MHA(LN1(x)))
+    if ((rc = norm(t.ln1_w, t.ln1_b, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.qkv, w.H, Himg, w.QKV, false, 1.0f, nullptr)) != AB_OK) return rc;
+    ++launches;
+    prof.begin(13, 4.0 * B * (double)T * T * C, 4.0 * el * 3 * C + (tc ? 2.0 : 4.0) * el * C);
+    rc = launch_facodec_attention(w.QKV, tc ? nullptr : w.A, tc ? reinterpret_cast<uint16_t*>(w.A) : nullptr,
+                                  g->precision == AB_PREC_TC_BF16, (int)B, Tn, st);
+    prof.end();
+    if (rc != AB_OK) return rc;
+    if ((rc = gemm(t.out_proj, w.A, reinterpret_cast<const uint16_t*>(w.A), w.S, true, 1.0f, nullptr)) != AB_OK) return rc;
+    // x = x + ffn_2(relu(ffn_1(LN2(x))))
+    if ((rc = norm(t.ln2_w, t.ln2_b, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.ffn_1, w.H, Himg, w.F, false, 1.0f, tc ? w.FI : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.ffn_2, w.F, w.FI, w.S, true, 0.0f, nullptr)) != AB_OK) return rc;
+  }
+  if ((rc = norm(g->fac.last_w, g->fac.last_b, w.H, nullptr)) != AB_OK) return rc;
+  ++launches;
+  prof.begin(12, el * C, 4.0 * el * C + 4.0 * B * C);
+  rc = launch_facodec_time_mean(w.H, dev_spk_out, (int)B, C, Tn, st);
+  prof.end();
+  if (rc != AB_OK) return rc;
+  g->launches = launches;
   return AB_OK;
 }
 

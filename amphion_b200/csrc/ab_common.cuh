@@ -243,6 +243,40 @@ int launch_facodec_style(const float* spk, int64_t spk_stride, const float* w, c
 int launch_facodec_film(const FacFilmParams& p, cudaStream_t s);
 int launch_facodec_vq2emb(const FacVqParams& p, cudaStream_t s);
 
+// ---- FACodecDecoder.forward(vq=True): the RVQ and the timbre encoder's own kernels (ab_facodec.cu) ----
+constexpr int FAC_TIMBRE_C = 256;         // encoder_hidden of the timbre encoder (transformer.py:154-217)
+constexpr int FAC_TIMBRE_HEADS = 4;
+constexpr int FAC_PE_ROWS = 5000;         // PositionalEncoding's max_len: the rows of "pe"
+struct FacRvqParams {       // quantize (facodec.py:408-445) for one tile of frames per CTA, and the positional add
+  const float* x;           // [B, C, T] with element strides xsb / xsc / xst
+  int64_t xsb, xsc, xst;
+  const float* w_in[AB_FACODEC_MAX_Q];     // in_proj, repacked [C][D] (weight norm folded)
+  const float* b_in[AB_FACODEC_MAX_Q];     // [D]
+  const float* w_out[AB_FACODEC_MAX_Q];    // out_proj, repacked [D][C]
+  const float* b_out[AB_FACODEC_MAX_Q];    // [C]
+  const float* cb[AB_FACODEC_MAX_Q];       // codebook [rows][D] (the unnormalised rows z_q reads)
+  const float* cbn[AB_FACODEC_MAX_Q];      // normalised codebook, rows padded to 16 floats [rows][16]
+  const float* cbn2[AB_FACODEC_MAX_Q];     // squared norms of the normalised rows [rows]
+  int64_t rows[AB_FACODEC_MAX_Q];
+  int layer0[3], nused[3];  // per group: first layer index, layers run (0: group absent)
+  int code_row0[3];         // per group: first row of codes_out
+  int ngroups;              // 2 or 3: the planes of quantized_out
+  int B, C, T, D;
+  float* emb;               // [B, C, T]
+  int64_t* codes;           // [n_used, B, T]
+  float* quantized;         // [ngroups, B, C, T]
+  const float* pe;          // nullable: [rows][C]; stream[b, c, t] = x[b, c, t] + pe[b][c]
+  float* stream;            // [B, C, T]
+};
+// normalised codebook rows (F.normalize, eps 1e-12) padded to 16 floats, and their squared norms
+int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows, int D, cudaStream_t s);
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s);
+// softmax(q k^T / 8) v per (utterance, head) from qkv [B, 3 * 256, T] (q, k, v rows; time fastest) -> y fp32 [B, 256, T]
+// or the operand image yimg [B][32][T][8]
+int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf16, int B, int T, cudaStream_t s);
+// spk[b][c] = sum_t y[b, c, t] / T (fixed order)
+int launch_facodec_time_mean(const float* y, float* spk, int B, int C, int T, cudaStream_t s);
+
 // launchers (ab_kernels_fp32.cu)
 int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);

@@ -1,6 +1,8 @@
 // FACodec decoder prologue kernels (models/codec/ns3_codec/facodec.py:556-576): the codebook decode (vq2emb), the
 // timbre projection and the LayerNorm + FiLM in front of conv_pre.  The generator itself runs on the BigVGAN path of
-// ab_capi.cu's forward_impl.
+// ab_capi.cu's forward_impl.  Then the kernels of FACodecDecoder.forward(vq=True) (facodec.py:408-471): the residual
+// vector quantizer, the timbre encoder's attention and the time mean; its GEMMs and LayerNorms run on the shared
+// convolution and LayerNorm kernels.
 #include <algorithm>
 
 #include "ab_common.cuh"
@@ -153,6 +155,326 @@ __global__ void __launch_bounds__(VQ_THREADS) facodec_vq2emb_kernel(FacVqParams 
   }
 }
 
+
+// ---- FACodecDecoder.forward(vq=True) ------------------------------------------------------------------------------
+
+// F.normalize(codebook) (eps 1e-12) into rows of 16 floats (zero padded) and the squared norms of the normalised rows,
+// as fvq.py:103-111 computes them.  One thread per row.
+__global__ void __launch_bounds__(256) facodec_cbnorm_kernel(const float* __restrict__ cb, float* __restrict__ cbn,
+                                                             float* __restrict__ cbn2, int64_t rows, int D) {
+  const int64_t r = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (r >= rows) return;
+  float v[FAC_MAX_CODEBOOK_DIM];
+  float n2 = 0.f;
+#pragma unroll
+  for (int d = 0; d < FAC_MAX_CODEBOOK_DIM; ++d) {
+    v[d] = d < D ? __ldg(cb + r * D + d) : 0.f;
+    n2 = __fmaf_rn(v[d], v[d], n2);
+  }
+  const float den = fmaxf(__fsqrt_rn(n2), 1e-12f);
+  float c2 = 0.f;
+#pragma unroll
+  for (int d = 0; d < FAC_MAX_CODEBOOK_DIM; ++d) {
+    const float c = d < D ? __fdiv_rn(v[d], den) : 0.f;
+    cbn[r * FAC_MAX_CODEBOOK_DIM + d] = c;
+    c2 = __fmaf_rn(c, c, c2);
+  }
+  cbn2[r] = c2;
+}
+
+// The residual vector quantizer, all groups in one launch.  One CTA per (utterance, tile of RVQ_TT frames): the tile's
+// x, the running residual, the current group's sum and prosody + content sit in shared memory [C][RVQ_TT]; each layer
+// streams its normalised codebook through shared memory in chunks of RVQ_CH rows, so any codebook size is served.
+// Per layer and frame (fvq.py:52-91):
+//   z_e = b_in + sum_c W_in[d][c] r[c]  (an fp32 FMA chain over c ascending, then the bias)
+//   e = z_e / max(|z_e|, 1e-12);  dist_i = (|e|^2 - 2 e.c_i) + |c_i|^2;  code = the lowest i of the least dist
+//   z_q = z_e + (codebook[code] - z_e)  (the straight-through step, two fp32 roundings)
+//   q = sum_d W_out[c][d] z_q[d] (an FMA chain from 0) + b_out[c];  r -= q;  group sum += q
+// The groups' sums are written as they complete; emb = (prosody + content) + residual.
+constexpr int RVQ_TT = 16;
+constexpr int RVQ_THREADS = 256;
+constexpr int RVQ_CH = 256;
+constexpr int RVQ_LANES = RVQ_THREADS / RVQ_TT;   // threads scanning one frame's codebook
+
+size_t rvq_smem_bytes(int C) {
+  return sizeof(float) * ((size_t)4 * C * RVQ_TT + RVQ_CH * (FAC_MAX_CODEBOOK_DIM + 1) +
+                          RVQ_TT * (2 * FAC_MAX_CODEBOOK_DIM + 1)) + sizeof(int) * RVQ_TT;
+}
+
+__global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(FacRvqParams p, int tiles) {
+  extern __shared__ __align__(16) float qsm[];
+  const int C = p.C, D = p.D, tid = threadIdx.x;
+  float* xs = qsm;                          // [C][TT] x
+  float* rs = xs + C * RVQ_TT;              // [C][TT] residual
+  float* gs = rs + C * RVQ_TT;              // [C][TT] current group's sum
+  float* s01 = gs + C * RVQ_TT;             // [C][TT] prosody, then prosody + content
+  float* cbs = s01 + C * RVQ_TT;            // [RVQ_CH][16] normalised codebook chunk
+  float* cb2s = cbs + RVQ_CH * FAC_MAX_CODEBOOK_DIM;    // [RVQ_CH]
+  float* zes = cb2s + RVQ_CH;               // [TT][16] z_e, then z_q
+  float* es = zes + RVQ_TT * FAC_MAX_CODEBOOK_DIM;      // [TT][16] normalised z_e
+  float* e2s = es + RVQ_TT * FAC_MAX_CODEBOOK_DIM;      // [TT] |e|^2
+  int* codes = reinterpret_cast<int*>(e2s + RVQ_TT);    // [TT]
+  const int b = blockIdx.x / tiles, t0 = (blockIdx.x - b * tiles) * RVQ_TT;
+  const int n = C * RVQ_TT;
+  const float* xb = p.x + (int64_t)b * p.xsb;
+  for (int i = tid; i < n; i += RVQ_THREADS) {
+    const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
+    float v = 0.f;
+    if (t < p.T) {
+      v = __ldg(xb + c * p.xsc + (int64_t)t * p.xst);
+      // transformer.py:43-45 on the batch-first stream: utterance b adds row b of pe at every time step
+      if (p.stream) p.stream[((int64_t)b * C + c) * p.T + t] = __fadd_rn(v, __ldg(p.pe + (int64_t)b * C + c));
+    }
+    xs[i] = v;
+  }
+  const int fu = tid / RVQ_LANES, lane = tid % RVQ_LANES;   // search: frame fu, rows lane, lane + RVQ_LANES, ...
+  for (int g = 0; g < 3; ++g) {
+    if (p.nused[g] == 0) continue;
+    __syncthreads();
+    for (int i = tid; i < n; i += RVQ_THREADS) {
+      rs[i] = g < 2 ? xs[i] : __fsub_rn(xs[i], s01[i]);   // facodec.py:436: x - (prosody + content)
+      gs[i] = 0.f;
+    }
+    for (int j = 0; j < p.nused[g]; ++j) {
+      const int q = p.layer0[g] + j;
+      __syncthreads();
+      // z_e: thread (d, u)
+      {
+        const int d = tid / RVQ_TT, u = tid % RVQ_TT;
+        if (d < D) {
+          const float* w = p.w_in[q] + d;
+          float a = 0.f;
+          for (int c = 0; c < C; ++c) a = __fmaf_rn(__ldg(w + (size_t)c * D), rs[c * RVQ_TT + u], a);
+          zes[u * FAC_MAX_CODEBOOK_DIM + d] = __fadd_rn(a, __ldg(p.b_in[q] + d));
+        }
+      }
+      __syncthreads();
+      if (tid < RVQ_TT) {   // F.normalize(z_e) and |e|^2
+        const float* z = zes + tid * FAC_MAX_CODEBOOK_DIM;
+        float n2 = 0.f;
+        for (int d = 0; d < D; ++d) n2 = __fmaf_rn(z[d], z[d], n2);
+        const float den = fmaxf(__fsqrt_rn(n2), 1e-12f);
+        float e2 = 0.f;
+        for (int d = 0; d < FAC_MAX_CODEBOOK_DIM; ++d) {
+          const float e = d < D ? __fdiv_rn(z[d], den) : 0.f;
+          es[tid * FAC_MAX_CODEBOOK_DIM + d] = e;
+          e2 = __fmaf_rn(e, e, e2);
+        }
+        e2s[tid] = e2;
+      }
+      __syncthreads();
+      float e[FAC_MAX_CODEBOOK_DIM];
+#pragma unroll
+      for (int d = 0; d < FAC_MAX_CODEBOOK_DIM; ++d) e[d] = es[fu * FAC_MAX_CODEBOOK_DIM + d];
+      const float e2 = e2s[fu];
+      float best = __int_as_float(0x7f800000);
+      int best_i = 0x7fffffff;
+      const int64_t rows = p.rows[q];
+      for (int64_t r0 = 0; r0 < rows; r0 += RVQ_CH) {
+        const int nr = rows - r0 < RVQ_CH ? (int)(rows - r0) : RVQ_CH;
+        __syncthreads();
+        const float4* src = reinterpret_cast<const float4*>(p.cbn[q] + r0 * FAC_MAX_CODEBOOK_DIM);
+        for (int i = tid; i < nr * (FAC_MAX_CODEBOOK_DIM / 4); i += RVQ_THREADS)
+          reinterpret_cast<float4*>(cbs)[i] = __ldg(src + i);
+        for (int i = tid; i < nr; i += RVQ_THREADS) cb2s[i] = __ldg(p.cbn2[q] + r0 + i);
+        __syncthreads();
+        for (int i = lane; i < nr; i += RVQ_LANES) {
+          const float4* c4 = reinterpret_cast<const float4*>(cbs + i * FAC_MAX_CODEBOOK_DIM);
+          float dot = 0.f;
+#pragma unroll
+          for (int k = 0; k < FAC_MAX_CODEBOOK_DIM / 4; ++k) {
+            const float4 c = c4[k];
+            dot = __fmaf_rn(e[4 * k], c.x, dot);
+            dot = __fmaf_rn(e[4 * k + 1], c.y, dot);
+            dot = __fmaf_rn(e[4 * k + 2], c.z, dot);
+            dot = __fmaf_rn(e[4 * k + 3], c.w, dot);
+          }
+          const float dist = __fadd_rn(__fsub_rn(e2, __fmul_rn(2.0f, dot)), cb2s[i]);
+          if (dist < best) { best = dist; best_i = (int)(r0 + i); }   // rows ascend: the first of equals stays
+        }
+      }
+      // the least dist over the frame's lanes, the lowest code among equals
+#pragma unroll
+      for (int m = RVQ_LANES / 2; m > 0; m >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, m);
+        const int oi = __shfl_xor_sync(0xffffffffu, best_i, m);
+        if (ob < best || (ob == best && oi < best_i)) { best = ob; best_i = oi; }
+      }
+      if (lane == 0) {
+        // no finite distance (a NaN input): code 0, as argmax over NaNs is not defined either way
+        codes[fu] = best_i == 0x7fffffff ? 0 : best_i;
+      }
+      __syncthreads();
+      if (tid < RVQ_TT * FAC_MAX_CODEBOOK_DIM) {   // z_q = z_e + (codebook[code] - z_e)
+        const int u = tid / FAC_MAX_CODEBOOK_DIM, d = tid % FAC_MAX_CODEBOOK_DIM;
+        if (d < D) {
+          const float z = zes[tid];
+          zes[tid] = __fadd_rn(z, __fsub_rn(__ldg(p.cb[q] + (int64_t)codes[u] * D + d), z));
+        }
+        if (d == 0 && t0 + u < p.T)
+          p.codes[((int64_t)(p.code_row0[g] + j) * p.B + b) * p.T + t0 + u] = codes[u];
+      }
+      __syncthreads();
+      const float* wo = p.w_out[q];
+      for (int i = tid; i < n; i += RVQ_THREADS) {
+        const int c = i / RVQ_TT, u = i - c * RVQ_TT;
+        const float* z = zes + u * FAC_MAX_CODEBOOK_DIM;
+        float a = 0.f;
+        for (int d = 0; d < D; ++d) a = __fmaf_rn(z[d], __ldg(wo + (size_t)d * C + c), a);
+        a = __fadd_rn(a, __ldg(p.b_out[q] + c));
+        rs[i] = __fsub_rn(rs[i], a);
+        gs[i] = __fadd_rn(gs[i], a);
+      }
+    }
+    __syncthreads();
+    for (int i = tid; i < n; i += RVQ_THREADS) {
+      const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
+      const float v = gs[i];
+      if (t < p.T) p.quantized[(((int64_t)g * p.B + b) * C + c) * p.T + t] = v;
+      if (g == 0) s01[i] = v;
+      else if (g == 1) s01[i] = __fadd_rn(s01[i], v);
+      else if (t < p.T) p.emb[((int64_t)b * C + c) * p.T + t] = __fadd_rn(s01[i], v);
+    }
+    if (g == 1 && p.nused[2] == 0) {
+      for (int i = tid; i < n; i += RVQ_THREADS) {
+        const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
+        if (t < p.T) p.emb[((int64_t)b * C + c) * p.T + t] = s01[i];
+      }
+    }
+  }
+}
+
+// Multi-head self-attention core of nn.MultiheadAttention(256, 4, batch_first=True) without a mask
+// (transformer.py:113-138): per head, softmax(q k^T / 8) v, flash style on the CUDA cores in fp32.  One CTA per
+// (64-query tile, head, utterance) loops over 64-key tiles with an online max and sum (precise expf); T x T is never
+// stored.  Thread (query i = tid / 4, quarter part = tid % 4) scores keys part*16 .. +15 of a tile and accumulates
+// output dims part*16 .. +15.  OUT: 0 fp32 [B, 256, T]; 1 / 2 the fp16 / bf16 operand image [B][32][T][8].
+constexpr int ATT_TILE = 64;
+constexpr int ATT_HD = FAC_TIMBRE_C / FAC_TIMBRE_HEADS;   // 64
+constexpr int ATT_THREADS = 256;
+constexpr size_t ATT_SMEM = sizeof(float) * (2 * ATT_HD * ATT_TILE + ATT_TILE * (ATT_TILE + 4));
+
+template <int OUT>
+__global__ void __launch_bounds__(ATT_THREADS, 1) facodec_attention_kernel(const float* __restrict__ qkv, float* y,
+                                                                       uint16_t* yimg, int T) {
+  extern __shared__ __align__(16) float asm_[];
+  float* ks = asm_;                          // [d][key] of the tile
+  float* vs = ks + ATT_HD * ATT_TILE;        // [d][key]
+  float* ps = vs + ATT_HD * ATT_TILE;        // [query][key] probabilities, rows padded to 68
+  constexpr int PSTR = ATT_TILE + 4;
+  const int h = blockIdx.y, b = blockIdx.z, q0 = blockIdx.x * ATT_TILE;
+  const int tid = threadIdx.x, qi = tid >> 2, part = tid & 3;
+  const int64_t base = (int64_t)b * 3 * FAC_TIMBRE_C * T;
+  const float* qrow = qkv + base + (int64_t)(h * ATT_HD) * T;
+  const float* krow = qkv + base + (int64_t)(FAC_TIMBRE_C + h * ATT_HD) * T;
+  const float* vrow = qkv + base + (int64_t)(2 * FAC_TIMBRE_C + h * ATT_HD) * T;
+  const int tq = q0 + qi;
+  float q[ATT_HD];
+#pragma unroll
+  for (int d = 0; d < ATT_HD; ++d) q[d] = tq < T ? __ldg(qrow + (int64_t)d * T + tq) : 0.f;
+  float o[16], l = 0.f, m = __int_as_float(0xff800000);
+#pragma unroll
+  for (int k = 0; k < 16; ++k) o[k] = 0.f;
+  for (int k0 = 0; k0 < T; k0 += ATT_TILE) {
+    __syncthreads();
+    for (int i = tid; i < ATT_HD * ATT_TILE; i += ATT_THREADS) {
+      const int d = i / ATT_TILE, j = i - d * ATT_TILE, t = k0 + j;
+      ks[i] = t < T ? __ldg(krow + (int64_t)d * T + t) : 0.f;
+      vs[i] = t < T ? __ldg(vrow + (int64_t)d * T + t) : 0.f;
+    }
+    __syncthreads();
+    float s[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s[k] = 0.f;
+#pragma unroll
+    for (int d = 0; d < ATT_HD; ++d) {
+      const float4* kr = reinterpret_cast<const float4*>(ks + d * ATT_TILE + part * 16);
+#pragma unroll
+      for (int k4 = 0; k4 < 4; ++k4) {
+        const float4 kv = kr[k4];
+        s[4 * k4] = __fmaf_rn(q[d], kv.x, s[4 * k4]);
+        s[4 * k4 + 1] = __fmaf_rn(q[d], kv.y, s[4 * k4 + 1]);
+        s[4 * k4 + 2] = __fmaf_rn(q[d], kv.z, s[4 * k4 + 2]);
+        s[4 * k4 + 3] = __fmaf_rn(q[d], kv.w, s[4 * k4 + 3]);
+      }
+    }
+    float mt = __int_as_float(0xff800000);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      s[k] = k0 + part * 16 + k < T ? __fmul_rn(s[k], 0.125f) : __int_as_float(0xff800000);
+      mt = fmaxf(mt, s[k]);
+    }
+    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+    const float mn = fmaxf(m, mt);               // every tile holds a key: finite
+    const float alpha = expf(__fsub_rn(m, mn));  // 0 on the first tile (m = -inf)
+    m = mn;
+    float ls = 0.f;
+    float4* pr = reinterpret_cast<float4*>(ps + qi * PSTR + part * 16);
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) {
+      float pv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        pv[e] = expf(__fsub_rn(s[4 * k4 + e], mn));   // exp(-inf) = 0 for the keys past T
+        ls = __fadd_rn(ls, pv[e]);
+      }
+      pr[k4] = make_float4(pv[0], pv[1], pv[2], pv[3]);
+    }
+    l = __fadd_rn(__fmul_rn(l, alpha), ls);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) o[k] = __fmul_rn(o[k], alpha);
+    __syncthreads();
+    const int nk = min(ATT_TILE, T - k0);
+    const float* prow = ps + qi * PSTR;
+    const float* vcol = vs + part * 16 * ATT_TILE;
+    for (int j = 0; j < nk; j += 4) {   // rows past nk hold zeros in v and p: 4-key steps stay exact
+      const float4 p4 = *reinterpret_cast<const float4*>(prow + j);
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        const float4 v4 = *reinterpret_cast<const float4*>(vcol + k * ATT_TILE + j);
+        o[k] = __fmaf_rn(p4.x, v4.x, o[k]);
+        o[k] = __fmaf_rn(p4.y, v4.y, o[k]);
+        o[k] = __fmaf_rn(p4.z, v4.z, o[k]);
+        o[k] = __fmaf_rn(p4.w, v4.w, o[k]);
+      }
+    }
+  }
+  // the row sum over the four quarters, in a fixed order
+  l = __fadd_rn(l, __shfl_xor_sync(0xffffffffu, l, 1));
+  l = __fadd_rn(l, __shfl_xor_sync(0xffffffffu, l, 2));
+  if (tq >= T) return;
+  float r[16];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) r[k] = __fdiv_rn(o[k], l);
+  const int c0 = h * ATT_HD + part * 16;
+  if (OUT == 0) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) y[((int64_t)b * FAC_TIMBRE_C + c0 + k) * T + tq] = r[k];
+  } else {
+    constexpr int c8n = FAC_TIMBRE_C / 8;
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+      *reinterpret_cast<uint4*>(yimg + (((size_t)b * c8n + c0 / 8 + hf) * T + tq) * 8) =
+          make_uint4(fac_cvt_pair<OUT - 1>(r[8 * hf], r[8 * hf + 1]), fac_cvt_pair<OUT - 1>(r[8 * hf + 2], r[8 * hf + 3]),
+                     fac_cvt_pair<OUT - 1>(r[8 * hf + 4], r[8 * hf + 5]), fac_cvt_pair<OUT - 1>(r[8 * hf + 6], r[8 * hf + 7]));
+  }
+}
+
+// spk[b][c] = (sum over t of y[b, c, t]) / T: one warp per row, lane-strided partial sums in time order, a butterfly
+// reduction (facodec.py:469, torch.mean(x_timbre, dim=2))
+__global__ void __launch_bounds__(256) facodec_time_mean_kernel(const float* __restrict__ y, float* __restrict__ spk,
+                                                               int rows, int T) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const float* yr = y + (int64_t)row * T;
+  float a = 0.f;
+  for (int t = lane; t < T; t += 32) a = __fadd_rn(a, __ldg(yr + t));
+#pragma unroll
+  for (int m = 16; m > 0; m >>= 1) a = __fadd_rn(a, __shfl_xor_sync(0xffffffffu, a, m));
+  if (lane == 0) spk[row] = __fdiv_rn(a, (float)T);
+}
+
 }  // namespace
 
 int launch_facodec_style(const float* spk, int64_t spk_stride, const float* w, const float* bias, float* style, int B,
@@ -198,6 +520,53 @@ int launch_facodec_vq2emb(const FacVqParams& p, cudaStream_t s) {
     AB_CUDA_TRY(cudaFuncSetAttribute(facodec_vq2emb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   facodec_vq2emb_kernel<<<(unsigned)grid, VQ_THREADS, smem, s>>>(p, (int)tiles);
   AB_LAUNCH_CHECK("facodec_vq2emb_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows, int D, cudaStream_t s) {
+  if (!cb || !cbn || !cbn2 || rows <= 0 || D <= 0 || D > FAC_MAX_CODEBOOK_DIM)
+    return fail(AB_ERR_ARG, "facodec cbnorm: bad argument");
+  facodec_cbnorm_kernel<<<(unsigned)ceil_div(rows, 256), 256, 0, s>>>(cb, cbn, cbn2, rows, D);
+  AB_LAUNCH_CHECK("facodec_cbnorm_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s) {
+  if (!p.x || !p.emb || !p.codes || !p.quantized || (!p.pe) != (!p.stream)) return fail(AB_ERR_ARG, "facodec rvq: null argument");
+  if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.D <= 0 || p.D > FAC_MAX_CODEBOOK_DIM || p.nused[0] <= 0 || p.nused[1] <= 0 ||
+      p.ngroups < 2 || p.ngroups > 3)
+    return fail(AB_ERR_ARG, "facodec rvq: bad shape");
+  const size_t smem = rvq_smem_bytes(p.C);
+  if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: %d channels do not fit shared memory", p.C);
+  const int64_t tiles = ceil_div(p.T, RVQ_TT), grid = (int64_t)p.B * tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: grid too large");
+  static DeviceOnce configured;
+  if (smem > 48 * 1024 && configured.need())
+    AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  facodec_rvq_kernel<<<(unsigned)grid, RVQ_THREADS, smem, s>>>(p, (int)tiles);
+  AB_LAUNCH_CHECK("facodec_rvq_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf16, int B, int T, cudaStream_t s) {
+  if (!qkv || (!y) == (!yimg)) return fail(AB_ERR_ARG, "facodec attention: null argument");
+  if (B <= 0 || B > 65535 || T <= 0) return fail(AB_ERR_ARG, "facodec attention: bad shape");
+  const int out = y ? 0 : (bf16 ? 2 : 1);
+  void (*kerns[3])(const float*, float*, uint16_t*, int) = {facodec_attention_kernel<0>, facodec_attention_kernel<1>,
+                                                            facodec_attention_kernel<2>};
+  static DeviceOnce configured[3];
+  if (configured[out].need())
+    AB_CUDA_TRY(cudaFuncSetAttribute(kerns[out], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM));
+  kerns[out]<<<dim3((unsigned)ceil_div(T, ATT_TILE), FAC_TIMBRE_HEADS, (unsigned)B), ATT_THREADS, ATT_SMEM, s>>>(qkv, y, yimg, T);
+  AB_LAUNCH_CHECK("facodec_attention_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_time_mean(const float* y, float* spk, int B, int C, int T, cudaStream_t s) {
+  if (!y || !spk || B <= 0 || C <= 0 || T <= 0) return fail(AB_ERR_ARG, "facodec time mean: bad argument");
+  const int rows = B * C;
+  facodec_time_mean_kernel<<<(unsigned)ceil_div(rows, 8), 256, 0, s>>>(y, spk, rows, T);
+  AB_LAUNCH_CHECK("facodec_time_mean_kernel");
   return AB_OK;
 }
 

@@ -1,8 +1,11 @@
 """FACodecDecoder — drop-in for the decoder of NaturalSpeech 3's FACodec (``models/codec/ns3_codec/facodec.py:242``):
 the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_proj,out_proj,_codebook}``, ``model.*``,
 ``timbre_encoder.*``, ``timbre_linear``, the ``CNNLSTM`` predictors and the ``use_gr_*`` heads), so the released
-``ns3_facodec_decoder.bin`` loads strictly.  The waveform path runs natively (``AB_GEN_FACODEC``):
+``ns3_facodec_decoder.bin`` loads strictly.  Served natively (``AB_GEN_FACODEC``):
 
+- ``forward(x, vq=True)`` in eval: latent ``[B, in_channels, T]`` -> ``(outs, qs, commit_loss, quantized_buf,
+  spk_embs)`` (:408-471): the three ResidualVQs on fp32 CUDA cores (codes are discrete) and the timbre transformer;
+  needs ``in_channels == 256``, the timbre encoder's width;
 - ``vq2emb(vq, use_residual_code=True)``: codes ``[n_q, B, T]`` -> ``[B, in_channels, T]`` (:556-566);
 - ``inference(x, speaker_embedding)``: the timbre FiLM (LayerNorm over channels, ``x * gamma + beta``) and the
   BigVGAN-family generator -> ``[B, 1, T * prod(up_ratios)]`` (:568-576).
@@ -10,8 +13,8 @@ the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_pr
 ``FACodecEncoder`` (:157-194) serves the waveform -> latent side natively (``AB_GEN_FACODEC_ENCODER``): ``forward`` /
 ``inference`` map ``[B, 1, N]`` to ``[B, out_channels, F]`` through the same ResidualUnits and strided convolutions.
 
-The decoder's encoder-side ``forward`` (quantization, the timbre transformer) and the training branch are not served;
-the modules only ``forward`` evaluates are kept as parameters."""
+The training branch (``vq=False``: the predictors, random residual masking, the losses), ``get_vq`` and a quantizer or
+timbre encoder in training mode are not served; the modules only those evaluate are kept as parameters."""
 from __future__ import annotations
 
 import ctypes as C
@@ -25,8 +28,8 @@ from .. import _capi
 from .activations import Activation1d, SnakeBeta
 from .generator import NativeGenerator
 
-_SERVED = ("amphion_b200 serves FACodecEncoder.forward() / .inference(), FACodecDecoder.vq2emb() and "
-           "FACodecDecoder.inference()")
+_SERVED = ("amphion_b200 serves FACodecEncoder.forward() / .inference(), FACodecDecoder.forward(vq=True) in eval, "
+           "FACodecDecoder.vq2emb() and FACodecDecoder.inference()")
 
 
 def _native_only(name):
@@ -179,6 +182,9 @@ class FACodecDecoder(NativeGenerator):
         self.codebook_size_content = codebook_size_content
         self.codebook_size_residual = codebook_size_residual
         self.codebook_dim = int(codebook_dim)
+        # set by the first forward(vq=True): the native handle then also holds the quantizers' in_proj and the timbre
+        # encoder (a decode-only handle keeps exactly the decoder's tensors)
+        self._quantize_handle = False
 
         def rvq(n, size):
             return ResidualVQ(num_quantizers=n, dim=vq_dim, codebook_size=size, codebook_dim=codebook_dim,
@@ -230,7 +236,7 @@ class FACodecDecoder(NativeGenerator):
     def _upsample_rates(self):
         return list(self.up_ratios)
 
-    def _c_config(self):
+    def _c_config_decode(self):
         if len(self.up_ratios) > _capi.AB_MAX_STAGES:
             raise ValueError("amphion_b200: too many up_ratios for the native decoder")
         c = _capi.GeneratorConfig()
@@ -336,13 +342,74 @@ class FACodecDecoder(NativeGenerator):
             self.last_launches = lib.ab_generator_last_launches(h)
         return wav
 
+    def _c_config(self):
+        c = self._c_config_decode()
+        c.facodec_quantize = int(self._quantize_handle)
+        return c
+
     def forward(self, x=None, vq=True, get_vq=False, eval_vq=True, speaker_embedding=None, n_quantizers=None,
                 quantized=None):
-        if vq is True:
-            raise NotImplementedError(f"amphion_b200: FACodecDecoder.forward(vq=True) (quantization and the timbre "
-                                      f"transformer) is not served; {_SERVED}")
-        raise NotImplementedError(f"amphion_b200: the training branch of FACodecDecoder.forward (the predictors, "
-                                  f"random residual masking) is not served; {_SERVED}")
+        """``vq=True``: x [B, 256, T] fp32 (any strides) -> ``(outs [B, 256, T], qs int64 [n_used, B, T],
+        commit_loss zeros [n_used], quantized_buf [2 or 3 x [B, 256, T]], spk_embs [B, 256])`` on x's device, without
+        autograd history (facodec.py:448-471 in eval).  ``n_quantizers = k`` keeps the first k layers of each group."""
+        if get_vq:
+            raise NotImplementedError(f"amphion_b200: FACodecDecoder.forward(get_vq=True) is not served; {_SERVED}")
+        if vq is not True:
+            raise NotImplementedError(f"amphion_b200: the training branch of FACodecDecoder.forward (the predictors, "
+                                      f"random residual masking) is not served; {_SERVED}")
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            dev = x.device if isinstance(x, torch.Tensor) else type(x).__name__
+            raise NotImplementedError(f"amphion_b200: FACodecDecoder.forward(vq=True) needs a CUDA tensor (got "
+                                      f"'{dev}'); there is no CPU fallback; {_SERVED}")
+        if self.in_channels != 256:
+            raise ValueError(f"amphion_b200: FACodecDecoder.forward(vq=True) needs in_channels == 256, the timbre "
+                             f"encoder's width (got {self.in_channels})")
+        if x.dim() != 3 or x.shape[1] != self.in_channels:
+            raise ValueError(f"FACodecDecoder.forward expects x of shape [B, {self.in_channels}, T], got {tuple(x.shape)}")
+        B, _, T = x.shape
+        if B == 0 or T == 0:
+            raise ValueError("amphion_b200: empty latent batch")
+        if B > self.timbre_encoder.position_emb.pe.shape[0]:
+            raise ValueError(f"amphion_b200: batch {B} > {self.timbre_encoder.position_emb.pe.shape[0]}, the rows of "
+                             f"the timbre encoder's positional encoding (the reference fails there too)")
+        k = max(self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r) if n_quantizers is None else int(n_quantizers)
+        if k < 1:
+            raise ValueError(f"amphion_b200: n_quantizers {n_quantizers} < 1 runs no layer (the reference raises too)")
+        if eval_vq:
+            self.quantizer.eval()   # facodec.py:460-461
+        if self.quantizer.training or any(m.training for m in self.quantizer.modules()):
+            raise NotImplementedError(f"amphion_b200: a quantizer in training mode (quantizer dropout, commitment "
+                                      f"losses) is not served; {_SERVED}")
+        if self.timbre_encoder.training or any(m.training for m in self.timbre_encoder.modules()):
+            raise NotImplementedError(f"amphion_b200: the timbre encoder in training mode (dropout) is not served; "
+                                      f"{_SERVED}")
+        if not self._quantize_handle:
+            # the decode-only handle lists no quantizer / timbre tensors: re-create it with them
+            self._quantize_handle = True
+            if self._handle is not None:
+                _capi.lib.ab_generator_destroy(self._handle)
+                self._handle = None
+            self._arena_key = None
+        if x.dtype != torch.float32:
+            x = x.float()
+        nq = [min(k, n) for n in (self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r)]
+        n_used, G = sum(nq), 3 if self.vq_num_q_r > 0 else 2
+        dev = x.device
+        with torch.cuda.device(dev):
+            self._sync_params(dev)
+            lib, h = _capi.lib, self._handle
+            need = lib.ab_facodec_quantize_workspace_bytes(h, B, T)
+            wbase = self._workspace_for(dev, need)
+            outs = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=dev)
+            qs = torch.empty(n_used, B, T, dtype=torch.int64, device=dev)
+            buf = torch.empty(G, B, self.in_channels, T, dtype=torch.float32, device=dev)
+            spk = torch.empty(B, self.in_channels, dtype=torch.float32, device=dev)
+            _capi.check(lib.ab_facodec_quantize(h, _capi.ptr(x), _capi.shape_array(x.stride()), B, T, k, _capi.ptr(outs),
+                                                _capi.ptr(qs), _capi.ptr(buf), _capi.ptr(spk), C.c_void_p(wbase), need,
+                                                _capi.stream_ptr()), "ab_facodec_quantize")
+            self.last_launches = lib.ab_generator_last_launches(h)
+        commit_loss = torch.zeros(n_used, dtype=torch.float32, device=dev)
+        return outs, qs, commit_loss, list(buf.unbind(0)), spk
 
     def remove_weight_norm(self):
         def _remove(m):

@@ -170,6 +170,9 @@ typedef struct ab_generator_config {
   int32_t vq_num_q[3];                          /* vq_num_q_p, vq_num_q_c, vq_num_q_r (the residual group may be 0) */
   int32_t vq_codebook_bits[3];                  /* codebook_size_{prosody,content,residual}: 2^bits rows */
   int32_t vq_codebook_dim;                      /* codebook_dim */
+  /* AB_GEN_FACODEC only (0 elsewhere): 1 = the handle also serves FACodecDecoder.forward(vq=True) (ab_facodec_quantize)
+   * and lists the quantizers' in_proj and the timbre encoder's tensors; needs n_mel == 256 */
+  int32_t facodec_quantize;
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -228,7 +231,10 @@ int ab_generator_last_launches(const ab_generator* g);
  * handle lists, when max_entries >= 11, also "diffwave_cond" (spectrogram upsampler and step embeddings, once per
  * call), "diffwave_input" (input projection), "diffwave_layer" (residual layers) and "diffwave_tail" (skip/output
  * projections and the sampler update).  A FACodec handle lists the first five and "facodec_prologue" (timbre_linear, the
- * LayerNorm and the FiLM, and vq2emb) when max_entries >= 12, the six unused classes with zero launches. */
+ * LayerNorm and the FiLM, and vq2emb) when max_entries >= 12, the six unused classes with zero launches; a handle created
+ * with facodec_quantize also lists "facodec_quantize" (the RVQ with the positional add, and the time mean) and
+ * "timbre_attention" (max_entries >= 14).  ab_facodec_quantize counts its GEMMs in "tc_conv" (tensor-core precision)
+ * or "conv1d_fp32", and its LayerNorms in "vocos_norm". */
 typedef struct ab_profile_entry {
   char name[32];
   int32_t launches;
@@ -300,6 +306,26 @@ int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t c
 int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t batch, int64_t frames, const int64_t x_strides[3],
                          const float* dev_spk, int64_t spk_row_stride, float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream);
+/* FACodecDecoder.forward(x, vq=True) in eval (facodec.py:408-471, quantize/rvq.py, quantize/fvq.py, transformer.py), on a
+ * handle created with facodec_quantize = 1 (else AB_ERR_STATE).  Extra tensors: "quantizer.{q}.layers.{j}.in_proj.weight"
+ * (weight norm) / ".in_proj.bias", "timbre_encoder.position_emb.pe" [5000, 1, 256], per layer l
+ * "timbre_encoder.layers.{l}.{ln_1,ln_2}.{weight,bias}", ".self_attn.in_proj_weight" [768, 256], ".self_attn.in_proj_bias",
+ * ".self_attn.out_proj.{weight,bias}", ".ffn.ffn_1.{weight,bias}" (k = 5), ".ffn.ffn_2.{weight,bias}", and
+ * "timbre_encoder.last_ln.{weight,bias}".
+ * x [B, 256, T] fp32 with any element strides.  Each ResidualVQ runs its first min(n_quantizers, layers) layers; per
+ * layer z_e = in_proj(residual), code = argmin over the L2-normalised codebook of the squared distance to the
+ * normalised z_e (ties: the lowest code), z_q = z_e + (codebook[code] - z_e) in fp32, q = out_proj(z_q), residual -= q,
+ * and the group's sum += q; the residual group reads x - (prosody + content).  All of it in fp32 on CUDA cores at every
+ * precision.  Outputs (contiguous): emb_out [B, 256, T] = prosody + content [+ residual], codes_out int64
+ * [n_used, B, T] (each group's rows in order), quantized_out [G, B, 256, T] (each group's sum; G = 2 + (residual group
+ * present)), spk_out [B, 256] = the time mean of the timbre encoder's output, which adds row b of "pe" to every time
+ * step of utterance b (the reference's batch-first PositionalEncoding), then 4 pre-LN layers (MHA with 4 heads, no mask;
+ * a k = 5 conv FFN with ReLU) and last_ln.  Refused before any launch: n_quantizers < 1, B > 5000 (the rows of pe).
+ * Workspace: ab_facodec_quantize_workspace_bytes, 256-byte aligned. */
+size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t batch, int64_t frames);
+int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t batch, int64_t frames,
+                        int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
+                        float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * FACodec encoder (AB_GEN_FACODEC_ENCODER): FACodecEncoder.forward / .inference (models/codec/ns3_codec/facodec.py:157-194).
