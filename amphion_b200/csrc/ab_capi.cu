@@ -120,7 +120,8 @@ struct StageRef {
   std::vector<BlockRef> blocks;
 };
 
-// FACodec (AB_GEN_FACODEC): timbre_linear and the codebook layers of the three ResidualVQs, in code-row order
+// FACodec (AB_GEN_FACODEC): timbre_linear and the codebook layers of the three ResidualVQs, in code-row order;
+// AB_GEN_FACODEC_REDECODER: timbre_linear and the embedding tables (cb, rows) of the three groups, in code-row order
 struct FacodecLayerRef {
   int cb = -1;
   ConvRef out_proj;
@@ -128,14 +129,14 @@ struct FacodecLayerRef {
   ConvRef in_proj;          // facodec_quantize only
   size_t cbn_offset = 0;    // facodec_quantize: arena offset of the normalised rows [rows][16], then their squared norms
 };
-struct TimbreLayerRef {     // one TransformerEncoderLayer (transformer.py:84-151), use_cln = False
-  int ln1_w = -1, ln1_b = -1, ln2_w = -1, ln2_b = -1;
+struct TimbreLayerRef {     // one TransformerEncoderLayer (transformer.py:84-151)
+  int ln1_w = -1, ln1_b = -1, ln2_w = -1, ln2_b = -1;   // LayerNorm weight / bias, or with use_cln the style Linear's
   ConvRef qkv, out_proj, ffn_1, ffn_2;
 };
 struct FacodecRef {
   int style_w = -1, style_b = -1;
   std::vector<FacodecLayerRef> layers;
-  // facodec_quantize: the timbre encoder (transformer.py:154-217)
+  // facodec_quantize: the timbre encoder (transformer.py:154-217); the redecoder: its prosody encoder (use_cln)
   int pe = -1, last_w = -1, last_b = -1;
   std::vector<TimbreLayerRef> timbre;
 };
@@ -279,8 +280,8 @@ int validate_diffwave_config(const ab_generator_config& c) {
   return AB_OK;
 }
 
-// AB_GEN_FACODEC: the decoder's fixed block structure (facodec.py:121-133, :220-240) and the ResidualVQ geometry
-int validate_facodec_config(const ab_generator_config& c) {
+// The generator of FACodec's decoder and redecoder: the fixed block structure (facodec.py:121-133, :220-240)
+int validate_facodec_generator_config(const ab_generator_config& c) {
   if (c.gin_channels || c.conv_post_no_bias || c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel ||
       c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop || c.dilation_cycle || c.embedding_rows)
     return fail(AB_ERR_ARG, "config: FACodec uses only the generator fields and vq_* (gin / trunk / Vocos / DiffWave fields must be 0)");
@@ -300,6 +301,13 @@ int validate_facodec_config(const ab_generator_config& c) {
                             "num_kernels 1, kernel 7, 3 dilations");
   if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
     return fail(AB_ERR_ARG, "config: FACodec uses SnakeBeta with alpha_logscale = True");
+  return AB_OK;
+}
+
+// AB_GEN_FACODEC: the generator and the ResidualVQ geometry
+int validate_facodec_config(const ab_generator_config& c) {
+  const int rc = validate_facodec_generator_config(c);
+  if (rc != AB_OK) return rc;
   if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
       c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
     return fail(AB_ERR_ARG, "config: FACodec vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, at most %d in all",
@@ -316,6 +324,26 @@ int validate_facodec_config(const ab_generator_config& c) {
   if (c.facodec_quantize && c.n_mel != FAC_TIMBRE_C)
     return fail(AB_ERR_UNSUPPORTED, "config: FACodec quantization needs in_channels == %d (the timbre encoder's width; "
                 "got %d)", FAC_TIMBRE_C, c.n_mel);
+  return AB_OK;
+}
+
+// AB_GEN_FACODEC_REDECODER: the generator and the embedding tables (facodec.py:602-689)
+int validate_facodec_redecoder_config(const ab_generator_config& c) {
+  const int rc = validate_facodec_generator_config(c);
+  if (rc != AB_OK) return rc;
+  // the prosody transformer is 256 wide, and its output is summed with the vq_dim-wide embeddings
+  if (c.n_mel != FAC_TIMBRE_C)
+    return fail(AB_ERR_UNSUPPORTED, "config: the FACodec redecoder needs in_channels == vq_dim == %d (the prosody "
+                "transformer's width; got %d)", FAC_TIMBRE_C, c.n_mel);
+  if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
+      c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
+    return fail(AB_ERR_ARG, "config: FACodec redecoder vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, "
+                "at most %d in all", c.vq_num_q[0], c.vq_num_q[1], c.vq_num_q[2], AB_FACODEC_MAX_Q);
+  for (int i = 0; i < 3; ++i)
+    if (c.vq_codebook_bits[i] <= 0 || c.vq_codebook_bits[i] > 24)
+      return fail(AB_ERR_ARG, "config: FACodec redecoder table size 2^%d out of range (bits 1..24)", c.vq_codebook_bits[i]);
+  if (c.vq_codebook_dim != 0 || c.facodec_quantize != 0)
+    return fail(AB_ERR_ARG, "config: the FACodec redecoder has no codebook_dim or facodec_quantize (both must be 0)");
   return AB_OK;
 }
 
@@ -350,9 +378,10 @@ int validate_facodec_encoder_config(const ab_generator_config& c) {
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
       c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC &&
-      c.kind != AB_GEN_FACODEC_ENCODER)
+      c.kind != AB_GEN_FACODEC_ENCODER && c.kind != AB_GEN_FACODEC_REDECODER)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
+  if (c.kind == AB_GEN_FACODEC_REDECODER) return validate_facodec_redecoder_config(c);
   if (c.facodec_quantize) return fail(AB_ERR_ARG, "config: facodec_quantize belongs to AB_GEN_FACODEC");
   for (int i = 0; i < 3; ++i)
     if (c.vq_num_q[i] || c.vq_codebook_bits[i]) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
@@ -538,8 +567,9 @@ void add_melgan_tensors(ab_generator* g) {
 
 ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout);   // below
 
-// FACodec decoder tensors (AB_GEN_FACODEC), the reference's names (facodec.py:121-133, :220-240, :286-369, fvq.py:23-29)
-void add_facodec_tensors(ab_generator* g) {
+// The generator and timbre_linear of FACodec's decoder and redecoder, the reference's names (facodec.py:121-133,
+// :220-240): model.* and timbre_linear.*
+void add_facodec_generator_tensors(ab_generator* g) {
   const ab_generator_config* cfg = &g->cfg;
   const int c0 = cfg->upsample_initial_channel, n = cfg->num_upsamples;
   auto mod = [](int i) { return "model." + std::to_string(i); };
@@ -571,10 +601,50 @@ void add_facodec_tensors(ab_generator* g) {
   }
   g->act_post = make_act(g, mod(1 + n), ch, true);
   g->conv_post = make_conv(g, mod(2 + n), ch, 1, 7, 1, false);
+  const int C = cfg->n_mel;
+  g->fac.style_w = g->add_slot("timbre_linear.weight", SLOT_VEC, {2 * C, C});
+  g->fac.style_b = g->add_slot("timbre_linear.bias", SLOT_VEC, {2 * C});
+}
+
+// A FACodec transformer (transformer.py:154-234) under `prefix`: pe, four layers, last_ln.  use_cln: each LayerNorm is
+// a StyleAdaptiveLayerNorm, listed as its style Linear [2H, H] / [2H] (transformer.py:13-32)
+void add_facodec_transformer_tensors(ab_generator* g, const std::string& prefix, bool use_cln) {
+  FacodecRef& f = g->fac;
+  const int H = FAC_TIMBRE_C;
+  f.pe = g->add_slot(prefix + "position_emb.pe", SLOT_VEC, {FAC_PE_ROWS, 1, H});
+  auto ln = [&](const std::string& name, int* w, int* b) {
+    if (use_cln) {
+      *w = g->add_slot(name + ".style.weight", SLOT_VEC, {2 * H, H});
+      *b = g->add_slot(name + ".style.bias", SLOT_VEC, {2 * H});
+    } else {
+      *w = g->add_slot(name + ".weight", SLOT_VEC, {H});
+      *b = g->add_slot(name + ".bias", SLOT_VEC, {H});
+    }
+  };
+  for (int i = 0; i < 4; ++i) {
+    const std::string pre = prefix + "layers." + std::to_string(i) + ".";
+    TimbreLayerRef t;
+    ln(pre + "ln_1", &t.ln1_w, &t.ln1_b);
+    ln(pre + "ln_2", &t.ln2_w, &t.ln2_b);
+    // nn.MultiheadAttention packs q, k and v into in_proj_weight [3H, H] / in_proj_bias [3H]
+    t.qkv.cin = H; t.qkv.cout = 3 * H; t.qkv.k = 1;
+    t.qkv.w = g->add_slot(pre + "self_attn.in_proj_weight", SLOT_CONV_W, {3 * H, H});
+    g->slots[t.qkv.w].shape[2] = 1;
+    t.qkv.b = g->add_slot(pre + "self_attn.in_proj_bias", SLOT_VEC, {3 * H});
+    t.out_proj = make_linear(g, pre + "self_attn.out_proj", H, H);
+    t.ffn_1 = make_conv(g, pre + "ffn.ffn_1", H, 4 * H, 5, 1, false);
+    t.ffn_2 = make_linear(g, pre + "ffn.ffn_2", 4 * H, H);
+    f.timbre.push_back(t);
+  }
+  ln(prefix + "last_ln", &f.last_w, &f.last_b);
+}
+
+// FACodec decoder tensors (AB_GEN_FACODEC), the reference's names (facodec.py:121-133, :220-240, :286-369, fvq.py:23-29)
+void add_facodec_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  add_facodec_generator_tensors(g);
   FacodecRef& f = g->fac;
   const int C = cfg->n_mel, D = cfg->vq_codebook_dim;
-  f.style_w = g->add_slot("timbre_linear.weight", SLOT_VEC, {2 * C, C});
-  f.style_b = g->add_slot("timbre_linear.bias", SLOT_VEC, {2 * C});
   for (int q = 0; q < 3; ++q)
     for (int j = 0; j < cfg->vq_num_q[q]; ++j) {
       const std::string pre = "quantizer." + std::to_string(q) + ".layers." + std::to_string(j) + ".";
@@ -594,27 +664,24 @@ void add_facodec_tensors(ab_generator* g) {
       l.in_proj = make_linear(g, "quantizer." + std::to_string(q) + ".layers." + std::to_string(j) + ".in_proj", C, D);
       g->slots[l.in_proj.w].no_tc = true;
     }
-  f.pe = g->add_slot("timbre_encoder.position_emb.pe", SLOT_VEC, {FAC_PE_ROWS, 1, FAC_TIMBRE_C});
-  const int H = FAC_TIMBRE_C;
-  for (int i = 0; i < 4; ++i) {
-    const std::string pre = "timbre_encoder.layers." + std::to_string(i) + ".";
-    TimbreLayerRef t;
-    t.ln1_w = g->add_slot(pre + "ln_1.weight", SLOT_VEC, {H});
-    t.ln1_b = g->add_slot(pre + "ln_1.bias", SLOT_VEC, {H});
-    t.ln2_w = g->add_slot(pre + "ln_2.weight", SLOT_VEC, {H});
-    t.ln2_b = g->add_slot(pre + "ln_2.bias", SLOT_VEC, {H});
-    // nn.MultiheadAttention packs q, k and v into in_proj_weight [3H, H] / in_proj_bias [3H]
-    t.qkv.cin = H; t.qkv.cout = 3 * H; t.qkv.k = 1;
-    t.qkv.w = g->add_slot(pre + "self_attn.in_proj_weight", SLOT_CONV_W, {3 * H, H});
-    g->slots[t.qkv.w].shape[2] = 1;
-    t.qkv.b = g->add_slot(pre + "self_attn.in_proj_bias", SLOT_VEC, {3 * H});
-    t.out_proj = make_linear(g, pre + "self_attn.out_proj", H, H);
-    t.ffn_1 = make_conv(g, pre + "ffn.ffn_1", H, 4 * H, 5, 1, false);
-    t.ffn_2 = make_linear(g, pre + "ffn.ffn_2", 4 * H, H);
-    f.timbre.push_back(t);
-  }
-  f.last_w = g->add_slot("timbre_encoder.last_ln.weight", SLOT_VEC, {H});
-  f.last_b = g->add_slot("timbre_encoder.last_ln.bias", SLOT_VEC, {H});
+  add_facodec_transformer_tensors(g, "timbre_encoder.", false);
+}
+
+// FACodec redecoder tensors (AB_GEN_FACODEC_REDECODER), the reference's names (facodec.py:602-689): the embedding
+// tables "{prosody,content,residual}_embs.{j}.weight" [2^bits, 256], the generator and timbre_linear, and the prosody
+// transformer "timbre_cond_prosody_enc.*" with style-adaptive LayerNorms
+void add_facodec_redecoder_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  static const char* kTables[3] = {"prosody_embs.", "content_embs.", "residual_embs."};
+  for (int q = 0; q < 3; ++q)
+    for (int j = 0; j < cfg->vq_num_q[q]; ++j) {
+      FacodecLayerRef l;
+      l.rows = (int64_t)1 << cfg->vq_codebook_bits[q];
+      l.cb = g->add_slot(kTables[q] + std::to_string(j) + ".weight", SLOT_VEC, {l.rows, cfg->n_mel});
+      g->fac.layers.push_back(l);
+    }
+  add_facodec_generator_tensors(g);
+  add_facodec_transformer_tensors(g, "timbre_cond_prosody_enc.", true);
 }
 
 // FACodec encoder tensors (AB_GEN_FACODEC_ENCODER), the reference's names (facodec.py:121-194): "block.0" (conv_pre,
@@ -803,6 +870,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     add_facodec_tensors(g);
   } else if (cfg->kind == AB_GEN_FACODEC_ENCODER) {
     add_facodec_encoder_tensors(g);
+  } else if (cfg->kind == AB_GEN_FACODEC_REDECODER) {
+    add_facodec_redecoder_tensors(g);
   } else {
     add_gan_tensors(g);
   }
@@ -971,11 +1040,12 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
       for (size_t j = 0; j < ups.size(); ++j) pack_snake_coef(&host[j * 24], &host[j * 24 + 12], &g->act_coef[ups[j]]);
     }
   }
+  // the transformers' GEMMs (the timbre encoder's, the prosody encoder's) all run on the wgmma kernel at 16 bits
+  for (const auto& t : g->fac.timbre)
+    for (const ConvRef* c : {&t.qkv, &t.out_proj, &t.ffn_1, &t.ffn_2})
+      if (precision != AB_PREC_FP32 && g->slots[c->w].tc_bytes == 0)
+        return fail(AB_ERR_UNSUPPORTED, "finalize: '%s' has no tensor-core image", g->slots[c->w].name.c_str());
   if (g->cfg.kind == AB_GEN_FACODEC && g->cfg.facodec_quantize) {
-    for (const auto& t : g->fac.timbre)   // the timbre encoder's GEMMs all run on the wgmma kernel at 16 bits
-      for (const ConvRef* c : {&t.qkv, &t.out_proj, &t.ffn_1, &t.ffn_2})
-        if (precision != AB_PREC_FP32 && g->slots[c->w].tc_bytes == 0)
-          return fail(AB_ERR_UNSUPPORTED, "finalize: '%s' has no tensor-core image", g->slots[c->w].name.c_str());
     for (const auto& l : g->fac.layers) {
       float* cbn = reinterpret_cast<float*>(g->arena + l.cbn_offset);
       float* cbn2 = reinterpret_cast<float*>(g->arena + l.cbn_offset +
@@ -1084,7 +1154,7 @@ size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T)
   if (!g || B <= 0 || T <= 0) return 0;
   if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return 0;
-  if (g->cfg.kind == AB_GEN_FACODEC)
+  if (g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER)
     return gan_workspace_bytes(g, B, T) + facodec_film_bytes(g, B, T) + align_up((size_t)B * 2 * g->cfg.n_mel * sizeof(float), 256);
   return gan_workspace_bytes(g, B, T);
 }
@@ -1139,8 +1209,10 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
   static const char* kNames[14] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
                                    "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
                                    "diffwave_tail", "facodec_prologue", "facodec_quantize", "timbre_attention"};
-  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder
-  const int n = g->cfg.kind == AB_GEN_FACODEC ? (g->cfg.facodec_quantize ? 14 : 12)
+  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder; the
+  // redecoder's prosody transformer reports its attention in class 13
+  const int n = g->cfg.kind == AB_GEN_FACODEC_REDECODER ? 14
+                : g->cfg.kind == AB_GEN_FACODEC ? (g->cfg.facodec_quantize ? 14 : 12)
                 : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
   for (int i = 0; i < n; ++i) {
@@ -1212,7 +1284,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   float *R[2] = {buf[0], buf[1]}, *U = buf[2], *P[2] = {buf[3], buf[4]}, *TMP = buf[5], *ACT = buf[6];
   // FACodec's generator is BigVGAN's pipeline with an activation in front of each transposed conv; its encoder the same
   // ResidualUnits with an activation and a strided conv closing each stage
-  const bool fac = g->cfg.kind == AB_GEN_FACODEC;
+  const bool fac = g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER;
   const bool big = g->cfg.kind == AB_GEN_BIGVGAN || fac || enc;
   const bool tc = g->precision != AB_PREC_FP32;
   const int nk = g->cfg.num_kernels;
@@ -1677,7 +1749,8 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
 int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64_t T,
                          const int64_t mel_strides[3], float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream) {
-  if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
+  if (g && (g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER))
+    return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
   return forward_impl(g, dev_mel, B, T, mel_strides, nullptr, 0, dev_wav, dev_workspace, workspace_bytes, stream);
@@ -1686,7 +1759,8 @@ int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64
 int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
                               const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
                               size_t workspace_bytes, void* stream) {
-  if (g && g->cfg.kind == AB_GEN_FACODEC) return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
+  if (g && (g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER))
+    return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
   return forward_impl(g, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes, stream);
@@ -1867,9 +1941,14 @@ int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t B, int6
 // ---------------------------------------------------------------------------
 // FACodec decoder
 // ---------------------------------------------------------------------------
-static int facodec_check(const ab_generator* g, int64_t B, int64_t T, const char* what) {
+// redecoder: 0 the entry serves the decoder only, 1 the decoder and the redecoder, 2 the redecoder only
+static int facodec_check(const ab_generator* g, int64_t B, int64_t T, const char* what, int redecoder = 0) {
   if (!g) return fail(AB_ERR_ARG, "%s: null handle", what);
-  if (g->cfg.kind != AB_GEN_FACODEC) return fail(AB_ERR_ARG, "%s: not a FACodec handle", what);
+  const bool ok = redecoder == 2 ? g->cfg.kind == AB_GEN_FACODEC_REDECODER
+                  : g->cfg.kind == AB_GEN_FACODEC || (redecoder == 1 && g->cfg.kind == AB_GEN_FACODEC_REDECODER);
+  if (!ok)
+    return fail(AB_ERR_ARG, "%s: not a FACodec %shandle", what,
+                redecoder == 2 ? "redecoder " : redecoder == 1 ? "decoder or redecoder " : "");
   if (!g->finalized) return fail(AB_ERR_STATE, "%s: finalize() the generator first", what);
   if (B <= 0 || T <= 0 || B > 65535) return fail(AB_ERR_ARG, "%s: batch %lld / frames %lld out of range", what, (long long)B, (long long)T);
   if (T * g->hop > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "%s: sequence too long", what);
@@ -1913,7 +1992,7 @@ int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t c
 int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
                          const float* dev_spk, int64_t spk_row_stride, float* dev_wav, void* dev_workspace,
                          size_t workspace_bytes, void* stream) {
-  int rc = facodec_check(g, B, T, "facodec_inference");
+  int rc = facodec_check(g, B, T, "facodec_inference", 1);
   if (rc == AB_OK && (!dev_x || !x_strides || !dev_spk || !dev_wav))
     rc = fail(AB_ERR_ARG, "facodec_inference: null argument");
   const int C = g ? g->cfg.n_mel : 0;
@@ -1982,6 +2061,67 @@ static size_t timbre_layout(int64_t B, int64_t T, char* base, TimbreWs* w) {
   return off;
 }
 
+// The four pre-LN layers of a FACodec transformer on the fp32 stream w.S (transformer.py:122-151): the decoder's timbre
+// encoder and the redecoder's prosody encoder differ only in their LayerNorms.  norm(layer, i, y, yimg) runs the
+// layer's ln_1 (i = 0) or ln_2 (i = 1) on w.S into y (fp32) or the operand image yimg.  Per layer: ln_1, the QKV GEMM,
+// the attention, out_proj onto S, ln_2, ffn_1 (k = 5; at 16 bits it also writes the image of its ReLU), ffn_2 onto S.
+extern "C++" {
+template <class Norm>
+static int facodec_transformer_layers(ab_generator* g, const TimbreWs& w, int64_t B, int Tn, DwProf& prof, int& launches,
+                                      Norm norm) {
+  cudaStream_t st = prof.st;
+  const int C = FAC_TIMBRE_C;
+  const bool tc = g->precision != AB_PREC_FP32;
+  const double el = (double)B * Tn;
+  const uint16_t* Himg = reinterpret_cast<const uint16_t*>(w.H);
+  // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual / acc_prev = y]
+  auto gemm = [&](const ConvRef& c, const float* x, const uint16_t* ximg, float* y, bool residual, float pre_slope,
+                  uint16_t* yimg) -> int {
+    ++launches;
+    prof.begin(tc ? 0 : 1, 2.0 * el * c.cin * c.cout * c.k,
+               el * c.cin * (tc ? 2.0 : 4.0) + 4.0 * el * c.cout * (residual ? 2 : 1) + (yimg ? 2.0 * el * c.cout : 0.0) +
+                   (tc ? 2.0 : 4.0) * c.cin * c.cout * c.k);
+    int r;
+    if (tc) {
+      TcConvParams t;
+      t.ximg = ximg; t.w = g->tcptr(c.w); t.bias = g->fptr(c.b);
+      t.acc_prev = residual ? y : nullptr; t.y = y; t.yimg = yimg; t.img_slope = 0.0f;
+      t.B = (int)B; t.Cin = c.cin; t.Cout = c.cout; t.T = Tn; t.k = c.k; t.d_or_u = 1; t.precision = g->precision;
+      r = launch_tc_conv(t, st);
+    } else {
+      // residual in place: each output element is read and then written by the same thread
+      ConvParams f;
+      f.x = x; f.xsb = (int64_t)c.cin * Tn; f.xsc = Tn; f.xst = 1;
+      f.w_t = g->fptr(c.w); f.bias = g->fptr(c.b);
+      f.residual = residual ? y : nullptr; f.acc_prev = nullptr; f.y = y;
+      f.B = (int)B; f.Cin = c.cin; f.Cout = c.cout; f.T = Tn; f.k = c.k; f.d = 1;
+      f.pre_slope = pre_slope; f.out_div = 1.0f; f.post_tanh = 0;
+      r = launch_conv1d_fp32(f, st);
+    }
+    prof.end();
+    return r;
+  };
+  int rc;
+  for (const TimbreLayerRef& t : g->fac.timbre) {
+    // x = x + out_proj(MHA(LN1(x)))
+    if ((rc = norm(t, 0, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.qkv, w.H, Himg, w.QKV, false, 1.0f, nullptr)) != AB_OK) return rc;
+    ++launches;
+    prof.begin(13, 4.0 * B * (double)Tn * Tn * C, 4.0 * el * 3 * C + (tc ? 2.0 : 4.0) * el * C);
+    rc = launch_facodec_attention(w.QKV, tc ? nullptr : w.A, tc ? reinterpret_cast<uint16_t*>(w.A) : nullptr,
+                                  g->precision == AB_PREC_TC_BF16, (int)B, Tn, st);
+    prof.end();
+    if (rc != AB_OK) return rc;
+    if ((rc = gemm(t.out_proj, w.A, reinterpret_cast<const uint16_t*>(w.A), w.S, true, 1.0f, nullptr)) != AB_OK) return rc;
+    // x = x + ffn_2(relu(ffn_1(LN2(x))))
+    if ((rc = norm(t, 1, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.ffn_1, w.H, Himg, w.F, false, 1.0f, tc ? w.FI : nullptr)) != AB_OK) return rc;
+    if ((rc = gemm(t.ffn_2, w.F, w.FI, w.S, true, 0.0f, nullptr)) != AB_OK) return rc;
+  }
+  return AB_OK;
+}
+}  // extern "C++"
+
 size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || g->cfg.kind != AB_GEN_FACODEC || !g->cfg.facodec_quantize || B <= 0 || T <= 0) return 0;
   return timbre_layout(B, T, nullptr, nullptr);
@@ -2007,7 +2147,6 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
   TimbreWs w;
   timbre_layout(B, T, static_cast<char*>(dev_workspace), &w);
   const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim, Tn = (int)T;
-  const bool tc = g->precision != AB_PREC_FP32;
   const double el = (double)B * T;
   int launches = 0;
   DwProf prof{g, st};
@@ -2052,7 +2191,6 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
   }
 
   // the timbre encoder on S (transformer.py:206-217)
-  const uint16_t* Himg = reinterpret_cast<const uint16_t*>(w.H);
   auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) -> int {
     NormParams n;
     n.x = w.S; n.ln_w = g->fptr(lw); n.ln_b = g->fptr(lb);
@@ -2064,55 +2202,119 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
     prof.end();
     return r;
   };
-  // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual / acc_prev = y]
-  auto gemm = [&](const ConvRef& c, const float* x, const uint16_t* ximg, float* y, bool residual, float pre_slope,
-                  uint16_t* yimg) -> int {
-    ++launches;
-    prof.begin(tc ? 0 : 1, 2.0 * el * c.cin * c.cout * c.k,
-               el * c.cin * (tc ? 2.0 : 4.0) + 4.0 * el * c.cout * (residual ? 2 : 1) + (yimg ? 2.0 * el * c.cout : 0.0) +
-                   (tc ? 2.0 : 4.0) * c.cin * c.cout * c.k);
-    int r;
-    if (tc) {
-      TcConvParams t;
-      t.ximg = ximg; t.w = g->tcptr(c.w); t.bias = g->fptr(c.b);
-      t.acc_prev = residual ? y : nullptr; t.y = y; t.yimg = yimg; t.img_slope = 0.0f;
-      t.B = (int)B; t.Cin = c.cin; t.Cout = c.cout; t.T = Tn; t.k = c.k; t.d_or_u = 1; t.precision = g->precision;
-      r = launch_tc_conv(t, st);
-    } else {
-      // residual in place: each output element is read and then written by the same thread
-      ConvParams f;
-      f.x = x; f.xsb = (int64_t)c.cin * Tn; f.xsc = Tn; f.xst = 1;
-      f.w_t = g->fptr(c.w); f.bias = g->fptr(c.b);
-      f.residual = residual ? y : nullptr; f.acc_prev = nullptr; f.y = y;
-      f.B = (int)B; f.Cin = c.cin; f.Cout = c.cout; f.T = Tn; f.k = c.k; f.d = 1;
-      f.pre_slope = pre_slope; f.out_div = 1.0f; f.post_tanh = 0;
-      r = launch_conv1d_fp32(f, st);
-    }
-    prof.end();
-    return r;
-  };
-  for (const TimbreLayerRef& t : g->fac.timbre) {
-    // x = x + out_proj(MHA(LN1(x)))
-    if ((rc = norm(t.ln1_w, t.ln1_b, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
-    if ((rc = gemm(t.qkv, w.H, Himg, w.QKV, false, 1.0f, nullptr)) != AB_OK) return rc;
-    ++launches;
-    prof.begin(13, 4.0 * B * (double)T * T * C, 4.0 * el * 3 * C + (tc ? 2.0 : 4.0) * el * C);
-    rc = launch_facodec_attention(w.QKV, tc ? nullptr : w.A, tc ? reinterpret_cast<uint16_t*>(w.A) : nullptr,
-                                  g->precision == AB_PREC_TC_BF16, (int)B, Tn, st);
-    prof.end();
-    if (rc != AB_OK) return rc;
-    if ((rc = gemm(t.out_proj, w.A, reinterpret_cast<const uint16_t*>(w.A), w.S, true, 1.0f, nullptr)) != AB_OK) return rc;
-    // x = x + ffn_2(relu(ffn_1(LN2(x))))
-    if ((rc = norm(t.ln2_w, t.ln2_b, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
-    if ((rc = gemm(t.ffn_1, w.H, Himg, w.F, false, 1.0f, tc ? w.FI : nullptr)) != AB_OK) return rc;
-    if ((rc = gemm(t.ffn_2, w.F, w.FI, w.S, true, 0.0f, nullptr)) != AB_OK) return rc;
-  }
+  rc = facodec_transformer_layers(g, w, B, Tn, prof, launches,
+                                  [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
+                                    return i == 0 ? norm(t.ln1_w, t.ln1_b, y, yimg) : norm(t.ln2_w, t.ln2_b, y, yimg);
+                                  });
+  if (rc != AB_OK) return rc;
   if ((rc = norm(g->fac.last_w, g->fac.last_b, w.H, nullptr)) != AB_OK) return rc;
   ++launches;
   prof.begin(12, el * C, 4.0 * el * C + 4.0 * B * C);
   rc = launch_facodec_time_mean(w.H, dev_spk_out, (int)B, C, Tn, st);
   prof.end();
   if (rc != AB_OK) return rc;
+  g->launches = launches;
+  return AB_OK;
+}
+
+// ---------------------------------------------------------------------------
+// FACodec redecoder
+// ---------------------------------------------------------------------------
+// FACodecRedecoder.vq2emb: the prosody transformer's workspace (TimbreWs), then the nine style vectors [9][B][2C]
+// (layer l's ln_1 at 2l, its ln_2 at 2l + 1, last_ln at 8)
+static size_t redecoder_layout(int64_t B, int64_t T, char* base, TimbreWs* w, float** styles) {
+  const size_t off = timbre_layout(B, T, base, w);
+  if (styles) *styles = base ? reinterpret_cast<float*>(base + off) : nullptr;
+  return off + align_up((size_t)9 * B * 2 * FAC_TIMBRE_C * sizeof(float), 256);
+}
+
+size_t ab_facodec_redecoder_vq2emb_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
+  if (!g || g->cfg.kind != AB_GEN_FACODEC_REDECODER || B <= 0 || T <= 0) return 0;
+  return redecoder_layout(B, T, nullptr, nullptr, nullptr);
+}
+
+int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q,
+                                int64_t B, int64_t T, const float* dev_spk, int64_t spk_row_stride, int32_t use_residual,
+                                float* dev_out, void* dev_workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "facodec_redecoder_vq2emb";
+  if (g && B > FAC_PE_ROWS)   // PositionalEncoding adds pe[:B] (transformer.py:43-45)
+    return fail(AB_ERR_ARG, "%s: batch %lld > %d, the rows of the positional encoding", what, (long long)B, FAC_PE_ROWS);
+  int rc = facodec_check(g, B, T, what, 2);
+  if (rc != AB_OK) return rc;
+  if (!dev_codes || !codes_strides || !dev_spk || !dev_out) return fail(AB_ERR_ARG, "%s: null argument", what);
+  const int C = FAC_TIMBRE_C, Tn = (int)T;
+  if (spk_row_stride < C) return fail(AB_ERR_ARG, "%s: speaker-embedding row stride < %d", what, C);
+  const int* nq = g->cfg.vq_num_q;
+  // code rows are read by position (facodec.py:739-756); extra rows are not read
+  const int rows = nq[0] + nq[1] + (use_residual ? nq[2] : 0);
+  if (n_q < rows)
+    return fail(AB_ERR_ARG, "%s: %d code rows; vq2emb reads %d (%d prosody, %d content, %d residual)", what, n_q, rows,
+                nq[0], nq[1], use_residual ? nq[2] : 0);
+  const size_t need = redecoder_layout(B, T, nullptr, nullptr, nullptr);
+  if (!dev_workspace || workspace_bytes < need)
+    return fail(AB_ERR_WORKSPACE, "%s: workspace %zu B < required %zu B", what, workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "%s: workspace must be 256-byte aligned", what);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  TimbreWs w;
+  float* styles = nullptr;
+  redecoder_layout(B, T, static_cast<char*>(dev_workspace), &w, &styles);
+  const FacodecRef& f = g->fac;
+  const double el = (double)B * T;
+  int launches = 0;
+  DwProf prof{g, st};
+
+  // (gamma, beta) of every StyleAdaptiveLayerNorm from the speaker embedding (transformer.py:25): the condition is the
+  // embedding expanded over time, whose time mean is the embedding itself
+  auto style_of = [&](int i) { return styles + (size_t)i * B * 2 * C; };
+  for (int i = 0; i < 9; ++i) {
+    const int sw = i == 8 ? f.last_w : (i & 1) ? f.timbre[i / 2].ln2_w : f.timbre[i / 2].ln1_w;
+    const int sb = i == 8 ? f.last_b : (i & 1) ? f.timbre[i / 2].ln2_b : f.timbre[i / 2].ln1_b;
+    ++launches;
+    prof.begin(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C));
+    rc = launch_facodec_style(dev_spk, spk_row_stride, g->fptr(sw), g->fptr(sb), style_of(i), (int)B, C, st);
+    prof.end();
+    if (rc != AB_OK) return rc;
+  }
+  // gamma * LayerNorm(S) + beta (transformer.py:29-31) into y (fp32) or the operand image yimg
+  auto film = [&](int i, float* y, uint16_t* yimg) -> int {
+    FacFilmParams p;
+    p.x = w.S; p.xsb = (int64_t)C * T; p.xsc = T; p.xst = 1;
+    p.style = style_of(i); p.y = y; p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
+    p.B = (int)B; p.C = C; p.T = Tn;
+    ++launches;
+    prof.begin(11, 10.0 * el * C, 4.0 * el * C + (y ? 4.0 : 2.0) * el * C);
+    const int r = launch_facodec_film(p, st);
+    prof.end();
+    return r;
+  };
+  // the gathers: prev + the tables' rows (+ pe) -> out
+  auto embed = [&](const float* prev, int row0, int ntab, const float* pe, float* out) -> int {
+    FacEmbedParams p;
+    memset(&p, 0, sizeof(p));
+    p.codes = dev_codes; p.cs0 = codes_strides[0]; p.cs1 = codes_strides[1]; p.cs2 = codes_strides[2];
+    p.row0 = row0; p.ntab = ntab;
+    for (int j = 0; j < ntab; ++j) { p.tab[j] = g->fptr(f.layers[row0 + j].cb); p.rows[j] = f.layers[row0 + j].rows; }
+    p.prev = prev; p.pe = pe; p.out = out;
+    p.B = (int)B; p.C = C; p.T = Tn;
+    ++launches;
+    prof.begin(11, el * C * (ntab + (prev ? 1 : 0) + (pe ? 1 : 0) - 1),
+               8.0 * el * ntab + 4.0 * el * C * (ntab + 1 + (prev ? 1 : 0)));
+    const int r = launch_facodec_embed(p, st);
+    prof.end();
+    return r;
+  };
+  // facodec.py:739-744: per prosody table, x_t = transformer(x_t + emb(codes)); the transformer adds pe each time
+  for (int i = 0; i < nq[0]; ++i) {
+    if ((rc = embed(i == 0 ? nullptr : w.H, i, 1, g->fptr(f.pe), w.S)) != AB_OK) return rc;
+    rc = facodec_transformer_layers(g, w, B, Tn, prof, launches,
+                                    [&](const TimbreLayerRef& t, int j, float* y, uint16_t* yimg) {
+                                      return film(2 * (int)(&t - f.timbre.data()) + j, y, yimg);
+                                    });
+    if (rc != AB_OK) return rc;
+    if ((rc = film(8, w.H, nullptr)) != AB_OK) return rc;   // last_ln
+  }
+  // facodec.py:746-756: out = x_t, + the content rows, + the residual rows, one add at a time
+  if ((rc = embed(w.H, nq[0], rows - nq[0], nullptr, dev_out)) != AB_OK) return rc;
   g->launches = launches;
   return AB_OK;
 }

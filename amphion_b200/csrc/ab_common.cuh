@@ -277,6 +277,21 @@ int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf1
 // spk[b][c] = sum_t y[b, c, t] / T (fixed order)
 int launch_facodec_time_mean(const float* y, float* spk, int B, int C, int T, cudaStream_t s);
 
+// ---- FACodecRedecoder.vq2emb: the embedding gathers and sums (ab_facodec.cu) ----
+struct FacEmbedParams {     // out[b, c, t] = ((prev[b, c, t] + tab[0][code_0][c]) + tab[1][code_1][c] ...) + pe[b][c],
+                            // one fp32 add per term in that order; without prev the first table's row is the first term
+  const int64_t* codes;     // [n_q, B, T] with element strides cs0 / cs1 / cs2; table j reads code row row0 + j
+  int64_t cs0, cs1, cs2;
+  int row0, ntab;
+  const float* tab[AB_FACODEC_MAX_Q];   // nn.Embedding weights [rows][C]
+  int64_t rows[AB_FACODEC_MAX_Q];
+  const float* prev;        // nullable: fp32 [B, C, T]
+  const float* pe;          // nullable: [>= B][C]; row b is added last
+  float* out;               // fp32 [B, C, T]; a time step with a code outside its table holds NaN in every channel
+  int B, C, T;
+};
+int launch_facodec_embed(const FacEmbedParams& p, cudaStream_t s);
+
 // launchers (ab_kernels_fp32.cu)
 int launch_vocos_norm(const NormParams& p, cudaStream_t s);
 int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);

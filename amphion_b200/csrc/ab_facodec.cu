@@ -2,7 +2,8 @@
 // timbre projection and the LayerNorm + FiLM in front of conv_pre.  The generator itself runs on the BigVGAN path of
 // ab_capi.cu's forward_impl.  Then the kernels of FACodecDecoder.forward(vq=True) (facodec.py:408-471): the residual
 // vector quantizer, the timbre encoder's attention and the time mean; its GEMMs and LayerNorms run on the shared
-// convolution and LayerNorm kernels.
+// convolution and LayerNorm kernels.  Last the embedding gathers of FACodecRedecoder.vq2emb (facodec.py:734-759); its
+// prosody transformer reuses the style, FiLM and attention kernels above.
 #include <algorithm>
 
 #include "ab_common.cuh"
@@ -475,6 +476,62 @@ __global__ void __launch_bounds__(256) facodec_time_mean_kernel(const float* __r
   if (lane == 0) spk[row] = __fdiv_rn(a, (float)T);
 }
 
+
+// ---- FACodecRedecoder.vq2emb ---------------------------------------------------------------------------------------
+
+// The embedding sums of FACodecRedecoder.vq2emb (facodec.py:734-759).  One CTA per (utterance, tile of EMB_TT time
+// steps).  The tile sits in shared memory [C][EMB_TT + 1]: prev is read into it along time, the table rows are then
+// read along channels and summed into it in the reference's order, and the tile is written along time.  The padded
+// row length keeps both access orders free of bank conflicts.  A code outside its table is not read and marks its
+// time step, which is written as NaN.  Two uses: the prosody stream fed to the transformer (prev = the previous run's
+// output or none, one prosody table, pe), and the tail (prev = last_ln's output, the content then residual tables).
+constexpr int EMB_TT = 16;
+constexpr int EMB_THREADS = 256;
+
+__global__ void __launch_bounds__(EMB_THREADS) facodec_embed_kernel(FacEmbedParams p, int tiles) {
+  extern __shared__ float esm[];   // [C][EMB_TT + 1]
+  __shared__ int code_s[AB_FACODEC_MAX_Q][EMB_TT];
+  __shared__ int bad[EMB_TT];
+  constexpr int LD = EMB_TT + 1;
+  const int b = blockIdx.x / tiles, t0 = (blockIdx.x - b * tiles) * EMB_TT;
+  const int C = p.C, tid = threadIdx.x, n = C * EMB_TT;
+  if (tid < EMB_TT) bad[tid] = 0;
+  __syncthreads();
+  for (int i = tid; i < p.ntab * EMB_TT; i += EMB_THREADS) {
+    const int j = i / EMB_TT, u = i - j * EMB_TT, t = t0 + u;
+    int code = 0;
+    if (t < p.T) {
+      const int64_t v = p.codes[(p.row0 + j) * p.cs0 + b * p.cs1 + t * p.cs2];
+      if (v < 0 || v >= p.rows[j]) bad[u] = 1;
+      else code = (int)v;
+    }
+    code_s[j][u] = code;
+  }
+  if (p.prev) {
+    const float* pb = p.prev + (int64_t)b * C * p.T;
+    for (int i = tid; i < n; i += EMB_THREADS) {
+      const int c = i / EMB_TT, u = i - c * EMB_TT, t = t0 + u;
+      esm[c * LD + u] = t < p.T ? __ldg(pb + (int64_t)c * p.T + t) : 0.f;
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < n; i += EMB_THREADS) {
+    const int u = i / C, c = i - u * C;
+    if (t0 + u >= p.T || bad[u]) continue;
+    int j = 0;
+    float a = p.prev ? esm[c * LD + u] : __ldg(p.tab[j++] + (int64_t)code_s[0][u] * C + c);
+    for (; j < p.ntab; ++j) a = __fadd_rn(a, __ldg(p.tab[j] + (int64_t)code_s[j][u] * C + c));
+    if (p.pe) a = __fadd_rn(a, __ldg(p.pe + (int64_t)b * C + c));
+    esm[c * LD + u] = a;
+  }
+  __syncthreads();
+  float* ob = p.out + (int64_t)b * C * p.T;
+  for (int i = tid; i < n; i += EMB_THREADS) {
+    const int c = i / EMB_TT, u = i - c * EMB_TT, t = t0 + u;
+    if (t < p.T) ob[(int64_t)c * p.T + t] = bad[u] ? __int_as_float(0x7fc00000) : esm[c * LD + u];
+  }
+}
+
 }  // namespace
 
 int launch_facodec_style(const float* spk, int64_t spk_stride, const float* w, const float* bias, float* style, int B,
@@ -567,6 +624,21 @@ int launch_facodec_time_mean(const float* y, float* spk, int B, int C, int T, cu
   const int rows = B * C;
   facodec_time_mean_kernel<<<(unsigned)ceil_div(rows, 8), 256, 0, s>>>(y, spk, rows, T);
   AB_LAUNCH_CHECK("facodec_time_mean_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_embed(const FacEmbedParams& p, cudaStream_t s) {
+  if (!p.codes || !p.out) return fail(AB_ERR_ARG, "facodec embed: null argument");
+  if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.ntab <= 0 || p.ntab > AB_FACODEC_MAX_Q || p.row0 < 0)
+    return fail(AB_ERR_ARG, "facodec embed: bad shape");
+  for (int j = 0; j < p.ntab; ++j)
+    if (!p.tab[j] || p.rows[j] <= 0 || p.rows[j] > (1 << 24)) return fail(AB_ERR_ARG, "facodec embed: bad table %d", j);
+  const size_t smem = sizeof(float) * (size_t)p.C * (EMB_TT + 1);
+  if (smem > 48 * 1024) return fail(AB_ERR_UNSUPPORTED, "facodec embed: %d channels do not fit shared memory", p.C);
+  const int64_t tiles = ceil_div(p.T, EMB_TT), grid = (int64_t)p.B * tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "facodec embed: grid too large");
+  facodec_embed_kernel<<<(unsigned)grid, EMB_THREADS, smem, s>>>(p, (int)tiles);
+  AB_LAUNCH_CHECK("facodec_embed_kernel");
   return AB_OK;
 }
 

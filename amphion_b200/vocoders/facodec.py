@@ -13,8 +13,13 @@ the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_pr
 ``FACodecEncoder`` (:157-194) serves the waveform -> latent side natively (``AB_GEN_FACODEC_ENCODER``): ``forward`` /
 ``inference`` map ``[B, 1, N]`` to ``[B, out_channels, F]`` through the same ResidualUnits and strided convolutions.
 
+``FACodecRedecoder`` (:602-769) serves the README's zero-shot voice conversion natively (``AB_GEN_FACODEC_REDECODER``):
+``vq2emb(vq, speaker_embedding, use_residual=True)`` gathers the prosody codes' embeddings, runs them through the
+speaker-conditioned prosody transformer (style-adaptive LayerNorms) and adds the content and residual embeddings ->
+``[B, 256, T]``; ``inference`` is the decoder's.  Its ``forward`` is broken in the reference and is refused.
+
 The training branch (``vq=False``: the predictors, random residual masking, the losses), ``get_vq`` and a quantizer or
-timbre encoder in training mode are not served; the modules only those evaluate are kept as parameters."""
+transformer in training mode are not served; the modules only those evaluate are kept as parameters."""
 from __future__ import annotations
 
 import ctypes as C
@@ -29,7 +34,8 @@ from .activations import Activation1d, SnakeBeta
 from .generator import NativeGenerator
 
 _SERVED = ("amphion_b200 serves FACodecEncoder.forward() / .inference(), FACodecDecoder.forward(vq=True) in eval, "
-           "FACodecDecoder.vq2emb() and FACodecDecoder.inference()")
+           "FACodecDecoder.vq2emb() and FACodecDecoder.inference(), and FACodecRedecoder.vq2emb() in eval and "
+           "FACodecRedecoder.inference()")
 
 
 def _native_only(name):
@@ -136,24 +142,121 @@ class _FFN(_Holder):
         self.ffn_2 = nn.Linear(filt, hidden)
 
 
-class _EncoderLayer(_Holder):
-    def __init__(self, hidden, heads, filt, k):
+class StyleAdaptiveLayerNorm(_Holder):
+    """Parameter holder for transformer.py:13-32: ``gamma * LayerNorm(x) + beta`` (no affine, eps 1e-5) with
+    ``(gamma, beta) = style(mean(condition, dim=1))``."""
+
+    def __init__(self, normalized_shape):
         super().__init__()
-        self.ln_1 = nn.LayerNorm(hidden)
-        self.ln_2 = nn.LayerNorm(hidden)
+        self.style = nn.Linear(normalized_shape, 2 * normalized_shape)
+        self.style.bias.data[:normalized_shape] = 1
+        self.style.bias.data[normalized_shape:] = 0
+
+
+class _EncoderLayer(_Holder):
+    def __init__(self, hidden, heads, filt, k, use_cln=False):
+        super().__init__()
+        norm = StyleAdaptiveLayerNorm if use_cln else nn.LayerNorm
+        self.ln_1 = norm(hidden)
+        self.ln_2 = norm(hidden)
         self.self_attn = nn.MultiheadAttention(hidden, heads, batch_first=True)
         self.ffn = _FFN(hidden, filt, k)
 
 
 class TransformerEncoder(_Holder):
-    """Parameter holder for transformer.py:154-217 (the timbre encoder, use_cln=False)."""
+    """Parameter holder for transformer.py:154-234: the decoder's timbre encoder (use_cln=False) or the redecoder's
+    speaker-conditioned prosody encoder (use_cln=True: style-adaptive ln_1, ln_2 and last_ln)."""
 
-    def __init__(self, encoder_layer=4, encoder_hidden=256, encoder_head=4, conv_filter_size=1024, conv_kernel_size=5):
+    def __init__(self, encoder_layer=4, encoder_hidden=256, encoder_head=4, conv_filter_size=1024, conv_kernel_size=5,
+                 use_cln=False):
         super().__init__()
         self.position_emb = _PositionalEncoding(encoder_hidden)
-        self.layers = nn.ModuleList([_EncoderLayer(encoder_hidden, encoder_head, conv_filter_size, conv_kernel_size)
-                                     for _ in range(encoder_layer)])
-        self.last_ln = nn.LayerNorm(encoder_hidden)
+        self.layers = nn.ModuleList([_EncoderLayer(encoder_hidden, encoder_head, conv_filter_size, conv_kernel_size,
+                                                   use_cln) for _ in range(encoder_layer)])
+        self.last_ln = StyleAdaptiveLayerNorm(encoder_hidden) if use_cln else nn.LayerNorm(encoder_hidden)
+
+
+def _generator_config(m, kind):
+    """The BigVGAN-family generator fields of the decoder and the redecoder (model.*, facodec.py:220-240)."""
+    if len(m.up_ratios) > _capi.AB_MAX_STAGES:
+        raise ValueError(f"amphion_b200: too many up_ratios for the native {type(m).__name__}")
+    c = _capi.GeneratorConfig()
+    c.kind = kind
+    c.n_mel = m.in_channels
+    c.upsample_initial_channel = m.upsample_initial_channel
+    c.num_upsamples = len(m.up_ratios)
+    for i, u in enumerate(m.up_ratios):
+        c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
+    c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
+    for p, d in enumerate((1, 3, 9)):
+        c.resblock_dilation_sizes[0][p] = d
+    c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
+    for i, (n, bits) in enumerate(((m.vq_num_q_p, m.codebook_size_prosody), (m.vq_num_q_c, m.codebook_size_content),
+                                   (m.vq_num_q_r, m.codebook_size_residual))):
+        c.vq_num_q[i], c.vq_codebook_bits[i] = n, int(bits)
+    return c
+
+
+def _workspace_for(m, device, need):
+    if m._workspace is None or m._workspace.numel() < need + 256 or m._workspace.device != device:
+        m._workspace = None
+        m._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
+    return (m._workspace.data_ptr() + 255) // 256 * 256
+
+
+def _inference(m, x, speaker_embedding, out, tail_events):
+    """FACodecDecoder.inference / FACodecRedecoder.inference (facodec.py:568-576, :761-769) on the native handle."""
+    who = type(m).__name__
+    if x.dim() != 3 or x.shape[1] != m.in_channels:
+        raise ValueError(f"{who}.inference expects x of shape [B, {m.in_channels}, T], got {tuple(x.shape)}")
+    spk = speaker_embedding
+    if spk.dim() != 2 or spk.shape[1] != m.in_channels or spk.shape[0] != x.shape[0]:
+        raise ValueError(f"{who}.inference expects a speaker embedding of shape [{x.shape[0]}, "
+                         f"{m.in_channels}], got {tuple(spk.shape)}")
+    if spk.device != x.device:
+        raise ValueError(f"{who}.inference: x and the speaker embedding are on different devices")
+    B, _, T = x.shape
+    if B == 0 or T == 0:
+        raise ValueError("amphion_b200: empty latent batch")
+    _capi.require_cuda(x, f"{who}.inference")
+    if x.dtype != torch.float32:
+        x = x.float()
+    spk = spk.float()
+    if spk.stride(1) != 1:
+        spk = spk.contiguous()
+    with torch.cuda.device(x.device):
+        m._sync_params(x.device)
+        lib, h = _capi.lib, m._handle
+        need = lib.ab_generator_workspace_bytes(h, B, T)
+        wbase = _workspace_for(m, x.device, need)
+        n_out = T * m.hop_length
+        if out is None:
+            wav = torch.empty(B, 1, n_out, dtype=torch.float32, device=x.device)
+        else:
+            if (tuple(out.shape) != (B, 1, n_out) or out.dtype != torch.float32 or out.device != x.device
+                    or not out.is_contiguous()):
+                raise ValueError(f"out must be a contiguous fp32 [{B}, 1, {n_out}] tensor on {x.device}")
+            wav = out
+        if tail_events:
+            for ev in tail_events:
+                ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded below
+            arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
+            _capi.check(lib.ab_generator_set_tail_events(h, arr, len(tail_events)), "ab_generator_set_tail_events")
+        _capi.check(lib.ab_facodec_inference(h, _capi.ptr(x), B, T, _capi.shape_array(x.stride()), _capi.ptr(spk),
+                                             spk.stride(0), _capi.ptr(wav), C.c_void_p(wbase), need,
+                                             _capi.stream_ptr()), "ab_facodec_inference")
+        m.last_launches = lib.ab_generator_last_launches(h)
+    return wav
+
+
+def _remove_all_weight_norm(m):
+    def _remove(mod):
+        try:
+            remove_weight_norm(mod)
+        except ValueError:   # this module has no weight norm
+            return
+    m.apply(_remove)
+    m.invalidate()
 
 
 class FACodecDecoder(NativeGenerator):
@@ -237,31 +340,12 @@ class FACodecDecoder(NativeGenerator):
         return list(self.up_ratios)
 
     def _c_config_decode(self):
-        if len(self.up_ratios) > _capi.AB_MAX_STAGES:
-            raise ValueError("amphion_b200: too many up_ratios for the native decoder")
-        c = _capi.GeneratorConfig()
-        c.kind = _capi.GEN_FACODEC
-        c.n_mel = self.in_channels
-        c.upsample_initial_channel = self.upsample_initial_channel
-        c.num_upsamples = len(self.up_ratios)
-        for i, u in enumerate(self.up_ratios):
-            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
-        c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
-        for p, d in enumerate((1, 3, 9)):
-            c.resblock_dilation_sizes[0][p] = d
-        c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
-        for i, (n, bits) in enumerate(((self.vq_num_q_p, self.codebook_size_prosody),
-                                       (self.vq_num_q_c, self.codebook_size_content),
-                                       (self.vq_num_q_r, self.codebook_size_residual))):
-            c.vq_num_q[i], c.vq_codebook_bits[i] = n, int(bits)
+        c = _generator_config(self, _capi.GEN_FACODEC)
         c.vq_codebook_dim = self.codebook_dim
         return c
 
     def _workspace_for(self, device, need):
-        if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != device:
-            self._workspace = None
-            self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
-        return (self._workspace.data_ptr() + 255) // 256 * 256
+        return _workspace_for(self, device, need)
 
     # ---- served methods --------------------------------------------------------------
     def vq2emb(self, vq, use_residual_code=True):
@@ -301,46 +385,7 @@ class FACodecDecoder(NativeGenerator):
         """x [B, in_channels, T] (any strides), speaker_embedding [B, in_channels] -> wav [B, 1, T * hop] fp32.
 
         ``out`` / ``tail_events`` (beyond the reference signature) behave as in the other generators' forward."""
-        if x.dim() != 3 or x.shape[1] != self.in_channels:
-            raise ValueError(f"FACodecDecoder.inference expects x of shape [B, {self.in_channels}, T], got {tuple(x.shape)}")
-        spk = speaker_embedding
-        if spk.dim() != 2 or spk.shape[1] != self.in_channels or spk.shape[0] != x.shape[0]:
-            raise ValueError(f"FACodecDecoder.inference expects a speaker embedding of shape [{x.shape[0]}, "
-                             f"{self.in_channels}], got {tuple(spk.shape)}")
-        if spk.device != x.device:
-            raise ValueError("FACodecDecoder.inference: x and the speaker embedding are on different devices")
-        B, _, T = x.shape
-        if B == 0 or T == 0:
-            raise ValueError("amphion_b200: empty latent batch")
-        _capi.require_cuda(x, "FACodecDecoder.inference")
-        if x.dtype != torch.float32:
-            x = x.float()
-        spk = spk.float()
-        if spk.stride(1) != 1:
-            spk = spk.contiguous()
-        with torch.cuda.device(x.device):
-            self._sync_params(x.device)
-            lib, h = _capi.lib, self._handle
-            need = lib.ab_generator_workspace_bytes(h, B, T)
-            wbase = self._workspace_for(x.device, need)
-            n_out = T * self.hop_length
-            if out is None:
-                wav = torch.empty(B, 1, n_out, dtype=torch.float32, device=x.device)
-            else:
-                if (tuple(out.shape) != (B, 1, n_out) or out.dtype != torch.float32 or out.device != x.device
-                        or not out.is_contiguous()):
-                    raise ValueError(f"out must be a contiguous fp32 [{B}, 1, {n_out}] tensor on {x.device}")
-                wav = out
-            if tail_events:
-                for ev in tail_events:
-                    ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded below
-                arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
-                _capi.check(lib.ab_generator_set_tail_events(h, arr, len(tail_events)), "ab_generator_set_tail_events")
-            _capi.check(lib.ab_facodec_inference(h, _capi.ptr(x), B, T, _capi.shape_array(x.stride()), _capi.ptr(spk),
-                                                 spk.stride(0), _capi.ptr(wav), C.c_void_p(wbase), need,
-                                                 _capi.stream_ptr()), "ab_facodec_inference")
-            self.last_launches = lib.ab_generator_last_launches(h)
-        return wav
+        return _inference(self, x, speaker_embedding, out, tail_events)
 
     def _c_config(self):
         c = self._c_config_decode()
@@ -412,13 +457,7 @@ class FACodecDecoder(NativeGenerator):
         return outs, qs, commit_loss, list(buf.unbind(0)), spk
 
     def remove_weight_norm(self):
-        def _remove(m):
-            try:
-                remove_weight_norm(m)
-            except ValueError:   # this module has no weight norm
-                return
-        self.apply(_remove)
-        self.invalidate()
+        _remove_all_weight_norm(self)
 
 
 class EncoderBlock(nn.Module):
@@ -542,10 +581,148 @@ class FACodecEncoder(NativeGenerator):
         return self.forward(x)
 
     def remove_weight_norm(self):
-        def _remove(m):
-            try:
-                remove_weight_norm(m)
-            except ValueError:   # this module has no weight norm
-                return
-        self.apply(_remove)
-        self.invalidate()
+        _remove_all_weight_norm(self)
+
+
+class FACodecRedecoder(NativeGenerator):
+    """Drop-in for FACodecRedecoder (facodec.py:602-769): the same constructor and parameter tree
+    (``{prosody,content,residual}_embs``, ``model.*``, ``timbre_linear``, ``timbre_cond_prosody_enc``), so the released
+    ``ns3_facodec_redecoder.bin`` loads strictly.  Served natively (``AB_GEN_FACODEC_REDECODER``), in eval:
+
+    - ``vq2emb(vq, speaker_embedding, use_residual=True)``: codes ``[n_q, B, T]`` (rows by position: prosody, content,
+      residual; extra rows ignored) and the target speaker's embedding ``[B, 256]`` -> ``[B, 256, T]``;
+    - ``inference(x, speaker_embedding)``: the decoder's FiLM and generator -> ``[B, 1, T * prod(up_ratios)]``.
+
+    The transformer's style Linears read the speaker embedding itself; the reference reads the time mean of the
+    embedding expanded over T, which equals it up to fp32 rounding of the sum."""
+
+    kind = "facodec_redecoder"
+
+    def __init__(self, in_channels=256, upsample_initial_channel=1280, up_ratios=(5, 5, 4, 2), vq_num_q_c=2,
+                 vq_num_q_p=1, vq_num_q_r=3, vq_dim=256, codebook_size_prosody=10, codebook_size_content=10,
+                 codebook_size_residual=10):
+        super().__init__()
+        if in_channels != 256 or vq_dim != 256:
+            # the prosody transformer is 256 wide and its output is summed with the vq_dim-wide embeddings
+            raise ValueError(f"amphion_b200: FACodecRedecoder needs in_channels == vq_dim == 256, the prosody "
+                             f"transformer's width (got {in_channels}, {vq_dim})")
+        self.hop_length = int(np.prod(up_ratios))
+        self.up_ratios = [int(u) for u in up_ratios]
+        self.in_channels, self.upsample_initial_channel = int(in_channels), int(upsample_initial_channel)
+        self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r = int(vq_num_q_p), int(vq_num_q_c), int(vq_num_q_r)
+        self.vq_dim = int(vq_dim)
+        self.codebook_size_prosody = codebook_size_prosody
+        self.codebook_size_content = codebook_size_content
+        self.codebook_size_residual = codebook_size_residual
+
+        def embs(n, bits):
+            out = nn.ModuleList()
+            for _ in range(n):
+                e = nn.Embedding(num_embeddings=2 ** bits, embedding_dim=vq_dim)
+                e.weight.data.normal_(mean=0.0, std=1e-5)
+                out.append(e)
+            return out
+
+        self.prosody_embs = embs(self.vq_num_q_p, codebook_size_prosody)
+        self.content_embs = embs(self.vq_num_q_c, codebook_size_content)
+        self.residual_embs = embs(self.vq_num_q_r, codebook_size_residual)
+
+        channels = upsample_initial_channel
+        layers = [weight_norm(nn.Conv1d(in_channels, channels, kernel_size=7, padding=3))]
+        for i, stride in enumerate(up_ratios):
+            layers.append(DecoderBlock(channels // 2 ** i, channels // 2 ** (i + 1), stride))
+        output_dim = channels // 2 ** len(up_ratios)
+        layers += [_act(output_dim), weight_norm(nn.Conv1d(output_dim, 1, kernel_size=7, padding=3)), nn.Tanh()]
+        self.model = nn.Sequential(*layers)
+
+        self.timbre_linear = nn.Linear(in_channels, in_channels * 2)
+        self.timbre_linear.bias.data[:in_channels] = 1
+        self.timbre_linear.bias.data[in_channels:] = 0
+        self.timbre_norm = nn.LayerNorm(in_channels, elementwise_affine=False)
+        self.timbre_cond_prosody_enc = TransformerEncoder(use_cln=True)
+
+    # ---- NativeGenerator hooks -------------------------------------------------------
+    def _input_channels(self):
+        return self.in_channels
+
+    def _hop(self):
+        return self.hop_length
+
+    def _upsample_rates(self):
+        return list(self.up_ratios)
+
+    def _c_config(self):
+        return _generator_config(self, _capi.GEN_FACODEC_REDECODER)
+
+    # ---- served methods --------------------------------------------------------------
+    def vq2emb(self, vq, speaker_embedding, use_residual=True):
+        """codes [n_q, B, T] (integer, any strides), speaker_embedding [B, 256] -> [B, 256, T] fp32 on the codes'
+        device (facodec.py:734-759)."""
+        p, c, r = self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r
+        if not isinstance(vq, torch.Tensor) or vq.dim() != 3 or vq.is_floating_point() or vq.is_complex() \
+                or vq.dtype == torch.bool:
+            got = f"{vq.dtype} {tuple(vq.shape)}" if isinstance(vq, torch.Tensor) else type(vq).__name__
+            raise ValueError(f"FACodecRedecoder.vq2emb expects integer codes [n_q, B, T], got {got}")
+        n_q, B, T = vq.shape
+        need = p + c + (r if use_residual else 0)
+        if n_q < need:
+            raise ValueError(f"FACodecRedecoder.vq2emb: {n_q} code rows, too few for {p} prosody, {c} content"
+                             + (f" and {r} residual" if use_residual else "") + " rows")
+        if B == 0 or T == 0:
+            raise ValueError("amphion_b200: empty code batch")
+        spk = speaker_embedding
+        if not isinstance(spk, torch.Tensor) or spk.dim() != 2 or tuple(spk.shape) != (B, self.in_channels):
+            got = tuple(spk.shape) if isinstance(spk, torch.Tensor) else type(spk).__name__
+            raise ValueError(f"FACodecRedecoder.vq2emb expects a speaker embedding of shape [{B}, {self.in_channels}], "
+                             f"got {got}")
+        if spk.device != vq.device:
+            raise ValueError("FACodecRedecoder.vq2emb: the codes and the speaker embedding are on different devices")
+        _capi.require_cuda(vq, "FACodecRedecoder.vq2emb")
+        if self.timbre_cond_prosody_enc.training or any(m.training for m in self.timbre_cond_prosody_enc.modules()):
+            raise NotImplementedError(f"amphion_b200: the prosody transformer in training mode (dropout) is not "
+                                      f"served; {_SERVED}")
+        n_pe = self.timbre_cond_prosody_enc.position_emb.pe.shape[0]
+        if B > n_pe:
+            raise ValueError(f"amphion_b200: batch {B} > {n_pe}, the rows of the prosody transformer's positional "
+                             f"encoding (the reference fails there too)")
+        vq = vq.long()
+        # codes the kernel would not read (it writes NaN there): refuse them before the launch, as F.embedding does
+        groups = [(0, p, self.codebook_size_prosody), (p, p + c, self.codebook_size_content)]
+        if use_residual and r > 0:
+            groups.append((p + c, p + c + r, self.codebook_size_residual))
+        for q0, q1, bits in groups:
+            part = vq[q0:q1]
+            lo, hi = int(part.min()), int(part.max())
+            if lo < 0 or hi >= 2 ** int(bits):
+                raise ValueError(f"FACodecRedecoder.vq2emb: code rows {q0}..{q1 - 1} hold {lo}..{hi}, outside the "
+                                 f"embedding table [0, {2 ** int(bits)})")
+        spk = spk.float()
+        if spk.stride(1) != 1:
+            spk = spk.contiguous()
+        with torch.cuda.device(vq.device):
+            self._sync_params(vq.device)
+            lib, h = _capi.lib, self._handle
+            ws = lib.ab_facodec_redecoder_vq2emb_workspace_bytes(h, B, T)
+            wbase = _workspace_for(self, vq.device, ws)
+            out = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=vq.device)
+            _capi.check(lib.ab_facodec_redecoder_vq2emb(h, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B, T,
+                                                        _capi.ptr(spk), spk.stride(0), int(bool(use_residual)),
+                                                        _capi.ptr(out), C.c_void_p(wbase), ws, _capi.stream_ptr()),
+                        "ab_facodec_redecoder_vq2emb")
+            self.last_launches = lib.ab_generator_last_launches(h)
+        return out
+
+    def inference(self, x, speaker_embedding, out=None, tail_events=None):
+        """x [B, 256, T] (any strides), speaker_embedding [B, 256] -> wav [B, 1, T * hop] fp32 (facodec.py:761-769).
+
+        ``out`` / ``tail_events`` (beyond the reference signature) behave as in the other generators' forward."""
+        return _inference(self, x, speaker_embedding, out, tail_events)
+
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError(
+            "amphion_b200: FACodecRedecoder.forward is not served: the reference builds the embedding sum as [B, T, d] "
+            "and transposes it before timbre_norm, so it raises unless T == 256, and at T == 256 it normalises over "
+            f"time and feeds [B, T, d] to conv_pre as channels.  Call vq2emb() and then inference(); {_SERVED}")
+
+    def remove_weight_norm(self):
+        _remove_all_weight_norm(self)

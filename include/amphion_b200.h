@@ -106,10 +106,21 @@ extern "C" {
  * reference's nn.Sequential names: "block.0" (conv_pre), "block.{1+i}.block.{0,1,2}.block.{0,1,2,3}" (a ResidualUnit's
  * act, k = 7 conv, act, k = 1 conv), "block.{1+i}.block.3" (the stage's activation), "block.{1+i}.block.4" (the strided
  * conv), "block.{1+n}" (final act), "block.{2+n}" (conv_post).  conv_pre (one input channel) runs on the fp32 CUDA cores
- * at every precision.  Runs through ab_facodec_encode, not ab_generator_forward. */
+ * at every precision.  Runs through ab_facodec_encode, not ab_generator_forward.
+ * AB_GEN_FACODEC_REDECODER: NaturalSpeech 3's FACodecRedecoder (models/codec/ns3_codec/facodec.py:602-769), the README's
+ * zero-shot voice conversion: vq2emb (ab_facodec_redecoder_vq2emb) and inference (ab_facodec_inference, the decoder's
+ * FiLM and generator).  Config fields: the generator fields as for AB_GEN_FACODEC, n_mel = in_channels = vq_dim = 256
+ * (the prosody transformer's width), vq_num_q = (prosody >= 1, content >= 1, residual >= 0) tables and
+ * vq_codebook_bits (1..24) their sizes; vq_codebook_dim = 0, facodec_quantize = 0; every other field 0.  Tensors keep the
+ * reference's names (the 265 entries of ns3_facodec_redecoder.bin at the default constructor):
+ * "{prosody,content,residual}_embs.{j}.weight" [2^bits, 256], the decoder's "model.*" and "timbre_linear.{weight,bias}",
+ * "timbre_cond_prosody_enc.position_emb.pe" [5000, 1, 256], per layer l "timbre_cond_prosody_enc.layers.{l}.{ln_1,ln_2}.
+ * style.{weight [512, 256], bias [512]}", ".self_attn.in_proj_{weight,bias}", ".self_attn.out_proj.{weight,bias}",
+ * ".ffn.ffn_1.{weight,bias}" (k = 5), ".ffn.ffn_2.{weight,bias}", and "timbre_cond_prosody_enc.last_ln.style.{weight,bias}".
+ * The reference's forward (:691-732) transposes the [B, T, d] sum before timbre_norm and is not served. */
 enum ab_generator_kind {
   AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
-  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8
+  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8, AB_GEN_FACODEC_REDECODER = 9
 };
 #define AB_FACODEC_MAX_Q 32   /* most codebook layers over the three ResidualVQs */
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
@@ -166,7 +177,8 @@ typedef struct ab_generator_config {
   /* AB_GEN_DIFFWAVE only (0 elsewhere) */
   int32_t dilation_cycle;                       /* dilation_cycle_length */
   int32_t embedding_rows;                       /* rows of the diffusion-step table, len(noise_schedule) */
-  /* AB_GEN_FACODEC only (0 elsewhere): the prosody, content and residual ResidualVQs (facodec.py:286-334) */
+  /* AB_GEN_FACODEC: the prosody, content and residual ResidualVQs (facodec.py:286-334); AB_GEN_FACODEC_REDECODER: its
+   * embedding tables (vq_num_q, vq_codebook_bits; vq_codebook_dim 0); 0 elsewhere */
   int32_t vq_num_q[3];                          /* vq_num_q_p, vq_num_q_c, vq_num_q_r (the residual group may be 0) */
   int32_t vq_codebook_bits[3];                  /* codebook_size_{prosody,content,residual}: 2^bits rows */
   int32_t vq_codebook_dim;                      /* codebook_dim */
@@ -234,7 +246,9 @@ int ab_generator_last_launches(const ab_generator* g);
  * LayerNorm and the FiLM, and vq2emb) when max_entries >= 12, the six unused classes with zero launches; a handle created
  * with facodec_quantize also lists "facodec_quantize" (the RVQ with the positional add, and the time mean) and
  * "timbre_attention" (max_entries >= 14).  ab_facodec_quantize counts its GEMMs in "tc_conv" (tensor-core precision)
- * or "conv1d_fp32", and its LayerNorms in "vocos_norm". */
+ * or "conv1d_fp32", and its LayerNorms in "vocos_norm".  A FACodec redecoder handle lists the same 14 classes:
+ * ab_facodec_redecoder_vq2emb counts its style Linears, style LayerNorms and embedding gathers in "facodec_prologue",
+ * its attention in "timbre_attention" and its GEMMs in "tc_conv" or "conv1d_fp32"; "facodec_quantize" stays empty. */
 typedef struct ab_profile_entry {
   char name[32];
   int32_t launches;
@@ -300,7 +314,7 @@ int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t batch, 
 int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q, int64_t batch,
                       int64_t frames, int32_t use_residual, float* dev_out, void* stream);
 /* x [B, in_channels, T] fp32 with any element strides, spk [B, in_channels] fp32 with row stride spk_row_stride ->
- * wav [B, 1, T * prod(up_ratios)].  Workspace: ab_generator_workspace_bytes.  Tail events (ab_generator_set_tail_events)
+ * wav [B, 1, T * prod(up_ratios)].  Also serves a redecoder handle (FACodecRedecoder.inference, facodec.py:761-769).  Workspace: ab_generator_workspace_bytes.  Tail events (ab_generator_set_tail_events)
  * split conv_post into batch chunks as for the other generators.  set_option's "resblock_fusion" is accepted and
  * changes nothing: every FACodec conv runs as a single conv. */
 int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t batch, int64_t frames, const int64_t x_strides[3],
@@ -326,6 +340,29 @@ size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t batch,
 int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t batch, int64_t frames,
                         int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
                         float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * FACodec redecoder (AB_GEN_FACODEC_REDECODER): FACodecRedecoder.vq2emb (models/codec/ns3_codec/facodec.py:734-759);
+ * its inference is ab_facodec_inference above.
+ * ---------------------------------------------------------------------- */
+/* codes int64 [n_q, B, T] with element strides codes_strides, read by position (prosody rows, content rows, then
+ * residual rows; rows past those read are ignored), spk [B, 256] fp32 with row stride spk_row_stride -> out [B, 256, T]
+ * fp32 contiguous.  Per prosody table i: x_t = Transformer(x_t + prosody_embs[i](codes[i])) (x_t starts at 0), where the
+ * transformer adds row b of "pe" to every time step of utterance b (the batch-first PositionalEncoding) and runs 4 pre-LN
+ * layers (MHA with 4 heads, no mask; a k = 5 conv FFN with ReLU) and last_ln, every LayerNorm style-adaptive:
+ * gamma * LayerNorm(x) + beta (eps 1e-5, no affine) with (gamma, beta) = style(speaker embedding).  (The reference feeds
+ * style the time mean of the embedding expanded over T, the embedding itself up to fp32 rounding of the sum.)  Then
+ * out = ((x_t + content_0) + content_1 ...) [+ residual_0 ...] with use_residual, one fp32 add per term.  The gathers,
+ * sums, style Linears and LayerNorm statistics are fp32 at every precision; the GEMMs take 16-bit operands at
+ * AB_PREC_TC_*.  A code outside its table is never read: its time step is written as NaN (a bad prosody code spreads
+ * through the attention to its whole utterance).  Refused before any launch: n_q below the rows read, B > 5000 (the rows
+ * of pe), a short or unaligned workspace.  Launches: 9 style Linears, per prosody table 30 (the gather, 4 x 7 layer
+ * launches, last_ln), and the tail gather.  Workspace: ab_facodec_redecoder_vq2emb_workspace_bytes, 256-byte aligned. */
+size_t ab_facodec_redecoder_vq2emb_workspace_bytes(const ab_generator* g, int64_t batch, int64_t frames);
+int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q,
+                                int64_t batch, int64_t frames, const float* dev_spk, int64_t spk_row_stride,
+                                int32_t use_residual, float* dev_out, void* dev_workspace, size_t workspace_bytes,
+                                void* stream);
 
 /* ------------------------------------------------------------------------
  * FACodec encoder (AB_GEN_FACODEC_ENCODER): FACodecEncoder.forward / .inference (models/codec/ns3_codec/facodec.py:157-194).
