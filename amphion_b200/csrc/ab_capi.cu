@@ -280,6 +280,31 @@ int validate_diffwave_config(const ab_generator_config& c) {
   return AB_OK;
 }
 
+// FACodec's DecoderBlocks / EncoderBlocks: three ResidualUnits k = 7, dilations (1, 3, 9), SnakeBeta with logscale
+// (facodec.py:121-154).  blocks and model name them in the messages.
+int check_facodec_units(const ab_generator_config& c, const char* blocks, const char* model) {
+  if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
+      c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
+    return fail(AB_ERR_ARG, "config: %s hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, num_kernels 1, kernel 7, "
+                            "3 dilations", blocks);
+  if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
+    return fail(AB_ERR_ARG, "config: %s uses SnakeBeta with alpha_logscale = True", model);
+  return AB_OK;
+}
+
+// The three code groups (prosody, content, residual) of FACodec's decoder and redecoder: vq_num_q and the table sizes.
+// model and table name them in the messages.
+int check_facodec_groups(const ab_generator_config& c, const char* model, const char* table) {
+  if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
+      c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
+    return fail(AB_ERR_ARG, "config: %s vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, at most %d in all",
+                model, c.vq_num_q[0], c.vq_num_q[1], c.vq_num_q[2], AB_FACODEC_MAX_Q);
+  for (int i = 0; i < 3; ++i)
+    if (c.vq_codebook_bits[i] <= 0 || c.vq_codebook_bits[i] > 24)
+      return fail(AB_ERR_ARG, "config: %s size 2^%d out of range (bits 1..24)", table, c.vq_codebook_bits[i]);
+  return AB_OK;
+}
+
 // The generator of FACodec's decoder and redecoder: the fixed block structure (facodec.py:121-133, :220-240)
 int validate_facodec_generator_config(const ab_generator_config& c) {
   if (c.gin_channels || c.conv_post_no_bias || c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel ||
@@ -295,26 +320,14 @@ int validate_facodec_generator_config(const ab_generator_config& c) {
     if (c.upsample_rates[i] <= 0 || c.upsample_rates[i] > 64 || c.upsample_kernel_sizes[i] != 2 * c.upsample_rates[i])
       return fail(AB_ERR_ARG, "config: FACodec stage %d: ratio %d (1..64) with kernel %d (must be 2 x ratio)", i,
                   c.upsample_rates[i], c.upsample_kernel_sizes[i]);
-  if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
-      c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
-    return fail(AB_ERR_ARG, "config: FACodec DecoderBlocks hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, "
-                            "num_kernels 1, kernel 7, 3 dilations");
-  if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
-    return fail(AB_ERR_ARG, "config: FACodec uses SnakeBeta with alpha_logscale = True");
-  return AB_OK;
+  return check_facodec_units(c, "FACodec DecoderBlocks", "FACodec");
 }
 
 // AB_GEN_FACODEC: the generator and the ResidualVQ geometry
 int validate_facodec_config(const ab_generator_config& c) {
-  const int rc = validate_facodec_generator_config(c);
+  int rc = validate_facodec_generator_config(c);
   if (rc != AB_OK) return rc;
-  if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
-      c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
-    return fail(AB_ERR_ARG, "config: FACodec vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, at most %d in all",
-                c.vq_num_q[0], c.vq_num_q[1], c.vq_num_q[2], AB_FACODEC_MAX_Q);
-  for (int i = 0; i < 3; ++i)
-    if (c.vq_codebook_bits[i] <= 0 || c.vq_codebook_bits[i] > 24)
-      return fail(AB_ERR_ARG, "config: FACodec codebook size 2^%d out of range (bits 1..24)", c.vq_codebook_bits[i]);
+  if ((rc = check_facodec_groups(c, "FACodec", "FACodec codebook")) != AB_OK) return rc;
   if (c.vq_codebook_dim <= 0 || c.vq_codebook_dim > FAC_MAX_CODEBOOK_DIM || c.vq_codebook_dim == c.n_mel)
     return fail(AB_ERR_UNSUPPORTED, "config: FACodec codebook_dim %d (1..%d, != vq_dim: out_proj must be a Linear)",
                 c.vq_codebook_dim, FAC_MAX_CODEBOOK_DIM);
@@ -329,19 +342,13 @@ int validate_facodec_config(const ab_generator_config& c) {
 
 // AB_GEN_FACODEC_REDECODER: the generator and the embedding tables (facodec.py:602-689)
 int validate_facodec_redecoder_config(const ab_generator_config& c) {
-  const int rc = validate_facodec_generator_config(c);
+  int rc = validate_facodec_generator_config(c);
   if (rc != AB_OK) return rc;
   // the prosody transformer is 256 wide, and its output is summed with the vq_dim-wide embeddings
   if (c.n_mel != FAC_TIMBRE_C)
     return fail(AB_ERR_UNSUPPORTED, "config: the FACodec redecoder needs in_channels == vq_dim == %d (the prosody "
                 "transformer's width; got %d)", FAC_TIMBRE_C, c.n_mel);
-  if (c.vq_num_q[0] <= 0 || c.vq_num_q[1] <= 0 || c.vq_num_q[2] < 0 ||
-      c.vq_num_q[0] + c.vq_num_q[1] + c.vq_num_q[2] > AB_FACODEC_MAX_Q)
-    return fail(AB_ERR_ARG, "config: FACodec redecoder vq_num_q (%d, %d, %d): prosody and content >= 1, residual >= 0, "
-                "at most %d in all", c.vq_num_q[0], c.vq_num_q[1], c.vq_num_q[2], AB_FACODEC_MAX_Q);
-  for (int i = 0; i < 3; ++i)
-    if (c.vq_codebook_bits[i] <= 0 || c.vq_codebook_bits[i] > 24)
-      return fail(AB_ERR_ARG, "config: FACodec redecoder table size 2^%d out of range (bits 1..24)", c.vq_codebook_bits[i]);
+  if ((rc = check_facodec_groups(c, "FACodec redecoder", "FACodec redecoder table")) != AB_OK) return rc;
   if (c.vq_codebook_dim != 0 || c.facodec_quantize != 0)
     return fail(AB_ERR_ARG, "config: the FACodec redecoder has no codebook_dim or facodec_quantize (both must be 0)");
   return AB_OK;
@@ -366,13 +373,7 @@ int validate_facodec_encoder_config(const ab_generator_config& c) {
         c.upsample_kernel_sizes[i] != 2 * c.upsample_rates[i])
       return fail(AB_ERR_UNSUPPORTED, "config: FACodec encoder stage %d: stride %d (1..%d) with kernel %d (must be 2 x stride)",
                   i, c.upsample_rates[i], AB_TC_MAX_STRIDE, c.upsample_kernel_sizes[i]);
-  if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
-      c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
-    return fail(AB_ERR_ARG, "config: FACodec EncoderBlocks hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, "
-                            "num_kernels 1, kernel 7, 3 dilations");
-  if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
-    return fail(AB_ERR_ARG, "config: the FACodec encoder uses SnakeBeta with alpha_logscale = True");
-  return AB_OK;
+  return check_facodec_units(c, "FACodec EncoderBlocks", "the FACodec encoder");
 }
 
 int validate_config(const ab_generator_config& c) {
@@ -1062,9 +1063,150 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
 // ---------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------
+extern "C++" {
 namespace {
 constexpr int NBUF = 7;  // fp32: R0 R1 U P0 P1 TMP ACT
 constexpr int NIMG = 4;  // 16-bit operand images: U P0 P1 R (stage output, HiFi-GAN)
+
+double rup16(int c) { return (double)((c + 15) / 16 * 16); }
+
+// Bump allocator over a workspace: take(bytes) returns the next 256-byte-aligned region, nullptr when base is null
+// (sizes only); off is the size of everything taken so far
+struct Carve {
+  char* base;
+  size_t off = 0;
+  template <class P = float>
+  P* take(size_t bytes) {
+    P* p = base ? reinterpret_cast<P*>(base + off) : nullptr;
+    off += align_up(bytes, 256);
+    return p;
+  }
+};
+
+int check_workspace(const char* what, const void* ws, size_t bytes, size_t need) {
+  if (!ws || bytes < need) return fail(AB_ERR_WORKSPACE, "%s: workspace %zu B < required %zu B", what, bytes, need);
+  if (reinterpret_cast<uintptr_t>(ws) & 255) return fail(AB_ERR_ARG, "%s: workspace must be 256-byte aligned", what);
+  return AB_OK;
+}
+
+// The launches of one entry-point call: counts them (ab_generator_last_launches), times each one when profiling is on
+// (ab_generator_set_profiling), and runs the layers the model kinds share
+struct Launch {
+  ab_generator* g;
+  cudaStream_t st;
+  int launches = 0;
+
+  template <class F>
+  int timed(int cls, double flops, double bytes, F launch) {
+    ++launches;
+    if (!g->profiling) return launch();
+    const ab_generator::ProfRec r{cls, g->get_event(), g->get_event(), flops, bytes};
+    cudaEventRecord(r.e0, st);
+    g->prof_recs.push_back(r);
+    const int rc = launch();
+    cudaEventRecord(g->prof_recs.back().e1, st);
+    return rc;
+  }
+  // n launches that are counted but not timed
+  template <class F>
+  int counted(int n, F launch) {
+    launches += n;
+    return launch();
+  }
+  // the count becomes ab_generator_last_launches when the call succeeds
+  int done(int rc) {
+    if (rc == AB_OK) g->launches = launches;
+    return rc;
+  }
+
+  // whether conv c runs on the wgmma kernel (tc_image_bytes decided it at create)
+  bool on_tc(const ConvRef& c) const { return g->precision != AB_PREC_FP32 && g->slots[c.w].tc_bytes > 0; }
+
+  // algorithmic HBM bytes of a Conv1d launch with fp32 activations and weights (profile)
+  static double conv_bytes(const ConvRef& c, int64_t B, int Tn, const float* residual, const float* acc_prev) {
+    const double el = (double)B * Tn;
+    return 4.0 * (el * c.cin + el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + (double)c.cin * c.cout * c.k);
+  }
+
+  // fp32 CUDA-core Conv1d; epi / gamma: Vocos' GELU or layer-scale residual epilogue in place of the branch mix
+  int conv(const ConvRef& c, int64_t B, const float* x, int64_t xsb, int64_t xsc, int64_t xst, float* y, int Tn,
+           float pre_slope, const float* residual, const float* acc_prev, float out_div, int post_tanh,
+           int epi = CONV_EPI_NONE, const float* gamma = nullptr) {
+    ConvParams p;
+    p.x = x; p.xsb = xsb; p.xsc = xsc; p.xst = xst;
+    p.w_t = g->fptr(c.w); p.bias = g->fptr(c.b);
+    p.residual = residual; p.acc_prev = acc_prev; p.y = y;
+    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d = c.d;
+    p.pre_slope = pre_slope; p.out_div = out_div; p.post_tanh = post_tanh; p.reflect = c.reflect;
+    p.epi = epi; p.gamma = gamma;
+    return timed(1, 2.0 * B * Tn * c.cout * c.cin * c.k, conv_bytes(c, B, Tn, residual, acc_prev),
+                 [&] { return launch_conv1d_fp32(p, st); });
+  }
+
+  // Conv1d c on the wgmma kernel, from fp32 x (lrelu(., pre_slope) in the loader) or the operand image ximg; with c2
+  // the ResBlock1 pair c -> lrelu(., pre_slope) -> c2 in one launch.  yimg: the image of lrelu(y, img_slope).  bytes:
+  // the launch's algorithmic HBM bytes; cls: the profile class, -1 for 0 on a pair / block-mode capable ResBlock conv
+  // and 4 on any other
+  int tc_conv(const ConvRef& c, const ConvRef* c2, int64_t B, const float* x, int64_t xsb, int64_t xsc, int64_t xst,
+              const uint16_t* ximg, float* y, uint16_t* yimg, int Tn, float pre_slope, const float* residual,
+              const float* acc_prev, float out_div, int post_tanh, double bytes, int cls = -1, float img_slope = 0.1f) {
+    TcConvParams p;
+    p.x = x; p.xsb = xsb; p.xsc = xsc; p.xst = xst; p.ximg = ximg; p.pre_slope = pre_slope;
+    p.w = g->tcptr(c.w); p.bias = g->fptr(c.b);
+    if (c2) { p.w2 = g->tcptr(c2->w); p.b2 = g->fptr(c2->b); p.mid_slope = pre_slope; }
+    p.residual = residual; p.acc_prev = acc_prev; p.out_div = out_div; p.post_tanh = post_tanh;
+    p.y = y; p.yimg = yimg; p.img_slope = img_slope;
+    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d_or_u = c.d;
+    p.precision = g->precision; p.reflect = c.reflect;
+    if (cls < 0) cls = c.cin == c.cout && tc_conv_supported(c.cin, c.k) ? 0 : 4;
+    return timed(cls, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes, [&] { return launch_tc_conv(p, st); });
+  }
+
+  // Activation1d: fp32 y and / or the 16-bit operand image yimg
+  int snake(const ActRef& a, int64_t B, const float* x, float* y, int C, int Tn, uint16_t* yimg = nullptr) {
+    SnakeParams p;
+    p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
+    p.x = x; p.y = y; p.alpha = g->fptr(a.alpha); p.beta = g->fptr(a.beta);
+    p.f_up = g->fptr(a.fup); p.f_down = g->fptr(a.fdown);
+    auto kc = g->act_coef.find(a.fup);
+    if (kc != g->act_coef.end()) { p.kc = kc->second; p.have_kc = 1; }
+    p.fast_snake = g->precision != AB_PREC_FP32;
+    p.B = (int)B; p.C = C; p.T = Tn; p.logscale = g->cfg.snake_logscale;
+    return timed(3, 0.0, (double)B * C * Tn * (4.0 + (y ? 4.0 : 0.0) + (yimg ? 2.0 : 0.0)),
+                 [&] { return launch_activation1d(p, st); });
+  }
+
+  // LayerNorm over channels [after Vocos' depthwise conv, slots dw_w / dw_b >= 0] -> fp32 y or the operand image yimg
+  int norm(int64_t B, int C, int Tn, const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float eps, float* y,
+           uint16_t* yimg) {
+    NormParams p;
+    p.x = x; p.dw_w = g->fptr(dw_w); p.dw_b = g->fptr(dw_b); p.ln_w = g->fptr(ln_w); p.ln_b = g->fptr(ln_b);
+    p.y = y; p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
+    p.B = (int)B; p.C = C; p.T = Tn; p.eps = eps;
+    const double el = (double)B * Tn;
+    return timed(6, el * C * ((dw_w >= 0 ? 14.0 : 0.0) + 8.0), 4.0 * el * C + (y ? 4.0 * el * C : 2.0 * el * rup16(C)),
+                 [&] { return launch_vocos_norm(p, st); });
+  }
+
+  // The last layer of a forward in contiguous batch chunks, chunk(b0, nb) each, and an event after each
+  // (ab_generator_set_tail_events): the caller's final gather of chunk i then runs under chunk i+1.  Runs nothing when
+  // rc is an error; consumes the tail events and nsf_source_frames either way.
+  template <class F>
+  int tail(int64_t B, int rc, F chunk) {
+    const size_t ne = g->tail_events.size();
+    const int nchunk = ne == 0 ? 1 : (int)std::min<int64_t>((int64_t)ne, B);
+    for (int ci = 0; rc == AB_OK && ci < nchunk; ++ci) {
+      const int64_t b0 = B * ci / nchunk, b1 = B * (ci + 1) / nchunk;
+      rc = chunk(b0, b1 - b0);
+      // when there are more events than utterances the surplus events fire with the last chunk
+      if (rc == AB_OK)
+        for (size_t e = ne * ci / nchunk; e < ne * (ci + 1) / nchunk; ++e) cudaEventRecord(g->tail_events[e], st);
+    }
+    g->tail_events.clear();
+    g->source_frames = 0;
+    return rc;
+  }
+};
 
 // Output length of the FACodec encoder's strided conv (k = 2s, padding s//2 + s%2) over t samples; 0 when the input is
 // empty or the padded input is shorter than the kernel (Conv1d raises), so an emptied stage stays empty
@@ -1091,9 +1233,30 @@ size_t stage_max(const ab_generator* g, int64_t B, int64_t T, bool image) {
   return mx;
 }
 
-size_t stage_max_image_bytes(const ab_generator* g, int64_t B, int64_t T) { return stage_max(g, B, T, true); }
+// Workspace of the generator pipeline: NBUF fp32 stage buffers and NIMG 16-bit operand images; FACodec's decoder and
+// redecoder then the FiLM output (fp32, or conv_pre's operand image) and the style [B][2C].  Returns its size.
+struct GanWs {
+  float* buf[NBUF];
+  uint16_t* img[NIMG];
+  char* film;
+  float* style;
+};
 
-size_t stage_max_elems(const ab_generator* g, int64_t B, int64_t T) { return stage_max(g, B, T, false); }
+size_t gan_layout(const ab_generator* g, int64_t B, int64_t T, char* base, GanWs* w) {
+  Carve c{base};
+  GanWs v = {};
+  const size_t bufsz = stage_max(g, B, T, false) * sizeof(float), imgsz = stage_max(g, B, T, true);
+  for (float*& b : v.buf) b = c.take(bufsz);
+  for (uint16_t*& i : v.img) i = c.take<uint16_t>(imgsz);
+  if (g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER) {
+    const int C = g->cfg.n_mel;
+    v.film = c.take<char>(std::max((size_t)B * C * T * sizeof(float), tc_act_image_bytes(B, C, T)));
+    v.style = c.take((size_t)B * 2 * C * sizeof(float));
+  }
+  if (w) *w = v;
+  return c.off;
+}
+
 // Vocos workspace: the fp32 residual stream X, the embed / final-norm output Y (fp32), the block input H and the
 // intermediate I (fp32 at AB_PREC_FP32, else 16-bit operand images; I also holds the fp32 head output), the spectrum S
 // [B*T][bins] complex and the iSTFT's workspace.  base == nullptr: sizes only.  0 when the iSTFT plan fails.
@@ -1109,21 +1272,20 @@ size_t vocos_layout(const ab_generator* g, int64_t B, int64_t T, char* base, Voc
   const size_t el = (size_t)B * T;
   const size_t ist = ab_istft_workspace_bytes(g->istft, B, T);
   if (ist == 0) return 0;
-  const size_t sz[6] = {el * D * 4, el * D * 4, fp32 ? el * D * 4 : tc_act_image_bytes(B, D, T),
-                        fp32 ? el * std::max(F, 2 * bins) * 4 : tc_act_image_bytes(B, F, T), el * bins * 8, ist};
-  char* p[6];
-  size_t off = 0;
-  for (int i = 0; i < 6; ++i) {
-    p[i] = base ? base + off : nullptr;
-    off += align_up(sz[i], 256);
-  }
-  if (w) {
-    w->X = reinterpret_cast<float*>(p[0]); w->Y = reinterpret_cast<float*>(p[1]); w->H = reinterpret_cast<float*>(p[2]);
-    w->I = reinterpret_cast<float*>(p[3]); w->S = reinterpret_cast<float*>(p[4]); w->ist = p[5]; w->ist_bytes = align_up(ist, 256);
-  }
-  return off;
+  Carve c{base};
+  VocosWs v;
+  v.X = c.take(el * D * 4);
+  v.Y = c.take(el * D * 4);
+  v.H = c.take(fp32 ? el * D * 4 : tc_act_image_bytes(B, D, T));
+  v.I = c.take(fp32 ? el * std::max(F, 2 * bins) * 4 : tc_act_image_bytes(B, F, T));
+  v.S = c.take(el * bins * 8);
+  v.ist = c.take<char>(ist);
+  v.ist_bytes = align_up(ist, 256);
+  if (w) *w = v;
+  return c.off;
 }
 }  // namespace
+}  // extern "C++"
 
 // NSF-HiFiGAN: length of stage i's output after `length = min(x.shape[-1], x_source.shape[-1])` (nsfhifigan.py:264-268).
 // noise_convs[i] = Conv1d(1, C, 2s, stride s, padding s/2), s = prod(rates[i+1:]) (:223-236; kernel 1 for the last stage),
@@ -1138,25 +1300,11 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
   return std::max<int64_t>(std::min(Tn, xs), 0);
 }
 
-// bytes of forward_impl's buffers (the stage buffers and operand images)
-static size_t gan_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
-  return NBUF * align_up(stage_max_elems(g, B, T) * sizeof(float), 256) +
-         NIMG * align_up(stage_max_image_bytes(g, B, T), 256);
-}
-
-// FACodec: forward_impl's buffers, then the FiLM output (fp32, or conv_pre's operand image) and the style [B][2C]
-static size_t facodec_film_bytes(const ab_generator* g, int64_t B, int64_t T) {
-  const int C = g->cfg.n_mel;
-  return align_up(std::max((size_t)B * C * T * sizeof(float), tc_act_image_bytes(B, C, T)), 256);
-}
-
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
   if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return 0;
-  if (g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER)
-    return gan_workspace_bytes(g, B, T) + facodec_film_bytes(g, B, T) + align_up((size_t)B * 2 * g->cfg.n_mel * sizeof(float), 256);
-  return gan_workspace_bytes(g, B, T);
+  return gan_layout(g, B, T, nullptr, nullptr);
 }
 
 int ab_generator_last_launches(const ab_generator* g) { return g ? g->launches : 0; }
@@ -1242,10 +1390,12 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
 // slower in block mode than as pairs on an H100 (DESIGN.md §6).
 static constexpr double kChainMaxRecompute = 1.5;
 
-// x_img (FACodec at tensor-core precision): conv_pre's input as an operand image, in place of dev_mel
-static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
-                        const float* dev_g, int64_t g_batch_stride, float* dev_wav, void* dev_workspace,
-                        size_t workspace_bytes, void* stream, const uint16_t* x_img = nullptr) {
+extern "C++" {
+namespace {
+// Checks every generator forward shares (ab_generator_forward[_cond], ab_facodec_inference, ab_facodec_encode)
+int check_forward(const ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
+                  const float* dev_g, int64_t g_batch_stride, const float* dev_wav, const void* dev_workspace,
+                  size_t workspace_bytes) {
   if (!g || !dev_mel || !dev_wav || !mel_strides) return fail(AB_ERR_ARG, "forward: null argument");
   if (dev_g != nullptr && g->cond_w < 0) return fail(AB_ERR_STATE, "forward: conditioning given but the generator has gin_channels == 0");
   if (dev_g != nullptr && g_batch_stride < g->cfg.gin_channels) return fail(AB_ERR_ARG, "forward: g row stride < gin_channels");
@@ -1256,11 +1406,9 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
   // FACodec's encoder: T counts input samples, and the stages shorten the sequence
   const bool enc = g->cfg.kind == AB_GEN_FACODEC_ENCODER;
   if ((int64_t)T * (enc ? 1 : g->hop) > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "forward: sequence too long");
-  const size_t need = ab_generator_workspace_bytes(g, B, T);
-  if (!dev_workspace || workspace_bytes < need) return fail(AB_ERR_WORKSPACE, "forward: workspace %zu B < required %zu B", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "forward: workspace must be 256-byte aligned");
-  const bool melgan = g->cfg.kind == AB_GEN_MELGAN;
-  if (melgan) {   // ReflectionPad1d(p) needs more than p samples (the reference raises a RuntimeError)
+  const int rc = check_workspace("forward", dev_workspace, workspace_bytes, ab_generator_workspace_bytes(g, B, T));
+  if (rc != AB_OK) return rc;
+  if (g->cfg.kind == AB_GEN_MELGAN) {   // ReflectionPad1d(p) needs more than p samples (the reference raises a RuntimeError)
     if (T <= 3) return fail(AB_ERR_ARG, "forward: conv_pre's ReflectionPad1d(3) needs more than 3 mel frames (got %lld)", (long long)T);
     int64_t t = T;
     for (size_t i = 0; i < g->stages.size(); ++i) {
@@ -1271,304 +1419,222 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
                       blk.dil[0], (long long)t);
     }
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t bufsz = align_up(stage_max_elems(g, B, T) * sizeof(float), 256);
-  const size_t imgsz = align_up(stage_max_image_bytes(g, B, T), 256);
-  float* buf[NBUF];
-  for (int i = 0; i < NBUF; ++i) buf[i] = reinterpret_cast<float*>(static_cast<char*>(dev_workspace) + i * bufsz);
-  uint16_t* img[NIMG];
-  for (int i = 0; i < NIMG; ++i)
-    img[i] = reinterpret_cast<uint16_t*>(static_cast<char*>(dev_workspace) + NBUF * bufsz + i * imgsz);
-  uint16_t *U16 = img[0], *P16[2] = {img[1], img[2]}, *R16 = img[3];
-  const uint16_t* r_img = nullptr;   // operand image of lrelu(stage input, 0.1) when the previous stage emitted it
-  float *R[2] = {buf[0], buf[1]}, *U = buf[2], *P[2] = {buf[3], buf[4]}, *TMP = buf[5], *ACT = buf[6];
+  return AB_OK;
+}
+
+// Vocos: x = norm(embed(x)), the ConvNeXt blocks, final_layer_norm, the head and the iSTFT (vocos.py:764-783, :343-360)
+int forward_vocos(Launch& L, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3], float* dev_wav,
+                  void* dev_workspace) {
+  ab_generator* g = L.g;
+  const VocosRef& v = g->vocos;
+  const ConvRef& cpre = g->conv_pre;
+  const int C0 = g->cfg.upsample_initial_channel, Tn = (int)T, bins = g->cfg.istft_n_fft / 2 + 1;
+  const bool tc = g->precision != AB_PREC_FP32;
+  VocosWs w;
+  if (vocos_layout(g, B, T, static_cast<char*>(dev_workspace), &w) == 0) return fail(AB_ERR_CUDA, "forward: iSTFT plan: %s", g_err);
+  uint16_t *Himg = reinterpret_cast<uint16_t*>(w.H), *Iimg = reinterpret_cast<uint16_t*>(w.I);
+  const double el = (double)B * T;
+  auto norm = [&](const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float* y, uint16_t* yimg) {
+    return L.norm(B, C0, Tn, x, dw_w, dw_b, ln_w, ln_b, 1e-6f, y, yimg);
+  };
+  // fp32 Linear over channels (k = 1 conv) with the GELU or layer-scale residual epilogue
+  auto linear_fp32 = [&](const ConvRef& c, const float* x, float* y, int epi, const float* gamma) {
+    return L.conv(c, B, x, (int64_t)c.cin * Tn, Tn, 1, y, Tn, 1.0f, epi == CONV_EPI_GAMMA_RESIDUAL ? y : nullptr, nullptr,
+                  1.0f, 0, epi, gamma);
+  };
+  // Linear over channels on the pointwise wgmma GEMM, from the operand image ximg
+  auto pointwise = [&](const ConvRef& c, int epi, const uint16_t* ximg, uint16_t* yimg, float* y, const float* gamma,
+                       float* spec) {
+    TcPwParams p;
+    p.epilogue = epi; p.ximg = ximg; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.gamma = gamma;
+    p.yimg = yimg; p.y = y; p.spec = spec;
+    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.precision = g->precision;
+    const double out = epi == AB_PW_GELU ? 2.0 * el * rup16(c.cout) : epi == AB_PW_GAMMA_RESIDUAL ? 8.0 * el * c.cout
+                                                                                                   : 8.0 * el * (c.cout / 2);
+    return L.timed(5, 2.0 * el * c.cin * c.cout, 2.0 * el * rup16(c.cin) + 2.0 * c.cin * c.cout + out,
+                   [&] { return launch_tc_pointwise(p, L.st); });
+  };
+  // x = norm(embed(x)) (vocos.py:764-772)
+  int rc = L.on_tc(cpre) ? L.tc_conv(cpre, nullptr, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, w.Y,
+                                     nullptr, Tn, 1.0f, nullptr, nullptr, 1.0f, 0, Launch::conv_bytes(cpre, B, Tn, nullptr, nullptr))
+                         : L.conv(cpre, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], w.Y, Tn, 1.0f, nullptr,
+                                  nullptr, 1.0f, 0);
+  if (rc == AB_OK) rc = norm(w.Y, -1, -1, v.norm_w, v.norm_b, w.X, nullptr);
+  // x = x + gamma * pwconv2(gelu(pwconv1(norm(dwconv(x))))) (vocos.py:509-527)
+  for (size_t i = 0; rc == AB_OK && i < v.blocks.size(); ++i) {
+    const VocosBlockRef& blk = v.blocks[i];
+    if (tc) {
+      rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, nullptr, Himg);
+      if (rc == AB_OK) rc = pointwise(blk.pw1, AB_PW_GELU, Himg, Iimg, nullptr, nullptr, nullptr);
+      if (rc == AB_OK) rc = pointwise(blk.pw2, AB_PW_GAMMA_RESIDUAL, Iimg, nullptr, w.X, g->fptr(blk.gamma), nullptr);
+    } else {
+      rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, w.H, nullptr);
+      if (rc == AB_OK) rc = linear_fp32(blk.pw1, w.H, w.I, CONV_EPI_GELU, nullptr);
+      if (rc == AB_OK) rc = linear_fp32(blk.pw2, w.I, w.X, CONV_EPI_GAMMA_RESIDUAL, g->fptr(blk.gamma));
+    }
+  }
+  // final_layer_norm (:781), then the head's Linear and S = min(exp(mag), 1e2) (cos p + i sin p) (:343-360)
+  if (rc == AB_OK) rc = norm(w.X, -1, -1, v.final_w, v.final_b, tc ? nullptr : w.Y, tc ? Himg : nullptr);
+  if (rc == AB_OK && tc) rc = pointwise(v.head, AB_PW_SPECTRUM, Himg, nullptr, nullptr, nullptr, w.S);
+  if (rc == AB_OK && !tc) {
+    rc = linear_fp32(v.head, w.Y, w.I, CONV_EPI_NONE, nullptr);
+    // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart
+    for (int64_t b = 0; rc == AB_OK && b < B; ++b) {
+      const float* hb = w.I + b * 2 * bins * T;
+      rc = L.counted(1, [&] {
+        return ab_spectral_head_forward(hb, hb + (int64_t)bins * T, nullptr, 1, bins, T, 1e2f, nullptr, nullptr, nullptr,
+                                        w.S + b * T * bins * 2, L.st);
+      });
+    }
+  }
+  // ISTFT "same" (:142-167)
+  return L.tail(B, rc, [&](int64_t b0, int64_t nb) {
+    return L.counted(2, [&] {
+      return ab_istft_forward(g->istft, w.S + b0 * T * bins * 2, nb, T, g->fptr(v.window), dev_wav + b0 * T * g->hop, w.ist,
+                              w.ist_bytes, L.st);
+    });
+  });
+}
+
+// The generator pipeline (HiFi-GAN, BigVGAN, NSF-HiFiGAN, the trunks, MelGAN, FACodec's generators and encoder), one
+// stage helper per step.  Between stages the stage input is R[cur_r]: cin channels of Tn samples.
+struct GanForward {
+  Launch& L;
+  ab_generator* g;
+  int64_t B;
   // FACodec's generator is BigVGAN's pipeline with an activation in front of each transposed conv; its encoder the same
   // ResidualUnits with an activation and a strided conv closing each stage
-  const bool fac = g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER;
-  const bool big = g->cfg.kind == AB_GEN_BIGVGAN || fac || enc;
-  const bool tc = g->precision != AB_PREC_FP32;
-  const int nk = g->cfg.num_kernels;
-  int launches = 0;
-  int rc;
-  // optional per-launch device timing
-  auto prof_begin = [&](int cls, double flops, double bytes) {
-    if (!g->profiling) return;
-    ab_generator::ProfRec r;
-    r.cls = cls; r.flops = flops; r.bytes = bytes;
-    r.e0 = g->get_event(); r.e1 = g->get_event();
-    cudaEventRecord(r.e0, st);
-    g->prof_recs.push_back(r);
-  };
-  auto prof_end = [&]() {
-    if (!g->profiling) return;
-    cudaEventRecord(g->prof_recs.back().e1, st);
-  };
+  bool melgan, fac, enc, big;
+  float *R[2], *U, *P[2], *TMP, *ACT;
+  uint16_t *U16, *P16[2], *R16;
+  const uint16_t* r_img = nullptr;   // operand image of lrelu(stage input, 0.1) when the previous stage emitted it
+  uint16_t* u_img = nullptr;         // operand image of lrelu(U, 0.1) when the ConvTranspose emitted it
+  int cur_r = 0, Tn, cin;
 
-  // algorithmic HBM bytes of a Conv1d launch with fp32 activations and weights (profile)
-  auto conv_bytes = [&](const ConvRef& c, int Tn, const float* residual, const float* acc_prev) {
-    const double el = (double)B * Tn;
-    return 4.0 * (el * c.cin + el * c.cout * (1 + (residual != nullptr) + (acc_prev != nullptr)) + (double)c.cin * c.cout * c.k);
-  };
-  // fp32 CUDA-core Conv1d
-  auto conv = [&](const ConvRef& c, const float* x, int64_t xsb, int64_t xsc, int64_t xst, float* y,
-                  int Tn, float pre_slope, const float* residual, const float* acc_prev, float out_div,
-                  int post_tanh) -> int {
-    ConvParams p;
-    p.x = x; p.xsb = xsb; p.xsc = xsc; p.xst = xst;
-    p.w_t = g->fptr(c.w); p.bias = g->fptr(c.b);
-    p.residual = residual; p.acc_prev = acc_prev; p.y = y;
-    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d = c.d;
-    p.pre_slope = pre_slope; p.out_div = out_div; p.post_tanh = post_tanh; p.reflect = c.reflect;
-    ++launches;
-    prof_begin(1, 2.0 * B * Tn * c.cout * c.cin * c.k, conv_bytes(c, Tn, residual, acc_prev));
-    const int r = launch_conv1d_fp32(p, st);
-    prof_end();
-    return r;
-  };
-  // whether conv c runs on the wgmma kernel (tc_image_bytes decided it at create)
-  auto on_tc = [&](const ConvRef& c) { return tc && g->slots[c.w].tc_bytes > 0; };
-  // Conv1d c on the wgmma kernel, from fp32 x (lrelu(., pre_slope) in the loader) or the operand image ximg; with c2
-  // the ResBlock1 pair c -> lrelu(., pre_slope) -> c2 in one launch.  bytes: the launch's algorithmic HBM bytes (profile)
-  auto tc_conv = [&](const ConvRef& c, const ConvRef* c2, const float* x, int64_t xsb, int64_t xsc, int64_t xst,
-                     const uint16_t* ximg, float* y, uint16_t* yimg, int Tn, float pre_slope, const float* residual,
-                     const float* acc_prev, float out_div, int post_tanh, double bytes) -> int {
-    TcConvParams p;
-    p.x = x; p.xsb = xsb; p.xsc = xsc; p.xst = xst; p.ximg = ximg; p.pre_slope = pre_slope;
-    p.w = g->tcptr(c.w); p.bias = g->fptr(c.b);
-    if (c2) { p.w2 = g->tcptr(c2->w); p.b2 = g->fptr(c2->b); p.mid_slope = pre_slope; }
-    p.residual = residual; p.acc_prev = acc_prev; p.out_div = out_div; p.post_tanh = post_tanh;
-    p.y = y; p.yimg = yimg; p.img_slope = 0.1f;
-    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = c.k; p.d_or_u = c.d;
-    p.precision = g->precision; p.reflect = c.reflect;
-    ++launches;
-    const bool rb = c.cin == c.cout && tc_conv_supported(c.cin, c.k);   // pair / block-mode capable ResBlock conv
-    prof_begin(rb ? 0 : 4, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes);
-    const int r = launch_tc_conv(p, st);
-    prof_end();
-    return r;
-  };
-  auto snake = [&](const ActRef& a, const float* x, float* y, int C, int Tn, uint16_t* yimg = nullptr) -> int {
-    SnakeParams p;
-    p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
-    p.x = x; p.y = y; p.alpha = g->fptr(a.alpha); p.beta = g->fptr(a.beta);
-    p.f_up = g->fptr(a.fup); p.f_down = g->fptr(a.fdown);
-    auto kc = g->act_coef.find(a.fup);
-    if (kc != g->act_coef.end()) { p.kc = kc->second; p.have_kc = 1; }
-    p.fast_snake = g->precision != AB_PREC_FP32;
-    p.B = (int)B; p.C = C; p.T = Tn; p.logscale = g->cfg.snake_logscale;
-    ++launches;
-    prof_begin(3, 0.0, (double)B * C * Tn * (4.0 + (y ? 4.0 : 0.0) + (yimg ? 2.0 : 0.0)));
-    const int r = launch_activation1d(p, st);
-    prof_end();
-    return r;
-  };
-  // conv_pre (hifigan.py:204, bigvgan.py:314)
-  const int C0 = g->cfg.upsample_initial_channel;
-  const ConvRef& cpre = g->conv_pre;
-  if (g->cfg.kind == AB_GEN_VOCOS) {
-    const VocosRef& v = g->vocos;
-    const int Tn = (int)T, bins = g->cfg.istft_n_fft / 2 + 1;
-    VocosWs w;
-    if (vocos_layout(g, B, T, static_cast<char*>(dev_workspace), &w) == 0) return fail(AB_ERR_CUDA, "forward: iSTFT plan: %s", g_err);
-    uint16_t *Himg = reinterpret_cast<uint16_t*>(w.H), *Iimg = reinterpret_cast<uint16_t*>(w.I);
-    const double el = (double)B * T;
-    auto rup16 = [](int c) { return (double)((c + 15) / 16 * 16); };
-    // LayerNorm over channels [after the depthwise conv] -> fp32 y or the operand image yimg
-    auto norm = [&](const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float* y, uint16_t* yimg) -> int {
-      NormParams p;
-      p.x = x; p.dw_w = g->fptr(dw_w); p.dw_b = g->fptr(dw_b); p.ln_w = g->fptr(ln_w); p.ln_b = g->fptr(ln_b);
-      p.y = y; p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
-      p.B = (int)B; p.C = C0; p.T = Tn; p.eps = 1e-6f;
-      ++launches;
-      prof_begin(6, el * C0 * ((dw_w >= 0 ? 14.0 : 0.0) + 8.0), 4.0 * el * C0 + (y ? 4.0 * el * C0 : 2.0 * el * rup16(C0)));
-      const int r = launch_vocos_norm(p, st);
-      prof_end();
-      return r;
-    };
-    // fp32 Linear over channels (k = 1 conv) with the GELU or layer-scale residual epilogue
-    auto linear_fp32 = [&](const ConvRef& c, const float* x, float* y, int epi, const float* gamma) -> int {
-      ConvParams p;
-      p.x = x; p.xsb = (int64_t)c.cin * Tn; p.xsc = Tn; p.xst = 1;
-      p.w_t = g->fptr(c.w); p.bias = g->fptr(c.b);
-      p.residual = epi == CONV_EPI_GAMMA_RESIDUAL ? y : nullptr; p.acc_prev = nullptr; p.y = y;
-      p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.k = 1; p.d = 1;
-      p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0; p.epi = epi; p.gamma = gamma;
-      ++launches;
-      prof_begin(1, 2.0 * el * c.cin * c.cout,
-                 4.0 * (el * c.cin + el * c.cout * (epi == CONV_EPI_GAMMA_RESIDUAL ? 2 : 1) + (double)c.cin * c.cout));
-      const int r = launch_conv1d_fp32(p, st);
-      prof_end();
-      return r;
-    };
-    // Linear over channels on the pointwise wgmma GEMM, from the operand image ximg
-    auto pointwise = [&](const ConvRef& c, int epi, const uint16_t* ximg, uint16_t* yimg, float* y, const float* gamma,
-                         float* spec) -> int {
-      TcPwParams p;
-      p.epilogue = epi; p.ximg = ximg; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.gamma = gamma;
-      p.yimg = yimg; p.y = y; p.spec = spec;
-      p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.precision = g->precision;
-      ++launches;
-      const double out = epi == AB_PW_GELU ? 2.0 * el * rup16(c.cout) : epi == AB_PW_GAMMA_RESIDUAL ? 8.0 * el * c.cout
-                                                                                                     : 8.0 * el * (c.cout / 2);
-      prof_begin(5, 2.0 * el * c.cin * c.cout, 2.0 * el * rup16(c.cin) + 2.0 * c.cin * c.cout + out);
-      const int r = launch_tc_pointwise(p, st);
-      prof_end();
-      return r;
-    };
-    // x = norm(embed(x)) (vocos.py:764-772)
-    rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, w.Y, nullptr, Tn,
-                               1.0f, nullptr, nullptr, 1.0f, 0, conv_bytes(cpre, Tn, nullptr, nullptr))
-                     : conv(cpre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], w.Y, Tn, 1.0f, nullptr, nullptr, 1.0f, 0);
-    if (rc == AB_OK) rc = norm(w.Y, -1, -1, v.norm_w, v.norm_b, w.X, nullptr);
-    // x = x + gamma * pwconv2(gelu(pwconv1(norm(dwconv(x))))) (vocos.py:509-527)
-    for (size_t i = 0; rc == AB_OK && i < v.blocks.size(); ++i) {
-      const VocosBlockRef& blk = v.blocks[i];
-      if (tc) {
-        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, nullptr, Himg);
-        if (rc == AB_OK) rc = pointwise(blk.pw1, AB_PW_GELU, Himg, Iimg, nullptr, nullptr, nullptr);
-        if (rc == AB_OK) rc = pointwise(blk.pw2, AB_PW_GAMMA_RESIDUAL, Iimg, nullptr, w.X, g->fptr(blk.gamma), nullptr);
-      } else {
-        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, w.H, nullptr);
-        if (rc == AB_OK) rc = linear_fp32(blk.pw1, w.H, w.I, CONV_EPI_GELU, nullptr);
-        if (rc == AB_OK) rc = linear_fp32(blk.pw2, w.I, w.X, CONV_EPI_GAMMA_RESIDUAL, g->fptr(blk.gamma));
-      }
-    }
-    // final_layer_norm (:781), then the head's Linear and S = min(exp(mag), 1e2) (cos p + i sin p) (:343-360)
-    if (rc == AB_OK) rc = norm(w.X, -1, -1, v.final_w, v.final_b, tc ? nullptr : w.Y, tc ? Himg : nullptr);
-    if (rc == AB_OK && tc) rc = pointwise(v.head, AB_PW_SPECTRUM, Himg, nullptr, nullptr, nullptr, w.S);
-    if (rc == AB_OK && !tc) {
-      rc = linear_fp32(v.head, w.Y, w.I, CONV_EPI_NONE, nullptr);
-      // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart
-      for (int64_t b = 0; rc == AB_OK && b < B; ++b) {
-        const float* hb = w.I + b * 2 * bins * T;
-        ++launches;
-        rc = ab_spectral_head_forward(hb, hb + (int64_t)bins * T, nullptr, 1, bins, T, 1e2f, nullptr, nullptr, nullptr,
-                                      w.S + b * T * bins * 2, stream);
-      }
-    }
-    // ISTFT "same" (:142-167) in contiguous batch chunks, an event after each (ab_generator_set_tail_events)
-    const int nchunk = g->tail_events.empty() ? 1 : (int)std::min<int64_t>((int64_t)g->tail_events.size(), B);
-    for (int ci = 0; rc == AB_OK && ci < nchunk; ++ci) {
-      const int64_t b0 = B * ci / nchunk, b1 = B * (ci + 1) / nchunk;
-      launches += 2;
-      rc = ab_istft_forward(g->istft, w.S + b0 * T * bins * 2, b1 - b0, T, g->fptr(v.window), dev_wav + b0 * T * g->hop, w.ist,
-                            w.ist_bytes, stream);
-      if (rc == AB_OK && !g->tail_events.empty()) {
-        const size_t e0 = g->tail_events.size() * (size_t)ci / nchunk, e1 = g->tail_events.size() * (size_t)(ci + 1) / nchunk;
-        for (size_t e = e0; e < e1; ++e) cudaEventRecord(g->tail_events[e], st);
-      }
-    }
-    g->tail_events.clear();
-    g->source_frames = 0;
-    if (rc != AB_OK) return rc;
-    g->launches = launches;
-    return AB_OK;
+  GanForward(Launch& l, int64_t b, int64_t T, const GanWs& w) : L(l), g(l.g), B(b), Tn((int)T), cin(g->cfg.upsample_initial_channel) {
+    melgan = g->cfg.kind == AB_GEN_MELGAN;
+    fac = g->cfg.kind == AB_GEN_FACODEC || g->cfg.kind == AB_GEN_FACODEC_REDECODER;
+    enc = g->cfg.kind == AB_GEN_FACODEC_ENCODER;
+    big = g->cfg.kind == AB_GEN_BIGVGAN || fac || enc;
+    R[0] = w.buf[0]; R[1] = w.buf[1]; U = w.buf[2]; P[0] = w.buf[3]; P[1] = w.buf[4]; TMP = w.buf[5]; ACT = w.buf[6];
+    U16 = w.img[0]; P16[0] = w.img[1]; P16[1] = w.img[2]; R16 = w.img[3];
   }
-  // HiFi-GAN: a tensor-core stage-0 ConvTranspose reads lrelu(x, 0.1) -> conv_pre emits that operand image, unless the
-  // conditioning add changes x after it
-  const bool pre_img = !big && !melgan && dev_g == nullptr && on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&
-                       on_tc(g->stages[0].up) && (C0 % 16) == 0 &&
-                       tc_can_emit_image(0, cpre.cin, cpre.cout, cpre.k, cpre.d);
-  rc = on_tc(cpre) ? tc_conv(cpre, nullptr, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], x_img, R[0],
-                             pre_img ? R16 : nullptr, (int)T, 1.0f, nullptr, nullptr, 1.0f, 0,
-                             conv_bytes(cpre, (int)T, nullptr, nullptr) + (pre_img ? 2.0 * B * T * C0 : 0.0))
-                   : conv(cpre, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], R[0], (int)T, 1.0f,
-                          nullptr, nullptr, 1.0f, 0);
-  if (rc != AB_OK) return rc;
-  if (dev_g != nullptr) {   // x = x + cond(g)  (hifigan.py:429-430)
-    ++launches;
-    rc = launch_cond_add(R[0], dev_g, g_batch_stride, g->fptr(g->cond_w), g->fptr(g->cond_b), (int)B, C0,
-                         g->cfg.gin_channels, (int)T, st);
+
+  // conv_pre (hifigan.py:204, bigvgan.py:314), then HiFiGAN_vits' x = x + cond(g) (hifigan.py:429-430)
+  int pre(const float* dev_mel, const int64_t mel_strides[3], const uint16_t* x_img, const float* dev_g, int64_t g_batch_stride) {
+    const ConvRef& cpre = g->conv_pre;
+    const int C0 = cin;
+    // HiFi-GAN: a tensor-core stage-0 ConvTranspose reads lrelu(x, 0.1) -> conv_pre emits that operand image, unless the
+    // conditioning add changes x after it
+    const bool pre_img = !big && !melgan && dev_g == nullptr && L.on_tc(cpre) && !g->stages.empty() && g->stages[0].has_up &&
+                         L.on_tc(g->stages[0].up) && (C0 % 16) == 0 && tc_can_emit_image(0, cpre.cin, cpre.cout, cpre.k, cpre.d);
+    int rc = L.on_tc(cpre) ? L.tc_conv(cpre, nullptr, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], x_img, R[0],
+                                       pre_img ? R16 : nullptr, Tn, 1.0f, nullptr, nullptr, 1.0f, 0,
+                                       Launch::conv_bytes(cpre, B, Tn, nullptr, nullptr) + (pre_img ? 2.0 * B * Tn * C0 : 0.0))
+                           : L.conv(cpre, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], R[0], Tn, 1.0f, nullptr,
+                                    nullptr, 1.0f, 0);
     if (rc != AB_OK) return rc;
-  }
-  if (pre_img) r_img = R16;
-  int cur_r = 0;
-  int Tn = (int)T;
-  int cin = C0;
-  for (size_t i = 0; i < g->stages.size(); ++i) {
-    const StageRef& sg = g->stages[i];
-    // x = leaky_relu(x, 0.1) (HiFi-GAN only) ; x = ups[i](x)   (hifigan.py:206-207, bigvgan.py:316-318)
-    uint16_t* u_img = nullptr;
-    if (!sg.has_up) {
-      std::swap(U, R[cur_r]);   // AB_GEN_TRUNK: the blocks read conv_pre's output in place
-    } else {
-      const bool up_tc = on_tc(sg.up);
-      // FACodec: x = Activation1d(SnakeBeta)(x) in front of the transposed conv (facodec.py:224-232), as the operand
-      // image the tensor-core ConvTranspose reads or as fp32
-      const float* up_x = R[cur_r];
-      if (fac) {
-        const bool img = up_tc && (cin % 16) == 0;
-        rc = img ? snake(sg.act, R[cur_r], nullptr, cin, Tn, P16[0]) : snake(sg.act, R[cur_r], ACT, cin, Tn);
-        if (rc != AB_OK) return rc;
-        r_img = img ? P16[0] : nullptr;
-        up_x = ACT;
-      }
-      // x = leaky_relu(x, 0.2) ; x = ConvTranspose1d(k = 2u, padding u//2 + u%2, output_padding u%2) (melgan.py:72-80)
-      const float pre_slope = big ? 1.0f : melgan ? 0.2f : 0.1f;
-      ++launches;
-      const double eo = (double)B * sg.ch * Tn * sg.u;
-      prof_begin(up_tc ? 4 : 2, 2.0 * eo * cin * ((double)sg.up.k / sg.u),
-                 4.0 * ((double)B * cin * Tn + eo + (double)cin * sg.ch * sg.up.k));
-      if (up_tc) {
-        TcConvParams p;
-        p.mode = 1;
-        p.x = up_x; p.xsb = (int64_t)cin * Tn; p.xsc = Tn; p.xst = 1; p.pre_slope = pre_slope;
-        p.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr;
-        p.w = g->tcptr(sg.up.w); p.bias = g->fptr(sg.up.b); p.y = U;
-        // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
-        u_img = (!big && !melgan && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
-        p.yimg = u_img; p.img_slope = 0.1f;
-        p.B = (int)B; p.Cin = cin; p.Cout = sg.ch; p.T = Tn; p.k = sg.up.k; p.d_or_u = sg.u; p.precision = g->precision;
-        p.pad = melgan || fac ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
-        rc = launch_tc_conv(p, st);
-      } else {
-        ConvTParams tp;
-        tp.x = up_x; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
-        tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u; tp.pre_slope = pre_slope;
-        tp.pad = melgan || fac ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
-        rc = launch_conv_transpose1d_fp32(tp, st);
-      }
-      prof_end();
+    if (dev_g != nullptr) {
+      rc = L.counted(1, [&] {
+        return launch_cond_add(R[0], dev_g, g_batch_stride, g->fptr(g->cond_w), g->fptr(g->cond_b), (int)B, C0,
+                               g->cfg.gin_channels, Tn, L.st);
+      });
       if (rc != AB_OK) return rc;
     }
-    Tn *= sg.u;
-    const int C = sg.ch;
-    {
-      // NSF-HiFiGAN with a source shorter than this stage (short f0, odd source stride): the reference truncates x
-      // to the source length before the ResBlocks (nsfhifigan.py:264-268).  Compact the rows; the operand image
-      // (laid out for the untruncated length) is dropped for this stage.
-      const int64_t Lt = nsf_stage_length(g, (int)i, Tn, g->source_frames);
-      if (Lt < Tn) {
-        if (Lt <= 0) return fail(AB_ERR_ARG, "forward: the f0 track leaves no samples in stage %d", (int)i);
-        AB_CUDA_TRY(cudaMemcpy2DAsync(TMP, (size_t)Lt * sizeof(float), U, (size_t)Tn * sizeof(float), (size_t)Lt * sizeof(float),
-                                      (size_t)B * C, cudaMemcpyDeviceToDevice, st));
-        std::swap(U, TMP);
-        u_img = nullptr;
-        Tn = (int)Lt;
-      }
+    if (pre_img) r_img = R16;
+    return AB_OK;
+  }
+
+  // x = leaky_relu(x, 0.1) (HiFi-GAN only) ; x = ups[i](x)   (hifigan.py:206-207, bigvgan.py:316-318) into U, FACodec's
+  // Activation1d in front (facodec.py:224-232); MelGAN: leaky_relu(x, 0.2), padding u//2 + u%2 (melgan.py:72-80)
+  int up(const StageRef& sg) {
+    u_img = nullptr;
+    if (!sg.has_up) {
+      std::swap(U, R[cur_r]);   // AB_GEN_TRUNK: the blocks read conv_pre's output in place
+      return AB_OK;
     }
-    float* Rout = R[cur_r ^ 1];
-    const int64_t sb = (int64_t)C * Tn, sc = Tn;
-    bool stage_img_written = false;
-    // MelGAN: x <- shortcut(x) + c2(lrelu(c1(lrelu(x, 0.2), reflect-padded, dilation 3^j), 0.2)) for each ResnetBlock
-    // (melgan.py:34-47), as three launches: c1 -> TMP, c2 -> P0, shortcut + P0 -> the block output.  The outputs
-    // alternate between P1 and Rout so that the stage's last block writes Rout.
-    for (size_t j = 0; melgan && j < sg.blocks.size(); ++j) {
+    const bool up_tc = L.on_tc(sg.up);
+    const float* up_x = R[cur_r];
+    if (fac) {   // the activation writes the operand image the tensor-core ConvTranspose reads, or fp32
+      const bool img = up_tc && (cin % 16) == 0;
+      const int rc = img ? L.snake(sg.act, B, R[cur_r], nullptr, cin, Tn, P16[0]) : L.snake(sg.act, B, R[cur_r], ACT, cin, Tn);
+      if (rc != AB_OK) return rc;
+      r_img = img ? P16[0] : nullptr;
+      up_x = ACT;
+    }
+    const float pre_slope = big ? 1.0f : melgan ? 0.2f : 0.1f;
+    const int pad = melgan || fac ? sg.u / 2 + sg.u % 2 : (sg.up.k - sg.u) / 2;
+    // HiFi-GAN: every consumer of U applies lrelu(., 0.1) first (hifigan.py:95) -> emit that operand image
+    if (up_tc) u_img = (!big && !melgan && tc_can_emit_image(1, cin, sg.ch, sg.up.k, sg.u)) ? U16 : nullptr;
+    const double eo = (double)B * sg.ch * Tn * sg.u;
+    return L.timed(up_tc ? 4 : 2, 2.0 * eo * cin * ((double)sg.up.k / sg.u),
+                   4.0 * ((double)B * cin * Tn + eo + (double)cin * sg.ch * sg.up.k), [&] {
+                     if (up_tc) {
+                       TcConvParams p;
+                       p.mode = 1;
+                       p.x = up_x; p.xsb = (int64_t)cin * Tn; p.xsc = Tn; p.xst = 1; p.pre_slope = pre_slope;
+                       p.ximg = (r_img != nullptr && (cin % 16) == 0) ? r_img : nullptr;
+                       p.w = g->tcptr(sg.up.w); p.bias = g->fptr(sg.up.b); p.y = U;
+                       p.yimg = u_img; p.img_slope = 0.1f;
+                       p.B = (int)B; p.Cin = cin; p.Cout = sg.ch; p.T = Tn; p.k = sg.up.k; p.d_or_u = sg.u;
+                       p.precision = g->precision; p.pad = pad;
+                       return launch_tc_conv(p, L.st);
+                     }
+                     ConvTParams tp;
+                     tp.x = up_x; tp.w_t = g->fptr(sg.up.w); tp.bias = g->fptr(sg.up.b); tp.y = U;
+                     tp.B = (int)B; tp.Cin = cin; tp.Cout = sg.ch; tp.Tin = Tn; tp.k = sg.up.k; tp.u = sg.u;
+                     tp.pre_slope = pre_slope; tp.pad = pad;
+                     return launch_conv_transpose1d_fp32(tp, L.st);
+                   });
+  }
+
+  // NSF-HiFiGAN with a source shorter than stage i (short f0, odd source stride): the reference truncates x to the
+  // source length before the ResBlocks (nsfhifigan.py:264-268).  Compact the rows of U (C channels); the operand image
+  // (laid out for the untruncated length) is dropped for this stage.
+  int nsf_truncate(int i, int C) {
+    const int64_t Lt = nsf_stage_length(g, i, Tn, g->source_frames);
+    if (Lt >= Tn) return AB_OK;
+    if (Lt <= 0) return fail(AB_ERR_ARG, "forward: the f0 track leaves no samples in stage %d", i);
+    AB_CUDA_TRY(cudaMemcpy2DAsync(TMP, (size_t)Lt * sizeof(float), U, (size_t)Tn * sizeof(float), (size_t)Lt * sizeof(float),
+                                  (size_t)B * C, cudaMemcpyDeviceToDevice, L.st));
+    std::swap(U, TMP);
+    u_img = nullptr;
+    Tn = (int)Lt;
+    return AB_OK;
+  }
+
+  // MelGAN: x <- shortcut(x) + c2(lrelu(c1(lrelu(x, 0.2), reflect-padded, dilation 3^j), 0.2)) for each ResnetBlock
+  // (melgan.py:34-47), as three launches: c1 -> TMP, c2 -> P0, shortcut + P0 -> the block output.  The outputs
+  // alternate between P1 and Rout so that the stage's last block writes Rout.
+  int melgan_blocks(const StageRef& sg, float* Rout) {
+    const int64_t sb = (int64_t)sg.ch * Tn;
+    auto run = [&](const ConvRef& c, const float* x, float* y, float slope, const float* acc_prev) -> int {
+      if (!L.on_tc(c)) return L.conv(c, B, x, sb, Tn, 1, y, Tn, slope, nullptr, acc_prev, 1.0f, 0);
+      const double el = (double)B * Tn;
+      return L.tc_conv(c, nullptr, B, x, sb, Tn, 1, nullptr, y, nullptr, Tn, slope, nullptr, acc_prev, 1.0f, 0,
+                       4.0 * el * c.cout * (1 + (acc_prev != nullptr)) + 4.0 * el * c.cin + 2.0 * c.cin * c.cout * c.k);
+    };
+    for (size_t j = 0; j < sg.blocks.size(); ++j) {
       const BlockRef& blk = sg.blocks[j];
       const float* cur = j == 0 ? U : ((sg.blocks.size() - j) % 2 == 0 ? Rout : P[1]);
       float* dst = (sg.blocks.size() - 1 - j) % 2 == 0 ? Rout : P[1];
-      auto run = [&](const ConvRef& c, const float* x, float* y, float slope, const float* acc_prev) -> int {
-        if (!on_tc(c)) return conv(c, x, sb, sc, 1, y, Tn, slope, nullptr, acc_prev, 1.0f, 0);
-        const double el = (double)B * Tn;
-        return tc_conv(c, nullptr, x, sb, sc, 1, nullptr, y, nullptr, Tn, slope, nullptr, acc_prev, 1.0f, 0,
-                       4.0 * el * c.cout * (1 + (acc_prev != nullptr)) + 4.0 * el * c.cin + 2.0 * c.cin * c.cout * c.k);
-      };
-      rc = run(blk.c1[0], cur, TMP, 0.2f, nullptr);
+      int rc = run(blk.c1[0], cur, TMP, 0.2f, nullptr);
       if (rc == AB_OK) rc = run(blk.c2[0], TMP, P[0], 0.2f, nullptr);
       if (rc == AB_OK) rc = run(blk.sc, cur, dst, 1.0f, P[0]);   // shortcut(x) + block(x)
       if (rc != AB_OK) return rc;
     }
-    for (int j = 0; !melgan && j < nk; ++j) {
+    return AB_OK;
+  }
+
+  // The ResBlocks / AMPBlocks of stage i on U into Rout: xs = rb_0(x) ; xs += rb_j(x) ; x = xs / num_kernels
+  // (hifigan.py:208-214), each block in one launch (block mode), as fused pairs or as single convs.  Sets r_img for the
+  // next stage.
+  int blocks(size_t i, const StageRef& sg, float* Rout) {
+    const int C = sg.ch, nk = g->cfg.num_kernels;
+    const int64_t sb = (int64_t)C * Tn, sc = Tn;
+    bool stage_img_written = false;
+    int rc;
+    for (int j = 0; j < nk; ++j) {
       const BlockRef& blk = sg.blocks[j];
       const float* cur = U;
       const uint16_t* cur_img = u_img;
@@ -1577,7 +1643,7 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
       const bool pair = !blk.c2.empty();
       const int ncv = pair ? 2 : 1;
       // every conv of a block has a weight image or none; fused: pair / block mode (HiFi-GAN) and tc_conv launch class
-      const bool blk_tc = on_tc(blk.c1[0]);
+      const bool blk_tc = L.on_tc(blk.c1[0]);
       const bool fused = blk_tc && tc_conv_supported(C, blk.k);
       if (fused && !big && g->rb_mode >= 2 && nd <= AB_TC_CHAIN_MAX_PAIRS) {
         // whole block in one launch when the halo recompute costs less than the per-pair HBM round trips of x
@@ -1600,11 +1666,9 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
           cp.npairs = nd; cp.nconv = ncv; cp.B = (int)B; cp.C = C; cp.T = Tn; cp.k = blk.k;
           cp.slope = 0.1f; cp.img_slope = 0.1f; cp.out_div = j == nk - 1 ? (float)nk : 1.0f;
           cp.precision = g->precision;
-          ++launches;
           const double el = (double)B * C * Tn;
-          prof_begin(0, 2.0 * el * C * blk.k * ncv * nd, 4.0 * (el * (2 + (j > 0)) + (double)ncv * nd * C * C * blk.k));
-          rc = launch_tc_chain(cp, st);
-          prof_end();
+          rc = L.timed(0, 2.0 * el * C * blk.k * ncv * nd, 4.0 * (el * (2 + (j > 0)) + (double)ncv * nd * C * C * blk.k),
+                       [&] { return launch_tc_chain(cp, L.st); });
           if (rc != AB_OK) return rc;
           if (stage_img) stage_img_written = true;
           continue;
@@ -1630,12 +1694,12 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
           img = blk_tc ? P16[0] : nullptr;
           in = blk_tc ? x : ACT;
           slope = 1.0f;
-          const int r = blk_tc ? snake(*a, x, nullptr, C, Tn, P16[0]) : snake(*a, x, ACT, C, Tn);
+          const int r = blk_tc ? L.snake(*a, B, x, nullptr, C, Tn, P16[0]) : L.snake(*a, B, x, ACT, C, Tn);
           if (r != AB_OK) return r;
         }
-        if (!blk_tc) return conv(c, in, sb, sc, 1, y, Tn, slope, residual, acc_prev, out_div, 0);
-        return tc_conv(c, nullptr, in, sb, sc, 1, img, y, nullptr, Tn, slope, residual, acc_prev, out_div, 0,
-                       rb_bytes(c, 1, x, residual, acc_prev));
+        if (!blk_tc) return L.conv(c, B, in, sb, sc, 1, y, Tn, slope, residual, acc_prev, out_div, 0);
+        return L.tc_conv(c, nullptr, B, in, sb, sc, 1, img, y, nullptr, Tn, slope, residual, acc_prev, out_div, 0,
+                         rb_bytes(c, 1, x, residual, acc_prev));
       };
       for (int p = 0; p < nd; ++p) {
         const bool last = p == nd - 1;
@@ -1645,12 +1709,11 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
         const bool stage_img = last && j == nk - 1 && !big && i + 1 < g->stages.size();
         if (stage_img) dst_img = R16;
         if (!last) pp ^= 1;
-        // xs = rb_0(x) ; xs += rb_j(x) ; x = xs / num_kernels  (hifigan.py:208-214)
         const float* accp = (last && j > 0) ? Rout : nullptr;
         const float div = (last && j == nk - 1) ? (float)nk : 1.0f;
         if (fused && !big) {
-          rc = tc_conv(blk.c1[p], pair ? &blk.c2[p] : nullptr, cur, sb, sc, 1, cur_img, dst, dst_img, Tn, 0.1f, cur, accp,
-                       div, 0, rb_bytes(blk.c1[p], ncv, cur, cur, accp));
+          rc = L.tc_conv(blk.c1[p], pair ? &blk.c2[p] : nullptr, B, cur, sb, sc, 1, cur_img, dst, dst_img, Tn, 0.1f, cur, accp,
+                         div, 0, rb_bytes(blk.c1[p], ncv, cur, cur, accp));
           if (rc != AB_OK) return rc;
           cur_img = dst_img;
           if (stage_img) stage_img_written = true;
@@ -1668,83 +1731,96 @@ static int forward_impl(ab_generator* g, const float* dev_mel, int64_t B, int64_
         cur = dst;
       }
     }
-    cur_r ^= 1;
-    cin = C;
     r_img = stage_img_written ? R16 : nullptr;
-    if (sg.down) {
-      // FACodec encoder: x = Conv1d(C, 2C, k = 2s, stride s, padding s//2 + s%2)(Activation1d(SnakeBeta)(x))
-      // (facodec.py:136-154); the activation writes the operand image the tensor-core conv reads, or fp32
-      const ConvRef& dc = sg.up;
-      const int sd = sg.down, pad = sd / 2 + sd % 2;
-      const bool dtc = on_tc(dc), img = dtc && (C % 16) == 0;
-      rc = img ? snake(sg.act, R[cur_r], nullptr, C, Tn, P16[0]) : snake(sg.act, R[cur_r], ACT, C, Tn);
-      if (rc != AB_OK) return rc;
-      const int To = (int)encoder_stage_length(Tn, sd);
-      float* dst = R[cur_r ^ 1];
-      ++launches;
-      prof_begin(dtc ? 4 : 1, 2.0 * B * To * dc.cout * dc.cin * dc.k,
-                 4.0 * ((double)B * C * Tn + (double)B * dc.cout * To + (double)dc.cin * dc.cout * dc.k));
-      if (dtc) {
-        TcConvParams p;
-        p.mode = 2;
-        p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1; p.ximg = img ? P16[0] : nullptr;
-        p.w = g->tcptr(dc.w); p.bias = g->fptr(dc.b); p.y = dst;
-        p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d_or_u = sd; p.pad = pad;
-        p.precision = g->precision;
-        rc = launch_tc_conv(p, st);
-      } else {
-        ConvParams p;
-        p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1;
-        p.w_t = g->fptr(dc.w); p.bias = g->fptr(dc.b); p.residual = nullptr; p.acc_prev = nullptr; p.y = dst;
-        p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d = 1;
-        p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0;
-        rc = launch_conv1d_strided_fp32(p, sd, pad, st);
-      }
-      prof_end();
-      if (rc != AB_OK) return rc;
-      cur_r ^= 1;
-      Tn = To;
-      cin = dc.cout;
-    }
+    return AB_OK;
   }
-  // post: leaky_relu(x) with the DEFAULT slope 0.01 (hifigan.py:215) or
-  // activation_post (bigvgan.py:327); conv_post; tanh
-  const float* xin = R[cur_r];
-  const int64_t sb = (int64_t)cin * Tn, sc = Tn;
-  if (big) {
-    rc = snake(g->act_post, xin, ACT, cin, Tn);
+
+  // FACodec encoder: x = Conv1d(C, 2C, k = 2s, stride s, padding s//2 + s%2)(Activation1d(SnakeBeta)(x))
+  // (facodec.py:136-154); the activation writes the operand image the tensor-core conv reads, or fp32
+  int down(const StageRef& sg) {
+    const ConvRef& dc = sg.up;
+    const int C = cin, sd = sg.down, pad = sd / 2 + sd % 2;
+    const bool dtc = L.on_tc(dc), img = dtc && (C % 16) == 0;
+    int rc = img ? L.snake(sg.act, B, R[cur_r], nullptr, C, Tn, P16[0]) : L.snake(sg.act, B, R[cur_r], ACT, C, Tn);
     if (rc != AB_OK) return rc;
-    xin = ACT;
+    const int To = (int)encoder_stage_length(Tn, sd);
+    float* dst = R[cur_r ^ 1];
+    rc = L.timed(dtc ? 4 : 1, 2.0 * B * To * dc.cout * dc.cin * dc.k,
+                 4.0 * ((double)B * C * Tn + (double)B * dc.cout * To + (double)dc.cin * dc.cout * dc.k), [&] {
+                   if (dtc) {
+                     TcConvParams p;
+                     p.mode = 2;
+                     p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1; p.ximg = img ? P16[0] : nullptr;
+                     p.w = g->tcptr(dc.w); p.bias = g->fptr(dc.b); p.y = dst;
+                     p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d_or_u = sd; p.pad = pad;
+                     p.precision = g->precision;
+                     return launch_tc_conv(p, L.st);
+                   }
+                   ConvParams p;
+                   p.x = ACT; p.xsb = (int64_t)C * Tn; p.xsc = Tn; p.xst = 1;
+                   p.w_t = g->fptr(dc.w); p.bias = g->fptr(dc.b); p.residual = nullptr; p.acc_prev = nullptr; p.y = dst;
+                   p.B = (int)B; p.Cin = C; p.Cout = dc.cout; p.T = Tn; p.k = dc.k; p.d = 1;
+                   p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0;
+                   return launch_conv1d_strided_fp32(p, sd, pad, L.st);
+                 });
+    if (rc != AB_OK) return rc;
+    cur_r ^= 1;
+    Tn = To;
+    cin = dc.cout;
+    return AB_OK;
   }
-  // conv_post in contiguous batch chunks, an event after each (ab_generator_set_tail_events): the caller's
-  // final gather of chunk i then runs under conv_post of chunk i+1
-  const int nchunk = g->tail_events.empty() ? 1 : (int)std::min<int64_t>((int64_t)g->tail_events.size(), B);
-  const int64_t Bfull = B;
-  const ConvRef& cpost = g->conv_post;
-  const float post_slope = big ? 1.0f : melgan ? 0.2f : 0.01f;
-  const int post_tanh = g->cfg.kind == AB_GEN_TRUNK || enc ? 0 : 1;
-  for (int ci = 0; ci < nchunk; ++ci) {
-    const int64_t b0 = Bfull * ci / nchunk, b1 = Bfull * (ci + 1) / nchunk;
-    B = b1 - b0;
-    const float* x = xin + b0 * sb;
-    float* y = dev_wav + b0 * cpost.cout * Tn;
-    rc = on_tc(cpost) ? tc_conv(cpost, nullptr, x, sb, sc, 1, nullptr, y, nullptr, Tn, post_slope, nullptr, nullptr, 1.0f,
-                                post_tanh, conv_bytes(cpost, Tn, nullptr, nullptr))
-                      : conv(cpost, x, sb, sc, 1, y, Tn, post_slope, nullptr, nullptr, 1.0f, post_tanh);
-    B = Bfull;
-    if (rc != AB_OK) break;
-    if (!g->tail_events.empty()) {
-      // when there are more events than utterances the surplus events fire with the last chunk
-      const size_t e0 = g->tail_events.size() * (size_t)ci / nchunk, e1 = g->tail_events.size() * (size_t)(ci + 1) / nchunk;
-      for (size_t e = e0; e < e1; ++e) cudaEventRecord(g->tail_events[e], st);
+
+  // post: leaky_relu(x) with the DEFAULT slope 0.01 (hifigan.py:215) or activation_post (bigvgan.py:327); conv_post;
+  // tanh.  conv_post runs in the tail chunks (Launch::tail).
+  int post(float* dev_wav) {
+    const float* xin = R[cur_r];
+    const int64_t sb = (int64_t)cin * Tn, sc = Tn;
+    if (big) {
+      const int rc = L.snake(g->act_post, B, xin, ACT, cin, Tn);
+      if (rc != AB_OK) return rc;
+      xin = ACT;
     }
+    const ConvRef& cpost = g->conv_post;
+    const float post_slope = big ? 1.0f : melgan ? 0.2f : 0.01f;
+    const int post_tanh = g->cfg.kind == AB_GEN_TRUNK || enc ? 0 : 1;
+    return L.tail(B, AB_OK, [&](int64_t b0, int64_t nb) {
+      const float* x = xin + b0 * sb;
+      float* y = dev_wav + b0 * cpost.cout * Tn;
+      return L.on_tc(cpost) ? L.tc_conv(cpost, nullptr, nb, x, sb, sc, 1, nullptr, y, nullptr, Tn, post_slope, nullptr, nullptr,
+                                        1.0f, post_tanh, Launch::conv_bytes(cpost, nb, Tn, nullptr, nullptr))
+                            : L.conv(cpost, nb, x, sb, sc, 1, y, Tn, post_slope, nullptr, nullptr, 1.0f, post_tanh);
+    });
   }
-  g->tail_events.clear();
-  g->source_frames = 0;
+};
+
+// A checked forward of any generator kind but DiffWave.  x_img (FACodec at tensor-core precision): conv_pre's input as
+// an operand image, in place of dev_mel.
+int forward_generator(Launch& L, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3], const float* dev_g,
+                      int64_t g_batch_stride, float* dev_wav, void* dev_workspace, size_t workspace_bytes,
+                      const uint16_t* x_img = nullptr) {
+  ab_generator* g = L.g;
+  int rc = check_forward(g, dev_mel, B, T, mel_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes);
   if (rc != AB_OK) return rc;
-  g->launches = launches;
-  return AB_OK;
+  if (g->cfg.kind == AB_GEN_VOCOS) return forward_vocos(L, dev_mel, B, T, mel_strides, dev_wav, dev_workspace);
+  GanWs w;
+  gan_layout(g, B, T, static_cast<char*>(dev_workspace), &w);
+  GanForward f(L, B, T, w);
+  if ((rc = f.pre(dev_mel, mel_strides, x_img, dev_g, g_batch_stride)) != AB_OK) return rc;
+  for (size_t i = 0; i < g->stages.size(); ++i) {
+    const StageRef& sg = g->stages[i];
+    if ((rc = f.up(sg)) != AB_OK) return rc;
+    f.Tn *= sg.u;
+    if ((rc = f.nsf_truncate((int)i, sg.ch)) != AB_OK) return rc;
+    float* Rout = f.R[f.cur_r ^ 1];
+    if ((rc = f.melgan ? f.melgan_blocks(sg, Rout) : f.blocks(i, sg, Rout)) != AB_OK) return rc;
+    f.cur_r ^= 1;
+    f.cin = sg.ch;
+    if (sg.down && (rc = f.down(sg)) != AB_OK) return rc;
+  }
+  return f.post(dev_wav);
 }
+}  // namespace
+}  // extern "C++"
 
 int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64_t T,
                          const int64_t mel_strides[3], float* dev_wav, void* dev_workspace,
@@ -1753,7 +1829,8 @@ int ab_generator_forward(ab_generator* g, const float* dev_mel, int64_t B, int64
     return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
-  return forward_impl(g, dev_mel, B, T, mel_strides, nullptr, 0, dev_wav, dev_workspace, workspace_bytes, stream);
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  return L.done(forward_generator(L, dev_mel, B, T, mel_strides, nullptr, 0, dev_wav, dev_workspace, workspace_bytes));
 }
 
 int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
@@ -1763,12 +1840,14 @@ int ab_generator_forward_cond(ab_generator* g, const float* dev_x, int64_t B, in
     return fail(AB_ERR_ARG, "forward: a FACodec handle runs through ab_facodec_inference");
   if (g && g->cfg.kind == AB_GEN_FACODEC_ENCODER)
     return fail(AB_ERR_ARG, "forward: a FACodec encoder handle runs through ab_facodec_encode");
-  return forward_impl(g, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes, stream);
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  return L.done(forward_generator(L, dev_x, B, T, x_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes));
 }
 
 // ---------------------------------------------------------------------------
 // DiffWave
 // ---------------------------------------------------------------------------
+extern "C++" {
 namespace {
 // Workspace: the fp32 residual stream in two buffers X0 / X1 (layer l reads one and writes the other), the skip sum,
 // the upsampled mel [B, n_mel, L], then the diffusion projections [n_steps][layers][C] and the step values.
@@ -1778,17 +1857,15 @@ struct DiffWaveWs {
 
 size_t diffwave_layout(const ab_generator* g, int64_t B, int64_t T, int n_steps, char* base, DiffWaveWs* w) {
   const size_t L = (size_t)T * g->hop;
-  const size_t sz[6] = {B * DW_CHANNELS * L * 4, B * DW_CHANNELS * L * 4, B * DW_CHANNELS * L * 4,
-                        B * (size_t)g->cfg.n_mel * L * 4, (size_t)n_steps * g->cfg.num_layers * DW_CHANNELS * 4,
-                        (size_t)n_steps * 4};
-  float* p[6];
-  size_t off = 0;
-  for (int i = 0; i < 6; ++i) {
-    p[i] = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += align_up(sz[i], 256);
-  }
-  if (w) *w = {{p[0], p[1]}, p[2], p[3], p[4], p[5]};
-  return off;
+  Carve c{base};
+  DiffWaveWs v;
+  for (float*& x : v.X) x = c.take(B * DW_CHANNELS * L * 4);
+  v.S = c.take(B * DW_CHANNELS * L * 4);
+  v.M = c.take(B * (size_t)g->cfg.n_mel * L * 4);
+  v.D = c.take((size_t)n_steps * g->cfg.num_layers * DW_CHANNELS * 4);
+  v.steps = c.take((size_t)n_steps * 4);
+  if (w) *w = v;
+  return c.off;
 }
 
 int diffwave_check(const ab_generator* g, int64_t B, int64_t T, int n_steps, void* ws, size_t ws_bytes, const char* what) {
@@ -1798,37 +1875,13 @@ int diffwave_check(const ab_generator* g, int64_t B, int64_t T, int n_steps, voi
   if (B <= 0 || T <= 0 || B > 65535) return fail(AB_ERR_ARG, "%s: batch %lld / frames %lld out of range", what, (long long)B, (long long)T);
   if (T * g->hop > (1ll << 30) || B * (int64_t)std::max(DW_CHANNELS, g->cfg.n_mel) * T * g->hop > (1ll << 40))
     return fail(AB_ERR_UNSUPPORTED, "%s: sequence too long", what);
-  const size_t need = diffwave_layout(g, B, T, n_steps, nullptr, nullptr);
-  if (!ws || ws_bytes < need) return fail(AB_ERR_WORKSPACE, "%s: workspace %zu B < required %zu B", what, ws_bytes, need);
-  if (reinterpret_cast<uintptr_t>(ws) & 255) return fail(AB_ERR_ARG, "%s: workspace must be 256-byte aligned", what);
-  return AB_OK;
+  return check_workspace(what, ws, ws_bytes, diffwave_layout(g, B, T, n_steps, nullptr, nullptr));
 }
 
-// per-launch device timing (ab_generator_set_profiling), classes 7-10
-struct DwProf {
-  ab_generator* g;
-  cudaStream_t st;
-  void begin(int cls, double flops, double bytes) {
-    if (!g->profiling) return;
-    ab_generator::ProfRec r;
-    r.cls = cls; r.flops = flops; r.bytes = bytes;
-    r.e0 = g->get_event(); r.e1 = g->get_event();
-    cudaEventRecord(r.e0, st);
-    g->prof_recs.push_back(r);
-  }
-  void end() {
-    if (g->profiling) cudaEventRecord(g->prof_recs.back().e1, st);
-  }
-};
-}  // namespace
-
-size_t ab_diffwave_workspace_bytes(const ab_generator* g, int64_t B, int64_t T, int32_t n_steps) {
-  if (!g || g->cfg.kind != AB_GEN_DIFFWAVE || B <= 0 || T <= 0 || n_steps <= 0) return 0;
-  return diffwave_layout(g, B, T, n_steps, nullptr, nullptr);
-}
-
-int ab_diffwave_condition(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
-                          const float* host_steps, int32_t n_steps, void* ws, size_t ws_bytes, void* stream) {
+// ab_diffwave_condition: the upsampled mel and the diffusion projections of every step
+int diffwave_condition(Launch& L, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
+                       const float* host_steps, int32_t n_steps, void* ws, size_t ws_bytes) {
+  ab_generator* g = L.g;
   if (!dev_mel || !mel_strides || !host_steps) return fail(AB_ERR_ARG, "diffwave_condition: null argument");
   if (n_steps <= 0 || n_steps > 65535) return fail(AB_ERR_ARG, "diffwave_condition: n_steps %d out of range", n_steps);
   int rc = diffwave_check(g, B, T, n_steps, ws, ws_bytes, "diffwave_condition");
@@ -1837,39 +1890,36 @@ int ab_diffwave_condition(ab_generator* g, const float* dev_mel, int64_t B, int6
     if (!(host_steps[i] >= 0.f) || !(ceilf(host_steps[i]) < (float)g->cfg.embedding_rows))
       return fail(AB_ERR_ARG, "diffwave_condition: diffusion step %g outside the embedding table [0, %d)", host_steps[i],
                   g->cfg.embedding_rows);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStream_t st = L.st;
   DiffWaveWs w;
   diffwave_layout(g, B, T, n_steps, static_cast<char*>(ws), &w);
   const DiffWaveRef& d = g->dw;
   const int nm = g->cfg.n_mel, nl = g->cfg.num_layers, C = DW_CHANNELS;
-  DwProf prof{g, st};
   g->dw.cond_B = 0;
   AB_CUDA_TRY(cudaMemcpyAsync(w.steps, host_steps, (size_t)n_steps * 4, cudaMemcpyHostToDevice, st));
   DwUpsampleParams up;
   up.mel = dev_mel; up.msb = mel_strides[0]; up.msc = mel_strides[1]; up.mst = mel_strides[2];
   up.w1 = g->fptr(d.wup[0]); up.b1 = g->fptr(d.bup[0]); up.w2 = g->fptr(d.wup[1]); up.b2 = g->fptr(d.bup[1]);
   up.out = w.M; up.B = (int)B; up.n_mel = nm; up.F = (int)T; up.f1 = g->cfg.upsample_rates[0]; up.f2 = g->cfg.upsample_rates[1];
-  const double L = (double)T * g->hop;
-  prof.begin(7, 2.0 * B * nm * L * 36.0, 4.0 * B * nm * (T + L));
-  rc = launch_dw_upsample(up, st);
-  prof.end();
+  const double Ls = (double)T * g->hop;
+  rc = L.timed(7, 2.0 * B * nm * Ls * 36.0, 4.0 * B * nm * (T + Ls), [&] { return launch_dw_upsample(up, st); });
   if (rc != AB_OK) return rc;
   DwEmbedParams e;
   const float* proj = reinterpret_cast<const float*>(g->arena + d.packed_offset) + nl * dw_layer_packed_floats(nm);
   e.steps = w.steps; e.table = g->fptr(d.table); e.w1 = g->fptr(d.wp1); e.b1 = g->fptr(d.bp1);
   e.w2 = g->fptr(d.wp2); e.b2 = g->fptr(d.bp2); e.wd = proj; e.bd = proj + (size_t)nl * C * 512; e.d = w.D; e.layers = nl;
-  prof.begin(7, 2.0 * n_steps * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512),
-             4.0 * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512 + (double)n_steps * nl * C));
-  rc = launch_dw_embed(e, n_steps, st);
-  prof.end();
+  rc = L.timed(7, 2.0 * n_steps * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512),
+               4.0 * (128.0 * 512 + 512.0 * 512 + (double)nl * C * 512 + (double)n_steps * nl * C),
+               [&] { return launch_dw_embed(e, n_steps, st); });
   if (rc != AB_OK) return rc;
   g->dw.cond_B = B; g->dw.cond_T = T; g->dw.cond_rows = n_steps;
-  g->launches = 2;
   return AB_OK;
 }
 
-int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t B, int64_t T, int32_t step_row, float c1, float c2,
-                     float sigma, const float* dev_noise, float* dev_eps, void* ws, size_t ws_bytes, void* stream) {
+// ab_diffwave_step: one pass of the network and the sampler update
+int diffwave_step(Launch& L, float* dev_audio, int64_t B, int64_t T, int32_t step_row, float c1, float c2, float sigma,
+                  const float* dev_noise, float* dev_eps, void* ws, size_t ws_bytes) {
+  ab_generator* g = L.g;
   if (!dev_audio) return fail(AB_ERR_ARG, "diffwave_step: null audio");
   if (!g || g->cfg.kind != AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "diffwave_step: not a DiffWave handle");
   if (g->dw.cond_B != B || g->dw.cond_T != T)
@@ -1880,19 +1930,15 @@ int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t B, int64_t T, in
   if (rc != AB_OK) return rc;
   if (step_row < -1 || step_row >= rows || (step_row == -1 && rows != B))
     return fail(AB_ERR_ARG, "diffwave_step: step row %d with %d conditioned steps and batch %lld", step_row, rows, (long long)B);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStream_t st = L.st;
   DiffWaveWs w;
   diffwave_layout(g, B, T, rows, static_cast<char*>(ws), &w);
   const DiffWaveRef& d = g->dw;
   const int nm = g->cfg.n_mel, nl = g->cfg.num_layers, C = DW_CHANNELS;
-  const int64_t L = T * g->hop;
-  const double el = (double)B * L;
-  DwProf prof{g, st};
-  int launches = 0;
-  ++launches;
-  prof.begin(8, 2.0 * el * C, 4.0 * el * (1 + C));
-  rc = launch_dw_input(dev_audio, g->fptr(d.win), g->fptr(d.bin), w.X[0], (int)B, L, st);
-  prof.end();
+  const int64_t Ls = T * g->hop;
+  const double el = (double)B * Ls;
+  rc = L.timed(8, 2.0 * el * C, 4.0 * el * (1 + C),
+               [&] { return launch_dw_input(dev_audio, g->fptr(d.win), g->fptr(d.bin), w.X[0], (int)B, Ls, st); });
   for (int l = 0; rc == AB_OK && l < nl; ++l) {
     DwLayerParams p;
     p.x_in = w.X[l & 1]; p.x_out = w.X[(l + 1) & 1]; p.skip = w.S; p.cond = w.M;
@@ -1900,25 +1946,37 @@ int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t B, int64_t T, in
     p.d_bstride = step_row < 0 ? (int64_t)nl * C : 0;
     const DwLayerPack lp = dw_layer_pack(g->arena + d.packed_offset, nm, l);
     p.w1 = lp.w1; p.b1 = lp.b1; p.w2 = lp.w2; p.b2 = lp.b2; p.w1h = lp.w1h; p.w2h = lp.w2h; p.precision = g->precision;
-    p.B = (int)B; p.n_mel = nm; p.dil = d.layers[l].dil; p.first = l == 0; p.L = L;
-    ++launches;
+    p.B = (int)B; p.n_mel = nm; p.dil = d.layers[l].dil; p.first = l == 0; p.L = Ls;
     // x read (3 taps, once from HBM), x written, skip read + written (stored by the first layer), mel read
-    prof.begin(9, 2.0 * el * 2 * C * (3 * C + nm + C), 4.0 * el * (C * (l == 0 ? 3 : 4) + nm));
-    rc = launch_dw_layer(p, st);
-    prof.end();
+    rc = L.timed(9, 2.0 * el * 2 * C * (3 * C + nm + C), 4.0 * el * (C * (l == 0 ? 3 : 4) + nm),
+                 [&] { return launch_dw_layer(p, st); });
   }
   if (rc != AB_OK) return rc;
   DwTailParams t;
   t.skip = w.S; t.wsk = g->fptr(d.wsk); t.bsk = g->fptr(d.bsk); t.wo = g->fptr(d.wo); t.bo = g->fptr(d.bo);
   t.skip_div = (float)sqrt((double)nl);
-  t.B = (int)B; t.L = L; t.eps = dev_eps; t.audio = dev_audio; t.noise = dev_noise; t.c1 = c1; t.c2 = c2; t.sigma = sigma;
-  ++launches;
-  prof.begin(10, 2.0 * el * (C * C + C), 4.0 * el * (C + (dev_eps ? 1 : 2) + (dev_noise ? 1 : 0)));
-  rc = launch_dw_tail(t, st);
-  prof.end();
-  if (rc != AB_OK) return rc;
-  g->launches = launches;
-  return AB_OK;
+  t.B = (int)B; t.L = Ls; t.eps = dev_eps; t.audio = dev_audio; t.noise = dev_noise; t.c1 = c1; t.c2 = c2; t.sigma = sigma;
+  return L.timed(10, 2.0 * el * (C * C + C), 4.0 * el * (C + (dev_eps ? 1 : 2) + (dev_noise ? 1 : 0)),
+                 [&] { return launch_dw_tail(t, st); });
+}
+}  // namespace
+}  // extern "C++"
+
+size_t ab_diffwave_workspace_bytes(const ab_generator* g, int64_t B, int64_t T, int32_t n_steps) {
+  if (!g || g->cfg.kind != AB_GEN_DIFFWAVE || B <= 0 || T <= 0 || n_steps <= 0) return 0;
+  return diffwave_layout(g, B, T, n_steps, nullptr, nullptr);
+}
+
+int ab_diffwave_condition(ab_generator* g, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3],
+                          const float* host_steps, int32_t n_steps, void* ws, size_t ws_bytes, void* stream) {
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  return L.done(diffwave_condition(L, dev_mel, B, T, mel_strides, host_steps, n_steps, ws, ws_bytes));
+}
+
+int ab_diffwave_step(ab_generator* g, float* dev_audio, int64_t B, int64_t T, int32_t step_row, float c1, float c2,
+                     float sigma, const float* dev_noise, float* dev_eps, void* ws, size_t ws_bytes, void* stream) {
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  return L.done(diffwave_step(L, dev_audio, B, T, step_row, c1, c2, sigma, dev_noise, dev_eps, ws, ws_bytes));
 }
 
 int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t B, int64_t T, const float* dev_mel,
@@ -1927,15 +1985,13 @@ int ab_diffwave_forward(ab_generator* g, const float* dev_audio, int64_t B, int6
   if (!dev_eps || !dev_audio) return fail(AB_ERR_ARG, "diffwave_forward: null argument");
   if (n_steps != 1 && n_steps != B)
     return fail(AB_ERR_ARG, "diffwave_forward: %d diffusion steps for a batch of %lld (need 1 or the batch)", n_steps, (long long)B);
-  int rc = ab_diffwave_condition(g, dev_mel, B, T, mel_strides, host_steps, n_steps, ws, ws_bytes, stream);
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  // the conditioning's count stands when the step then fails
+  const int rc = L.done(diffwave_condition(L, dev_mel, B, T, mel_strides, host_steps, n_steps, ws, ws_bytes));
   if (rc != AB_OK) return rc;
-  const int cond_launches = g->launches;
   // the audio is only read when eps is given
-  rc = ab_diffwave_step(g, const_cast<float*>(dev_audio), B, T, n_steps == 1 ? 0 : -1, 1.f, 0.f, 0.f, nullptr, dev_eps, ws,
-                        ws_bytes, stream);
-  if (rc != AB_OK) return rc;
-  g->launches += cond_launches;
-  return AB_OK;
+  return L.done(diffwave_step(L, const_cast<float*>(dev_audio), B, T, n_steps == 1 ? 0 : -1, 1.f, 0.f, 0.f, nullptr, dev_eps,
+                              ws, ws_bytes));
 }
 
 // ---------------------------------------------------------------------------
@@ -1978,15 +2034,11 @@ int ab_facodec_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t c
   p.group_end[0] = nq[0]; p.group_end[1] = n_pc; p.group_end[2] = n_all;
   p.ngroups = resid ? 3 : 2;
   p.B = (int)B; p.C = g->cfg.n_mel; p.T = (int)T; p.D = g->cfg.vq_codebook_dim; p.out = dev_out;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  DwProf prof{g, st};
+  Launch L{g, static_cast<cudaStream_t>(stream)};
   const double el = (double)B * T;
-  prof.begin(11, 2.0 * el * p.nq * p.C * p.D, 8.0 * el * p.nq + 4.0 * el * p.C + 4.0 * p.nq * (double)p.C * (p.D + 1));
-  rc = launch_facodec_vq2emb(p, st);
-  prof.end();
-  if (rc != AB_OK) return rc;
-  g->launches = 1;
-  return AB_OK;
+  rc = L.timed(11, 2.0 * el * p.nq * p.C * p.D, 8.0 * el * p.nq + 4.0 * el * p.C + 4.0 * p.nq * (double)p.C * (p.D + 1),
+               [&] { return launch_facodec_vq2emb(p, L.st); });
+  return L.done(rc);
 }
 
 int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t T, const int64_t x_strides[3],
@@ -1997,45 +2049,38 @@ int ab_facodec_inference(ab_generator* g, const float* dev_x, int64_t B, int64_t
     rc = fail(AB_ERR_ARG, "facodec_inference: null argument");
   const int C = g ? g->cfg.n_mel : 0;
   if (rc == AB_OK && spk_row_stride < C) rc = fail(AB_ERR_ARG, "facodec_inference: speaker-embedding row stride < %d", C);
-  const size_t need = ab_generator_workspace_bytes(g, B, T);
-  if (rc == AB_OK && (!dev_workspace || workspace_bytes < need))
-    rc = fail(AB_ERR_WORKSPACE, "facodec_inference: workspace %zu B < required %zu B", workspace_bytes, need);
-  if (rc == AB_OK && (reinterpret_cast<uintptr_t>(dev_workspace) & 255))
-    rc = fail(AB_ERR_ARG, "facodec_inference: workspace must be 256-byte aligned");
+  if (rc == AB_OK)
+    rc = check_workspace("facodec_inference", dev_workspace, workspace_bytes, ab_generator_workspace_bytes(g, B, T));
   if (rc != AB_OK) {
     if (g) g->tail_events.clear();
     return rc;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  char* film = static_cast<char*>(dev_workspace) + gan_workspace_bytes(g, B, T);
-  float* style = reinterpret_cast<float*>(film + facodec_film_bytes(g, B, T));
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  GanWs w;
+  gan_layout(g, B, T, static_cast<char*>(dev_workspace), &w);
   // conv_pre reads the FiLM output as its operand image when it runs on the wgmma kernel
-  const bool img = g->precision != AB_PREC_FP32 && g->slots[g->conv_pre.w].tc_bytes > 0;
-  DwProf prof{g, st};
+  const bool img = L.on_tc(g->conv_pre);
   const double el = (double)B * T;
-  prof.begin(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C));
-  rc = launch_facodec_style(dev_spk, spk_row_stride, g->fptr(g->fac.style_w), g->fptr(g->fac.style_b), style, (int)B, C, st);
-  prof.end();
+  rc = L.timed(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C), [&] {
+    return launch_facodec_style(dev_spk, spk_row_stride, g->fptr(g->fac.style_w), g->fptr(g->fac.style_b), w.style, (int)B, C,
+                                L.st);
+  });
   if (rc == AB_OK) {
     FacFilmParams p;
     p.x = dev_x; p.xsb = x_strides[0]; p.xsc = x_strides[1]; p.xst = x_strides[2];
-    p.style = style; p.y = img ? nullptr : reinterpret_cast<float*>(film);
-    p.yimg = img ? reinterpret_cast<uint16_t*>(film) : nullptr; p.bf16 = g->precision == AB_PREC_TC_BF16;
+    p.style = w.style; p.y = img ? nullptr : reinterpret_cast<float*>(w.film);
+    p.yimg = img ? reinterpret_cast<uint16_t*>(w.film) : nullptr; p.bf16 = g->precision == AB_PREC_TC_BF16;
     p.B = (int)B; p.C = C; p.T = (int)T;
-    prof.begin(11, 10.0 * el * C, 4.0 * el * C + (img ? 2.0 * el * ((C + 15) / 16 * 16) : 4.0 * el * C));
-    rc = launch_facodec_film(p, st);
-    prof.end();
+    rc = L.timed(11, 10.0 * el * C, 4.0 * el * C + (img ? 2.0 * el * rup16(C) : 4.0 * el * C),
+                 [&] { return launch_facodec_film(p, L.st); });
   }
   if (rc != AB_OK) {
     g->tail_events.clear();
     return rc;
   }
   const int64_t strides[3] = {(int64_t)C * T, T, 1};
-  rc = forward_impl(g, reinterpret_cast<const float*>(film), B, T, strides, nullptr, 0, dev_wav, dev_workspace,
-                    workspace_bytes, stream, img ? reinterpret_cast<const uint16_t*>(film) : nullptr);
-  if (rc != AB_OK) return rc;
-  g->launches += 2;
-  return AB_OK;
+  return L.done(forward_generator(L, reinterpret_cast<const float*>(w.film), B, T, strides, nullptr, 0, dev_wav, dev_workspace,
+                                  workspace_bytes, img ? reinterpret_cast<const uint16_t*>(w.film) : nullptr));
 }
 
 // FACodecDecoder.forward(vq=True): workspace of the timbre encoder.  S the fp32 stream [B, 256, T]; H a LayerNorm's
@@ -2045,72 +2090,58 @@ struct TimbreWs {
   float *S, *H, *QKV, *A, *F;
   uint16_t* FI;
 };
-static size_t timbre_layout(int64_t B, int64_t T, char* base, TimbreWs* w) {
+extern "C++" {
+static TimbreWs timbre_layout(Carve& c, int64_t B, int64_t T) {
   const size_t el = (size_t)B * T, C = FAC_TIMBRE_C;
-  const size_t sz[6] = {el * C * 4, el * C * 4, el * 3 * C * 4, el * C * 4, el * 4 * C * 4, tc_act_image_bytes(B, 4 * C, T)};
-  char* p[6];
-  size_t off = 0;
-  for (int i = 0; i < 6; ++i) {
-    p[i] = base ? base + off : nullptr;
-    off += align_up(sz[i], 256);
-  }
-  if (w) {
-    w->S = reinterpret_cast<float*>(p[0]); w->H = reinterpret_cast<float*>(p[1]); w->QKV = reinterpret_cast<float*>(p[2]);
-    w->A = reinterpret_cast<float*>(p[3]); w->F = reinterpret_cast<float*>(p[4]); w->FI = reinterpret_cast<uint16_t*>(p[5]);
-  }
-  return off;
+  TimbreWs w;
+  w.S = c.take(el * C * 4);
+  w.H = c.take(el * C * 4);
+  w.QKV = c.take(el * 3 * C * 4);
+  w.A = c.take(el * C * 4);
+  w.F = c.take(el * 4 * C * 4);
+  w.FI = c.take<uint16_t>(tc_act_image_bytes(B, 4 * C, T));
+  return w;
+}
+
+// FACodecRedecoder.vq2emb: the prosody transformer's workspace (TimbreWs), then the nine style vectors [9][B][2C]
+// (layer l's ln_1 at 2l, its ln_2 at 2l + 1, last_ln at 8)
+static TimbreWs redecoder_layout(Carve& c, int64_t B, int64_t T, float** styles) {
+  const TimbreWs w = timbre_layout(c, B, T);
+  *styles = c.take((size_t)9 * B * 2 * FAC_TIMBRE_C * sizeof(float));
+  return w;
 }
 
 // The four pre-LN layers of a FACodec transformer on the fp32 stream w.S (transformer.py:122-151): the decoder's timbre
 // encoder and the redecoder's prosody encoder differ only in their LayerNorms.  norm(layer, i, y, yimg) runs the
 // layer's ln_1 (i = 0) or ln_2 (i = 1) on w.S into y (fp32) or the operand image yimg.  Per layer: ln_1, the QKV GEMM,
 // the attention, out_proj onto S, ln_2, ffn_1 (k = 5; at 16 bits it also writes the image of its ReLU), ffn_2 onto S.
-extern "C++" {
 template <class Norm>
-static int facodec_transformer_layers(ab_generator* g, const TimbreWs& w, int64_t B, int Tn, DwProf& prof, int& launches,
-                                      Norm norm) {
-  cudaStream_t st = prof.st;
+static int facodec_transformer_layers(Launch& L, const TimbreWs& w, int64_t B, int Tn, Norm norm) {
+  ab_generator* g = L.g;
   const int C = FAC_TIMBRE_C;
   const bool tc = g->precision != AB_PREC_FP32;
   const double el = (double)B * Tn;
   const uint16_t* Himg = reinterpret_cast<const uint16_t*>(w.H);
-  // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual / acc_prev = y]
+  // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual = y]; all in profile class 0 at
+  // 16 bits, and the image of relu(y)
   auto gemm = [&](const ConvRef& c, const float* x, const uint16_t* ximg, float* y, bool residual, float pre_slope,
                   uint16_t* yimg) -> int {
-    ++launches;
-    prof.begin(tc ? 0 : 1, 2.0 * el * c.cin * c.cout * c.k,
-               el * c.cin * (tc ? 2.0 : 4.0) + 4.0 * el * c.cout * (residual ? 2 : 1) + (yimg ? 2.0 * el * c.cout : 0.0) +
-                   (tc ? 2.0 : 4.0) * c.cin * c.cout * c.k);
-    int r;
-    if (tc) {
-      TcConvParams t;
-      t.ximg = ximg; t.w = g->tcptr(c.w); t.bias = g->fptr(c.b);
-      t.acc_prev = residual ? y : nullptr; t.y = y; t.yimg = yimg; t.img_slope = 0.0f;
-      t.B = (int)B; t.Cin = c.cin; t.Cout = c.cout; t.T = Tn; t.k = c.k; t.d_or_u = 1; t.precision = g->precision;
-      r = launch_tc_conv(t, st);
-    } else {
-      // residual in place: each output element is read and then written by the same thread
-      ConvParams f;
-      f.x = x; f.xsb = (int64_t)c.cin * Tn; f.xsc = Tn; f.xst = 1;
-      f.w_t = g->fptr(c.w); f.bias = g->fptr(c.b);
-      f.residual = residual ? y : nullptr; f.acc_prev = nullptr; f.y = y;
-      f.B = (int)B; f.Cin = c.cin; f.Cout = c.cout; f.T = Tn; f.k = c.k; f.d = 1;
-      f.pre_slope = pre_slope; f.out_div = 1.0f; f.post_tanh = 0;
-      r = launch_conv1d_fp32(f, st);
-    }
-    prof.end();
-    return r;
+    // residual in place: each output element is read and then written by the same thread
+    if (!tc) return L.conv(c, B, x, (int64_t)c.cin * Tn, Tn, 1, y, Tn, pre_slope, residual ? y : nullptr, nullptr, 1.0f, 0);
+    return L.tc_conv(c, nullptr, B, nullptr, 0, 0, 0, ximg, y, yimg, Tn, 1.0f, nullptr, residual ? y : nullptr, 1.0f, 0,
+                     el * c.cin * 2.0 + 4.0 * el * c.cout * (residual ? 2 : 1) + (yimg ? 2.0 * el * c.cout : 0.0) +
+                         2.0 * c.cin * c.cout * c.k,
+                     0, 0.0f);
   };
   int rc;
   for (const TimbreLayerRef& t : g->fac.timbre) {
     // x = x + out_proj(MHA(LN1(x)))
     if ((rc = norm(t, 0, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
     if ((rc = gemm(t.qkv, w.H, Himg, w.QKV, false, 1.0f, nullptr)) != AB_OK) return rc;
-    ++launches;
-    prof.begin(13, 4.0 * B * (double)Tn * Tn * C, 4.0 * el * 3 * C + (tc ? 2.0 : 4.0) * el * C);
-    rc = launch_facodec_attention(w.QKV, tc ? nullptr : w.A, tc ? reinterpret_cast<uint16_t*>(w.A) : nullptr,
-                                  g->precision == AB_PREC_TC_BF16, (int)B, Tn, st);
-    prof.end();
+    rc = L.timed(13, 4.0 * B * (double)Tn * Tn * C, 4.0 * el * 3 * C + (tc ? 2.0 : 4.0) * el * C, [&] {
+      return launch_facodec_attention(w.QKV, tc ? nullptr : w.A, tc ? reinterpret_cast<uint16_t*>(w.A) : nullptr,
+                                      g->precision == AB_PREC_TC_BF16, (int)B, Tn, L.st);
+    });
     if (rc != AB_OK) return rc;
     if ((rc = gemm(t.out_proj, w.A, reinterpret_cast<const uint16_t*>(w.A), w.S, true, 1.0f, nullptr)) != AB_OK) return rc;
     // x = x + ffn_2(relu(ffn_1(LN2(x))))
@@ -2124,7 +2155,9 @@ static int facodec_transformer_layers(ab_generator* g, const TimbreWs& w, int64_
 
 size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || g->cfg.kind != AB_GEN_FACODEC || !g->cfg.facodec_quantize || B <= 0 || T <= 0) return 0;
-  return timbre_layout(B, T, nullptr, nullptr);
+  Carve c{nullptr};
+  timbre_layout(c, B, T);
+  return c.off;
 }
 
 int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t B, int64_t T,
@@ -2139,17 +2172,13 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
   if (n_quantizers < 1) return fail(AB_ERR_ARG, "facodec_quantize: n_quantizers %d < 1 (no layer would run)", n_quantizers);
   if (B > FAC_PE_ROWS)   // PositionalEncoding adds pe[:B] (transformer.py:43-45)
     return fail(AB_ERR_ARG, "facodec_quantize: batch %lld > %d, the rows of the positional encoding", (long long)B, FAC_PE_ROWS);
-  const size_t need = ab_facodec_quantize_workspace_bytes(g, B, T);
-  if (!dev_workspace || workspace_bytes < need)
-    return fail(AB_ERR_WORKSPACE, "facodec_quantize: workspace %zu B < required %zu B", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "facodec_quantize: workspace must be 256-byte aligned");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  TimbreWs w;
-  timbre_layout(B, T, static_cast<char*>(dev_workspace), &w);
+  rc = check_workspace("facodec_quantize", dev_workspace, workspace_bytes, ab_facodec_quantize_workspace_bytes(g, B, T));
+  if (rc != AB_OK) return rc;
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  Carve ws{static_cast<char*>(dev_workspace)};
+  const TimbreWs w = timbre_layout(ws, B, T);
   const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim, Tn = (int)T;
   const double el = (double)B * T;
-  int launches = 0;
-  DwProf prof{g, st};
 
   // the quantizers (all groups, one launch) and the positional add into S
   FacRvqParams p;
@@ -2178,59 +2207,34 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
   p.B = (int)B; p.C = C; p.T = Tn; p.D = D;
   p.emb = dev_emb_out; p.codes = dev_codes_out; p.quantized = dev_quantized_out;
   p.pe = g->fptr(g->fac.pe); p.stream = w.S;
-  {
-    double cb_flops = 0.0, cb_bytes = 0.0;
-    for (int q = 0; q < AB_FACODEC_MAX_Q; ++q)
-      if (p.cb[q]) { cb_flops += 2.0 * el * p.rows[q] * D; cb_bytes += 4.0 * p.rows[q] * (FAC_MAX_CODEBOOK_DIM + 1); }
-    ++launches;
-    prof.begin(12, 4.0 * el * nq_run * C * D + cb_flops,
-               4.0 * el * C * (2 + p.ngroups + 1) + 8.0 * el * n_used + cb_bytes + 8.0 * nq_run * (double)C * D);
-    rc = launch_facodec_rvq(p, st);
-    prof.end();
-    if (rc != AB_OK) return rc;
-  }
+  double cb_flops = 0.0, cb_bytes = 0.0;
+  for (int q = 0; q < AB_FACODEC_MAX_Q; ++q)
+    if (p.cb[q]) { cb_flops += 2.0 * el * p.rows[q] * D; cb_bytes += 4.0 * p.rows[q] * (FAC_MAX_CODEBOOK_DIM + 1); }
+  rc = L.timed(12, 4.0 * el * nq_run * C * D + cb_flops,
+               4.0 * el * C * (2 + p.ngroups + 1) + 8.0 * el * n_used + cb_bytes + 8.0 * nq_run * (double)C * D,
+               [&] { return launch_facodec_rvq(p, L.st); });
+  if (rc != AB_OK) return rc;
 
   // the timbre encoder on S (transformer.py:206-217)
-  auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) -> int {
-    NormParams n;
-    n.x = w.S; n.ln_w = g->fptr(lw); n.ln_b = g->fptr(lb);
-    n.y = y; n.yimg = yimg; n.bf16 = g->precision == AB_PREC_TC_BF16;
-    n.B = (int)B; n.C = C; n.T = Tn; n.eps = 1e-5f;
-    ++launches;
-    prof.begin(6, 8.0 * el * C, 4.0 * el * C + (y ? 4.0 : 2.0) * el * C);
-    const int r = launch_vocos_norm(n, st);
-    prof.end();
-    return r;
-  };
-  rc = facodec_transformer_layers(g, w, B, Tn, prof, launches,
-                                  [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
-                                    return i == 0 ? norm(t.ln1_w, t.ln1_b, y, yimg) : norm(t.ln2_w, t.ln2_b, y, yimg);
-                                  });
+  auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) { return L.norm(B, C, Tn, w.S, -1, -1, lw, lb, 1e-5f, y, yimg); };
+  rc = facodec_transformer_layers(L, w, B, Tn, [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
+    return i == 0 ? norm(t.ln1_w, t.ln1_b, y, yimg) : norm(t.ln2_w, t.ln2_b, y, yimg);
+  });
   if (rc != AB_OK) return rc;
   if ((rc = norm(g->fac.last_w, g->fac.last_b, w.H, nullptr)) != AB_OK) return rc;
-  ++launches;
-  prof.begin(12, el * C, 4.0 * el * C + 4.0 * B * C);
-  rc = launch_facodec_time_mean(w.H, dev_spk_out, (int)B, C, Tn, st);
-  prof.end();
-  if (rc != AB_OK) return rc;
-  g->launches = launches;
-  return AB_OK;
+  rc = L.timed(12, el * C, 4.0 * el * C + 4.0 * B * C, [&] { return launch_facodec_time_mean(w.H, dev_spk_out, (int)B, C, Tn, L.st); });
+  return L.done(rc);
 }
 
 // ---------------------------------------------------------------------------
 // FACodec redecoder
 // ---------------------------------------------------------------------------
-// FACodecRedecoder.vq2emb: the prosody transformer's workspace (TimbreWs), then the nine style vectors [9][B][2C]
-// (layer l's ln_1 at 2l, its ln_2 at 2l + 1, last_ln at 8)
-static size_t redecoder_layout(int64_t B, int64_t T, char* base, TimbreWs* w, float** styles) {
-  const size_t off = timbre_layout(B, T, base, w);
-  if (styles) *styles = base ? reinterpret_cast<float*>(base + off) : nullptr;
-  return off + align_up((size_t)9 * B * 2 * FAC_TIMBRE_C * sizeof(float), 256);
-}
-
 size_t ab_facodec_redecoder_vq2emb_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || g->cfg.kind != AB_GEN_FACODEC_REDECODER || B <= 0 || T <= 0) return 0;
-  return redecoder_layout(B, T, nullptr, nullptr, nullptr);
+  Carve c{nullptr};
+  float* styles;
+  redecoder_layout(c, B, T, &styles);
+  return c.off;
 }
 
 int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_q,
@@ -2250,18 +2254,14 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
   if (n_q < rows)
     return fail(AB_ERR_ARG, "%s: %d code rows; vq2emb reads %d (%d prosody, %d content, %d residual)", what, n_q, rows,
                 nq[0], nq[1], use_residual ? nq[2] : 0);
-  const size_t need = redecoder_layout(B, T, nullptr, nullptr, nullptr);
-  if (!dev_workspace || workspace_bytes < need)
-    return fail(AB_ERR_WORKSPACE, "%s: workspace %zu B < required %zu B", what, workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(dev_workspace) & 255) return fail(AB_ERR_ARG, "%s: workspace must be 256-byte aligned", what);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  TimbreWs w;
+  rc = check_workspace(what, dev_workspace, workspace_bytes, ab_facodec_redecoder_vq2emb_workspace_bytes(g, B, T));
+  if (rc != AB_OK) return rc;
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  Carve ws{static_cast<char*>(dev_workspace)};
   float* styles = nullptr;
-  redecoder_layout(B, T, static_cast<char*>(dev_workspace), &w, &styles);
+  const TimbreWs w = redecoder_layout(ws, B, T, &styles);
   const FacodecRef& f = g->fac;
   const double el = (double)B * T;
-  int launches = 0;
-  DwProf prof{g, st};
 
   // (gamma, beta) of every StyleAdaptiveLayerNorm from the speaker embedding (transformer.py:25): the condition is the
   // embedding expanded over time, whose time mean is the embedding itself
@@ -2269,10 +2269,9 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
   for (int i = 0; i < 9; ++i) {
     const int sw = i == 8 ? f.last_w : (i & 1) ? f.timbre[i / 2].ln2_w : f.timbre[i / 2].ln1_w;
     const int sb = i == 8 ? f.last_b : (i & 1) ? f.timbre[i / 2].ln2_b : f.timbre[i / 2].ln1_b;
-    ++launches;
-    prof.begin(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C));
-    rc = launch_facodec_style(dev_spk, spk_row_stride, g->fptr(sw), g->fptr(sb), style_of(i), (int)B, C, st);
-    prof.end();
+    rc = L.timed(11, 4.0 * B * C * C, 4.0 * (2.0 * C * C + B * 3.0 * C), [&] {
+      return launch_facodec_style(dev_spk, spk_row_stride, g->fptr(sw), g->fptr(sb), style_of(i), (int)B, C, L.st);
+    });
     if (rc != AB_OK) return rc;
   }
   // gamma * LayerNorm(S) + beta (transformer.py:29-31) into y (fp32) or the operand image yimg
@@ -2281,11 +2280,7 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
     p.x = w.S; p.xsb = (int64_t)C * T; p.xsc = T; p.xst = 1;
     p.style = style_of(i); p.y = y; p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
     p.B = (int)B; p.C = C; p.T = Tn;
-    ++launches;
-    prof.begin(11, 10.0 * el * C, 4.0 * el * C + (y ? 4.0 : 2.0) * el * C);
-    const int r = launch_facodec_film(p, st);
-    prof.end();
-    return r;
+    return L.timed(11, 10.0 * el * C, 4.0 * el * C + (y ? 4.0 : 2.0) * el * C, [&] { return launch_facodec_film(p, L.st); });
   };
   // the gathers: prev + the tables' rows (+ pe) -> out
   auto embed = [&](const float* prev, int row0, int ntab, const float* pe, float* out) -> int {
@@ -2296,27 +2291,20 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
     for (int j = 0; j < ntab; ++j) { p.tab[j] = g->fptr(f.layers[row0 + j].cb); p.rows[j] = f.layers[row0 + j].rows; }
     p.prev = prev; p.pe = pe; p.out = out;
     p.B = (int)B; p.C = C; p.T = Tn;
-    ++launches;
-    prof.begin(11, el * C * (ntab + (prev ? 1 : 0) + (pe ? 1 : 0) - 1),
-               8.0 * el * ntab + 4.0 * el * C * (ntab + 1 + (prev ? 1 : 0)));
-    const int r = launch_facodec_embed(p, st);
-    prof.end();
-    return r;
+    return L.timed(11, el * C * (ntab + (prev ? 1 : 0) + (pe ? 1 : 0) - 1), 8.0 * el * ntab + 4.0 * el * C * (ntab + 1 + (prev ? 1 : 0)),
+                   [&] { return launch_facodec_embed(p, L.st); });
   };
   // facodec.py:739-744: per prosody table, x_t = transformer(x_t + emb(codes)); the transformer adds pe each time
   for (int i = 0; i < nq[0]; ++i) {
     if ((rc = embed(i == 0 ? nullptr : w.H, i, 1, g->fptr(f.pe), w.S)) != AB_OK) return rc;
-    rc = facodec_transformer_layers(g, w, B, Tn, prof, launches,
-                                    [&](const TimbreLayerRef& t, int j, float* y, uint16_t* yimg) {
-                                      return film(2 * (int)(&t - f.timbre.data()) + j, y, yimg);
-                                    });
+    rc = facodec_transformer_layers(L, w, B, Tn, [&](const TimbreLayerRef& t, int j, float* y, uint16_t* yimg) {
+      return film(2 * (int)(&t - f.timbre.data()) + j, y, yimg);
+    });
     if (rc != AB_OK) return rc;
     if ((rc = film(8, w.H, nullptr)) != AB_OK) return rc;   // last_ln
   }
   // facodec.py:746-756: out = x_t, + the content rows, + the residual rows, one add at a time
-  if ((rc = embed(w.H, nq[0], rows - nq[0], nullptr, dev_out)) != AB_OK) return rc;
-  g->launches = launches;
-  return AB_OK;
+  return L.done(embed(w.H, nq[0], rows - nq[0], nullptr, dev_out));
 }
 
 // ---------------------------------------------------------------------------
@@ -2338,7 +2326,8 @@ int ab_facodec_encode(ab_generator* g, const float* dev_wav, int64_t B, int64_t 
   if (ab_facodec_encoder_frames(g, N) <= 0)
     return fail(AB_ERR_ARG, "facodec_encode: %lld samples leave a stage with no output (a strided conv's padded input is "
                 "shorter than its kernel)", (long long)N);
-  return forward_impl(g, dev_wav, B, N, wav_strides, nullptr, 0, dev_out, dev_workspace, workspace_bytes, stream);
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  return L.done(forward_generator(L, dev_wav, B, N, wav_strides, nullptr, 0, dev_out, dev_workspace, workspace_bytes));
 }
 
 // ---------------------------------------------------------------------------
