@@ -120,6 +120,12 @@ SIGNATURES = {
     "ab_tc_conv_forward": (C.c_int, [C.c_int32, _P, _I64P, C.c_float, _P, _P, _P, _P, _P, C.c_float, C.c_int32, _P, _P,
                                      C.c_float, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, _P, C.c_size_t, _P]),
+    "ab_vocos_norm_forward": (C.c_int, [_P, _P, _P, _P, _P, C.c_float, _P, _P, C.c_int32, C.c_int64, C.c_int64,
+                                        C.c_int64, _P]),
+    "ab_vocos_pointwise_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+                                                        C.c_int32]),
+    "ab_vocos_pointwise_forward": (C.c_int, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_int64,
+                                             C.c_int64, C.c_int64, C.c_int32, _P, C.c_size_t, _P]),
     "ab_diffwave_layer_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "ab_diffwave_layer_forward": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_int64,
                                             C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),

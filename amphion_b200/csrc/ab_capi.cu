@@ -2452,6 +2452,100 @@ int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides
   return launch_tc_conv(p, st);
 }
 
+int ab_vocos_norm_forward(const float* dev_x, const float* dev_dw_w, const float* dev_dw_b, const float* dev_ln_w,
+                          const float* dev_ln_b, float eps, float* dev_y, uint16_t* dev_yimg, int32_t precision, int64_t B,
+                          int64_t C, int64_t T, void* stream) {
+  if (!dev_x || !dev_ln_w || !dev_ln_b) return fail(AB_ERR_ARG, "vocos_norm: null argument");
+  if ((!dev_y) == (!dev_yimg)) return fail(AB_ERR_ARG, "vocos_norm: give exactly one of y and yimg");
+  if ((!dev_dw_w) != (!dev_dw_b)) return fail(AB_ERR_ARG, "vocos_norm: give both or neither of dw_w and dw_b");
+  if (dev_yimg && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
+    return fail(AB_ERR_ARG, "vocos_norm: the operand image needs a tensor-core precision (got %d)", precision);
+  if (B < 1 || C < 1 || T < 1 || B > INT32_MAX || C > INT32_MAX || T > (1ll << 30))
+    return fail(AB_ERR_ARG, "vocos_norm: batch %lld, %lld channels, length %lld", (long long)B, (long long)C, (long long)T);
+  NormParams p;
+  p.x = dev_x; p.dw_w = dev_dw_w; p.dw_b = dev_dw_b; p.ln_w = dev_ln_w; p.ln_b = dev_ln_b;
+  p.y = dev_y; p.yimg = dev_yimg; p.bf16 = precision == AB_PREC_TC_BF16;
+  p.B = (int)B; p.C = (int)C; p.T = (int)T; p.eps = eps;
+  return launch_vocos_norm(p, static_cast<cudaStream_t>(stream));
+}
+
+static_assert(AB_VOCOS_PW_GELU == AB_PW_GELU && AB_VOCOS_PW_GAMMA == AB_PW_GAMMA_RESIDUAL &&
+                  AB_VOCOS_PW_SPECTRUM == AB_PW_SPECTRUM,
+              "the public pointwise epilogues name launch_tc_pointwise's");
+
+size_t ab_vocos_pointwise_workspace_bytes(int32_t epilogue, int64_t B, int64_t cin, int64_t cout, int64_t T,
+                                          int32_t precision) {
+  if (B < 1 || cin < 1 || cout < 1 || T < 1 || cin > INT32_MAX || cout > INT32_MAX) return 0;
+  const size_t w = align_up((size_t)cin * cout * sizeof(float), 256);
+  if (precision != AB_PREC_FP32) {
+    const size_t img = tc_weight_image_bytes(0, (int)cin, (int)cout, 1, 1);
+    return img == 0 ? 0 : w + align_up(img, 256);
+  }
+  // SPECTRUM: the Linear's output [B, C_out, T] before the spectral head
+  return w + (epilogue == AB_VOCOS_PW_SPECTRUM ? align_up((size_t)B * cout * T * sizeof(float), 256) : 0);
+}
+
+int ab_vocos_pointwise_forward(int32_t epilogue, const float* dev_x, const uint16_t* dev_ximg, const float* dev_w,
+                               const float* dev_bias, const float* dev_gamma, float* dev_y, uint16_t* dev_yimg,
+                               float* dev_spec, int64_t B, int64_t cin, int64_t cout, int64_t T, int32_t precision,
+                               void* ws, size_t ws_bytes, void* stream) {
+  if (epilogue < AB_VOCOS_PW_GELU || epilogue > AB_VOCOS_PW_SPECTRUM)
+    return fail(AB_ERR_ARG, "vocos_pointwise: unknown epilogue %d", epilogue);
+  if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
+    return fail(AB_ERR_ARG, "vocos_pointwise: unknown precision %d", precision);
+  const bool tc = precision != AB_PREC_FP32;
+  if (!dev_w || !dev_bias) return fail(AB_ERR_ARG, "vocos_pointwise: null weight or bias");
+  if (tc ? (!dev_ximg || dev_x) : (!dev_x || dev_ximg))
+    return fail(AB_ERR_ARG, "vocos_pointwise: precision %d takes its input as %s", precision, tc ? "ximg" : "x");
+  const bool out_ok = epilogue == AB_VOCOS_PW_GELU ? (tc ? dev_yimg != nullptr : dev_y != nullptr)
+                      : epilogue == AB_VOCOS_PW_GAMMA ? dev_y && dev_gamma
+                                                      : dev_spec != nullptr;
+  if (!out_ok) return fail(AB_ERR_ARG, "vocos_pointwise: epilogue %d: missing output or gamma", epilogue);
+  if (epilogue == AB_VOCOS_PW_SPECTRUM && (cout & 1))
+    return fail(AB_ERR_ARG, "vocos_pointwise: the spectrum needs an even C_out (magnitude and phase halves), got %lld",
+                (long long)cout);
+  if (B < 1 || cin < 1 || cout < 1 || T < 1 || B > 65535 || cin > INT32_MAX || cout > INT32_MAX || T > (1ll << 30))
+    return fail(AB_ERR_ARG, "vocos_pointwise: batch %lld, C_in %lld, C_out %lld, length %lld", (long long)B,
+                (long long)cin, (long long)cout, (long long)T);
+  const size_t need = ab_vocos_pointwise_workspace_bytes(epilogue, B, cin, cout, T, precision);
+  if (need == 0) return fail(AB_ERR_UNSUPPORTED, "vocos_pointwise: %s", ab_last_error());
+  int rc = check_workspace("vocos_pointwise", ws, ws_bytes, need);
+  if (rc != AB_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* w_t = static_cast<float*>(ws);
+  char* rest = static_cast<char*>(ws) + align_up((size_t)cin * cout * sizeof(float), 256);
+  rc = launch_repack_weight(dev_w, nullptr, w_t, (int)cout, (int)cin, 1, 0, st);
+  if (rc != AB_OK) return rc;
+  if (tc) {
+    rc = epilogue == AB_VOCOS_PW_SPECTRUM ? launch_tc_pack_head_weight(w_t, rest, (int)cin, (int)cout, precision, st)
+                                          : launch_tc_pack_weight(w_t, rest, 0, (int)cin, (int)cout, 1, 1, precision, st);
+    if (rc != AB_OK) return rc;
+    TcPwParams p;
+    p.epilogue = epilogue; p.ximg = dev_ximg; p.w = rest; p.bias = dev_bias; p.gamma = dev_gamma;
+    p.yimg = dev_yimg; p.y = dev_y; p.spec = dev_spec;
+    p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)T; p.precision = precision;
+    return launch_tc_pointwise(p, st);
+  }
+  float* head = reinterpret_cast<float*>(rest);
+  ConvParams p;
+  p.x = dev_x; p.xsb = cin * T; p.xsc = T; p.xst = 1; p.w_t = w_t; p.bias = dev_bias;
+  p.residual = epilogue == AB_VOCOS_PW_GAMMA ? dev_y : nullptr; p.acc_prev = nullptr;
+  p.y = epilogue == AB_VOCOS_PW_SPECTRUM ? head : dev_y;
+  p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)T; p.k = 1; p.d = 1;
+  p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0;
+  p.epi = epilogue == AB_VOCOS_PW_GELU ? CONV_EPI_GELU : epilogue == AB_VOCOS_PW_GAMMA ? CONV_EPI_GAMMA_RESIDUAL : CONV_EPI_NONE;
+  p.gamma = dev_gamma;
+  rc = launch_conv1d_fp32(p, st);
+  // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart (forward_vocos)
+  const int64_t bins = cout / 2;
+  for (int64_t b = 0; rc == AB_OK && epilogue == AB_VOCOS_PW_SPECTRUM && b < B; ++b) {
+    const float* hb = head + b * cout * T;
+    rc = ab_spectral_head_forward(hb, hb + bins * T, nullptr, 1, bins, T, 1e2f, nullptr, nullptr, nullptr,
+                                  dev_spec + b * T * bins * 2, st);
+  }
+  return rc;
+}
+
 size_t ab_diffwave_layer_workspace_bytes(int32_t n_mel) {
   return n_mel < 1 ? 0 : dw_layer_packed_floats(n_mel) * sizeof(float);
 }

@@ -97,8 +97,8 @@ __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
       const int t = t0 + tx + 16 * i;
       if (t >= p.T) continue;
       float v = acc[c][i] + bv;
-      if constexpr (EPI == CONV_EPI_GELU) {
-        v = 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f));
+      if constexpr (EPI == CONV_EPI_GELU) {   // (0.5 v) (1 + erff(v / sqrt 2)), every step rounded
+        v = __fmul_rn(__fmul_rn(0.5f, v), __fadd_rn(1.0f, erff(__fmul_rn(v, 0.70710678118654752440f))));
       } else if constexpr (EPI == CONV_EPI_GAMMA_RESIDUAL) {
         v = __fadd_rn(__ldg(p.residual + row + t), __fmul_rn(__ldg(p.gamma + co), v));
       } else {
@@ -1082,6 +1082,9 @@ int launch_cond_add(float* x, const float* g, int64_t g_batch_stride, const floa
 // TT time steps): the values of all C channels of the tile go to shared memory [C][TT] once, then the mean, the
 // biased variance (a second pass over the centred values, as torch.layer_norm) and the affine output per time step.
 // DW: the k = 7 zero-padded depthwise conv with bias first.  OUT: 0 fp32 [B, C, T]; 1 / 2 the fp16 / bf16 operand image.
+// The divisions, the square root and the output (v - mean) * rstd * w + b (a multiply, then an FMA) are explicit
+// __f*_rn intrinsics, so that no build can contract or reorder them differently: tests/vocos_exact_oracle.py restates
+// every rounding step.
 // ===========================================================================
 namespace {
 constexpr int LN_THREADS = 256;
@@ -1123,13 +1126,13 @@ __global__ void __launch_bounds__(LN_THREADS) vocos_norm_kernel(NormParams p, in
   if (tid < TT) {
     float s = 0.f;
     for (int q = 0; q < ngrp; ++q) s += part[q * TT + tid];
-    mean_s[tid] = s / (float)p.C;
+    mean_s[tid] = __fdiv_rn(s, (float)p.C);
   }
   __syncthreads();
   const float mu = mean_s[tt];
   a = 0.f;
   for (int c = grp; c < p.C; c += ngrp) {
-    const float d = lsm[c * TT + tt] - mu;
+    const float d = __fsub_rn(lsm[c * TT + tt], mu);
     a = fmaf(d, d, a);
   }
   part[tid] = a;
@@ -1137,11 +1140,11 @@ __global__ void __launch_bounds__(LN_THREADS) vocos_norm_kernel(NormParams p, in
   if (tid < TT) {
     float s = 0.f;
     for (int q = 0; q < ngrp; ++q) s += part[q * TT + tid];
-    rstd_s[tid] = 1.0f / sqrtf(s / (float)p.C + p.eps);
+    rstd_s[tid] = __frcp_rn(__fsqrt_rn(__fadd_rn(__fdiv_rn(s, (float)p.C), p.eps)));
   }
   __syncthreads();
   auto norm = [&](int c, int u) {
-    return (lsm[c * TT + u] - mean_s[u]) * rstd_s[u] * __ldg(p.ln_w + c) + __ldg(p.ln_b + c);
+    return __fmaf_rn(__fmul_rn(__fsub_rn(lsm[c * TT + u], mean_s[u]), rstd_s[u]), __ldg(p.ln_w + c), __ldg(p.ln_b + c));
   };
   if (OUT == 0) {
     for (int i = tid; i < n; i += LN_THREADS) {

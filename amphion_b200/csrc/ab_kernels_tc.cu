@@ -1117,7 +1117,8 @@ __device__ __forceinline__ void epilogue_convt(const HcArgs& p, const HcGeom& g,
 
 // Epilogues of Vocos' pointwise (1x1) GEMM D[t, n] = sum_ci A[t, ci] W[n, ci] (launch_tc_pointwise) on hitem_kernel,
 // output channels co0 + column at time O + row:
-//   PW_GELU:     yimg = cvt(gelu(acc + b))                           (pwconv1 + nn.GELU(), exact erf)
+//   PW_GELU:     yimg = cvt(gelu(acc + b))                           (pwconv1 + nn.GELU(), exact erf; (0.5 v) (1 + erff),
+//                                                                     every step an explicit __f*_rn)
 //   PW_GAMMA:    y = y + gamma * (acc + b), fp32 in place            (pwconv2, layer scale and residual, vocos.py:509-527)
 //   PW_SPECTRUM: columns 2j, 2j + 1 hold bin j's log-magnitude and phase (launch_tc_pack_head_weight):
 //                spec[b T + t][j] = min(exp(m), 1e2) (cos p, sin p)  (ISTFTHead, vocos.py:343-361)
@@ -1145,7 +1146,10 @@ __device__ __forceinline__ void epilogue_pw(const HcArgs& p, const HcGeom& g, co
           if ((co >> 3) >= g.c8n_out) continue;
           float v[2] = {a0 + bias_s[co], a1 + bias_s[co + 1]};
 #pragma unroll
-          for (int q = 0; q < 2; ++q) v[q] = co + q < p.Cout ? 0.5f * v[q] * (1.0f + erff(v[q] * 0.70710678118654752440f)) : 0.f;
+          for (int q = 0; q < 2; ++q)
+            v[q] = co + q < p.Cout
+                       ? __fmul_rn(__fmul_rn(0.5f, v[q]), __fadd_rn(1.0f, erff(__fmul_rn(v[q], 0.70710678118654752440f))))
+                       : 0.f;
           *reinterpret_cast<uint32_t*>(p.yimg + (((size_t)b * g.c8n_out + (co >> 3)) * g.Tout + t) * 8 + (co & 7)) =
               pack2t<BF16>(v[0], v[1]);
         } else if constexpr (EPI == PW_GAMMA) {

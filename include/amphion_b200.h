@@ -443,6 +443,37 @@ int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides
  * diffwave_upsample: SpectrogramUpsampler (diffwave.py:68-93) of mel [B, n_mel, frames] with element strides mel_strides:
  *   two ConvTranspose2d(1, 1, [3, 2f], stride [1, f], padding [1, f / 2]) (weights [3, 2f], biases [1]), each followed by
  *   leaky_relu(0.4), even f1, f2 -> out [B, n_mel, frames f1 f2]. */
+/* Vocos building blocks: one launch each of the kernels forward_vocos runs for a ConvNeXt block and the head (no
+ * reference counterpart; exposed for the bit-exact tests).  Every fp32 tensor contiguous.
+ * vocos_norm: LayerNorm over channels (two-pass mean and biased variance, then (x - mean) * rstd * ln_w + ln_b) of x
+ *   [B, C, T], optionally after the k = 7 zero-padded depthwise conv (dw_w [C, 1, 7] and dw_b [C], both or neither).
+ *   Exactly one of y (fp32 [B, C, T]) and yimg (operand image [B][ceil16(C)/8][T][8], padding channels zero, rounded
+ *   to `precision` = AB_PREC_TC_F16 | AB_PREC_TC_BF16; ignored for y) is given.  AB_ERR_UNSUPPORTED, nothing launched,
+ *   when a time tile of C channels does not fit shared memory.
+ * vocos_pointwise: Linear over channels, w [C_out, C_in] (nn.Linear) and bias [C_out], packed into the workspace
+ *   (ab_vocos_pointwise_workspace_bytes, 256-byte aligned) as ab_generator_finalize packs it, then
+ *     AB_VOCOS_PW_GELU:     tc: ximg in -> yimg = the image of gelu(W x + b) (padding channels zero);
+ *                           fp32: x [B, C_in, T] in -> y = gelu(W x + b)
+ *     AB_VOCOS_PW_GAMMA:    y = y + gamma * (W x + b) in place, fp32 [B, C_out, T] (tc: from ximg; fp32: from x)
+ *     AB_VOCOS_PW_SPECTRUM: spec [B*T][C_out/2] complex (interleaved re, im) = min(exp(m), 1e2) (cos p + i sin p), m and
+ *                           p the first and second halves of W x + b (Vocos' ISTFTHead; even C_out)
+ *   At AB_PREC_TC_F16 / TC_BF16 the input is the operand image ximg [B][ceil16(C_in)/8][T][8] and one pointwise wgmma
+ *   GEMM launch runs; at AB_PREC_FP32 the input is x and the CUDA-core conv kernel runs with k = 1 (SPECTRUM: into the
+ *   workspace, then ab_spectral_head_forward per utterance).  The other input and the outputs an epilogue does not
+ *   write may be NULL.  AB_ERR_ARG before any launch for an input that does not match the precision, a missing
+ *   output or gamma, or an odd C_out with SPECTRUM. */
+#define AB_VOCOS_PW_GELU 0
+#define AB_VOCOS_PW_GAMMA 1
+#define AB_VOCOS_PW_SPECTRUM 2
+int ab_vocos_norm_forward(const float* dev_x, const float* dev_dw_w, const float* dev_dw_b, const float* dev_ln_w,
+                          const float* dev_ln_b, float eps, float* dev_y, uint16_t* dev_yimg, int32_t precision,
+                          int64_t batch, int64_t channels, int64_t length, void* stream);
+size_t ab_vocos_pointwise_workspace_bytes(int32_t epilogue, int64_t batch, int64_t cin, int64_t cout, int64_t length,
+                                          int32_t precision);
+int ab_vocos_pointwise_forward(int32_t epilogue, const float* dev_x, const uint16_t* dev_ximg, const float* dev_w,
+                               const float* dev_bias, const float* dev_gamma, float* dev_y, uint16_t* dev_yimg,
+                               float* dev_spec, int64_t batch, int64_t cin, int64_t cout, int64_t length,
+                               int32_t precision, void* dev_workspace, size_t workspace_bytes, void* stream);
 size_t ab_diffwave_layer_workspace_bytes(int32_t n_mel);
 int ab_diffwave_layer_forward(const float* dev_x_in, const float* dev_d, int64_t d_batch_stride, const float* dev_cond,
                               const float* dev_wdil, const float* dev_bdil, const float* dev_wcond, const float* dev_bcond,
