@@ -110,6 +110,8 @@ SIGNATURES = {
     "ab_facodec_encoder_frames": (C.c_int64, [_P, C.c_int64]),
     "ab_facodec_encode": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _I64P, _P, _P, C.c_size_t, _P]),
     "ab_activation1d_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P, C.c_int32, _P, _P, _P]),
+    "ab_activation1d_packed_forward": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P, C.c_int32,
+                                                 C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, _P]),
     "ab_conv1d_forward": (C.c_int, [_P, _P, _P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                     C.c_int32, C.c_float, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),
     "ab_conv1d_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32]),

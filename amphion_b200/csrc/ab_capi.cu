@@ -1089,6 +1089,21 @@ int check_workspace(const char* what, const void* ws, size_t bytes, size_t need)
   return AB_OK;
 }
 
+// One Activation1d launch as a generator issues it: the taps packed on the host (kc; null: the kernel reads f_up /
+// f_down), and at 16 bits the short snake, which launch_activation1d takes on image-only launches.  Shared by
+// Launch::snake and ab_activation1d_packed_forward, so that the standalone entry point runs the generator's launch.
+SnakeParams generator_snake_params(const SnakeCoef* kc, int precision, const float* x, float* y, uint16_t* yimg,
+                                   const float* alpha, const float* beta, const float* f_up, const float* f_down,
+                                   int logscale, int B, int C, int T) {
+  SnakeParams p;
+  if (kc) { p.kc = *kc; p.have_kc = 1; }
+  p.fast_snake = precision != AB_PREC_FP32;
+  p.yimg = yimg; p.bf16 = precision == AB_PREC_TC_BF16;
+  p.x = x; p.y = y; p.alpha = alpha; p.beta = beta; p.f_up = f_up; p.f_down = f_down;
+  p.B = B; p.C = C; p.T = T; p.logscale = logscale;
+  return p;
+}
+
 // The launches of one entry-point call: counts them (ab_generator_last_launches), times each one when profiling is on
 // (ab_generator_set_profiling), and runs the layers the model kinds share
 struct Launch {
@@ -1164,14 +1179,10 @@ struct Launch {
 
   // Activation1d: fp32 y and / or the 16-bit operand image yimg
   int snake(const ActRef& a, int64_t B, const float* x, float* y, int C, int Tn, uint16_t* yimg = nullptr) {
-    SnakeParams p;
-    p.yimg = yimg; p.bf16 = g->precision == AB_PREC_TC_BF16;
-    p.x = x; p.y = y; p.alpha = g->fptr(a.alpha); p.beta = g->fptr(a.beta);
-    p.f_up = g->fptr(a.fup); p.f_down = g->fptr(a.fdown);
     auto kc = g->act_coef.find(a.fup);
-    if (kc != g->act_coef.end()) { p.kc = kc->second; p.have_kc = 1; }
-    p.fast_snake = g->precision != AB_PREC_FP32;
-    p.B = (int)B; p.C = C; p.T = Tn; p.logscale = g->cfg.snake_logscale;
+    const SnakeParams p = generator_snake_params(kc != g->act_coef.end() ? &kc->second : nullptr, g->precision, x, y,
+                                                 yimg, g->fptr(a.alpha), g->fptr(a.beta), g->fptr(a.fup),
+                                                 g->fptr(a.fdown), g->cfg.snake_logscale, (int)B, C, Tn);
     return timed(3, 0.0, (double)B * C * Tn * (4.0 + (y ? 4.0 : 0.0) + (yimg ? 2.0 : 0.0)),
                  [&] { return launch_activation1d(p, st); });
   }
@@ -2342,6 +2353,25 @@ int ab_activation1d_forward(const float* dev_x, float* dev_y, int64_t B, int64_t
   p.x = dev_x; p.y = dev_y; p.alpha = dev_alpha; p.beta = dev_beta; p.f_up = f_up; p.f_down = f_down;
   p.B = (int)B; p.C = (int)C; p.T = (int)T; p.logscale = logscale;
   p.yimg = nullptr; p.bf16 = 0;
+  return launch_activation1d(p, static_cast<cudaStream_t>(stream));
+}
+
+int ab_activation1d_packed_forward(const float* dev_x, float* dev_y, uint16_t* dev_yimg, int64_t B, int64_t C,
+                                   int64_t T, const float* dev_alpha, const float* dev_beta, int32_t logscale,
+                                   const float* f_up, const float* f_down, int32_t precision, void* stream) {
+  if (!dev_x || !dev_alpha || !dev_beta || !f_up || !f_down) return fail(AB_ERR_ARG, "activation1d_packed: null argument");
+  if (!dev_y && !dev_yimg) return fail(AB_ERR_ARG, "activation1d_packed: no output requested");
+  if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
+    return fail(AB_ERR_ARG, "activation1d_packed: unknown precision %d", precision);
+  if (dev_yimg && precision == AB_PREC_FP32)
+    return fail(AB_ERR_ARG, "activation1d_packed: the operand image needs a tensor-core precision");
+  if (B < 1 || C < 1 || T < 1) return fail(AB_ERR_ARG, "activation1d_packed: bad shape");
+  if (B > 65535 || C > 65535 * 8) return fail(AB_ERR_UNSUPPORTED, "activation1d_packed: B or C too large");
+  if (T > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "activation1d_packed: sequence too long");
+  SnakeCoef kc;
+  pack_snake_coef(f_up, f_down, &kc);
+  const SnakeParams p = generator_snake_params(&kc, precision, dev_x, dev_y, dev_yimg, dev_alpha, dev_beta, nullptr,
+                                               nullptr, logscale, (int)B, (int)C, (int)T);
   return launch_activation1d(p, static_cast<cudaStream_t>(stream));
 }
 

@@ -107,7 +107,7 @@ __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
 __device__ __forceinline__ float hsum2(f32x2 v) {
   float lo, hi;
   upk2(v, lo, hi);
-  return lo + hi;
+  return __fadd_rn(lo, hi);
 }
 
 __device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {

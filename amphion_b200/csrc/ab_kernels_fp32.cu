@@ -648,13 +648,14 @@ constexpr int SN_TR = 8 * 32 * 2;          // image transposition: [8 ch][32 lan
 constexpr int WT = 8 * SN_WS;              // outputs per CTA tile (8 warps)
 
 __device__ __forceinline__ float snake_eval(float u, float a, float invb) {
-  // sin(u*a)^2 with explicit range reduction to [-pi, pi] before the MUFU
-  const float arg = u * a;
-  const float kf = rintf(arg * 0.15915494309189535f);
-  float r = fmaf(-kf, 6.2831854820251465f, arg);
-  r = fmaf(-kf, -1.7484555314695172e-07f, r);
+  // sin(u*a)^2 with explicit range reduction to [-pi, pi] before the MUFU (Cody-Waite: 2 pi as a high and a low part);
+  // every rounding is an explicit intrinsic, restated step by step in tests/activation1d_exact_oracle.py
+  const float arg = __fmul_rn(u, a);
+  const float kf = rintf(__fmul_rn(arg, 0.15915494309189535f));
+  float r = __fmaf_rn(-kf, 6.2831854820251465f, arg);
+  r = __fmaf_rn(-kf, -1.7484555314695172e-07f, r);
   const float sv = __sinf(r);
-  return fmaf(invb, sv * sv, u);
+  return __fmaf_rn(invb, __fmul_rn(sv, sv), u);
 }
 
 // Two snake evaluations at once, without explicit range reduction: sin.approx multiplies by 1/2pi and the MUFU
@@ -938,7 +939,7 @@ __global__ void __launch_bounds__(NT, AB_SNAKE_BLOCKS) activation1d_warp_kernel(
       }
     }
     prm[threadIdx.x][0] = a;
-    prm[threadIdx.x][1] = 1.0f / (bb + 1e-9f);
+    prm[threadIdx.x][1] = __frcp_rn(__fadd_rn(bb, 1e-9f));
   }
   __syncthreads();
   if (t0 >= T) return;                           // warp-uniform; no block barriers below

@@ -383,6 +383,17 @@ int ab_activation1d_forward(const float* dev_x, float* dev_y, int64_t batch, int
                             int64_t length, const float* dev_alpha, const float* dev_beta,
                             int32_t logscale, const float* dev_filter_up12,
                             const float* dev_filter_down12, void* stream);
+/* The same Activation1d as one launch of what a generator handle runs (no reference counterpart; exposed for the
+ * bit-exact tests): the 12 + 12 taps are HOST arrays, packed as ab_generator_finalize packs them and passed by value.
+ * y (fp32 [B, C, T]) and yimg (operand image [B][ceil16(C)/8][T][8] of y, padding channels zero, rounded to
+ * `precision` = AB_PREC_TC_F16 | AB_PREC_TC_BF16) may each be NULL, not both.  At a tensor-core precision a launch
+ * with yimg and no y evaluates sin(u a) without the explicit range reduction, as the tensor-core generators do
+ * (DESIGN 4.3); every launch with y keeps it.  AB_ERR_ARG before any launch for a NULL input, no output, yimg at
+ * AB_PREC_FP32 or an unknown precision. */
+int ab_activation1d_packed_forward(const float* dev_x, float* dev_y, uint16_t* dev_yimg, int64_t batch,
+                                   int64_t channels, int64_t length, const float* dev_alpha, const float* dev_beta,
+                                   int32_t logscale, const float* filter_up12, const float* filter_down12,
+                                   int32_t precision, void* stream);
 
 /* ------------------------------------------------------------------------
  * Building blocks exposed for parity tests (each is one launch of the kernel
