@@ -48,6 +48,7 @@ class GeneratorConfig(C.Structure):
         ("vq_codebook_bits", C.c_int32 * 3),
         ("vq_codebook_dim", C.c_int32),
         ("facodec_quantize", C.c_int32),
+        ("facodec_prosody_encoder", C.c_int32),
     ]
 
 
@@ -104,6 +105,9 @@ SIGNATURES = {
     "ab_facodec_inference": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _I64P, _P, C.c_int64, _P, _P, C.c_size_t, _P]),
     "ab_facodec_quantize_workspace_bytes": (C.c_size_t, [_P, C.c_int64, C.c_int64]),
     "ab_facodec_quantize": (C.c_int, [_P, _P, _I64P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "ab_facodec_quantize_prosody": (C.c_int, [_P, _P, _I64P, _P, _I64P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, _P,
+                                              _P, C.c_size_t, _P]),
+    "ab_facodec_prosody_input_forward": (C.c_int, [_P, _I64P, _P, _P, _P, C.c_int64, C.c_int64, _P, _P]),
     "ab_facodec_redecoder_vq2emb_workspace_bytes": (C.c_size_t, [_P, C.c_int64, C.c_int64]),
     "ab_facodec_redecoder_vq2emb": (C.c_int, [_P, _P, _I64P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int32,
                                               _P, _P, C.c_size_t, _P]),

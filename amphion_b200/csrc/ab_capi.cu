@@ -139,6 +139,9 @@ struct FacodecRef {
   // facodec_quantize: the timbre encoder (transformer.py:154-217); the redecoder: its prosody encoder (use_cln)
   int pe = -1, last_w = -1, last_b = -1;
   std::vector<TimbreLayerRef> timbre;
+  // facodec_prosody_encoder (FACodecDecoderV2): melspec_linear and the prosody transformer melspec_encoder
+  int mel_w = -1, mel_b = -1, pros_pe = -1, pros_last_w = -1, pros_last_b = -1;
+  std::vector<TimbreLayerRef> prosody;
 };
 
 }  // namespace
@@ -337,6 +340,10 @@ int validate_facodec_config(const ab_generator_config& c) {
   if (c.facodec_quantize && c.n_mel != FAC_TIMBRE_C)
     return fail(AB_ERR_UNSUPPORTED, "config: FACodec quantization needs in_channels == %d (the timbre encoder's width; "
                 "got %d)", FAC_TIMBRE_C, c.n_mel);
+  // FACodecDecoderV2: the prosody transformer feeds the quantizer, so it comes with facodec_quantize
+  if (c.facodec_prosody_encoder != 0 && (c.facodec_prosody_encoder != 1 || !c.facodec_quantize))
+    return fail(AB_ERR_ARG, "config: facodec_prosody_encoder must be 0, or 1 with facodec_quantize = 1 (got %d, %d)",
+                c.facodec_prosody_encoder, c.facodec_quantize);
   return AB_OK;
 }
 
@@ -349,8 +356,9 @@ int validate_facodec_redecoder_config(const ab_generator_config& c) {
     return fail(AB_ERR_UNSUPPORTED, "config: the FACodec redecoder needs in_channels == vq_dim == %d (the prosody "
                 "transformer's width; got %d)", FAC_TIMBRE_C, c.n_mel);
   if ((rc = check_facodec_groups(c, "FACodec redecoder", "FACodec redecoder table")) != AB_OK) return rc;
-  if (c.vq_codebook_dim != 0 || c.facodec_quantize != 0)
-    return fail(AB_ERR_ARG, "config: the FACodec redecoder has no codebook_dim or facodec_quantize (both must be 0)");
+  if (c.vq_codebook_dim != 0 || c.facodec_quantize != 0 || c.facodec_prosody_encoder != 0)
+    return fail(AB_ERR_ARG, "config: the FACodec redecoder has no codebook_dim, facodec_quantize or "
+                            "facodec_prosody_encoder (all must be 0)");
   return AB_OK;
 }
 
@@ -383,7 +391,8 @@ int validate_config(const ab_generator_config& c) {
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
   if (c.kind == AB_GEN_FACODEC_REDECODER) return validate_facodec_redecoder_config(c);
-  if (c.facodec_quantize) return fail(AB_ERR_ARG, "config: facodec_quantize belongs to AB_GEN_FACODEC");
+  if (c.facodec_quantize || c.facodec_prosody_encoder)
+    return fail(AB_ERR_ARG, "config: facodec_quantize / facodec_prosody_encoder belong to AB_GEN_FACODEC");
   for (int i = 0; i < 3; ++i)
     if (c.vq_num_q[i] || c.vq_codebook_bits[i]) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
   if (c.vq_codebook_dim) return fail(AB_ERR_ARG, "config: vq_* fields belong to AB_GEN_FACODEC");
@@ -607,12 +616,14 @@ void add_facodec_generator_tensors(ab_generator* g) {
   g->fac.style_b = g->add_slot("timbre_linear.bias", SLOT_VEC, {2 * C});
 }
 
-// A FACodec transformer (transformer.py:154-234) under `prefix`: pe, four layers, last_ln.  use_cln: each LayerNorm is
-// a StyleAdaptiveLayerNorm, listed as its style Linear [2H, H] / [2H] (transformer.py:13-32)
-void add_facodec_transformer_tensors(ab_generator* g, const std::string& prefix, bool use_cln) {
-  FacodecRef& f = g->fac;
+// A FACodec transformer (transformer.py:154-234) under `prefix`: pe, four layers, last_ln, into pe / layers / last_w /
+// last_b.  use_cln: each LayerNorm is a StyleAdaptiveLayerNorm, listed as its style Linear [2H, H] / [2H]
+// (transformer.py:13-32).  fp32_only: the GEMMs run on the CUDA cores at every precision (no tensor-core image).
+void add_facodec_transformer_tensors(ab_generator* g, const std::string& prefix, bool use_cln, int* pe,
+                                     std::vector<TimbreLayerRef>* layers, int* last_w, int* last_b,
+                                     bool fp32_only = false) {
   const int H = FAC_TIMBRE_C;
-  f.pe = g->add_slot(prefix + "position_emb.pe", SLOT_VEC, {FAC_PE_ROWS, 1, H});
+  *pe = g->add_slot(prefix + "position_emb.pe", SLOT_VEC, {FAC_PE_ROWS, 1, H});
   auto ln = [&](const std::string& name, int* w, int* b) {
     if (use_cln) {
       *w = g->add_slot(name + ".style.weight", SLOT_VEC, {2 * H, H});
@@ -635,9 +646,11 @@ void add_facodec_transformer_tensors(ab_generator* g, const std::string& prefix,
     t.out_proj = make_linear(g, pre + "self_attn.out_proj", H, H);
     t.ffn_1 = make_conv(g, pre + "ffn.ffn_1", H, 4 * H, 5, 1, false);
     t.ffn_2 = make_linear(g, pre + "ffn.ffn_2", 4 * H, H);
-    f.timbre.push_back(t);
+    if (fp32_only)
+      for (const ConvRef* c : {&t.qkv, &t.out_proj, &t.ffn_1, &t.ffn_2}) g->slots[c->w].no_tc = true;
+    layers->push_back(t);
   }
-  ln(prefix + "last_ln", &f.last_w, &f.last_b);
+  ln(prefix + "last_ln", last_w, last_b);
 }
 
 // FACodec decoder tensors (AB_GEN_FACODEC), the reference's names (facodec.py:121-133, :220-240, :286-369, fvq.py:23-29)
@@ -665,7 +678,14 @@ void add_facodec_tensors(ab_generator* g) {
       l.in_proj = make_linear(g, "quantizer." + std::to_string(q) + ".layers." + std::to_string(j) + ".in_proj", C, D);
       g->slots[l.in_proj.w].no_tc = true;
     }
-  add_facodec_transformer_tensors(g, "timbre_encoder.", false);
+  add_facodec_transformer_tensors(g, "timbre_encoder.", false, &f.pe, &f.timbre, &f.last_w, &f.last_b);
+  if (!cfg->facodec_prosody_encoder) return;
+  // FACodecDecoderV2 (facodec.py:1006-1017): melspec_linear (read by the prosody input kernel in its nn.Linear layout)
+  // and melspec_encoder, which runs in fp32 at every precision because its output is quantized
+  f.mel_w = g->add_slot("melspec_linear.weight", SLOT_VEC, {FAC_TIMBRE_C, FAC_PROSODY_BINS});
+  f.mel_b = g->add_slot("melspec_linear.bias", SLOT_VEC, {FAC_TIMBRE_C});
+  add_facodec_transformer_tensors(g, "melspec_encoder.", false, &f.pros_pe, &f.prosody, &f.pros_last_w, &f.pros_last_b,
+                                  true);
 }
 
 // FACodec redecoder tensors (AB_GEN_FACODEC_REDECODER), the reference's names (facodec.py:602-689): the embedding
@@ -682,7 +702,8 @@ void add_facodec_redecoder_tensors(ab_generator* g) {
       g->fac.layers.push_back(l);
     }
   add_facodec_generator_tensors(g);
-  add_facodec_transformer_tensors(g, "timbre_cond_prosody_enc.", true);
+  FacodecRef& f = g->fac;
+  add_facodec_transformer_tensors(g, "timbre_cond_prosody_enc.", true, &f.pe, &f.timbre, &f.last_w, &f.last_b);
 }
 
 // FACodec encoder tensors (AB_GEN_FACODEC_ENCODER), the reference's names (facodec.py:121-194): "block.0" (conv_pre,
@@ -2126,11 +2147,12 @@ static TimbreWs redecoder_layout(Carve& c, int64_t B, int64_t T, float** styles)
 // encoder and the redecoder's prosody encoder differ only in their LayerNorms.  norm(layer, i, y, yimg) runs the
 // layer's ln_1 (i = 0) or ln_2 (i = 1) on w.S into y (fp32) or the operand image yimg.  Per layer: ln_1, the QKV GEMM,
 // the attention, out_proj onto S, ln_2, ffn_1 (k = 5; at 16 bits it also writes the image of its ReLU), ffn_2 onto S.
+// tc: the GEMMs take 16-bit operands (the handle's precision); false runs them and the attention in fp32 on CUDA cores.
 template <class Norm>
-static int facodec_transformer_layers(Launch& L, const TimbreWs& w, int64_t B, int Tn, Norm norm) {
+static int facodec_transformer_layers(Launch& L, const TimbreWs& w, int64_t B, int Tn,
+                                      const std::vector<TimbreLayerRef>& layers, bool tc, Norm norm) {
   ab_generator* g = L.g;
   const int C = FAC_TIMBRE_C;
-  const bool tc = g->precision != AB_PREC_FP32;
   const double el = (double)B * Tn;
   const uint16_t* Himg = reinterpret_cast<const uint16_t*>(w.H);
   // a GEMM (k = 1) or the k = 5 ffn_1 conv: x fp32 or ximg, y = (bias + W x) [+ residual = y]; all in profile class 0 at
@@ -2145,7 +2167,7 @@ static int facodec_transformer_layers(Launch& L, const TimbreWs& w, int64_t B, i
                      0, 0.0f);
   };
   int rc;
-  for (const TimbreLayerRef& t : g->fac.timbre) {
+  for (const TimbreLayerRef& t : layers) {
     // x = x + out_proj(MHA(LN1(x)))
     if ((rc = norm(t, 0, tc ? nullptr : w.H, tc ? reinterpret_cast<uint16_t*>(w.H) : nullptr)) != AB_OK) return rc;
     if ((rc = gemm(t.qkv, w.H, Himg, w.QKV, false, 1.0f, nullptr)) != AB_OK) return rc;
@@ -2168,28 +2190,59 @@ size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t B, int
   if (!g || g->cfg.kind != AB_GEN_FACODEC || !g->cfg.facodec_quantize || B <= 0 || T <= 0) return 0;
   Carve c{nullptr};
   timbre_layout(c, B, T);
+  if (g->cfg.facodec_prosody_encoder) c.take((size_t)B * T * FAC_TIMBRE_C * sizeof(float));   // melspec_encoder's output
   return c.off;
 }
 
-int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t B, int64_t T,
-                        int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
-                        float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream) {
-  int rc = facodec_check(g, B, T, "facodec_quantize");
+// FACodecDecoder.forward(vq=True) (dev_pf null) and FACodecDecoderV2.forward(vq=True) (dev_pf: the prosody feature)
+static int facodec_quantize_impl(ab_generator* g, const char* what, const float* dev_x, const int64_t x_strides[3],
+                                 const float* dev_pf, const int64_t pf_strides[3], int64_t B, int64_t T,
+                                 int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out,
+                                 float* dev_quantized_out, float* dev_spk_out, void* dev_workspace,
+                                 size_t workspace_bytes, void* stream) {
+  int rc = facodec_check(g, B, T, what);
   if (rc != AB_OK) return rc;
-  if (!g->cfg.facodec_quantize)
-    return fail(AB_ERR_STATE, "facodec_quantize: the handle was created without facodec_quantize");
-  if (!dev_x || !x_strides || !dev_emb_out || !dev_codes_out || !dev_quantized_out || !dev_spk_out)
-    return fail(AB_ERR_ARG, "facodec_quantize: null argument");
-  if (n_quantizers < 1) return fail(AB_ERR_ARG, "facodec_quantize: n_quantizers %d < 1 (no layer would run)", n_quantizers);
+  if (!g->cfg.facodec_quantize) return fail(AB_ERR_STATE, "%s: the handle was created without facodec_quantize", what);
+  const bool v2 = g->cfg.facodec_prosody_encoder != 0;
+  if (v2 && !dev_pf)
+    return fail(AB_ERR_STATE, "%s: the handle serves FACodecDecoderV2, whose forward reads the prosody feature "
+                              "(ab_facodec_quantize_prosody)", what);
+  if (!v2 && dev_pf)
+    return fail(AB_ERR_STATE, "%s: the handle was created without facodec_prosody_encoder", what);
+  if (!dev_x || !x_strides || (v2 && !pf_strides) || !dev_emb_out || !dev_codes_out || !dev_quantized_out || !dev_spk_out)
+    return fail(AB_ERR_ARG, "%s: null argument", what);
+  if (n_quantizers < 1) return fail(AB_ERR_ARG, "%s: n_quantizers %d < 1 (no layer would run)", what, n_quantizers);
   if (B > FAC_PE_ROWS)   // PositionalEncoding adds pe[:B] (transformer.py:43-45)
-    return fail(AB_ERR_ARG, "facodec_quantize: batch %lld > %d, the rows of the positional encoding", (long long)B, FAC_PE_ROWS);
-  rc = check_workspace("facodec_quantize", dev_workspace, workspace_bytes, ab_facodec_quantize_workspace_bytes(g, B, T));
+    return fail(AB_ERR_ARG, "%s: batch %lld > %d, the rows of the positional encoding", what, (long long)B, FAC_PE_ROWS);
+  rc = check_workspace(what, dev_workspace, workspace_bytes, ab_facodec_quantize_workspace_bytes(g, B, T));
   if (rc != AB_OK) return rc;
   Launch L{g, static_cast<cudaStream_t>(stream)};
   Carve ws{static_cast<char*>(dev_workspace)};
   const TimbreWs w = timbre_layout(ws, B, T);
   const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim, Tn = (int)T;
   const double el = (double)B * T;
+  auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) { return L.norm(B, C, Tn, w.S, -1, -1, lw, lb, 1e-5f, y, yimg); };
+
+  // FACodecDecoderV2 (facodec.py:1034-1038): melspec_encoder(melspec_linear(prosody_feature^T)) into P, all fp32: the
+  // input projection and pe into S, four layers on S, last_ln into P
+  float* P = nullptr;
+  if (v2) {
+    const FacodecRef& f = g->fac;
+    P = ws.take((size_t)B * T * C * sizeof(float));
+    FacProsodyInParams q;
+    q.x = dev_pf; q.xsb = pf_strides[0]; q.xsi = pf_strides[1]; q.xst = pf_strides[2];
+    q.w = g->fptr(f.mel_w); q.bias = g->fptr(f.mel_b); q.pe = g->fptr(f.pros_pe); q.y = w.S;
+    q.B = (int)B; q.T = Tn;
+    rc = L.timed(11, el * C * (2.0 * FAC_PROSODY_BINS + 2.0), 4.0 * el * (FAC_PROSODY_BINS + C) + 4.0 * C * (FAC_PROSODY_BINS + 2.0),
+                 [&] { return launch_facodec_prosody_input(q, L.st); });
+    if (rc != AB_OK) return rc;
+    rc = facodec_transformer_layers(L, w, B, Tn, f.prosody, false,
+                                    [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
+      return i == 0 ? norm(t.ln1_w, t.ln1_b, y, yimg) : norm(t.ln2_w, t.ln2_b, y, yimg);
+    });
+    if (rc != AB_OK) return rc;
+    if ((rc = norm(f.pros_last_w, f.pros_last_b, P, nullptr)) != AB_OK) return rc;
+  }
 
   // the quantizers (all groups, one launch) and the positional add into S
   FacRvqParams p;
@@ -2222,19 +2275,50 @@ int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_str
   for (int q = 0; q < AB_FACODEC_MAX_Q; ++q)
     if (p.cb[q]) { cb_flops += 2.0 * el * p.rows[q] * D; cb_bytes += 4.0 * p.rows[q] * (FAC_MAX_CODEBOOK_DIM + 1); }
   rc = L.timed(12, 4.0 * el * nq_run * C * D + cb_flops,
-               4.0 * el * C * (2 + p.ngroups + 1) + 8.0 * el * n_used + cb_bytes + 8.0 * nq_run * (double)C * D,
-               [&] { return launch_facodec_rvq(p, L.st); });
+               4.0 * el * C * (2 + p.ngroups + 1 + (v2 ? 1 : 0)) + 8.0 * el * n_used + cb_bytes + 8.0 * nq_run * (double)C * D,
+               [&] { return launch_facodec_rvq(p, L.st, P); });
   if (rc != AB_OK) return rc;
 
   // the timbre encoder on S (transformer.py:206-217)
-  auto norm = [&](int lw, int lb, float* y, uint16_t* yimg) { return L.norm(B, C, Tn, w.S, -1, -1, lw, lb, 1e-5f, y, yimg); };
-  rc = facodec_transformer_layers(L, w, B, Tn, [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
+  rc = facodec_transformer_layers(L, w, B, Tn, g->fac.timbre, g->precision != AB_PREC_FP32,
+                                  [&](const TimbreLayerRef& t, int i, float* y, uint16_t* yimg) {
     return i == 0 ? norm(t.ln1_w, t.ln1_b, y, yimg) : norm(t.ln2_w, t.ln2_b, y, yimg);
   });
   if (rc != AB_OK) return rc;
   if ((rc = norm(g->fac.last_w, g->fac.last_b, w.H, nullptr)) != AB_OK) return rc;
   rc = L.timed(12, el * C, 4.0 * el * C + 4.0 * B * C, [&] { return launch_facodec_time_mean(w.H, dev_spk_out, (int)B, C, Tn, L.st); });
   return L.done(rc);
+}
+
+int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t B, int64_t T,
+                        int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
+                        float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream) {
+  return facodec_quantize_impl(g, "facodec_quantize", dev_x, x_strides, nullptr, nullptr, B, T, n_quantizers, dev_emb_out,
+                               dev_codes_out, dev_quantized_out, dev_spk_out, dev_workspace, workspace_bytes, stream);
+}
+
+int ab_facodec_quantize_prosody(ab_generator* g, const float* dev_x, const int64_t x_strides[3], const float* dev_prosody,
+                                const int64_t prosody_strides[3], int64_t B, int64_t T, int32_t n_quantizers,
+                                float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out, float* dev_spk_out,
+                                void* dev_workspace, size_t workspace_bytes, void* stream) {
+  if (g && !dev_prosody) return fail(AB_ERR_ARG, "facodec_quantize_prosody: null argument");
+  return facodec_quantize_impl(g, "facodec_quantize_prosody", dev_x, x_strides, dev_prosody, prosody_strides, B, T,
+                               n_quantizers, dev_emb_out, dev_codes_out, dev_quantized_out, dev_spk_out, dev_workspace,
+                               workspace_bytes, stream);
+}
+
+int ab_facodec_prosody_input_forward(const float* dev_x, const int64_t x_strides[3], const float* dev_w,
+                                     const float* dev_bias, const float* dev_pe, int64_t B, int64_t T, float* dev_y,
+                                     void* stream) {
+  if (!x_strides) return fail(AB_ERR_ARG, "facodec_prosody_input_forward: null argument");
+  if (B <= 0 || T <= 0 || B > FAC_PE_ROWS || T > (1ll << 30))
+    return fail(AB_ERR_ARG, "facodec_prosody_input_forward: batch %lld / frames %lld out of range", (long long)B,
+                (long long)T);
+  FacProsodyInParams p;
+  p.x = dev_x; p.xsb = x_strides[0]; p.xsi = x_strides[1]; p.xst = x_strides[2];
+  p.w = dev_w; p.bias = dev_bias; p.pe = dev_pe; p.y = dev_y;
+  p.B = (int)B; p.T = (int)T;
+  return launch_facodec_prosody_input(p, static_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------
@@ -2308,7 +2392,8 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
   // facodec.py:739-744: per prosody table, x_t = transformer(x_t + emb(codes)); the transformer adds pe each time
   for (int i = 0; i < nq[0]; ++i) {
     if ((rc = embed(i == 0 ? nullptr : w.H, i, 1, g->fptr(f.pe), w.S)) != AB_OK) return rc;
-    rc = facodec_transformer_layers(L, w, B, Tn, [&](const TimbreLayerRef& t, int j, float* y, uint16_t* yimg) {
+    rc = facodec_transformer_layers(L, w, B, Tn, f.timbre, g->precision != AB_PREC_FP32,
+                                    [&](const TimbreLayerRef& t, int j, float* y, uint16_t* yimg) {
       return film(2 * (int)(&t - f.timbre.data()) + j, y, yimg);
     });
     if (rc != AB_OK) return rc;

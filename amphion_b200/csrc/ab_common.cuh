@@ -270,12 +270,27 @@ struct FacRvqParams {       // quantize (facodec.py:408-445) for one tile of fra
 };
 // normalised codebook rows (F.normalize, eps 1e-12) padded to 16 floats, and their squared norms
 int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows, int D, cudaStream_t s);
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s);
+// prosody == nullptr: FACodecDecoder's RVQ (every group reads x); else FACodecDecoderV2's (facodec.py:1027-1094): the
+// prosody group reads prosody [B, C, T] (contiguous), the content group x, the residual group x - (prosody + content)
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody = nullptr);
 // softmax(q k^T / 8) v per (utterance, head) from qkv [B, 3 * 256, T] (q, k, v rows; time fastest) -> y fp32 [B, 256, T]
 // or the operand image yimg [B][32][T][8]
 int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf16, int B, int T, cudaStream_t s);
 // spk[b][c] = sum_t y[b, c, t] / T (fixed order)
 int launch_facodec_time_mean(const float* y, float* spk, int B, int C, int T, cudaStream_t s);
+
+// ---- FACodecDecoderV2.forward(vq=True): the prosody transformer's input (ab_facodec.cu) ----
+constexpr int FAC_PROSODY_BINS = 20;      // melspec_linear's in_features: the first 20 mel rows
+struct FacProsodyInParams { // y[b, c, t] = ((sum_i w[c][i] x[b, i, t]) + bias[c]) + pe[b][c]
+  const float* x;           // [B, 20, T] with element strides xsb / xsi / xst
+  int64_t xsb, xsi, xst;
+  const float* w;           // melspec_linear.weight [256][20] (nn.Linear layout)
+  const float* bias;        // [256]
+  const float* pe;          // [>= B][256]
+  float* y;                 // fp32 [B, 256, T]
+  int B, T;
+};
+int launch_facodec_prosody_input(const FacProsodyInParams& p, cudaStream_t s);
 
 // ---- FACodecRedecoder.vq2emb: the embedding gathers and sums (ab_facodec.cu) ----
 struct FacEmbedParams {     // out[b, c, t] = ((prev[b, c, t] + tab[0][code_0][c]) + tab[1][code_1][c] ...) + pe[b][c],

@@ -2,9 +2,11 @@
 // timbre projection and the LayerNorm + FiLM in front of conv_pre.  The generator itself runs on the BigVGAN path of
 // ab_capi.cu's forward_impl.  Then the kernels of FACodecDecoder.forward(vq=True) (facodec.py:408-471): the residual
 // vector quantizer, the timbre encoder's attention and the time mean; its GEMMs and LayerNorms run on the shared
-// convolution and LayerNorm kernels.  Last the embedding gathers of FACodecRedecoder.vq2emb (facodec.py:734-759); its
+// convolution and LayerNorm kernels; FACodecDecoderV2 adds the prosody transformer's input and an RVQ whose prosody
+// group reads that transformer's output.  Last the embedding gathers of FACodecRedecoder.vq2emb (facodec.py:734-759); its
 // prosody transformer reuses the style, FiLM and attention kernels above.
 #include <algorithm>
+#include <type_traits>
 
 #include "ab_common.cuh"
 
@@ -191,7 +193,10 @@ __global__ void __launch_bounds__(256) facodec_cbnorm_kernel(const float* __rest
 //   e = z_e / max(|z_e|, 1e-12);  dist_i = (|e|^2 - 2 e.c_i) + |c_i|^2;  code = the lowest i of the least dist
 //   z_q = z_e + (codebook[code] - z_e)  (the straight-through step, two fp32 roundings)
 //   q = sum_d W_out[c][d] z_q[d] (an FMA chain from 0) + b_out[c];  r -= q;  group sum += q
-// The groups' sums are written as they complete; emb = (prosody + content) + residual.
+// The groups' sums are written as they complete; emb = (prosody + content) + residual.  PROSODY (FACodecDecoderV2,
+// facodec.py:1027-1094): the prosody group's residual starts from the prosody transformer's output instead of x; the
+// content and residual groups and the positional add are V1's.  Two instantiations, so that V1's code holds no prosody
+// source.
 constexpr int RVQ_TT = 16;
 constexpr int RVQ_THREADS = 256;
 constexpr int RVQ_CH = 256;
@@ -202,7 +207,14 @@ size_t rvq_smem_bytes(int C) {
                           RVQ_TT * (2 * FAC_MAX_CODEBOOK_DIM + 1)) + sizeof(int) * RVQ_TT;
 }
 
-__global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(FacRvqParams p, int tiles) {
+struct FacRvqProsodyParams : FacRvqParams {
+  const float* prosody;     // [B, C, T], the prosody transformer's output
+};
+template <bool PROSODY>
+using RvqArgs = typename std::conditional<PROSODY, FacRvqProsodyParams, FacRvqParams>::type;
+
+template <bool PROSODY>
+__global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<PROSODY> p, int tiles) {
   extern __shared__ __align__(16) float qsm[];
   const int C = p.C, D = p.D, tid = threadIdx.x;
   float* xs = qsm;                          // [C][TT] x
@@ -235,6 +247,14 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(FacRvqParam
     for (int i = tid; i < n; i += RVQ_THREADS) {
       rs[i] = g < 2 ? xs[i] : __fsub_rn(xs[i], s01[i]);   // facodec.py:436: x - (prosody + content)
       gs[i] = 0.f;
+    }
+    if constexpr (PROSODY) {
+      if (g == 0) {   // facodec.py:1038-1042: the prosody group quantizes melspec_encoder's output
+        for (int i = tid; i < n; i += RVQ_THREADS) {
+          const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
+          rs[i] = t < p.T ? __ldg(p.prosody + ((int64_t)b * C + c) * p.T + t) : 0.f;
+        }
+      }
     }
     for (int j = 0; j < p.nused[g]; ++j) {
       const int q = p.layer0[g] + j;
@@ -342,6 +362,45 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(FacRvqParam
         if (t < p.T) p.emb[((int64_t)b * C + c) * p.T + t] = s01[i];
       }
     }
+  }
+}
+
+// FACodecDecoderV2's prosody input (facodec.py:1036-1038 and transformer.py:43-45): melspec_linear over the 20 mel rows
+// of each frame, then the batch-first PositionalEncoding's row b.  One CTA per (utterance, tile of PIN_TT frames),
+// thread c = output channel: the input tile [20][PIN_TT] is read along time into shared memory (every thread then reads
+// the same element: a broadcast), thread c holds row c of the weight, and the output tile [256][PIN_TT + 1] is written
+// back along time.  Per output, in this order:
+//   a = 0;  a = fma(w[c][i], x[i], a) for i = 0 .. 19;  a = a + bias[c];  a = a + pe[b][c]
+constexpr int PIN_TT = 16;
+constexpr int PIN_THREADS = FAC_TIMBRE_C;
+
+__global__ void __launch_bounds__(PIN_THREADS) facodec_prosody_input_kernel(FacProsodyInParams p, int tiles) {
+  __shared__ float xs[FAC_PROSODY_BINS][PIN_TT];
+  __shared__ float ys[FAC_TIMBRE_C][PIN_TT + 1];
+  const int b = blockIdx.x / tiles, t0 = (blockIdx.x - b * tiles) * PIN_TT;
+  const int tid = threadIdx.x;
+  const float* xb = p.x + (int64_t)b * p.xsb;
+  for (int i = tid; i < FAC_PROSODY_BINS * PIN_TT; i += PIN_THREADS) {
+    const int j = i / PIN_TT, u = i - j * PIN_TT, t = t0 + u;
+    xs[j][u] = t < p.T ? __ldg(xb + j * p.xsi + (int64_t)t * p.xst) : 0.f;
+  }
+  float w[FAC_PROSODY_BINS];
+#pragma unroll
+  for (int j = 0; j < FAC_PROSODY_BINS; ++j) w[j] = __ldg(p.w + tid * FAC_PROSODY_BINS + j);
+  const float bias = __ldg(p.bias + tid), pe = __ldg(p.pe + (int64_t)b * FAC_TIMBRE_C + tid);
+  __syncthreads();
+#pragma unroll 4
+  for (int u = 0; u < PIN_TT; ++u) {
+    float a = 0.f;
+#pragma unroll
+    for (int j = 0; j < FAC_PROSODY_BINS; ++j) a = __fmaf_rn(w[j], xs[j][u], a);
+    ys[tid][u] = __fadd_rn(__fadd_rn(a, bias), pe);
+  }
+  __syncthreads();
+  float* yb = p.y + (int64_t)b * FAC_TIMBRE_C * p.T;
+  for (int i = tid; i < FAC_TIMBRE_C * PIN_TT; i += PIN_THREADS) {
+    const int c = i / PIN_TT, u = i - c * PIN_TT, t = t0 + u;
+    if (t < p.T) yb[(int64_t)c * p.T + t] = ys[c][u];
   }
 }
 
@@ -588,7 +647,7 @@ int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows
   return AB_OK;
 }
 
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s) {
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody) {
   if (!p.x || !p.emb || !p.codes || !p.quantized || (!p.pe) != (!p.stream)) return fail(AB_ERR_ARG, "facodec rvq: null argument");
   if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.D <= 0 || p.D > FAC_MAX_CODEBOOK_DIM || p.nused[0] <= 0 || p.nused[1] <= 0 ||
       p.ngroups < 2 || p.ngroups > 3)
@@ -597,11 +656,32 @@ int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s) {
   if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: %d channels do not fit shared memory", p.C);
   const int64_t tiles = ceil_div(p.T, RVQ_TT), grid = (int64_t)p.B * tiles;
   if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: grid too large");
+  if (prosody) {
+    static DeviceOnce configured;
+    if (smem > 48 * 1024 && configured.need())
+      AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FacRvqProsodyParams q;
+    static_cast<FacRvqParams&>(q) = p;
+    q.prosody = prosody;
+    facodec_rvq_kernel<true><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(q, (int)tiles);
+    AB_LAUNCH_CHECK("facodec_rvq_kernel<true>");
+    return AB_OK;
+  }
   static DeviceOnce configured;
   if (smem > 48 * 1024 && configured.need())
-    AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  facodec_rvq_kernel<<<(unsigned)grid, RVQ_THREADS, smem, s>>>(p, (int)tiles);
+    AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  facodec_rvq_kernel<false><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(p, (int)tiles);
   AB_LAUNCH_CHECK("facodec_rvq_kernel");
+  return AB_OK;
+}
+
+int launch_facodec_prosody_input(const FacProsodyInParams& p, cudaStream_t s) {
+  if (!p.x || !p.w || !p.bias || !p.pe || !p.y) return fail(AB_ERR_ARG, "facodec prosody input: null argument");
+  if (p.B <= 0 || p.T <= 0) return fail(AB_ERR_ARG, "facodec prosody input: bad shape");
+  const int64_t tiles = ceil_div(p.T, PIN_TT), grid = (int64_t)p.B * tiles;
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "facodec prosody input: grid too large");
+  facodec_prosody_input_kernel<<<(unsigned)grid, PIN_THREADS, 0, s>>>(p, (int)tiles);
+  AB_LAUNCH_CHECK("facodec_prosody_input_kernel");
   return AB_OK;
 }
 

@@ -18,6 +18,11 @@ the same constructor, the same parameter tree (``quantizer.{q}.layers.{j}.{in_pr
 speaker-conditioned prosody transformer (style-adaptive LayerNorms) and adds the content and residual embeddings ->
 ``[B, 256, T]``; ``inference`` is the decoder's.  Its ``forward`` is broken in the reference and is refused.
 
+``FACodecEncoderV2`` / ``FACodecDecoderV2`` (:772-1199) serve the README's second voice-conversion flow: the encoder adds
+``get_prosody_feature`` (the first 20 rows of an 80-row log-mel on the native mel pipeline), and the decoder's
+``forward(x, prosody_feature, vq=True)`` quantizes the prosody group from ``melspec_encoder(melspec_linear(feature))``,
+a second transformer that runs in fp32 at every precision.
+
 The training branch (``vq=False``: the predictors, random residual masking, the losses), ``get_vq`` and a quantizer or
 transformer in training mode are not served; the modules only those evaluate are kept as parameters."""
 from __future__ import annotations
@@ -36,6 +41,9 @@ from .generator import NativeGenerator
 _SERVED = ("amphion_b200 serves FACodecEncoder.forward() / .inference(), FACodecDecoder.forward(vq=True) in eval, "
            "FACodecDecoder.vq2emb() and FACodecDecoder.inference(), and FACodecRedecoder.vq2emb() in eval and "
            "FACodecRedecoder.inference()")
+_SERVED_V2 = ("amphion_b200 serves FACodecEncoderV2.forward() / .inference() / .get_prosody_feature(), "
+              "FACodecDecoderV2.forward(x, prosody_feature, vq=True) in eval, FACodecDecoderV2.vq2emb() and "
+              "FACodecDecoderV2.inference()")
 
 
 def _native_only(name):
@@ -726,3 +734,167 @@ class FACodecRedecoder(NativeGenerator):
 
     def remove_weight_norm(self):
         _remove_all_weight_norm(self)
+
+
+# ---- FACodec V2 (facodec.py:772-1199) ---------------------------------------------------------------------------------
+_PROSODY_BINS = 20
+
+
+class MelSpectrogram(_Holder):
+    """Buffer holder for ns3_codec/melspec.py:39-102 as FACodecEncoderV2 builds it: ``mel_basis`` [num_mels, n_fft/2+1]
+    (Slaney mel filterbank) and ``hann_window`` [win_size].  The transform runs on the native mel pipeline."""
+
+    def __init__(self, n_fft, num_mels, sampling_rate, hop_size, win_size, fmin, fmax, center=False):
+        super().__init__()
+        from ..mel import librosa_mel_fn
+        self.n_fft, self.hop_size, self.win_size = int(n_fft), int(hop_size), int(win_size)
+        self.sampling_rate, self.num_mels, self.fmin, self.fmax, self.center = sampling_rate, num_mels, fmin, fmax, center
+        self.register_buffer("mel_basis", librosa_mel_fn(sampling_rate, n_fft, num_mels, fmin, fmax).float())
+        self.register_buffer("hann_window", torch.hann_window(win_size))
+
+
+class FACodecEncoderV2(FACodecEncoder):
+    """Drop-in for FACodecEncoderV2 (facodec.py:772-845): FACodecEncoder's parameter tree plus the buffers
+    ``mel_transform.{mel_basis, hann_window}``, so ``ns3_facodec_encoder_v2.bin`` loads strictly.  ``forward`` /
+    ``inference`` are FACodecEncoder's; ``get_prosody_feature(x)`` is served natively."""
+
+    def __init__(self, ngf=32, up_ratios=(2, 4, 5, 5), out_channels=1024):
+        super().__init__(ngf=ngf, up_ratios=up_ratios, out_channels=out_channels)
+        self.mel_transform = MelSpectrogram(n_fft=1024, num_mels=80, sampling_rate=16000, hop_size=200, win_size=800,
+                                            fmin=0, fmax=8000)
+
+    def prosody_frames(self, n_samples):
+        """Frames of get_prosody_feature for n_samples samples: (N + 2 pad - n_fft) // hop + 1, pad = (n_fft - hop) / 2."""
+        mt = self.mel_transform
+        pad = (mt.n_fft - mt.hop_size) // 2
+        return (int(n_samples) + 2 * pad - mt.n_fft) // mt.hop_size + 1
+
+    def get_prosody_feature(self, x):
+        """wav [B, 1, N] (any strides) -> [B, 20, F] fp32 log-mel, the first 20 of the 80 mel rows (facodec.py:820-821):
+        reflect pad (n_fft - hop) / 2, |STFT| with sqrt(re^2 + im^2 + 1e-9), the module's mel_basis rows, log(clamp(.,
+        1e-5)).  Runs on the native STFT + mel pipeline with the module's own buffers."""
+        from ..mel import native_stft_mel
+        if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[1] != 1:
+            got = tuple(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__
+            raise ValueError(f"FACodecEncoderV2.get_prosody_feature expects a waveform of shape [B, 1, N], got {got}")
+        mt = self.mel_transform
+        pad = (mt.n_fft - mt.hop_size) // 2
+        B, _, N = x.shape
+        if B == 0:
+            raise ValueError("amphion_b200: empty waveform batch")
+        if N <= pad:
+            raise ValueError(f"FACodecEncoderV2.get_prosody_feature: {N} samples are too few for the reflect pad of {pad} "
+                             f"(the reference raises there too); it needs at least {pad + 1}")
+        _capi.require_cuda(x, "FACodecEncoderV2.get_prosody_feature")
+        basis = mt.mel_basis[:_PROSODY_BINS].to(device=x.device, dtype=torch.float32).contiguous()
+        window = mt.hann_window.to(device=x.device, dtype=torch.float32).contiguous()
+        with torch.no_grad():
+            _, mel, _ = native_stft_mel(x[:, 0, :].float(), mt.n_fft, mt.hop_size, mt.win_size, window, basis, pad, 1e-9,
+                                        clamp=1e-5)
+        return mel
+
+
+class FACodecDecoderV2(FACodecDecoder):
+    """Drop-in for FACodecDecoderV2 (facodec.py:848-1199): FACodecDecoder's constructor and parameter tree plus
+    ``melspec_linear`` (Linear 20 -> 256) and ``melspec_encoder`` (a 4-layer, 256-wide transformer), so
+    ``ns3_facodec_decoder_v2.bin`` loads strictly.  Served natively, in eval:
+
+    - ``forward(x, prosody_feature, vq=True)``: latent ``[B, 256, T]`` and prosody feature ``[B, 20, T]`` -> V1's
+      5-tuple; the prosody group quantizes the prosody transformer's output (fp32 at every precision), the content
+      group x, the residual group x - (prosody + content);
+    - ``vq2emb(vq, use_residual=True)`` and ``inference(x, speaker_embedding)``: FACodecDecoder's."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.melspec_linear = nn.Linear(_PROSODY_BINS, 256)
+        self.melspec_encoder = TransformerEncoder()
+        self.apply(_init_weights)   # reset_parameters (facodec.py:1025): every Conv1d bias 0, as a fresh V2 decoder has
+
+    def _c_config(self):
+        c = super()._c_config()
+        c.facodec_prosody_encoder = int(self._quantize_handle)
+        return c
+
+    def vq2emb(self, vq, use_residual=True):
+        """codes [n_q, B, T] -> [B, in_channels, T] fp32 (facodec.py:1179-1190; FACodecDecoder.vq2emb's code path)."""
+        return super().vq2emb(vq, use_residual_code=use_residual)
+
+    def forward(self, x=None, prosody_feature=None, vq=True, get_vq=False, eval_vq=True, speaker_embedding=None,
+                n_quantizers=None, quantized=None):
+        """``vq=True``: x [B, 256, T] fp32 and prosody_feature [B, 20, T] (any strides) -> ``(outs [B, 256, T], qs int64
+        [n_used, B, T], commit_loss zeros [n_used], quantized_buf [2 or 3 x [B, 256, T]], spk_embs [B, 256])`` on x's
+        device, without autograd history (facodec.py:1064-1094 in eval).  ``n_quantizers = k`` keeps the first k layers
+        of each group."""
+        if get_vq:
+            raise NotImplementedError(f"amphion_b200: FACodecDecoderV2.forward(get_vq=True) is not served; {_SERVED_V2}")
+        if vq is not True:
+            raise NotImplementedError(f"amphion_b200: the training branch of FACodecDecoderV2.forward (the predictors, "
+                                      f"random residual masking) is not served; {_SERVED_V2}")
+        if self.in_channels != 256:
+            raise ValueError(f"amphion_b200: FACodecDecoderV2.forward(vq=True) needs in_channels == 256, the timbre "
+                             f"encoder's width (got {self.in_channels})")
+        if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[1] != self.in_channels:
+            got = tuple(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__
+            raise ValueError(f"FACodecDecoderV2.forward expects x of shape [B, {self.in_channels}, T], got {got}")
+        pf = prosody_feature
+        B, _, T = x.shape
+        if not isinstance(pf, torch.Tensor) or pf.dim() != 3 or pf.shape[0] != B or pf.shape[1] != _PROSODY_BINS:
+            got = tuple(pf.shape) if isinstance(pf, torch.Tensor) else type(pf).__name__
+            raise ValueError(f"FACodecDecoderV2.forward expects a prosody feature of shape [{B}, {_PROSODY_BINS}, T], "
+                             f"got {got}")
+        if pf.shape[2] != T:
+            # at hop 200 about a quarter of waveform lengths give one more encoder frame than mel frames
+            raise ValueError(f"FACodecDecoderV2.forward: x has {T} frames and the prosody feature {pf.shape[2]}; they "
+                             f"must match (the reference fails there too).  Trim the longer one to the shorter")
+        if B == 0 or T == 0:
+            raise ValueError("amphion_b200: empty latent batch")
+        if not x.is_cuda:
+            raise NotImplementedError(f"amphion_b200: FACodecDecoderV2.forward(vq=True) needs a CUDA tensor (got "
+                                      f"'{x.device}'); there is no CPU fallback; {_SERVED_V2}")
+        if pf.device != x.device:
+            raise ValueError("FACodecDecoderV2.forward: x and the prosody feature are on different devices")
+        n_pe = min(self.timbre_encoder.position_emb.pe.shape[0], self.melspec_encoder.position_emb.pe.shape[0])
+        if B > n_pe:
+            raise ValueError(f"amphion_b200: batch {B} > {n_pe}, the rows of the transformers' positional encoding "
+                             f"(the reference fails there too)")
+        k = max(self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r) if n_quantizers is None else int(n_quantizers)
+        if k < 1:
+            raise ValueError(f"amphion_b200: n_quantizers {n_quantizers} < 1 runs no layer (the reference raises too)")
+        if eval_vq:
+            self.quantizer.eval()   # facodec.py:1076-1077
+        if self.quantizer.training or any(m.training for m in self.quantizer.modules()):
+            raise NotImplementedError(f"amphion_b200: a quantizer in training mode (quantizer dropout, commitment "
+                                      f"losses) is not served; {_SERVED_V2}")
+        for name in ("timbre_encoder", "melspec_encoder"):
+            mod = getattr(self, name)
+            if mod.training or any(m.training for m in mod.modules()):
+                raise NotImplementedError(f"amphion_b200: the {name} in training mode (dropout) is not served; "
+                                          f"{_SERVED_V2}")
+        if not self._quantize_handle:
+            # the decode-only handle lists no quantizer / transformer tensors: re-create it with them
+            self._quantize_handle = True
+            if self._handle is not None:
+                _capi.lib.ab_generator_destroy(self._handle)
+                self._handle = None
+            self._arena_key = None
+        x = x.float()
+        pf = pf.float()
+        nq = [min(k, n) for n in (self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r)]
+        n_used, G = sum(nq), 3 if self.vq_num_q_r > 0 else 2
+        dev = x.device
+        with torch.cuda.device(dev):
+            self._sync_params(dev)
+            lib, h = _capi.lib, self._handle
+            need = lib.ab_facodec_quantize_workspace_bytes(h, B, T)
+            wbase = self._workspace_for(dev, need)
+            outs = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=dev)
+            qs = torch.empty(n_used, B, T, dtype=torch.int64, device=dev)
+            buf = torch.empty(G, B, self.in_channels, T, dtype=torch.float32, device=dev)
+            spk = torch.empty(B, self.in_channels, dtype=torch.float32, device=dev)
+            _capi.check(lib.ab_facodec_quantize_prosody(h, _capi.ptr(x), _capi.shape_array(x.stride()), _capi.ptr(pf),
+                                                        _capi.shape_array(pf.stride()), B, T, k, _capi.ptr(outs),
+                                                        _capi.ptr(qs), _capi.ptr(buf), _capi.ptr(spk), C.c_void_p(wbase),
+                                                        need, _capi.stream_ptr()), "ab_facodec_quantize_prosody")
+            self.last_launches = lib.ab_generator_last_launches(h)
+        commit_loss = torch.zeros(n_used, dtype=torch.float32, device=dev)
+        return outs, qs, commit_loss, list(buf.unbind(0)), spk

@@ -185,6 +185,10 @@ typedef struct ab_generator_config {
   /* AB_GEN_FACODEC only (0 elsewhere): 1 = the handle also serves FACodecDecoder.forward(vq=True) (ab_facodec_quantize)
    * and lists the quantizers' in_proj and the timbre encoder's tensors; needs n_mel == 256 */
   int32_t facodec_quantize;
+  /* AB_GEN_FACODEC with facodec_quantize = 1 only (0 elsewhere): 1 = FACodecDecoderV2 (facodec.py:848-1094): the handle
+   * also lists "melspec_linear.{weight,bias}" ([256, 20], [256]) and the prosody transformer "melspec_encoder.*" (named
+   * as "timbre_encoder.*"), and its forward(vq=True) is ab_facodec_quantize_prosody (ab_facodec_quantize refuses it) */
+  int32_t facodec_prosody_encoder;
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -340,6 +344,19 @@ size_t ab_facodec_quantize_workspace_bytes(const ab_generator* g, int64_t batch,
 int ab_facodec_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t batch, int64_t frames,
                         int32_t n_quantizers, float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out,
                         float* dev_spk_out, void* dev_workspace, size_t workspace_bytes, void* stream);
+/* FACodecDecoderV2.forward(x, prosody_feature, vq=True) in eval (facodec.py:1027-1094), on a handle created with
+ * facodec_prosody_encoder = 1 (else AB_ERR_STATE; ab_facodec_quantize refuses such a handle with AB_ERR_STATE, as the V2
+ * forward has no form without the prosody feature).  prosody [B, 20, T] fp32 with any element strides, T the frames of
+ * x.  The prosody group quantizes melspec_encoder(melspec_linear(prosody^T))^T instead of x: per frame the input
+ * projection (an fp32 FMA chain over the 20 rows from 0, then the bias) plus row b of "melspec_encoder.position_emb.pe",
+ * then 4 pre-LN layers and last_ln, all fp32 on CUDA cores at every precision (its output is quantized).  The content
+ * group reads x, the residual group x - (prosody + content); everything else, the outputs and their layout are as in
+ * ab_facodec_quantize.  Launches: 1 input projection, 4 x 7 layer launches, last_ln, then ab_facodec_quantize's 31.
+ * Workspace: ab_facodec_quantize_workspace_bytes (on such a handle it sizes this call), 256-byte aligned. */
+int ab_facodec_quantize_prosody(ab_generator* g, const float* dev_x, const int64_t x_strides[3], const float* dev_prosody,
+                                const int64_t prosody_strides[3], int64_t batch, int64_t frames, int32_t n_quantizers,
+                                float* dev_emb_out, int64_t* dev_codes_out, float* dev_quantized_out, float* dev_spk_out,
+                                void* dev_workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * FACodec redecoder (AB_GEN_FACODEC_REDECODER): FACodecRedecoder.vq2emb (models/codec/ns3_codec/facodec.py:734-759);
@@ -454,6 +471,13 @@ int ab_tc_conv_forward(int32_t mode, const float* dev_x, const int64_t x_strides
  * diffwave_upsample: SpectrogramUpsampler (diffwave.py:68-93) of mel [B, n_mel, frames] with element strides mel_strides:
  *   two ConvTranspose2d(1, 1, [3, 2f], stride [1, f], padding [1, f / 2]) (weights [3, 2f], biases [1]), each followed by
  *   leaky_relu(0.4), even f1, f2 -> out [B, n_mel, frames f1 f2]. */
+/* FACodecDecoderV2's prosody input projection: the first launch of ab_facodec_quantize_prosody, alone (no reference
+ * counterpart; exposed for the bit-exact tests).  x [B, 20, T] fp32 with any element
+ *   strides, w [256, 20] (nn.Linear layout), bias [256], pe [>= B][256] (row b for utterance b) -> y [B, 256, T] fp32
+ *   contiguous, y[b, c, t] = ((fma chain over i = 0..19 of w[c][i] x[b, i, t], from 0) + bias[c]) + pe[b][c]. */
+int ab_facodec_prosody_input_forward(const float* dev_x, const int64_t x_strides[3], const float* dev_w,
+                                     const float* dev_bias, const float* dev_pe, int64_t batch, int64_t frames,
+                                     float* dev_y, void* stream);
 /* Vocos building blocks: one launch each of the kernels forward_vocos runs for a ConvNeXt block and the head (no
  * reference counterpart; exposed for the bit-exact tests).  Every fp32 tensor contiguous.
  * vocos_norm: LayerNorm over channels (two-pass mean and biased variance, then (x - mean) * rstd * ln_w + ln_b) of x
