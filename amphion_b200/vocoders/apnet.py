@@ -139,19 +139,14 @@ class _Trunk(NativeGenerator):
         if mel.dtype != torch.float32:
             mel = mel.float()
         B, _, T = mel.shape
-        with torch.cuda.device(mel.device):
-            self._sync_params(mel.device)
-            lib, h = _capi.lib, self._handle
-            need = lib.ab_generator_workspace_bytes(h, B, T)
-            if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != mel.device:
-                self._workspace = None
-                self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=mel.device)
-            wbase = (self._workspace.data_ptr() + 255) // 256 * 256
+        with self._launch(mel.device) as h:
+            need = _capi.lib.ab_generator_workspace_bytes(h, B, T)
+            ws = self._scratch(need, mel.device)
             cout = self._c_config().trunk_out_channels
             out = torch.empty(B, cout, T, dtype=torch.float32, device=mel.device)
-            _capi.check(lib.ab_generator_forward(h, _capi.ptr(mel), B, T, _capi.shape_array(mel.stride()), _capi.ptr(out),
-                                                 C.c_void_p(wbase), need, _capi.stream_ptr()), "ab_generator_forward")
-            self.last_launches = lib.ab_generator_last_launches(h)
+            _capi.check(_capi.lib.ab_generator_forward(h, _capi.ptr(mel), B, T, _capi.shape_array(mel.stride()),
+                                                       _capi.ptr(out), ws, need, _capi.stream_ptr()),
+                        "ab_generator_forward")
         return out
 
 

@@ -132,30 +132,29 @@ class DiffWave(NativeGenerator):
         need = _capi.lib.ab_diffwave_workspace_bytes(self._handle, B, F, n_steps)
         if need == 0:
             raise RuntimeError(f"amphion_b200: DiffWave workspace query failed: {_capi.last_error()}")
-        if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != device:
-            self._workspace = None
-            self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
-        return C.c_void_p((self._workspace.data_ptr() + 255) // 256 * 256), need
+        return self._scratch(need, device), need
 
     def _condition(self, spectrogram, steps):
         """Upsampled mel and the diffusion projections of every value in ``steps`` (host floats) into the workspace;
         returns (workspace pointer, bytes)."""
-        self._sync_params(spectrogram.device)
         B, _, F = spectrogram.shape
         steps = np.ascontiguousarray(steps, dtype=np.float32)
-        ws, need = self._ensure_workspace(B, F, len(steps), spectrogram.device)
-        _capi.check(_capi.lib.ab_diffwave_condition(
-            self._handle, _capi.ptr(spectrogram), B, F, _capi.shape_array(spectrogram.stride()),
-            steps.ctypes.data_as(C.POINTER(C.c_float)), len(steps), ws, need, _capi.stream_ptr()), "ab_diffwave_condition")
+        with self._launch(spectrogram.device) as h:
+            ws, need = self._ensure_workspace(B, F, len(steps), spectrogram.device)
+            _capi.check(_capi.lib.ab_diffwave_condition(
+                h, _capi.ptr(spectrogram), B, F, _capi.shape_array(spectrogram.stride()),
+                steps.ctypes.data_as(C.POINTER(C.c_float)), len(steps), ws, need, _capi.stream_ptr()),
+                "ab_diffwave_condition")
         return ws, need
 
     def _step(self, audio, row, c1, c2, sigma, noise, ws, need):
-        """One sampler update of ``audio`` [B, L] in place with conditioning row ``row``."""
+        """One sampler update of ``audio`` [B, L] in place with conditioning row ``row``, on the workspace and the
+        parameters ``_condition`` left (the sampler calls it under the audio's device)."""
         B, L = audio.shape
         _capi.check(_capi.lib.ab_diffwave_step(self._handle, _capi.ptr(audio), B, L // self._hop(), row, float(c1), float(c2),
                                                float(sigma), _capi.ptr(noise), None, ws, need, _capi.stream_ptr()),
                     "ab_diffwave_step")
-        self.last_launches = _capi.lib.ab_generator_last_launches(self._handle)
+        self._count_launches()
 
     def forward(self, audio, diffusion_step, spectrogram):
         """audio [B, L], diffusion_step [1] or [B] (integer: a table row; float: lerp between rows), spectrogram
@@ -173,14 +172,11 @@ class DiffWave(NativeGenerator):
         if audio.device != spectrogram.device:
             raise ValueError("amphion_b200: audio and spectrogram must be on the same device")
         audio = audio.float().contiguous()
-        with torch.cuda.device(spectrogram.device):
-            self._sync_params(spectrogram.device)
-            B, _, F = spectrogram.shape
+        with self._launch(spectrogram.device) as h:
             ws, need = self._ensure_workspace(B, F, len(steps), spectrogram.device)
             eps = torch.empty(B, 1, audio.shape[1], dtype=torch.float32, device=audio.device)
             _capi.check(_capi.lib.ab_diffwave_forward(
-                self._handle, _capi.ptr(audio), B, F, _capi.ptr(spectrogram), _capi.shape_array(spectrogram.stride()),
+                h, _capi.ptr(audio), B, F, _capi.ptr(spectrogram), _capi.shape_array(spectrogram.stride()),
                 steps.ctypes.data_as(C.POINTER(C.c_float)), len(steps), _capi.ptr(eps), ws, need, _capi.stream_ptr()),
                 "ab_diffwave_forward")
-            self.last_launches = _capi.lib.ab_generator_last_launches(self._handle)
         return eps

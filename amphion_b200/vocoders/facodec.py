@@ -27,8 +27,6 @@ The training branch (``vq=False``: the predictors, random residual masking, the 
 transformer in training mode are not served; the modules only those evaluate are kept as parameters."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 from torch import nn
@@ -184,32 +182,91 @@ class TransformerEncoder(_Holder):
         self.last_ln = StyleAdaptiveLayerNorm(encoder_hidden) if use_cln else nn.LayerNorm(encoder_hidden)
 
 
-def _generator_config(m, kind):
-    """The BigVGAN-family generator fields of the decoder and the redecoder (model.*, facodec.py:220-240)."""
-    if len(m.up_ratios) > _capi.AB_MAX_STAGES:
-        raise ValueError(f"amphion_b200: too many up_ratios for the native {type(m).__name__}")
+def _block_config(kind, n_in, channels, up_ratios):
+    """The fixed fields of every FACodec generator: a stage per ratio u (kernel 2u), one ResidualUnit kernel (k = 7,
+    dilations 1, 3, 9) and SnakeBeta with logscale."""
     c = _capi.GeneratorConfig()
-    c.kind = kind
-    c.n_mel = m.in_channels
-    c.upsample_initial_channel = m.upsample_initial_channel
-    c.num_upsamples = len(m.up_ratios)
-    for i, u in enumerate(m.up_ratios):
+    c.kind, c.n_mel, c.upsample_initial_channel = kind, n_in, channels
+    c.num_upsamples = len(up_ratios)
+    for i, u in enumerate(up_ratios):
         c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
     c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
     for p, d in enumerate((1, 3, 9)):
         c.resblock_dilation_sizes[0][p] = d
     c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
+    return c
+
+
+def _generator_config(m, kind):
+    """The BigVGAN-family generator fields of the decoder and the redecoder (model.*, facodec.py:220-240)."""
+    if len(m.up_ratios) > _capi.AB_MAX_STAGES:
+        raise ValueError(f"amphion_b200: too many up_ratios for the native {type(m).__name__}")
+    c = _block_config(kind, m.in_channels, m.upsample_initial_channel, m.up_ratios)
     for i, (n, bits) in enumerate(((m.vq_num_q_p, m.codebook_size_prosody), (m.vq_num_q_c, m.codebook_size_content),
                                    (m.vq_num_q_r, m.codebook_size_residual))):
         c.vq_num_q[i], c.vq_codebook_bits[i] = n, int(bits)
     return c
 
 
-def _workspace_for(m, device, need):
-    if m._workspace is None or m._workspace.numel() < need + 256 or m._workspace.device != device:
-        m._workspace = None
-        m._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
-    return (m._workspace.data_ptr() + 255) // 256 * 256
+def _build_generator(m, in_channels, upsample_initial_channel, up_ratios, timbre_encoder=False):
+    """The decoder's and the redecoder's ``model.*``, ``timbre_linear`` and ``timbre_norm`` (facodec.py:337-369,
+    :656-677); with ``timbre_encoder``, the decoder's timbre encoder between them.  The order is the reference's, so a
+    seeded construction draws the same initial weights."""
+    channels = upsample_initial_channel
+    layers = [weight_norm(nn.Conv1d(in_channels, channels, kernel_size=7, padding=3))]
+    for i, stride in enumerate(up_ratios):
+        layers.append(DecoderBlock(channels // 2 ** i, channels // 2 ** (i + 1), stride))
+    output_dim = channels // 2 ** len(up_ratios)
+    layers += [_act(output_dim), weight_norm(nn.Conv1d(output_dim, 1, kernel_size=7, padding=3)), nn.Tanh()]
+    m.model = nn.Sequential(*layers)
+    if timbre_encoder:
+        m.timbre_encoder = TransformerEncoder()
+    m.timbre_linear = nn.Linear(in_channels, in_channels * 2)
+    m.timbre_linear.bias.data[:in_channels] = 1
+    m.timbre_linear.bias.data[in_channels:] = 0
+    m.timbre_norm = nn.LayerNorm(in_channels, elementwise_affine=False)
+
+
+def _refuse_training(module, what, why, served):
+    """Dropout and the training losses are not served: refuse ``module`` when it or a submodule is in training mode."""
+    if any(m.training for m in module.modules()):
+        raise NotImplementedError(f"amphion_b200: {what} in training mode ({why}) is not served; {served}")
+
+
+def _check_codes(m, vq, use_residual, who, table):
+    """Codes the kernel would not read (it writes NaN there): refuse them before the launch, as F.embedding does."""
+    p, c, r = m.vq_num_q_p, m.vq_num_q_c, m.vq_num_q_r
+    groups = [(0, p, m.codebook_size_prosody), (p, p + c, m.codebook_size_content)]
+    if use_residual and r > 0:
+        groups.append((p + c, p + c + r, m.codebook_size_residual))
+    for q0, q1, bits in groups:
+        part = vq[q0:q1]
+        lo, hi = int(part.min()), int(part.max())
+        if lo < 0 or hi >= 2 ** int(bits):
+            raise ValueError(f"{who}.vq2emb: code rows {q0}..{q1 - 1} hold {lo}..{hi}, outside the {table} "
+                             f"[0, {2 ** int(bits)})")
+
+
+class _FACodecGenerator(NativeGenerator):
+    """The hooks the FACodec encoder, decoder and redecoder share."""
+
+    def _input_channels(self):
+        return self.in_channels
+
+    def _hop(self):
+        return self.hop_length
+
+    def _upsample_rates(self):
+        return list(self.up_ratios)
+
+    def remove_weight_norm(self):
+        def _remove(mod):
+            try:
+                remove_weight_norm(mod)
+            except ValueError:   # this module has no weight norm
+                return
+        self.apply(_remove)
+        self.invalidate()
 
 
 def _inference(m, x, speaker_embedding, out, tail_events):
@@ -232,42 +289,18 @@ def _inference(m, x, speaker_embedding, out, tail_events):
     spk = spk.float()
     if spk.stride(1) != 1:
         spk = spk.contiguous()
-    with torch.cuda.device(x.device):
-        m._sync_params(x.device)
-        lib, h = _capi.lib, m._handle
-        need = lib.ab_generator_workspace_bytes(h, B, T)
-        wbase = _workspace_for(m, x.device, need)
-        n_out = T * m.hop_length
-        if out is None:
-            wav = torch.empty(B, 1, n_out, dtype=torch.float32, device=x.device)
-        else:
-            if (tuple(out.shape) != (B, 1, n_out) or out.dtype != torch.float32 or out.device != x.device
-                    or not out.is_contiguous()):
-                raise ValueError(f"out must be a contiguous fp32 [{B}, 1, {n_out}] tensor on {x.device}")
-            wav = out
-        if tail_events:
-            for ev in tail_events:
-                ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded below
-            arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
-            _capi.check(lib.ab_generator_set_tail_events(h, arr, len(tail_events)), "ab_generator_set_tail_events")
-        _capi.check(lib.ab_facodec_inference(h, _capi.ptr(x), B, T, _capi.shape_array(x.stride()), _capi.ptr(spk),
-                                             spk.stride(0), _capi.ptr(wav), C.c_void_p(wbase), need,
-                                             _capi.stream_ptr()), "ab_facodec_inference")
-        m.last_launches = lib.ab_generator_last_launches(h)
+    with m._launch(x.device) as h:
+        need = _capi.lib.ab_generator_workspace_bytes(h, B, T)
+        ws = m._scratch(need, x.device)
+        wav = m._output(out, (B, 1, T * m.hop_length), x.device)
+        m._arm_tail_events(tail_events)
+        _capi.check(_capi.lib.ab_facodec_inference(h, _capi.ptr(x), B, T, _capi.shape_array(x.stride()),
+                                                   _capi.ptr(spk), spk.stride(0), _capi.ptr(wav), ws, need,
+                                                   _capi.stream_ptr()), "ab_facodec_inference")
     return wav
 
 
-def _remove_all_weight_norm(m):
-    def _remove(mod):
-        try:
-            remove_weight_norm(mod)
-        except ValueError:   # this module has no weight norm
-            return
-    m.apply(_remove)
-    m.invalidate()
-
-
-class FACodecDecoder(NativeGenerator):
+class FACodecDecoder(_FACodecGenerator):
     kind = "facodec"
 
     def __init__(self, in_channels=256, upsample_initial_channel=1536, ngf=32, up_ratios=(5, 5, 4, 2), vq_num_q_c=2,
@@ -305,19 +338,7 @@ class FACodecDecoder(NativeGenerator):
         if self.vq_num_q_r > 0:
             self.quantizer.append(rvq(vq_num_q_r, codebook_size_residual))
 
-        channels = upsample_initial_channel
-        layers = [weight_norm(nn.Conv1d(in_channels, channels, kernel_size=7, padding=3))]
-        for i, stride in enumerate(up_ratios):
-            layers.append(DecoderBlock(channels // 2 ** i, channels // 2 ** (i + 1), stride))
-        output_dim = channels // 2 ** len(up_ratios)
-        layers += [_act(output_dim), weight_norm(nn.Conv1d(output_dim, 1, kernel_size=7, padding=3)), nn.Tanh()]
-        self.model = nn.Sequential(*layers)
-
-        self.timbre_encoder = TransformerEncoder()
-        self.timbre_linear = nn.Linear(in_channels, in_channels * 2)
-        self.timbre_linear.bias.data[:in_channels] = 1
-        self.timbre_linear.bias.data[in_channels:] = 0
-        self.timbre_norm = nn.LayerNorm(in_channels, elementwise_affine=False)
+        _build_generator(self, in_channels, upsample_initial_channel, up_ratios, timbre_encoder=True)
         self.f0_predictor = CNNLSTM(in_channels, 1, 2)
         self.phone_predictor = CNNLSTM(in_channels, 5003, 1)
         self.use_gr_content_f0 = use_gr_content_f0
@@ -338,22 +359,15 @@ class FACodecDecoder(NativeGenerator):
                                                     CNNLSTM(in_channels, 245200, 1, global_pred=True))
 
     # ---- NativeGenerator hooks -------------------------------------------------------
-    def _input_channels(self):
-        return self.in_channels
-
-    def _hop(self):
-        return self.hop_length
-
-    def _upsample_rates(self):
-        return list(self.up_ratios)
-
     def _c_config_decode(self):
         c = _generator_config(self, _capi.GEN_FACODEC)
         c.vq_codebook_dim = self.codebook_dim
         return c
 
-    def _workspace_for(self, device, need):
-        return _workspace_for(self, device, need)
+    def _c_config(self):
+        c = self._c_config_decode()
+        c.facodec_quantize = int(self._quantize_handle)
+        return c
 
     # ---- served methods --------------------------------------------------------------
     def vq2emb(self, vq, use_residual_code=True):
@@ -370,23 +384,12 @@ class FACodecDecoder(NativeGenerator):
             raise ValueError("amphion_b200: empty code batch")
         _capi.require_cuda(vq, "FACodecDecoder.vq2emb")
         vq = vq.long()
-        # codes the kernel would not read (it writes NaN there): refuse them before the launch, as F.embedding does
-        groups = [(0, self.vq_num_q_p, self.codebook_size_prosody), (self.vq_num_q_p, n_pc, self.codebook_size_content)]
-        if use_residual_code and self.vq_num_q_r > 0:
-            groups.append((n_pc, n_all, self.codebook_size_residual))
-        for q0, q1, bits in groups:
-            part = vq[q0:q1]
-            lo, hi = int(part.min()), int(part.max())
-            if lo < 0 or hi >= 2 ** int(bits):
-                raise ValueError(f"FACodecDecoder.vq2emb: code rows {q0}..{q1 - 1} hold {lo}..{hi}, outside the "
-                                 f"codebook [0, {2 ** int(bits)})")
-        with torch.cuda.device(vq.device):
-            self._sync_params(vq.device)
+        _check_codes(self, vq, use_residual_code, "FACodecDecoder", "codebook")
+        with self._launch(vq.device) as h:
             out = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=vq.device)
-            _capi.check(_capi.lib.ab_facodec_vq2emb(self._handle, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B, T,
+            _capi.check(_capi.lib.ab_facodec_vq2emb(h, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B, T,
                                                     int(bool(use_residual_code)), _capi.ptr(out), _capi.stream_ptr()),
                         "ab_facodec_vq2emb")
-            self.last_launches = _capi.lib.ab_generator_last_launches(self._handle)
         return out
 
     def inference(self, x, speaker_embedding, out=None, tail_events=None):
@@ -394,11 +397,6 @@ class FACodecDecoder(NativeGenerator):
 
         ``out`` / ``tail_events`` (beyond the reference signature) behave as in the other generators' forward."""
         return _inference(self, x, speaker_embedding, out, tail_events)
-
-    def _c_config(self):
-        c = self._c_config_decode()
-        c.facodec_quantize = int(self._quantize_handle)
-        return c
 
     def forward(self, x=None, vq=True, get_vq=False, eval_vq=True, speaker_embedding=None, n_quantizers=None,
                 quantized=None):
@@ -422,50 +420,61 @@ class FACodecDecoder(NativeGenerator):
         B, _, T = x.shape
         if B == 0 or T == 0:
             raise ValueError("amphion_b200: empty latent batch")
-        if B > self.timbre_encoder.position_emb.pe.shape[0]:
-            raise ValueError(f"amphion_b200: batch {B} > {self.timbre_encoder.position_emb.pe.shape[0]}, the rows of "
-                             f"the timbre encoder's positional encoding (the reference fails there too)")
+        return self._quantize(x, None, n_quantizers, eval_vq)
+
+    def _quantize(self, x, pf, n_quantizers, eval_vq):
+        """forward(vq=True) once its arguments are checked: V1 (``pf`` None) quantizes the prosody group from x, V2 from
+        ``pf``, the prosody feature, through the melspec encoder."""
+        served = _SERVED if pf is None else _SERVED_V2
+        # the transformers the pass runs, under the names the refusals give them
+        encoders = {"timbre encoder": self.timbre_encoder} if pf is None else \
+            {"timbre_encoder": self.timbre_encoder, "melspec_encoder": self.melspec_encoder}
+        B, _, T = x.shape
+        n_pe = min(e.position_emb.pe.shape[0] for e in encoders.values())
+        if B > n_pe:
+            rows = "the timbre encoder's" if pf is None else "the transformers'"
+            raise ValueError(f"amphion_b200: batch {B} > {n_pe}, the rows of {rows} positional encoding (the reference "
+                             f"fails there too)")
         k = max(self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r) if n_quantizers is None else int(n_quantizers)
         if k < 1:
             raise ValueError(f"amphion_b200: n_quantizers {n_quantizers} < 1 runs no layer (the reference raises too)")
         if eval_vq:
-            self.quantizer.eval()   # facodec.py:460-461
-        if self.quantizer.training or any(m.training for m in self.quantizer.modules()):
-            raise NotImplementedError(f"amphion_b200: a quantizer in training mode (quantizer dropout, commitment "
-                                      f"losses) is not served; {_SERVED}")
-        if self.timbre_encoder.training or any(m.training for m in self.timbre_encoder.modules()):
-            raise NotImplementedError(f"amphion_b200: the timbre encoder in training mode (dropout) is not served; "
-                                      f"{_SERVED}")
+            self.quantizer.eval()   # facodec.py:460-461, :1076-1077
+        _refuse_training(self.quantizer, "a quantizer", "quantizer dropout, commitment losses", served)
+        for name, mod in encoders.items():
+            _refuse_training(mod, f"the {name}", "dropout", served)
         if not self._quantize_handle:
-            # the decode-only handle lists no quantizer / timbre tensors: re-create it with them
+            # the decode-only handle lists no quantizer / transformer tensors: re-create it with them
             self._quantize_handle = True
             if self._handle is not None:
                 _capi.lib.ab_generator_destroy(self._handle)
                 self._handle = None
             self._arena_key = None
-        if x.dtype != torch.float32:
-            x = x.float()
+        x = x.float()
         nq = [min(k, n) for n in (self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r)]
         n_used, G = sum(nq), 3 if self.vq_num_q_r > 0 else 2
         dev = x.device
-        with torch.cuda.device(dev):
-            self._sync_params(dev)
-            lib, h = _capi.lib, self._handle
-            need = lib.ab_facodec_quantize_workspace_bytes(h, B, T)
-            wbase = self._workspace_for(dev, need)
+        with self._launch(dev) as h:
+            need = _capi.lib.ab_facodec_quantize_workspace_bytes(h, B, T)
+            ws = self._scratch(need, dev)
             outs = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=dev)
             qs = torch.empty(n_used, B, T, dtype=torch.int64, device=dev)
             buf = torch.empty(G, B, self.in_channels, T, dtype=torch.float32, device=dev)
             spk = torch.empty(B, self.in_channels, dtype=torch.float32, device=dev)
-            _capi.check(lib.ab_facodec_quantize(h, _capi.ptr(x), _capi.shape_array(x.stride()), B, T, k, _capi.ptr(outs),
-                                                _capi.ptr(qs), _capi.ptr(buf), _capi.ptr(spk), C.c_void_p(wbase), need,
-                                                _capi.stream_ptr()), "ab_facodec_quantize")
-            self.last_launches = lib.ab_generator_last_launches(h)
+            xs = _capi.shape_array(x.stride())
+            if pf is None:
+                _capi.check(_capi.lib.ab_facodec_quantize(h, _capi.ptr(x), xs, B, T, k, _capi.ptr(outs), _capi.ptr(qs),
+                                                          _capi.ptr(buf), _capi.ptr(spk), ws, need, _capi.stream_ptr()),
+                            "ab_facodec_quantize")
+            else:
+                pf = pf.float()
+                _capi.check(_capi.lib.ab_facodec_quantize_prosody(h, _capi.ptr(x), xs, _capi.ptr(pf),
+                                                                  _capi.shape_array(pf.stride()), B, T, k,
+                                                                  _capi.ptr(outs), _capi.ptr(qs), _capi.ptr(buf),
+                                                                  _capi.ptr(spk), ws, need, _capi.stream_ptr()),
+                            "ab_facodec_quantize_prosody")
         commit_loss = torch.zeros(n_used, dtype=torch.float32, device=dev)
         return outs, qs, commit_loss, list(buf.unbind(0)), spk
-
-    def remove_weight_norm(self):
-        _remove_all_weight_norm(self)
 
 
 class EncoderBlock(nn.Module):
@@ -490,7 +499,7 @@ def _init_weights(m):
         nn.init.constant_(m.bias, 0)
 
 
-class FACodecEncoder(NativeGenerator):
+class FACodecEncoder(_FACodecGenerator):
     """Drop-in for FACodecEncoder (facodec.py:157-194): the same constructor and parameter tree (``block.*``), so the
     released ``ns3_facodec_encoder.bin`` loads strictly.  ``forward(x)`` / ``inference(x)``: wav ``[B, 1, N]`` (any
     strides) -> ``[B, out_channels, F]`` fp32, F = ``frames(N)``."""
@@ -516,26 +525,10 @@ class FACodecEncoder(NativeGenerator):
     def _input_channels(self):
         return 1
 
-    def _hop(self):
-        return self.hop_length
-
-    def _upsample_rates(self):
-        return list(self.up_ratios)
-
     def _c_config(self):
         if len(self.up_ratios) > _capi.AB_MAX_STAGES:
             raise ValueError("amphion_b200: too many up_ratios for the native encoder")
-        c = _capi.GeneratorConfig()
-        c.kind = _capi.GEN_FACODEC_ENCODER
-        c.n_mel = 1
-        c.upsample_initial_channel = self.ngf
-        c.num_upsamples = len(self.up_ratios)
-        for i, u in enumerate(self.up_ratios):
-            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, 2 * u
-        c.resblock, c.num_kernels, c.resblock_kernel_sizes[0], c.num_dilations[0] = 1, 1, 7, 3
-        for p, d in enumerate((1, 3, 9)):
-            c.resblock_dilation_sizes[0][p] = d
-        c.activation, c.snake_logscale = _capi.ACT_SNAKEBETA, 1
+        c = _block_config(_capi.GEN_FACODEC_ENCODER, 1, self.ngf, self.up_ratios)
         c.trunk_out_channels = self.out_channels
         return c
 
@@ -565,34 +558,19 @@ class FACodecEncoder(NativeGenerator):
         _capi.require_cuda(x, "FACodecEncoder.forward")
         if x.dtype != torch.float32:
             x = x.float()
-        with torch.cuda.device(x.device):
-            self._sync_params(x.device)
-            lib, h = _capi.lib, self._handle
-            need = lib.ab_generator_workspace_bytes(h, B, N)
-            if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != x.device:
-                self._workspace = None
-                self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=x.device)
-            wbase = (self._workspace.data_ptr() + 255) // 256 * 256
-            if out is None:
-                y = torch.empty(B, self.out_channels, F, dtype=torch.float32, device=x.device)
-            else:
-                if (tuple(out.shape) != (B, self.out_channels, F) or out.dtype != torch.float32 or out.device != x.device
-                        or not out.is_contiguous()):
-                    raise ValueError(f"out must be a contiguous fp32 [{B}, {self.out_channels}, {F}] tensor on {x.device}")
-                y = out
-            _capi.check(lib.ab_facodec_encode(h, _capi.ptr(x), B, N, _capi.shape_array(x.stride()), _capi.ptr(y),
-                                              C.c_void_p(wbase), need, _capi.stream_ptr()), "ab_facodec_encode")
-            self.last_launches = lib.ab_generator_last_launches(h)
+        with self._launch(x.device) as h:
+            need = _capi.lib.ab_generator_workspace_bytes(h, B, N)
+            ws = self._scratch(need, x.device)
+            y = self._output(out, (B, self.out_channels, F), x.device)
+            _capi.check(_capi.lib.ab_facodec_encode(h, _capi.ptr(x), B, N, _capi.shape_array(x.stride()), _capi.ptr(y),
+                                                    ws, need, _capi.stream_ptr()), "ab_facodec_encode")
         return y
 
     def inference(self, x):
         return self.forward(x)
 
-    def remove_weight_norm(self):
-        _remove_all_weight_norm(self)
 
-
-class FACodecRedecoder(NativeGenerator):
+class FACodecRedecoder(_FACodecGenerator):
     """Drop-in for FACodecRedecoder (facodec.py:602-769): the same constructor and parameter tree
     (``{prosody,content,residual}_embs``, ``model.*``, ``timbre_linear``, ``timbre_cond_prosody_enc``), so the released
     ``ns3_facodec_redecoder.bin`` loads strictly.  Served natively (``AB_GEN_FACODEC_REDECODER``), in eval:
@@ -634,31 +612,10 @@ class FACodecRedecoder(NativeGenerator):
         self.prosody_embs = embs(self.vq_num_q_p, codebook_size_prosody)
         self.content_embs = embs(self.vq_num_q_c, codebook_size_content)
         self.residual_embs = embs(self.vq_num_q_r, codebook_size_residual)
-
-        channels = upsample_initial_channel
-        layers = [weight_norm(nn.Conv1d(in_channels, channels, kernel_size=7, padding=3))]
-        for i, stride in enumerate(up_ratios):
-            layers.append(DecoderBlock(channels // 2 ** i, channels // 2 ** (i + 1), stride))
-        output_dim = channels // 2 ** len(up_ratios)
-        layers += [_act(output_dim), weight_norm(nn.Conv1d(output_dim, 1, kernel_size=7, padding=3)), nn.Tanh()]
-        self.model = nn.Sequential(*layers)
-
-        self.timbre_linear = nn.Linear(in_channels, in_channels * 2)
-        self.timbre_linear.bias.data[:in_channels] = 1
-        self.timbre_linear.bias.data[in_channels:] = 0
-        self.timbre_norm = nn.LayerNorm(in_channels, elementwise_affine=False)
+        _build_generator(self, in_channels, upsample_initial_channel, up_ratios)
         self.timbre_cond_prosody_enc = TransformerEncoder(use_cln=True)
 
     # ---- NativeGenerator hooks -------------------------------------------------------
-    def _input_channels(self):
-        return self.in_channels
-
-    def _hop(self):
-        return self.hop_length
-
-    def _upsample_rates(self):
-        return list(self.up_ratios)
-
     def _c_config(self):
         return _generator_config(self, _capi.GEN_FACODEC_REDECODER)
 
@@ -686,38 +643,24 @@ class FACodecRedecoder(NativeGenerator):
         if spk.device != vq.device:
             raise ValueError("FACodecRedecoder.vq2emb: the codes and the speaker embedding are on different devices")
         _capi.require_cuda(vq, "FACodecRedecoder.vq2emb")
-        if self.timbre_cond_prosody_enc.training or any(m.training for m in self.timbre_cond_prosody_enc.modules()):
-            raise NotImplementedError(f"amphion_b200: the prosody transformer in training mode (dropout) is not "
-                                      f"served; {_SERVED}")
+        _refuse_training(self.timbre_cond_prosody_enc, "the prosody transformer", "dropout", _SERVED)
         n_pe = self.timbre_cond_prosody_enc.position_emb.pe.shape[0]
         if B > n_pe:
             raise ValueError(f"amphion_b200: batch {B} > {n_pe}, the rows of the prosody transformer's positional "
                              f"encoding (the reference fails there too)")
         vq = vq.long()
-        # codes the kernel would not read (it writes NaN there): refuse them before the launch, as F.embedding does
-        groups = [(0, p, self.codebook_size_prosody), (p, p + c, self.codebook_size_content)]
-        if use_residual and r > 0:
-            groups.append((p + c, p + c + r, self.codebook_size_residual))
-        for q0, q1, bits in groups:
-            part = vq[q0:q1]
-            lo, hi = int(part.min()), int(part.max())
-            if lo < 0 or hi >= 2 ** int(bits):
-                raise ValueError(f"FACodecRedecoder.vq2emb: code rows {q0}..{q1 - 1} hold {lo}..{hi}, outside the "
-                                 f"embedding table [0, {2 ** int(bits)})")
+        _check_codes(self, vq, use_residual, "FACodecRedecoder", "embedding table")
         spk = spk.float()
         if spk.stride(1) != 1:
             spk = spk.contiguous()
-        with torch.cuda.device(vq.device):
-            self._sync_params(vq.device)
-            lib, h = _capi.lib, self._handle
-            ws = lib.ab_facodec_redecoder_vq2emb_workspace_bytes(h, B, T)
-            wbase = _workspace_for(self, vq.device, ws)
+        with self._launch(vq.device) as h:
+            ws_bytes = _capi.lib.ab_facodec_redecoder_vq2emb_workspace_bytes(h, B, T)
+            ws = self._scratch(ws_bytes, vq.device)
             out = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=vq.device)
-            _capi.check(lib.ab_facodec_redecoder_vq2emb(h, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B, T,
-                                                        _capi.ptr(spk), spk.stride(0), int(bool(use_residual)),
-                                                        _capi.ptr(out), C.c_void_p(wbase), ws, _capi.stream_ptr()),
+            _capi.check(_capi.lib.ab_facodec_redecoder_vq2emb(h, _capi.ptr(vq), _capi.shape_array(vq.stride()), n_q, B,
+                                                              T, _capi.ptr(spk), spk.stride(0), int(bool(use_residual)),
+                                                              _capi.ptr(out), ws, ws_bytes, _capi.stream_ptr()),
                         "ab_facodec_redecoder_vq2emb")
-            self.last_launches = lib.ab_generator_last_launches(h)
         return out
 
     def inference(self, x, speaker_embedding, out=None, tail_events=None):
@@ -731,9 +674,6 @@ class FACodecRedecoder(NativeGenerator):
             "amphion_b200: FACodecRedecoder.forward is not served: the reference builds the embedding sum as [B, T, d] "
             "and transposes it before timbre_norm, so it raises unless T == 256, and at T == 256 it normalises over "
             f"time and feeds [B, T, d] to conv_pre as channels.  Call vq2emb() and then inference(); {_SERVED}")
-
-    def remove_weight_norm(self):
-        _remove_all_weight_norm(self)
 
 
 # ---- FACodec V2 (facodec.py:772-1199) ---------------------------------------------------------------------------------
@@ -853,48 +793,4 @@ class FACodecDecoderV2(FACodecDecoder):
                                       f"'{x.device}'); there is no CPU fallback; {_SERVED_V2}")
         if pf.device != x.device:
             raise ValueError("FACodecDecoderV2.forward: x and the prosody feature are on different devices")
-        n_pe = min(self.timbre_encoder.position_emb.pe.shape[0], self.melspec_encoder.position_emb.pe.shape[0])
-        if B > n_pe:
-            raise ValueError(f"amphion_b200: batch {B} > {n_pe}, the rows of the transformers' positional encoding "
-                             f"(the reference fails there too)")
-        k = max(self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r) if n_quantizers is None else int(n_quantizers)
-        if k < 1:
-            raise ValueError(f"amphion_b200: n_quantizers {n_quantizers} < 1 runs no layer (the reference raises too)")
-        if eval_vq:
-            self.quantizer.eval()   # facodec.py:1076-1077
-        if self.quantizer.training or any(m.training for m in self.quantizer.modules()):
-            raise NotImplementedError(f"amphion_b200: a quantizer in training mode (quantizer dropout, commitment "
-                                      f"losses) is not served; {_SERVED_V2}")
-        for name in ("timbre_encoder", "melspec_encoder"):
-            mod = getattr(self, name)
-            if mod.training or any(m.training for m in mod.modules()):
-                raise NotImplementedError(f"amphion_b200: the {name} in training mode (dropout) is not served; "
-                                          f"{_SERVED_V2}")
-        if not self._quantize_handle:
-            # the decode-only handle lists no quantizer / transformer tensors: re-create it with them
-            self._quantize_handle = True
-            if self._handle is not None:
-                _capi.lib.ab_generator_destroy(self._handle)
-                self._handle = None
-            self._arena_key = None
-        x = x.float()
-        pf = pf.float()
-        nq = [min(k, n) for n in (self.vq_num_q_p, self.vq_num_q_c, self.vq_num_q_r)]
-        n_used, G = sum(nq), 3 if self.vq_num_q_r > 0 else 2
-        dev = x.device
-        with torch.cuda.device(dev):
-            self._sync_params(dev)
-            lib, h = _capi.lib, self._handle
-            need = lib.ab_facodec_quantize_workspace_bytes(h, B, T)
-            wbase = self._workspace_for(dev, need)
-            outs = torch.empty(B, self.in_channels, T, dtype=torch.float32, device=dev)
-            qs = torch.empty(n_used, B, T, dtype=torch.int64, device=dev)
-            buf = torch.empty(G, B, self.in_channels, T, dtype=torch.float32, device=dev)
-            spk = torch.empty(B, self.in_channels, dtype=torch.float32, device=dev)
-            _capi.check(lib.ab_facodec_quantize_prosody(h, _capi.ptr(x), _capi.shape_array(x.stride()), _capi.ptr(pf),
-                                                        _capi.shape_array(pf.stride()), B, T, k, _capi.ptr(outs),
-                                                        _capi.ptr(qs), _capi.ptr(buf), _capi.ptr(spk), C.c_void_p(wbase),
-                                                        need, _capi.stream_ptr()), "ab_facodec_quantize_prosody")
-            self.last_launches = lib.ab_generator_last_launches(h)
-        commit_loss = torch.zeros(n_used, dtype=torch.float32, device=dev)
-        return outs, qs, commit_loss, list(buf.unbind(0)), spk
+        return self._quantize(x, pf, n_quantizers, eval_vq)

@@ -62,7 +62,7 @@ def _forward_chunked_to_host(model, mels):
     flat = output.detach().squeeze(1)
     with torch.cuda.stream(side):
         for i in range(n):
-            b0, b1 = B * i // n, B * (i + 1) // n                # the chunk bounds of ab_generator_set_tail_events
+            b0, b1 = B * i // n, B * (i + 1) // n                # the chunk bounds of NativeGenerator._arm_tail_events
             side.wait_event(events[i])
             host[b0:b1].copy_(flat[b0:b1], non_blocking=True)
     output.record_stream(side)

@@ -1,4 +1,5 @@
-"""Shared host logic of the native GAN generators (HiFi-GAN / BigVGAN).
+"""Shared host logic of the native vocoders: the C-ABI handle, the parameter arena and the one launch path every native
+entry point takes (HiFi-GAN, BigVGAN, NSF-HiFiGAN, MelGAN, Vocos, DiffWave, APNet's trunks and FACodec).
 
 The module keeps the reference's parameter names and weight-norm decomposition
 (``weight_g`` / ``weight_v``) so reference checkpoints load unchanged
@@ -6,6 +7,7 @@ The module keeps the reference's parameter names and weight-norm decomposition
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -71,7 +73,7 @@ class ConvBlock(nn.Module):
 class NativeGenerator(nn.Module):
     """Base class: owns the C-ABI handle, the packed-parameter arena and the workspace."""
 
-    kind = None       # "hifigan" | "bigvgan" | "nsfhifigan"
+    kind = None       # "hifigan" | "bigvgan" | "nsfhifigan" | "melgan" | "vocos" | "diffwave" | "trunk" | "facodec*"
     hp_key = None     # cfg.model.<hp_key>
 
     def __init__(self):
@@ -197,38 +199,61 @@ class NativeGenerator(nn.Module):
         B, _, T = x.shape
         if B == 0 or T == 0:
             raise ValueError("amphion_b200: empty mel batch")
-        with torch.cuda.device(x.device):
-            self._sync_params(x.device)
-            lib, h = _capi.lib, self._handle
-            hop = self._hop()
-            need = lib.ab_generator_workspace_bytes(h, B, T)
-            if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != x.device:
-                self._workspace = None
-                self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=x.device)
-            wbase = (self._workspace.data_ptr() + 255) // 256 * 256
-            n_out = T * hop if out_samples is None else int(out_samples)
-            if out is None:
-                wav = torch.empty(B, 1, n_out, dtype=torch.float32, device=x.device)
-            else:
-                if (tuple(out.shape) != (B, 1, n_out) or out.dtype != torch.float32 or out.device != x.device
-                        or not out.is_contiguous()):
-                    raise ValueError(f"out must be a contiguous fp32 [{B}, 1, {n_out}] tensor on {x.device}")
-                wav = out
-            if tail_events:
-                for ev in tail_events:
-                    ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded below
-                arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
-                _capi.check(lib.ab_generator_set_tail_events(h, arr, len(tail_events)), "ab_generator_set_tail_events")
+        with self._launch(x.device) as h:
+            need = _capi.lib.ab_generator_workspace_bytes(h, B, T)
+            ws = self._scratch(need, x.device)
+            n_out = T * self._hop() if out_samples is None else int(out_samples)
+            wav = self._output(out, (B, 1, n_out), x.device)
+            self._arm_tail_events(tail_events)
             strides = _capi.shape_array(x.stride())
             if g is None:
-                _capi.check(lib.ab_generator_forward(h, _capi.ptr(x), B, T, strides, _capi.ptr(wav), C.c_void_p(wbase),
-                                                     need, _capi.stream_ptr()), "ab_generator_forward")
+                _capi.check(_capi.lib.ab_generator_forward(h, _capi.ptr(x), B, T, strides, _capi.ptr(wav), ws, need,
+                                                           _capi.stream_ptr()), "ab_generator_forward")
             else:
-                _capi.check(lib.ab_generator_forward_cond(h, _capi.ptr(x), B, T, strides, _capi.ptr(g), g.stride(0),
-                                                          _capi.ptr(wav), C.c_void_p(wbase), need, _capi.stream_ptr()),
+                _capi.check(_capi.lib.ab_generator_forward_cond(h, _capi.ptr(x), B, T, strides, _capi.ptr(g),
+                                                                g.stride(0), _capi.ptr(wav), ws, need,
+                                                                _capi.stream_ptr()),
                             "ab_generator_forward_cond")
-            self.last_launches = lib.ab_generator_last_launches(h)
         return wav
+
+    # ---- the launch path of every native entry point ------------------------------------------------------------
+    @contextlib.contextmanager
+    def _launch(self, device):
+        """Runs the body, which makes one C call on the yielded handle, on ``device`` with the parameters synced;
+        ``last_launches`` becomes that call's count once the body returned without raising."""
+        with torch.cuda.device(device):
+            self._sync_params(device)
+            yield self._handle
+            self._count_launches()
+
+    def _count_launches(self):
+        self.last_launches = _capi.lib.ab_generator_last_launches(self._handle)
+
+    def _scratch(self, need, device):
+        """Pointer to ``need`` bytes of 256-byte-aligned device workspace; the buffer only grows, and moves with the
+        device."""
+        if self._workspace is None or self._workspace.numel() < need + 256 or self._workspace.device != device:
+            self._workspace = None
+            self._workspace = torch.empty(need + 256, dtype=torch.uint8, device=device)
+        return C.c_void_p((self._workspace.data_ptr() + 255) // 256 * 256)
+
+    @staticmethod
+    def _output(out, shape, device):
+        """A new fp32 tensor of ``shape``, or the caller's ``out`` once it is checked to be one."""
+        if out is None:
+            return torch.empty(shape, dtype=torch.float32, device=device)
+        if tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != device or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous fp32 [{', '.join(map(str, shape))}] tensor on {device}")
+        return out
+
+    def _arm_tail_events(self, tail_events):
+        """The last layer runs in ``len(tail_events)`` batch chunks and records event i when chunk i is complete."""
+        if tail_events:
+            for ev in tail_events:
+                ev.record()   # creates the underlying cudaEvent_t (torch creates it lazily); re-recorded by the call
+            arr = (C.c_void_p * len(tail_events))(*[C.c_void_p(ev.cuda_event) for ev in tail_events])
+            _capi.check(_capi.lib.ab_generator_set_tail_events(self._handle, arr, len(tail_events)),
+                        "ab_generator_set_tail_events")
 
     def set_option(self, key: str, value: int):
         """Execution-plan knob of the C ABI (`ab_generator_set_option`), e.g. ("nsf_source_frames", n)."""
