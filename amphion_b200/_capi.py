@@ -13,8 +13,9 @@ AB_MAX_DILATIONS = 8
 GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN, GEN_VOCOS, GEN_DIFFWAVE, GEN_FACODEC = 0, 1, 2, 3, 4, 5, 6, 7
 GEN_FACODEC_ENCODER = 8
 GEN_FACODEC_REDECODER = 9
+GEN_RVQ = 10
 AB_FACODEC_MAX_Q = 32
-ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA = 0, 1, 2
+ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA, ACT_SNAKE1D = 0, 1, 2, 3
 PRECISIONS = {"fp32": 0, "tc_f16": 1, "tc_bf16": 2}
 
 
@@ -49,6 +50,7 @@ class GeneratorConfig(C.Structure):
         ("vq_codebook_dim", C.c_int32),
         ("facodec_quantize", C.c_int32),
         ("facodec_prosody_encoder", C.c_int32),
+        ("vq_codebook_size", C.c_int32),
     ]
 
 
@@ -111,11 +113,14 @@ SIGNATURES = {
     "ab_facodec_redecoder_vq2emb_workspace_bytes": (C.c_size_t, [_P, C.c_int64, C.c_int64]),
     "ab_facodec_redecoder_vq2emb": (C.c_int, [_P, _P, _I64P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int32,
                                               _P, _P, C.c_size_t, _P]),
+    "ab_rvq_quantize": (C.c_int, [_P, _P, _I64P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, _P]),
+    "ab_rvq_vq2emb": (C.c_int, [_P, _P, _I64P, C.c_int32, C.c_int64, C.c_int64, _P, _P]),
     "ab_facodec_encoder_frames": (C.c_int64, [_P, C.c_int64]),
     "ab_facodec_encode": (C.c_int, [_P, _P, C.c_int64, C.c_int64, _I64P, _P, _P, C.c_size_t, _P]),
     "ab_activation1d_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P, C.c_int32, _P, _P, _P]),
     "ab_activation1d_packed_forward": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, _P, _P, C.c_int32,
                                                  C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, _P]),
+    "ab_snake1d_forward": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64, _P, C.c_int32, _P]),
     "ab_conv1d_forward": (C.c_int, [_P, _P, _P, _P, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                     C.c_int32, C.c_float, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),
     "ab_conv1d_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32]),

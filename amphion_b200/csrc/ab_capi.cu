@@ -284,14 +284,20 @@ int validate_diffwave_config(const ab_generator_config& c) {
 }
 
 // FACodec's DecoderBlocks / EncoderBlocks: three ResidualUnits k = 7, dilations (1, 3, 9), SnakeBeta with logscale
-// (facodec.py:121-154).  blocks and model name them in the messages.
-int check_facodec_units(const ab_generator_config& c, const char* blocks, const char* model) {
+// (facodec.py:121-154), or with snake1d the codec encoder's plain Snake1d (amphion_codec/codec.py:42-97, no logscale).
+// blocks and model name them in the messages.
+int check_facodec_units(const ab_generator_config& c, const char* blocks, const char* model, bool snake1d = false) {
   if (c.resblock != 1 || c.num_kernels != 1 || c.resblock_kernel_sizes[0] != 7 || c.num_dilations[0] != 3 ||
       c.resblock_dilation_sizes[0][0] != 1 || c.resblock_dilation_sizes[0][1] != 3 || c.resblock_dilation_sizes[0][2] != 9)
     return fail(AB_ERR_ARG, "config: %s hold ResidualUnits k = 7, dilations (1, 3, 9): resblock 1, num_kernels 1, kernel 7, "
                             "3 dilations", blocks);
+  if (snake1d && c.activation == AB_ACT_SNAKE1D) {
+    if (c.snake_logscale != 0) return fail(AB_ERR_ARG, "config: Snake1d has no logscale (snake_logscale must be 0)");
+    return AB_OK;
+  }
   if (c.activation != AB_ACT_SNAKEBETA || c.snake_logscale != 1)
-    return fail(AB_ERR_ARG, "config: %s uses SnakeBeta with alpha_logscale = True", model);
+    return fail(AB_ERR_ARG, snake1d ? "config: %s uses SnakeBeta with alpha_logscale = True, or Snake1d"
+                                    : "config: %s uses SnakeBeta with alpha_logscale = True", model);
   return AB_OK;
 }
 
@@ -381,16 +387,40 @@ int validate_facodec_encoder_config(const ab_generator_config& c) {
         c.upsample_kernel_sizes[i] != 2 * c.upsample_rates[i])
       return fail(AB_ERR_UNSUPPORTED, "config: FACodec encoder stage %d: stride %d (1..%d) with kernel %d (must be 2 x stride)",
                   i, c.upsample_rates[i], AB_TC_MAX_STRIDE, c.upsample_kernel_sizes[i]);
-  return check_facodec_units(c, "FACodec EncoderBlocks", "the FACodec encoder");
+  return check_facodec_units(c, "FACodec EncoderBlocks", "the FACodec encoder", true);
+}
+
+// AB_GEN_RVQ: a ResidualVQ of FactorizedVectorQuantize layers (amphion_codec/quantize/residual_vq.py,
+// factorized_vector_quantize.py) and nothing else
+int validate_rvq_config(const ab_generator_config& c) {
+  ab_generator_config z;
+  memset(&z, 0, sizeof(z));
+  z.kind = c.kind; z.n_mel = c.n_mel; z.vq_num_q[0] = c.vq_num_q[0]; z.vq_codebook_dim = c.vq_codebook_dim;
+  z.vq_codebook_size = c.vq_codebook_size;
+  if (memcmp(&z, &c, sizeof(z)) != 0)
+    return fail(AB_ERR_ARG, "config: a residual VQ uses only n_mel (input_dim), vq_num_q[0] (num_quantizers), "
+                            "vq_codebook_size and vq_codebook_dim (every other field must be 0)");
+  if (c.n_mel <= 0 || c.n_mel > 4096 || c.vq_num_q[0] <= 0 || c.vq_num_q[0] > AB_FACODEC_MAX_Q || c.vq_codebook_size <= 0 ||
+      c.vq_codebook_size > (1 << 24))
+    return fail(AB_ERR_ARG, "config: residual VQ input_dim %d (1..4096), num_quantizers %d (1..%d) or codebook_size %d "
+                "(1..2^24) out of range", c.n_mel, c.vq_num_q[0], AB_FACODEC_MAX_Q, c.vq_codebook_size);
+  if (c.vq_codebook_dim <= 0 || c.vq_codebook_dim > FAC_MAX_CODEBOOK_DIM || c.vq_codebook_dim == c.n_mel)
+    return fail(AB_ERR_UNSUPPORTED, "config: residual VQ codebook_dim %d (1..%d, != input_dim: the projections must be "
+                "convolutions)", c.vq_codebook_dim, FAC_MAX_CODEBOOK_DIM);
+  return AB_OK;
 }
 
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
       c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC &&
-      c.kind != AB_GEN_FACODEC_ENCODER && c.kind != AB_GEN_FACODEC_REDECODER)
+      c.kind != AB_GEN_FACODEC_ENCODER && c.kind != AB_GEN_FACODEC_REDECODER && c.kind != AB_GEN_RVQ)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
+  if (c.kind == AB_GEN_RVQ) return validate_rvq_config(c);
+  if (c.vq_codebook_size) return fail(AB_ERR_ARG, "config: vq_codebook_size belongs to AB_GEN_RVQ");
   if (c.kind == AB_GEN_FACODEC) return validate_facodec_config(c);
   if (c.kind == AB_GEN_FACODEC_REDECODER) return validate_facodec_redecoder_config(c);
+  if (c.activation == AB_ACT_SNAKE1D && c.kind != AB_GEN_FACODEC_ENCODER)
+    return fail(AB_ERR_ARG, "config: Snake1d is served in the FACodec encoder kind only");
   if (c.facodec_quantize || c.facodec_prosody_encoder)
     return fail(AB_ERR_ARG, "config: facodec_quantize / facodec_prosody_encoder belong to AB_GEN_FACODEC");
   for (int i = 0; i < 3; ++i)
@@ -709,11 +739,18 @@ void add_facodec_redecoder_tensors(ab_generator* g) {
 // FACodec encoder tensors (AB_GEN_FACODEC_ENCODER), the reference's names (facodec.py:121-194): "block.0" (conv_pre,
 // 1 -> ngf, k = 7), per stride i "block.{1+i}.block.{0,1,2}.block.{0..3}" (three ResidualUnits at C = ngf 2^i),
 // ".block.3" (Activation1d) and ".block.4" (the strided conv C -> 2C, k = 2s), "block.{1+n}" (final Activation1d),
-// "block.{2+n}" (conv_post, k = 3)
+// "block.{2+n}" (conv_post, k = 3).  With AB_ACT_SNAKE1D (the codec's CodecEncoder, codec.py:60-143) each activation
+// is a Snake1d whose one tensor is "<module>.alpha" [1, C, 1].
 void add_facodec_encoder_tensors(ab_generator* g) {
   const ab_generator_config* cfg = &g->cfg;
   const int n = cfg->num_upsamples;
   auto mod = [](int i) { return "block." + std::to_string(i); };
+  auto act = [&](const std::string& prefix, int ch) {
+    if (cfg->activation != AB_ACT_SNAKE1D) return make_act(g, prefix, ch, true);
+    ActRef a;
+    a.alpha = g->add_slot(prefix + ".alpha", SLOT_VEC, {1, ch, 1});
+    return a;
+  };
   g->conv_pre = make_conv(g, mod(0), 1, cfg->upsample_initial_channel, 7, 1, false);
   g->slots[g->conv_pre.w].no_tc = true;   // one input channel: 31 of the wgmma kernel's 32 K lanes would be zero
   int ch = cfg->upsample_initial_channel;
@@ -731,20 +768,20 @@ void add_facodec_encoder_tensors(ab_generator* g) {
       const int d = cfg->resblock_dilation_sizes[0][p];
       const std::string pre = base + std::to_string(p) + ".block.";
       blk.dil.push_back(d);
-      blk.acts.push_back(make_act(g, pre + "0", ch, true));
+      blk.acts.push_back(act(pre + "0", ch));
       blk.c1.push_back(make_conv(g, pre + "1", ch, ch, 7, d, false));
-      blk.acts.push_back(make_act(g, pre + "2", ch, true));
+      blk.acts.push_back(act(pre + "2", ch));
       blk.c2.push_back(make_conv(g, pre + "3", ch, ch, 1, 1, false));
     }
     st.blocks.push_back(blk);
-    st.act = make_act(g, base + "3", ch, true);
+    st.act = act(base + "3", ch);
     st.up = make_conv(g, base + "4", ch, 2 * ch, 2 * st.down, 1, false);
     g->slots[st.up.w].stride = st.down;
     g->slots[st.up.w].strided = true;
     g->stages.push_back(st);
     ch *= 2;
   }
-  g->act_post = make_act(g, mod(1 + n), ch, true);
+  g->act_post = act(mod(1 + n), ch);
   g->conv_post = make_conv(g, mod(2 + n), ch, cfg->trunk_out_channels, 3, 1, false);
 }
 
@@ -758,6 +795,25 @@ ConvRef make_linear(ab_generator* g, const std::string& name, int cin, int cout)
   g->slots[c.w].shape[2] = 1;
   c.b = g->add_slot(name + ".bias", SLOT_VEC, {cout});
   return c;
+}
+
+// The codec's ResidualVQ (AB_GEN_RVQ), the reference's names (residual_vq.py:55-66, factorized_vector_quantize.py:40-50):
+// per layer i "quantizers.{i}.in_project" (WNConv1d input_dim -> codebook_dim, k = 1), ".out_project" (WNConv1d
+// codebook_dim -> input_dim, k = 1) and ".codebook.weight" [codebook_size, codebook_dim].  Repacked as every k = 1 conv,
+// in_project is [input_dim][codebook_dim] and out_project [codebook_dim][input_dim], the layouts the RVQ kernels read.
+void add_rvq_tensors(ab_generator* g) {
+  const ab_generator_config* cfg = &g->cfg;
+  const int C = cfg->n_mel, D = cfg->vq_codebook_dim;
+  for (int i = 0; i < cfg->vq_num_q[0]; ++i) {
+    const std::string pre = "quantizers." + std::to_string(i) + ".";
+    FacodecLayerRef l;
+    l.rows = cfg->vq_codebook_size;
+    l.in_proj = make_conv(g, pre + "in_project", C, D, 1, 1, false);
+    l.out_proj = make_conv(g, pre + "out_project", D, C, 1, 1, false);
+    l.cb = g->add_slot(pre + "codebook.weight", SLOT_VEC, {l.rows, D});
+    g->slots[l.in_proj.w].no_tc = g->slots[l.out_proj.w].no_tc = true;
+    g->fac.layers.push_back(l);
+  }
 }
 
 // Vocos tensors (AB_GEN_VOCOS), the reference's state-dict names (vocos.py:469-527, :720-783, :314-361, :824-881)
@@ -894,6 +950,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     add_facodec_encoder_tensors(g);
   } else if (cfg->kind == AB_GEN_FACODEC_REDECODER) {
     add_facodec_redecoder_tensors(g);
+  } else if (cfg->kind == AB_GEN_RVQ) {
+    add_rvq_tensors(g);
   } else {
     add_gan_tensors(g);
   }
@@ -911,7 +969,7 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
     g->dw.packed_offset = g->arena_need;
     g->arena_need += align_up(diffwave_packed_floats(*cfg) * sizeof(float), 256);
   }
-  if (cfg->kind == AB_GEN_FACODEC && cfg->facodec_quantize) {   // normalised codebooks, built at finalize
+  if ((cfg->kind == AB_GEN_FACODEC && cfg->facodec_quantize) || cfg->kind == AB_GEN_RVQ) {   // normalised codebooks, built at finalize
     for (auto& l : g->fac.layers) {
       l.cbn_offset = g->arena_need;
       g->arena_need += align_up((size_t)l.rows * FAC_MAX_CODEBOOK_DIM * sizeof(float), 256) +
@@ -1067,7 +1125,7 @@ int ab_generator_finalize(ab_generator* g, int32_t precision, void* stream) {
     for (const ConvRef* c : {&t.qkv, &t.out_proj, &t.ffn_1, &t.ffn_2})
       if (precision != AB_PREC_FP32 && g->slots[c->w].tc_bytes == 0)
         return fail(AB_ERR_UNSUPPORTED, "finalize: '%s' has no tensor-core image", g->slots[c->w].name.c_str());
-  if (g->cfg.kind == AB_GEN_FACODEC && g->cfg.facodec_quantize) {
+  if ((g->cfg.kind == AB_GEN_FACODEC && g->cfg.facodec_quantize) || g->cfg.kind == AB_GEN_RVQ) {
     for (const auto& l : g->fac.layers) {
       float* cbn = reinterpret_cast<float*>(g->arena + l.cbn_offset);
       float* cbn2 = reinterpret_cast<float*>(g->arena + l.cbn_offset +
@@ -1198,8 +1256,12 @@ struct Launch {
     return timed(cls, 2.0 * B * Tn * c.cout * c.cin * c.k * (c2 ? 2 : 1), bytes, [&] { return launch_tc_conv(p, st); });
   }
 
-  // Activation1d: fp32 y and / or the 16-bit operand image yimg
+  // Activation1d, or the codec encoder's Snake1d: fp32 y and / or the 16-bit operand image yimg
   int snake(const ActRef& a, int64_t B, const float* x, float* y, int C, int Tn, uint16_t* yimg = nullptr) {
+    if (g->cfg.activation == AB_ACT_SNAKE1D)
+      return timed(3, 0.0, (double)B * C * Tn * (4.0 + (y ? 4.0 : 0.0)) + (yimg ? 2.0 * B * rup16(C) * Tn : 0.0), [&] {
+        return launch_snake1d(x, y, yimg, g->precision == AB_PREC_TC_BF16, g->fptr(a.alpha), (int)B, C, Tn, st);
+      });
     auto kc = g->act_coef.find(a.fup);
     const SnakeParams p = generator_snake_params(kc != g->act_coef.end() ? &kc->second : nullptr, g->precision, x, y,
                                                  yimg, g->fptr(a.alpha), g->fptr(a.beta), g->fptr(a.fup),
@@ -1335,7 +1397,7 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
   if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
-  if (g->cfg.kind == AB_GEN_DIFFWAVE) return 0;
+  if (g->cfg.kind == AB_GEN_DIFFWAVE || g->cfg.kind == AB_GEN_RVQ) return 0;
   return gan_layout(g, B, T, nullptr, nullptr);
 }
 
@@ -1390,8 +1452,10 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
                                    "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
                                    "diffwave_tail", "facodec_prologue", "facodec_quantize", "timbre_attention"};
   // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder; the
-  // redecoder's prosody transformer reports its attention in class 13
+  // redecoder's prosody transformer reports its attention in class 13; a residual VQ handle reports vq2emb in 11 and
+  // quantization in 12
   const int n = g->cfg.kind == AB_GEN_FACODEC_REDECODER ? 14
+                : g->cfg.kind == AB_GEN_RVQ ? 13
                 : g->cfg.kind == AB_GEN_FACODEC ? (g->cfg.facodec_quantize ? 14 : 12)
                 : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
@@ -1433,6 +1497,7 @@ int check_forward(const ab_generator* g, const float* dev_mel, int64_t B, int64_
   if (dev_g != nullptr && g_batch_stride < g->cfg.gin_channels) return fail(AB_ERR_ARG, "forward: g row stride < gin_channels");
   if (!g->finalized) return fail(AB_ERR_STATE, "forward: finalize() the generator first");
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "forward: a DiffWave handle runs through ab_diffwave_forward");
+  if (g->cfg.kind == AB_GEN_RVQ) return fail(AB_ERR_ARG, "forward: a residual VQ handle runs through ab_rvq_*");
   if (B <= 0 || T <= 0) return fail(AB_ERR_ARG, "forward: batch and frames must be positive (got %lld, %lld)", (long long)B, (long long)T);
   if (B > 65535) return fail(AB_ERR_UNSUPPORTED, "forward: batch %lld > 65535", (long long)B);
   // FACodec's encoder: T counts input samples, and the stages shorten the sequence
@@ -2406,6 +2471,76 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
 // ---------------------------------------------------------------------------
 // FACodec encoder
 // ---------------------------------------------------------------------------
+// ---------------------------------------------------------------------------
+// The codec's ResidualVQ (AB_GEN_RVQ)
+// ---------------------------------------------------------------------------
+static int rvq_check(const ab_generator* g, int64_t B, int64_t T, int32_t n, const char* what) {
+  if (!g) return fail(AB_ERR_ARG, "%s: null handle", what);
+  if (g->cfg.kind != AB_GEN_RVQ) return fail(AB_ERR_ARG, "%s: not a residual VQ handle", what);
+  if (!g->finalized) return fail(AB_ERR_STATE, "%s: finalize() the handle first", what);
+  if (B <= 0 || T <= 0 || B > 65535 || T > (1ll << 30))
+    return fail(AB_ERR_ARG, "%s: batch %lld / frames %lld out of range", what, (long long)B, (long long)T);
+  if (n < 1 || n > g->cfg.vq_num_q[0])
+    return fail(AB_ERR_ARG, "%s: n_quantizers %d outside 1..%d", what, n, g->cfg.vq_num_q[0]);
+  return AB_OK;
+}
+
+int ab_rvq_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t B, int64_t T,
+                    int32_t n_quantizers, float* dev_quantized_out, int64_t* dev_codes_out, float* dev_layers_out,
+                    void* stream) {
+  int rc = rvq_check(g, B, T, n_quantizers, "rvq_quantize");
+  if (rc != AB_OK) return rc;
+  if (!dev_x || !x_strides || !dev_quantized_out || !dev_codes_out || !dev_layers_out)
+    return fail(AB_ERR_ARG, "rvq_quantize: null argument");
+  const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim;
+  FacRvqParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = dev_x; p.xsb = x_strides[0]; p.xsc = x_strides[1]; p.xst = x_strides[2];
+  p.nused[0] = n_quantizers;
+  for (int q = 0; q < n_quantizers; ++q) {
+    const FacodecLayerRef& l = g->fac.layers[q];
+    p.w_in[q] = g->fptr(l.in_proj.w); p.b_in[q] = g->fptr(l.in_proj.b);
+    p.w_out[q] = g->fptr(l.out_proj.w); p.b_out[q] = g->fptr(l.out_proj.b);
+    p.cb[q] = g->fptr(l.cb);
+    p.cbn[q] = reinterpret_cast<const float*>(g->arena + l.cbn_offset);
+    p.cbn2[q] = reinterpret_cast<const float*>(g->arena + l.cbn_offset +
+                                               align_up((size_t)l.rows * FAC_MAX_CODEBOOK_DIM * sizeof(float), 256));
+    p.rows[q] = l.rows;
+  }
+  p.ngroups = 1;
+  p.B = (int)B; p.C = C; p.T = (int)T; p.D = D;
+  p.codes = dev_codes_out; p.quantized = dev_quantized_out;
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  const double el = (double)B * T, n = n_quantizers, rows = (double)g->cfg.vq_codebook_size;
+  rc = L.timed(12, 4.0 * el * n * C * D + 2.0 * el * n * rows * D,
+               4.0 * el * C * (2 + n) + 8.0 * el * n + 4.0 * n * rows * (FAC_MAX_CODEBOOK_DIM + 1) + 8.0 * n * C * D,
+               [&] { return launch_facodec_rvq(p, L.st, nullptr, dev_layers_out); });
+  return L.done(rc);
+}
+
+int ab_rvq_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_quantizers,
+                  int64_t B, int64_t T, float* dev_out, void* stream) {
+  int rc = rvq_check(g, B, T, n_quantizers, "rvq_vq2emb");
+  if (rc != AB_OK) return rc;
+  if (!dev_codes || !codes_strides || !dev_out) return fail(AB_ERR_ARG, "rvq_vq2emb: null argument");
+  FacVqParams p;
+  memset(&p, 0, sizeof(p));
+  p.codes = dev_codes; p.cs0 = codes_strides[0]; p.cs1 = codes_strides[1]; p.cs2 = codes_strides[2];
+  p.nq = n_quantizers;
+  for (int q = 0; q < p.nq; ++q) {
+    const FacodecLayerRef& l = g->fac.layers[q];
+    p.cb[q] = g->fptr(l.cb); p.w[q] = g->fptr(l.out_proj.w); p.bias[q] = g->fptr(l.out_proj.b); p.rows[q] = l.rows;
+  }
+  p.group_end[0] = p.nq;
+  p.ngroups = 1;
+  p.B = (int)B; p.C = g->cfg.n_mel; p.T = (int)T; p.D = g->cfg.vq_codebook_dim; p.out = dev_out;
+  Launch L{g, static_cast<cudaStream_t>(stream)};
+  const double el = (double)B * T;
+  rc = L.timed(11, 2.0 * el * p.nq * p.C * p.D, 8.0 * el * p.nq + 4.0 * el * p.C + 4.0 * p.nq * (double)p.C * (p.D + 1),
+               [&] { return launch_facodec_vq2emb(p, L.st); });
+  return L.done(rc);
+}
+
 int64_t ab_facodec_encoder_frames(const ab_generator* g, int64_t samples) {
   if (!g || g->cfg.kind != AB_GEN_FACODEC_ENCODER || samples <= 0) return 0;
   int64_t t = samples;
@@ -2458,6 +2593,19 @@ int ab_activation1d_packed_forward(const float* dev_x, float* dev_y, uint16_t* d
   const SnakeParams p = generator_snake_params(&kc, precision, dev_x, dev_y, dev_yimg, dev_alpha, dev_beta, nullptr,
                                                nullptr, logscale, (int)B, (int)C, (int)T);
   return launch_activation1d(p, static_cast<cudaStream_t>(stream));
+}
+
+int ab_snake1d_forward(const float* dev_x, float* dev_y, uint16_t* dev_yimg, int64_t B, int64_t C, int64_t T,
+                       const float* dev_alpha, int32_t precision, void* stream) {
+  if (!dev_x || !dev_alpha) return fail(AB_ERR_ARG, "snake1d: null argument");
+  if (!dev_y && !dev_yimg) return fail(AB_ERR_ARG, "snake1d: no output requested");
+  if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
+    return fail(AB_ERR_ARG, "snake1d: unknown precision %d", precision);
+  if (dev_yimg && precision == AB_PREC_FP32) return fail(AB_ERR_ARG, "snake1d: the operand image needs a tensor-core precision");
+  if (B < 1 || C < 1 || T < 1) return fail(AB_ERR_ARG, "snake1d: bad shape");
+  if (B > 65535 || C > 65536 || T > (1ll << 30)) return fail(AB_ERR_UNSUPPORTED, "snake1d: shape too large");
+  return launch_snake1d(dev_x, dev_y, dev_yimg, precision == AB_PREC_TC_BF16, dev_alpha, (int)B, (int)C, (int)T,
+                        static_cast<cudaStream_t>(stream));
 }
 
 size_t ab_conv1d_workspace_bytes(int64_t cin, int64_t cout, int32_t k, int32_t precision) {

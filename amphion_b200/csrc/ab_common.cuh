@@ -271,8 +271,10 @@ struct FacRvqParams {       // quantize (facodec.py:408-445) for one tile of fra
 // normalised codebook rows (F.normalize, eps 1e-12) padded to 16 floats, and their squared norms
 int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows, int D, cudaStream_t s);
 // prosody == nullptr: FACodecDecoder's RVQ (every group reads x); else FACodecDecoderV2's (facodec.py:1027-1094): the
-// prosody group reads prosody [B, C, T] (contiguous), the content group x, the residual group x - (prosody + content)
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody = nullptr);
+// prosody group reads prosody [B, C, T] (contiguous), the content group x, the residual group x - (prosody + content).
+// layers != nullptr: the codec's ResidualVQ, one group (ngroups 1, emb unused): quantized [B, C, T] is its sum and
+// layers [n_used, B, C, T] each layer's term
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody = nullptr, float* layers = nullptr);
 // softmax(q k^T / 8) v per (utterance, head) from qkv [B, 3 * 256, T] (q, k, v rows; time fastest) -> y fp32 [B, 256, T]
 // or the operand image yimg [B][32][T][8]
 int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf16, int B, int T, cudaStream_t s);
@@ -315,6 +317,9 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s);
 int launch_conv1d_strided_fp32(const ConvParams& p, int stride, int pad, cudaStream_t s);
 int launch_conv_transpose1d_fp32(const ConvTParams& p, cudaStream_t s);
 int launch_activation1d(const SnakeParams& p, cudaStream_t s);
+// Snake1d (codec.py:32-48) of contiguous x [B, C, T]: fp32 y and / or the operand image yimg [B][ceil16(C)/8][T][8]
+int launch_snake1d(const float* x, float* y, uint16_t* yimg, int bf16, const float* alpha, int B, int C, int T,
+                   cudaStream_t s);
 // Repack a conv weight into [Cin][k][Cout] fp32, folding weight norm if g != nullptr.
 // transposed == 0: src is [Cout][Cin][k] (Conv1d); 1: src is [Cin][Cout][k] (ConvTranspose1d).
 int launch_repack_weight(const float* v, const float* g, float* dst, int d0, int d1, int k,

@@ -193,10 +193,11 @@ __global__ void __launch_bounds__(256) facodec_cbnorm_kernel(const float* __rest
 //   e = z_e / max(|z_e|, 1e-12);  dist_i = (|e|^2 - 2 e.c_i) + |c_i|^2;  code = the lowest i of the least dist
 //   z_q = z_e + (codebook[code] - z_e)  (the straight-through step, two fp32 roundings)
 //   q = sum_d W_out[c][d] z_q[d] (an FMA chain from 0) + b_out[c];  r -= q;  group sum += q
-// The groups' sums are written as they complete; emb = (prosody + content) + residual.  PROSODY (FACodecDecoderV2,
-// facodec.py:1027-1094): the prosody group's residual starts from the prosody transformer's output instead of x; the
-// content and residual groups and the positional add are V1's.  Two instantiations, so that V1's code holds no prosody
-// source.
+// The groups' sums are written as they complete; emb = (prosody + content) + residual.  Three instantiations, so that
+// V1's code holds neither of the others' sources: RVQ_FACODEC; RVQ_PROSODY (FACodecDecoderV2, facodec.py:1027-1094): the
+// prosody group's residual starts from the prosody transformer's output instead of x, the content and residual groups
+// and the positional add are V1's; RVQ_LAYERS (the codec's ResidualVQ, amphion_codec/quantize/residual_vq.py:69-134):
+// one group, whose sum ((0 + q_0) + q_1) + ... is quantized_out, and each layer's q also written to its plane of `layers`.
 constexpr int RVQ_TT = 16;
 constexpr int RVQ_THREADS = 256;
 constexpr int RVQ_CH = 256;
@@ -207,14 +208,20 @@ size_t rvq_smem_bytes(int C) {
                           RVQ_TT * (2 * FAC_MAX_CODEBOOK_DIM + 1)) + sizeof(int) * RVQ_TT;
 }
 
+enum RvqMode { RVQ_FACODEC = 0, RVQ_PROSODY = 1, RVQ_LAYERS = 2 };
 struct FacRvqProsodyParams : FacRvqParams {
   const float* prosody;     // [B, C, T], the prosody transformer's output
 };
-template <bool PROSODY>
-using RvqArgs = typename std::conditional<PROSODY, FacRvqProsodyParams, FacRvqParams>::type;
+struct FacRvqLayersParams : FacRvqParams {
+  float* layers;            // [n_used, B, C, T]: layer q's out_proj(z_q) in plane q
+};
+template <int MODE>
+using RvqArgs = typename std::conditional<MODE == RVQ_PROSODY, FacRvqProsodyParams,
+                                          typename std::conditional<MODE == RVQ_LAYERS, FacRvqLayersParams,
+                                                                    FacRvqParams>::type>::type;
 
-template <bool PROSODY>
-__global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<PROSODY> p, int tiles) {
+template <int MODE>
+__global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<MODE> p, int tiles) {
   extern __shared__ __align__(16) float qsm[];
   const int C = p.C, D = p.D, tid = threadIdx.x;
   float* xs = qsm;                          // [C][TT] x
@@ -248,7 +255,7 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<PRO
       rs[i] = g < 2 ? xs[i] : __fsub_rn(xs[i], s01[i]);   // facodec.py:436: x - (prosody + content)
       gs[i] = 0.f;
     }
-    if constexpr (PROSODY) {
+    if constexpr (MODE == RVQ_PROSODY) {
       if (g == 0) {   // facodec.py:1038-1042: the prosody group quantizes melspec_encoder's output
         for (int i = tid; i < n; i += RVQ_THREADS) {
           const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
@@ -345,6 +352,10 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<PRO
         a = __fadd_rn(a, __ldg(p.b_out[q] + c));
         rs[i] = __fsub_rn(rs[i], a);
         gs[i] = __fadd_rn(gs[i], a);
+        if constexpr (MODE == RVQ_LAYERS) {
+          const int t = t0 + u;
+          if (t < p.T) p.layers[(((int64_t)q * p.B + b) * C + c) * p.T + t] = a;
+        }
       }
     }
     __syncthreads();
@@ -647,10 +658,13 @@ int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows
   return AB_OK;
 }
 
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody) {
-  if (!p.x || !p.emb || !p.codes || !p.quantized || (!p.pe) != (!p.stream)) return fail(AB_ERR_ARG, "facodec rvq: null argument");
-  if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.D <= 0 || p.D > FAC_MAX_CODEBOOK_DIM || p.nused[0] <= 0 || p.nused[1] <= 0 ||
-      p.ngroups < 2 || p.ngroups > 3)
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody, float* layers) {
+  // layers: the codec's single group, which writes quantized_out through `quantized` and no emb
+  if (!p.x || (!layers && !p.emb) || !p.codes || !p.quantized || (!p.pe) != (!p.stream) || (prosody && layers))
+    return fail(AB_ERR_ARG, "facodec rvq: null argument");
+  const bool groups_ok = layers ? p.ngroups == 1 && p.nused[1] == 0 && p.nused[2] == 0
+                                : p.nused[1] > 0 && p.ngroups >= 2 && p.ngroups <= 3;
+  if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.D <= 0 || p.D > FAC_MAX_CODEBOOK_DIM || p.nused[0] <= 0 || !groups_ok)
     return fail(AB_ERR_ARG, "facodec rvq: bad shape");
   const size_t smem = rvq_smem_bytes(p.C);
   if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: %d channels do not fit shared memory", p.C);
@@ -659,18 +673,29 @@ int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* proso
   if (prosody) {
     static DeviceOnce configured;
     if (smem > 48 * 1024 && configured.need())
-      AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<RVQ_PROSODY>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     FacRvqProsodyParams q;
     static_cast<FacRvqParams&>(q) = p;
     q.prosody = prosody;
-    facodec_rvq_kernel<true><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(q, (int)tiles);
-    AB_LAUNCH_CHECK("facodec_rvq_kernel<true>");
+    facodec_rvq_kernel<RVQ_PROSODY><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(q, (int)tiles);
+    AB_LAUNCH_CHECK("facodec_rvq_kernel<RVQ_PROSODY>");
+    return AB_OK;
+  }
+  if (layers) {
+    static DeviceOnce configured;
+    if (smem > 48 * 1024 && configured.need())
+      AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<RVQ_LAYERS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    FacRvqLayersParams q;
+    static_cast<FacRvqParams&>(q) = p;
+    q.layers = layers;
+    facodec_rvq_kernel<RVQ_LAYERS><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(q, (int)tiles);
+    AB_LAUNCH_CHECK("facodec_rvq_kernel<RVQ_LAYERS>");
     return AB_OK;
   }
   static DeviceOnce configured;
   if (smem > 48 * 1024 && configured.need())
-    AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  facodec_rvq_kernel<false><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(p, (int)tiles);
+    AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<RVQ_FACODEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  facodec_rvq_kernel<RVQ_FACODEC><<<(unsigned)grid, RVQ_THREADS, smem, s>>>(p, (int)tiles);
   AB_LAUNCH_CHECK("facodec_rvq_kernel");
   return AB_OK;
 }

@@ -1192,6 +1192,58 @@ int launch_vocos_norm(const NormParams& p, cudaStream_t s) {
   return AB_OK;
 }
 
+// ===========================================================================
+// Snake1d (models/codec/amphion_codec/codec.py:32-48): y = x + (alpha[c] + 1e-9)^-1 * sin(alpha[c] x)^2 with every step
+// rounded as the reference's TorchScript snake rounds it: u = alpha x, s = sinf(u) (the accurate sinf torch.sin calls),
+// r = 1 / (alpha + 1e-9) (correctly rounded), y = x + r (s s); nothing contracted into an FMA.  The same arithmetic at
+// every precision.  One thread per (utterance, 8-channel group, time step): consecutive threads take consecutive time
+// steps, so the 8 fp32 loads and stores and the 16-byte image store of a warp are each coalesced.  IMG: 0 no image,
+// 1 / 2 the fp16 / bf16 operand image [B][ceil16(C)/8][T][8] (saturating round to nearest, padding channels zero).
+// ===========================================================================
+namespace {
+template <int IMG>
+__global__ void __launch_bounds__(256) snake1d_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                      uint16_t* __restrict__ yimg, const float* __restrict__ alpha,
+                                                      int C, int c8n, int T, int64_t total) {
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (i >= total) return;
+  const int t = (int)(i % T);
+  const int64_t bc = i / T;
+  const int c8 = (int)(bc % c8n), b = (int)(bc / c8n);
+  float v[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int c = c8 * 8 + e;
+    v[e] = 0.f;
+    if (c < C) {
+      const int64_t at = ((int64_t)b * C + c) * T + t;
+      const float xv = __ldg(x + at), a = __ldg(alpha + c);
+      const float s = sinf(__fmul_rn(a, xv));
+      v[e] = __fadd_rn(xv, __fmul_rn(__frcp_rn(__fadd_rn(a, 1e-9f)), __fmul_rn(s, s)));
+      if (y) y[at] = v[e];
+    }
+  }
+  if (IMG)
+    *reinterpret_cast<uint4*>(yimg + (((size_t)b * c8n + c8) * T + t) * 8) =
+        make_uint4(cvt_pair<IMG - 1>(v[0], v[1]), cvt_pair<IMG - 1>(v[2], v[3]), cvt_pair<IMG - 1>(v[4], v[5]),
+                   cvt_pair<IMG - 1>(v[6], v[7]));
+}
+}  // namespace
+
+int launch_snake1d(const float* x, float* y, uint16_t* yimg, int bf16, const float* alpha, int B, int C, int T,
+                   cudaStream_t s) {
+  if (!x || !alpha || (!y && !yimg)) return fail(AB_ERR_ARG, "snake1d: null argument");
+  if (B <= 0 || C <= 0 || T <= 0) return fail(AB_ERR_ARG, "snake1d: bad shape");
+  const int c8n = (C + 15) / 16 * 2;
+  const int64_t total = (int64_t)B * c8n * T, grid = ceil_div(total, 256);
+  if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "snake1d: grid too large");
+  void (*kerns[3])(const float*, float*, uint16_t*, const float*, int, int, int, int64_t) = {
+      snake1d_kernel<0>, snake1d_kernel<1>, snake1d_kernel<2>};
+  kerns[yimg ? (bf16 ? 2 : 1) : 0]<<<(unsigned)grid, 256, 0, s>>>(x, y, yimg, alpha, C, c8n, T, total);
+  AB_LAUNCH_CHECK("snake1d_kernel");
+  return AB_OK;
+}
+
 int launch_scale_inplace(float* p, size_t n, float gain, cudaStream_t s) {
   if (n == 0) return AB_OK;
   const int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 8);

@@ -107,6 +107,17 @@ extern "C" {
  * act, k = 7 conv, act, k = 1 conv), "block.{1+i}.block.3" (the stage's activation), "block.{1+i}.block.4" (the strided
  * conv), "block.{1+n}" (final act), "block.{2+n}" (conv_post).  conv_pre (one input channel) runs on the fp32 CUDA cores
  * at every precision.  Runs through ab_facodec_encode, not ab_generator_forward.
+ * The same kind with activation = AB_ACT_SNAKE1D and snake_logscale = 0 serves the codec encoder of MaskGCT, Metis and
+ * DebaTTS, CodecEncoder.forward (models/codec/amphion_codec/codec.py:60-143, use_tanh = False): d_model is ngf, and every
+ * activation is a plain Snake1d, y = x + (alpha + 1e-9)^-1 sin(alpha x)^2 per channel (no anti-aliasing, no logscale; see
+ * ab_snake1d_forward for its rounding).  Its tensors are then "<module>.alpha" [1, C, 1] in place of each Activation1d's
+ * alpha, beta and filters; the convolutions, their routing and the workspace are the FACodec encoder's.
+ * AB_GEN_RVQ: the codec's ResidualVQ of FactorizedVectorQuantize layers (models/codec/amphion_codec/quantize/residual_vq.py,
+ * factorized_vector_quantize.py, quantizer_type "fvq", use_l2_normlize = True), alone.  Config fields: n_mel = input_dim,
+ * vq_num_q[0] = num_quantizers (1..AB_FACODEC_MAX_Q), vq_codebook_size (any size >= 1), vq_codebook_dim (1..16, !=
+ * input_dim); every other field 0.  Tensors keep the reference's names: "quantizers.{i}.in_project.weight" [codebook_dim,
+ * input_dim, 1] (weight norm over every dim but 0) / ".bias", "quantizers.{i}.out_project.weight" [input_dim, codebook_dim,
+ * 1] / ".bias", "quantizers.{i}.codebook.weight" [codebook_size, codebook_dim].  Runs through ab_rvq_*.
  * AB_GEN_FACODEC_REDECODER: NaturalSpeech 3's FACodecRedecoder (models/codec/ns3_codec/facodec.py:602-769), the README's
  * zero-shot voice conversion: vq2emb (ab_facodec_redecoder_vq2emb) and inference (ab_facodec_inference, the decoder's
  * FiLM and generator).  Config fields: the generator fields as for AB_GEN_FACODEC, n_mel = in_channels = vq_dim = 256
@@ -120,10 +131,10 @@ extern "C" {
  * The reference's forward (:691-732) transposes the [B, T, d] sum before timbre_norm and is not served. */
 enum ab_generator_kind {
   AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
-  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8, AB_GEN_FACODEC_REDECODER = 9
+  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8, AB_GEN_FACODEC_REDECODER = 9, AB_GEN_RVQ = 10
 };
 #define AB_FACODEC_MAX_Q 32   /* most codebook layers over the three ResidualVQs */
-enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2 };
+enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2, AB_ACT_SNAKE1D = 3 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
   AB_PREC_FP32 = 0,   /* CUDA-core FFMA, fp32 operands and accumulation */
@@ -189,6 +200,8 @@ typedef struct ab_generator_config {
    * also lists "melspec_linear.{weight,bias}" ([256, 20], [256]) and the prosody transformer "melspec_encoder.*" (named
    * as "timbre_encoder.*"), and its forward(vq=True) is ab_facodec_quantize_prosody (ab_facodec_quantize refuses it) */
   int32_t facodec_prosody_encoder;
+  /* AB_GEN_RVQ only (0 elsewhere): rows of every codebook, any size >= 1 */
+  int32_t vq_codebook_size;
 } ab_generator_config;
 
 int ab_generator_create(const ab_generator_config* cfg, ab_generator** out);
@@ -382,6 +395,25 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
                                 void* stream);
 
 /* ------------------------------------------------------------------------
+ * The codec's ResidualVQ (AB_GEN_RVQ): ResidualVQ.forward in eval and ResidualVQ.vq2emb
+ * (models/codec/amphion_codec/quantize/residual_vq.py:69-144).  The first n_quantizers layers run (1..num_quantizers).
+ * Per layer, in fp32 on CUDA cores: z_e = in_project(residual) (an FMA chain over the input channels from 0, then the
+ * bias); code = argmin over the L2-normalised codebook of the squared distance to the normalised z_e (ties: the lowest
+ * code); z_q = z_e + (codebook[code] - z_e); q = out_project(z_q) (an FMA chain from 0, then the bias); residual -= q.
+ * quantized_out = ((0 + q_0) + q_1) + ..., the reference's order.  No workspace.
+ * ---------------------------------------------------------------------- */
+/* x [B, input_dim, T] fp32 with any element strides -> quantized_out [B, input_dim, T], codes_out int64 [n, B, T] and
+ * layers_out [n, B, input_dim, T] (each layer's q, the reference's all_quantized), all contiguous.  One launch. */
+int ab_rvq_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t batch, int64_t frames,
+                    int32_t n_quantizers, float* dev_quantized_out, int64_t* dev_codes_out, float* dev_layers_out,
+                    void* stream);
+/* codes int64 [>= n, B, T] with element strides codes_strides -> out [B, input_dim, T] fp32 contiguous, the sum of
+ * out_project(codebook[code]) over the first n layers in layer order, from 0.  A code outside [0, codebook_size) is never
+ * read: its time step of `out` is written as NaN.  One launch. */
+int ab_rvq_vq2emb(ab_generator* g, const int64_t* dev_codes, const int64_t codes_strides[3], int32_t n_quantizers,
+                  int64_t batch, int64_t frames, float* dev_out, void* stream);
+
+/* ------------------------------------------------------------------------
  * FACodec encoder (AB_GEN_FACODEC_ENCODER): FACodecEncoder.forward / .inference (models/codec/ns3_codec/facodec.py:157-194).
  * ---------------------------------------------------------------------- */
 /* frames F of the encoder's output for `samples` input samples; 0 when a stage would be empty (or g is not an encoder) */
@@ -411,6 +443,16 @@ int ab_activation1d_packed_forward(const float* dev_x, float* dev_y, uint16_t* d
                                    int64_t channels, int64_t length, const float* dev_alpha, const float* dev_beta,
                                    int32_t logscale, const float* filter_up12, const float* filter_down12,
                                    int32_t precision, void* stream);
+
+/* Snake1d (models/codec/amphion_codec/codec.py:32-48) as one launch of what the codec encoder runs (no reference
+ * counterpart; exposed for the bit-exact tests).  x [B, C, T] fp32 contiguous, alpha [C] -> y (fp32 [B, C, T]) and / or
+ * yimg (the operand image [B][ceil16(C)/8][T][8] of y, padding channels zero, rounded to nearest with saturation to
+ * `precision` = AB_PREC_TC_F16 | AB_PREC_TC_BF16); either may be NULL, not both.  Per element, in fp32 with no
+ * contraction: s = sinf(alpha x) (CUDA's sinf), y = x + (1 / (alpha + 1e-9)) * (s * s), the reciprocal correctly
+ * rounded; the same at every precision.  AB_ERR_ARG before any launch for a NULL input, no output, yimg at AB_PREC_FP32
+ * or an unknown precision. */
+int ab_snake1d_forward(const float* dev_x, float* dev_y, uint16_t* dev_yimg, int64_t batch, int64_t channels,
+                       int64_t length, const float* dev_alpha, int32_t precision, void* stream);
 
 /* ------------------------------------------------------------------------
  * Building blocks exposed for parity tests (each is one launch of the kernel
