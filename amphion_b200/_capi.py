@@ -14,6 +14,7 @@ GEN_HIFIGAN, GEN_BIGVGAN, GEN_NSFHIFIGAN, GEN_TRUNK, GEN_MELGAN, GEN_VOCOS, GEN_
 GEN_FACODEC_ENCODER = 8
 GEN_FACODEC_REDECODER = 9
 GEN_RVQ = 10
+GEN_VOCOS_LINEAR = 11
 AB_FACODEC_MAX_Q = 32
 ACT_LRELU, ACT_SNAKE, ACT_SNAKEBETA, ACT_SNAKE1D = 0, 1, 2, 3
 PRECISIONS = {"fp32": 0, "tc_f16": 1, "tc_bf16": 2}

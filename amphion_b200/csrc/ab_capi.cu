@@ -80,7 +80,8 @@ struct BlockRef {  // one ResBlock / AMPBlock
   ConvRef sc;                   // MelGAN ResnetBlock: the 1x1 shortcut (c1, c2 then hold one conv each)
 };
 
-// Vocos (AB_GEN_VOCOS): slot indices of the backbone and head; the Linear layers are k = 1 convs
+// Vocos (AB_GEN_VOCOS) and VocosBackbone + nn.Linear (AB_GEN_VOCOS_LINEAR): slot indices of the backbone and head;
+// the Linear layers are k = 1 convs
 struct VocosBlockRef {   // one ConvNeXtBlock (vocos.py:469-527)
   int dw_w = -1, dw_b = -1, ln_w = -1, ln_b = -1, gamma = -1;
   ConvRef pw1, pw2;
@@ -89,7 +90,7 @@ struct VocosBlockRef {   // one ConvNeXtBlock (vocos.py:469-527)
 struct VocosRef {
   int norm_w = -1, norm_b = -1, final_w = -1, final_b = -1, window = -1;
   std::vector<VocosBlockRef> blocks;
-  ConvRef head;   // head.out: [n_fft + 2, dim]
+  ConvRef head;   // head.out: [n_fft + 2, dim]; AB_GEN_VOCOS_LINEAR: the Linear "1" [out, dim]
 };
 
 // DiffWave (AB_GEN_DIFFWAVE): slot indices; every tensor is a SLOT_VEC copied as is, the layer weights are repacked
@@ -244,17 +245,27 @@ ActRef make_act(ab_generator* g, const std::string& prefix, int ch, bool has_bet
   return a;
 }
 
-// AB_GEN_VOCOS: only its own fields; the ISTFT needs what ab_istft_forward serves
+// AB_GEN_VOCOS: only its own fields; the ISTFT needs what ab_istft_forward serves.  AB_GEN_VOCOS_LINEAR: the backbone's
+// fields and trunk_out_channels (the Linear's out_features)
 int validate_vocos_config(const ab_generator_config& c) {
+  const bool linear = c.kind == AB_GEN_VOCOS_LINEAR;
   if (c.num_upsamples || c.resblock || c.num_kernels || c.activation || c.snake_logscale || c.gin_channels ||
-      c.conv_post_no_bias || c.trunk_out_channels || c.trunk_in_kernel || c.trunk_out_kernel)
-    return fail(AB_ERR_ARG, "config: Vocos uses only n_mel, upsample_initial_channel, ffn_channels, num_layers, istft_n_fft "
-                            "and istft_hop (every other field must be 0)");
+      c.conv_post_no_bias || (!linear && c.trunk_out_channels) || c.trunk_in_kernel || c.trunk_out_kernel ||
+      (linear && (c.istft_n_fft || c.istft_hop)))
+    return fail(AB_ERR_ARG, linear ? "config: VocosBackbone + Linear uses only n_mel, upsample_initial_channel, ffn_channels, "
+                                     "num_layers and trunk_out_channels (every other field must be 0)"
+                                   : "config: Vocos uses only n_mel, upsample_initial_channel, ffn_channels, num_layers, "
+                                     "istft_n_fft and istft_hop (every other field must be 0)");
   const int lim = 1 << 16;
   if (c.n_mel <= 0 || c.n_mel > lim || c.upsample_initial_channel <= 0 || c.upsample_initial_channel > lim ||
       c.ffn_channels <= 0 || c.ffn_channels > lim || c.num_layers <= 0 || c.num_layers > 4096)
     return fail(AB_ERR_ARG, "config: Vocos input_channels %d, dim %d, intermediate_dim %d, num_layers %d out of range", c.n_mel,
                 c.upsample_initial_channel, c.ffn_channels, c.num_layers);
+  if (linear) {
+    if (c.trunk_out_channels <= 0 || c.trunk_out_channels > lim)
+      return fail(AB_ERR_ARG, "config: the Linear's out_features %d out of range", c.trunk_out_channels);
+    return AB_OK;
+  }
   if (c.istft_n_fft <= 0 || c.istft_hop <= 0 || c.istft_n_fft > lim)
     return fail(AB_ERR_ARG, "config: Vocos n_fft %d / hop %d out of range", c.istft_n_fft, c.istft_hop);
   if ((c.istft_n_fft & 1) || c.istft_hop > c.istft_n_fft || ((c.istft_n_fft - c.istft_hop) & 1))
@@ -404,6 +415,10 @@ int validate_rvq_config(const ab_generator_config& c) {
       c.vq_codebook_size > (1 << 24))
     return fail(AB_ERR_ARG, "config: residual VQ input_dim %d (1..4096), num_quantizers %d (1..%d) or codebook_size %d "
                 "(1..2^24) out of range", c.n_mel, c.vq_num_q[0], AB_FACODEC_MAX_Q, c.vq_codebook_size);
+  // the quantize kernel keeps the residual and the running sum of a 16-frame tile in shared memory
+  if (c.n_mel > AB_RVQ_MAX_INPUT_DIM)
+    return fail(AB_ERR_UNSUPPORTED, "config: residual VQ input_dim %d does not fit the quantize kernel's shared memory "
+                "(at most %d)", c.n_mel, AB_RVQ_MAX_INPUT_DIM);
   if (c.vq_codebook_dim <= 0 || c.vq_codebook_dim > FAC_MAX_CODEBOOK_DIM || c.vq_codebook_dim == c.n_mel)
     return fail(AB_ERR_UNSUPPORTED, "config: residual VQ codebook_dim %d (1..%d, != input_dim: the projections must be "
                 "convolutions)", c.vq_codebook_dim, FAC_MAX_CODEBOOK_DIM);
@@ -413,7 +428,8 @@ int validate_rvq_config(const ab_generator_config& c) {
 int validate_config(const ab_generator_config& c) {
   if (c.kind != AB_GEN_HIFIGAN && c.kind != AB_GEN_BIGVGAN && c.kind != AB_GEN_NSFHIFIGAN && c.kind != AB_GEN_TRUNK &&
       c.kind != AB_GEN_MELGAN && c.kind != AB_GEN_VOCOS && c.kind != AB_GEN_DIFFWAVE && c.kind != AB_GEN_FACODEC &&
-      c.kind != AB_GEN_FACODEC_ENCODER && c.kind != AB_GEN_FACODEC_REDECODER && c.kind != AB_GEN_RVQ)
+      c.kind != AB_GEN_FACODEC_ENCODER && c.kind != AB_GEN_FACODEC_REDECODER && c.kind != AB_GEN_RVQ &&
+      c.kind != AB_GEN_VOCOS_LINEAR)
     return fail(AB_ERR_ARG, "config: unknown generator kind %d", c.kind);
   if (c.kind == AB_GEN_RVQ) return validate_rvq_config(c);
   if (c.vq_codebook_size) return fail(AB_ERR_ARG, "config: vq_codebook_size belongs to AB_GEN_RVQ");
@@ -429,7 +445,7 @@ int validate_config(const ab_generator_config& c) {
   if (c.kind == AB_GEN_DIFFWAVE) return validate_diffwave_config(c);
   if (c.dilation_cycle || c.embedding_rows) return fail(AB_ERR_ARG, "config: dilation_cycle / embedding_rows belong to AB_GEN_DIFFWAVE");
   if (c.kind == AB_GEN_FACODEC_ENCODER) return validate_facodec_encoder_config(c);
-  if (c.kind == AB_GEN_VOCOS) return validate_vocos_config(c);
+  if (c.kind == AB_GEN_VOCOS || c.kind == AB_GEN_VOCOS_LINEAR) return validate_vocos_config(c);
   if (c.ffn_channels || c.num_layers || c.istft_n_fft || c.istft_hop)
     return fail(AB_ERR_ARG, "config: ffn_channels / num_layers / istft_* belong to AB_GEN_VOCOS");
   const bool trunk = c.kind == AB_GEN_TRUNK;
@@ -816,16 +832,19 @@ void add_rvq_tensors(ab_generator* g) {
   }
 }
 
-// Vocos tensors (AB_GEN_VOCOS), the reference's state-dict names (vocos.py:469-527, :720-783, :314-361, :824-881)
+// Vocos tensors (AB_GEN_VOCOS), the reference's state-dict names (vocos.py:469-527, :720-783, :314-361, :824-881);
+// AB_GEN_VOCOS_LINEAR: nn.Sequential(VocosBackbone, nn.Linear)'s, "0.*" and "1.{weight,bias}" (repcodec_model.py:108-127)
 void add_vocos_tensors(ab_generator* g) {
   const ab_generator_config* cfg = &g->cfg;
   const int D = cfg->upsample_initial_channel, F = cfg->ffn_channels;
+  const bool linear = cfg->kind == AB_GEN_VOCOS_LINEAR;
+  const std::string bb = linear ? "0." : "backbone.";
   VocosRef& v = g->vocos;
-  g->conv_pre = make_conv(g, "backbone.embed", cfg->n_mel, D, 7, 1, false);
-  v.norm_w = g->add_slot("backbone.norm.weight", SLOT_VEC, {D});
-  v.norm_b = g->add_slot("backbone.norm.bias", SLOT_VEC, {D});
+  g->conv_pre = make_conv(g, bb + "embed", cfg->n_mel, D, 7, 1, false);
+  v.norm_w = g->add_slot(bb + "norm.weight", SLOT_VEC, {D});
+  v.norm_b = g->add_slot(bb + "norm.bias", SLOT_VEC, {D});
   for (int i = 0; i < cfg->num_layers; ++i) {
-    const std::string pre = "backbone.convnext." + std::to_string(i);
+    const std::string pre = bb + "convnext." + std::to_string(i);
     VocosBlockRef b;
     b.dw_w = g->add_slot(pre + ".dwconv.weight", SLOT_VEC, {D, 1, 7});
     b.dw_b = g->add_slot(pre + ".dwconv.bias", SLOT_VEC, {D});
@@ -836,8 +855,12 @@ void add_vocos_tensors(ab_generator* g) {
     b.gamma = g->add_slot(pre + ".gamma", SLOT_VEC, {D});
     v.blocks.push_back(b);
   }
-  v.final_w = g->add_slot("backbone.final_layer_norm.weight", SLOT_VEC, {D});
-  v.final_b = g->add_slot("backbone.final_layer_norm.bias", SLOT_VEC, {D});
+  v.final_w = g->add_slot(bb + "final_layer_norm.weight", SLOT_VEC, {D});
+  v.final_b = g->add_slot(bb + "final_layer_norm.bias", SLOT_VEC, {D});
+  if (linear) {
+    v.head = make_linear(g, "1", D, cfg->trunk_out_channels);
+    return;
+  }
   v.head = make_linear(g, "head.out", D, cfg->istft_n_fft + 2);
   g->slots[v.head.w].head_cols = true;
   v.window = g->add_slot("head.istft.window", SLOT_VEC, {cfg->istft_n_fft});
@@ -942,6 +965,8 @@ int ab_generator_create(const ab_generator_config* cfg, ab_generator** out) {
       delete g;
       return rc;
     }
+  } else if (cfg->kind == AB_GEN_VOCOS_LINEAR) {
+    add_vocos_tensors(g);
   } else if (cfg->kind == AB_GEN_DIFFWAVE) {
     add_diffwave_tensors(g);
   } else if (cfg->kind == AB_GEN_FACODEC) {
@@ -1354,6 +1379,7 @@ size_t gan_layout(const ab_generator* g, int64_t B, int64_t T, char* base, GanWs
 // Vocos workspace: the fp32 residual stream X, the embed / final-norm output Y (fp32), the block input H and the
 // intermediate I (fp32 at AB_PREC_FP32, else 16-bit operand images; I also holds the fp32 head output), the spectrum S
 // [B*T][bins] complex and the iSTFT's workspace.  base == nullptr: sizes only.  0 when the iSTFT plan fails.
+// AB_GEN_VOCOS_LINEAR: X, Y, H and I only (the Linear writes the output).
 struct VocosWs {
   float *X, *Y, *H, *I, *S;
   void* ist;
@@ -1362,15 +1388,20 @@ struct VocosWs {
 
 size_t vocos_layout(const ab_generator* g, int64_t B, int64_t T, char* base, VocosWs* w) {
   const int D = g->cfg.upsample_initial_channel, F = g->cfg.ffn_channels, bins = g->cfg.istft_n_fft / 2 + 1;
-  const bool fp32 = g->precision == AB_PREC_FP32;
+  const bool fp32 = g->precision == AB_PREC_FP32, linear = g->cfg.kind == AB_GEN_VOCOS_LINEAR;
   const size_t el = (size_t)B * T;
-  const size_t ist = ab_istft_workspace_bytes(g->istft, B, T);
-  if (ist == 0) return 0;
   Carve c{base};
-  VocosWs v;
+  VocosWs v = {};
   v.X = c.take(el * D * 4);
   v.Y = c.take(el * D * 4);
   v.H = c.take(fp32 ? el * D * 4 : tc_act_image_bytes(B, D, T));
+  if (linear) {
+    v.I = c.take(fp32 ? el * F * 4 : tc_act_image_bytes(B, F, T));
+    if (w) *w = v;
+    return c.off;
+  }
+  const size_t ist = ab_istft_workspace_bytes(g->istft, B, T);
+  if (ist == 0) return 0;
   v.I = c.take(fp32 ? el * std::max(F, 2 * bins) * 4 : tc_act_image_bytes(B, F, T));
   v.S = c.take(el * bins * 8);
   v.ist = c.take<char>(ist);
@@ -1396,7 +1427,7 @@ static int64_t nsf_stage_length(const ab_generator* g, int stage, int64_t Tn, in
 
 size_t ab_generator_workspace_bytes(const ab_generator* g, int64_t B, int64_t T) {
   if (!g || B <= 0 || T <= 0) return 0;
-  if (g->cfg.kind == AB_GEN_VOCOS) return vocos_layout(g, B, T, nullptr, nullptr);
+  if (g->cfg.kind == AB_GEN_VOCOS || g->cfg.kind == AB_GEN_VOCOS_LINEAR) return vocos_layout(g, B, T, nullptr, nullptr);
   if (g->cfg.kind == AB_GEN_DIFFWAVE || g->cfg.kind == AB_GEN_RVQ) return 0;
   return gan_layout(g, B, T, nullptr, nullptr);
 }
@@ -1430,7 +1461,8 @@ int64_t ab_generator_output_samples(const ab_generator* g, int64_t frames, int64
 
 int ab_generator_set_option(ab_generator* g, const char* key, int32_t value) {
   if (!g || !key) return fail(AB_ERR_ARG, "set_option: null argument");
-  if (g->cfg.kind == AB_GEN_VOCOS) return fail(AB_ERR_ARG, "set_option: Vocos has no execution-plan option ('%s')", key);
+  if (g->cfg.kind == AB_GEN_VOCOS || g->cfg.kind == AB_GEN_VOCOS_LINEAR)
+    return fail(AB_ERR_ARG, "set_option: Vocos has no execution-plan option ('%s')", key);
   if (g->cfg.kind == AB_GEN_DIFFWAVE) return fail(AB_ERR_ARG, "set_option: DiffWave has no execution-plan option ('%s')", key);
   if (strcmp(key, "nsf_source_frames") == 0) {   // one-shot: consumed by the next forward
     if (value < 0) return fail(AB_ERR_ARG, "set_option: nsf_source_frames must be >= 0");
@@ -1451,13 +1483,14 @@ int ab_generator_get_profile(ab_generator* g, ab_profile_entry* out, int32_t max
   static const char* kNames[14] = {"tc_conv", "conv1d_fp32", "conv_transpose1d_fp32", "activation1d", "tc_gemmconv",
                                    "tc_pointwise", "vocos_norm", "diffwave_cond", "diffwave_input", "diffwave_layer",
                                    "diffwave_tail", "facodec_prologue", "facodec_quantize", "timbre_attention"};
-  // classes 5-6 are Vocos' kernels, 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder; the
+  // classes 5-6 are Vocos' kernels (and the Linear head's), 7-10 DiffWave's, 11 FACodec's, 12-13 FACodec's quantization and timbre encoder; the
   // redecoder's prosody transformer reports its attention in class 13; a residual VQ handle reports vq2emb in 11 and
   // quantization in 12
   const int n = g->cfg.kind == AB_GEN_FACODEC_REDECODER ? 14
                 : g->cfg.kind == AB_GEN_RVQ ? 13
                 : g->cfg.kind == AB_GEN_FACODEC ? (g->cfg.facodec_quantize ? 14 : 12)
-                : g->cfg.kind == AB_GEN_DIFFWAVE ? 11 : g->cfg.kind == AB_GEN_VOCOS ? 7 : 5;
+                : g->cfg.kind == AB_GEN_DIFFWAVE ? 11
+                : g->cfg.kind == AB_GEN_VOCOS || g->cfg.kind == AB_GEN_VOCOS_LINEAR ? 7 : 5;
   if (max_entries < n) return fail(AB_ERR_ARG, "get_profile: need room for %d entries", n);
   for (int i = 0; i < n; ++i) {
     memset(&out[i], 0, sizeof(out[i]));
@@ -1519,62 +1552,86 @@ int check_forward(const ab_generator* g, const float* dev_mel, int64_t B, int64_
   return AB_OK;
 }
 
-// Vocos: x = norm(embed(x)), the ConvNeXt blocks, final_layer_norm, the head and the iSTFT (vocos.py:764-783, :343-360)
+// Vocos' layers on one workspace (vocos_layout): the backbone and the Linear heads
+struct VocosForward {
+  Launch& L;
+  ab_generator* g;
+  int64_t B;
+  int Tn;
+  bool tc;
+  VocosWs w;
+  uint16_t *Himg, *Iimg;
+
+  VocosForward(Launch& l, int64_t b, int64_t T, const VocosWs& ws)
+      : L(l), g(l.g), B(b), Tn((int)T), tc(l.g->precision != AB_PREC_FP32), w(ws),
+        Himg(reinterpret_cast<uint16_t*>(ws.H)), Iimg(reinterpret_cast<uint16_t*>(ws.I)) {}
+
+  int norm(const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float* y, uint16_t* yimg) {
+    return L.norm(B, g->cfg.upsample_initial_channel, Tn, x, dw_w, dw_b, ln_w, ln_b, 1e-6f, y, yimg);
+  }
+  // fp32 Linear over channels (k = 1 conv) of nb utterances with the GELU, layer-scale residual or time-major epilogue
+  int linear_fp32(const ConvRef& c, int64_t nb, const float* x, float* y, int epi, const float* gamma) {
+    return L.conv(c, nb, x, (int64_t)c.cin * Tn, Tn, 1, y, Tn, 1.0f, epi == CONV_EPI_GAMMA_RESIDUAL ? y : nullptr, nullptr,
+                  1.0f, 0, epi, gamma);
+  }
+  // Linear over channels of nb utterances on the pointwise wgmma GEMM, from the operand image ximg
+  int pointwise(const ConvRef& c, int epi, int64_t nb, const uint16_t* ximg, uint16_t* yimg, float* y,
+                const float* gamma, float* spec) {
+    TcPwParams p;
+    p.epilogue = epi; p.ximg = ximg; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.gamma = gamma;
+    p.yimg = yimg; p.y = y; p.spec = spec;
+    p.B = (int)nb; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.precision = g->precision;
+    const double el = (double)nb * Tn;
+    const double out = epi == AB_PW_GELU ? 2.0 * el * rup16(c.cout) : epi == AB_PW_GAMMA_RESIDUAL ? 8.0 * el * c.cout
+                       : epi == AB_PW_LINEAR ? 4.0 * el * c.cout : 8.0 * el * (c.cout / 2);
+    return L.timed(5, 2.0 * el * c.cin * c.cout, 2.0 * el * rup16(c.cin) + 2.0 * c.cin * c.cout + out,
+                   [&] { return launch_tc_pointwise(p, L.st); });
+  }
+
+  // VocosBackbone.forward (vocos.py:764-783): x = norm(embed(x)), the ConvNeXt blocks and final_layer_norm, whose output
+  // is left in w.Y (fp32) or, at 16 bits, as the operand image in w.H
+  int backbone(const float* dev_mel, const int64_t mel_strides[3]) {
+    const VocosRef& v = g->vocos;
+    const ConvRef& cpre = g->conv_pre;
+    // x = norm(embed(x)) (vocos.py:764-772)
+    int rc = L.on_tc(cpre) ? L.tc_conv(cpre, nullptr, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr,
+                                       w.Y, nullptr, Tn, 1.0f, nullptr, nullptr, 1.0f, 0,
+                                       Launch::conv_bytes(cpre, B, Tn, nullptr, nullptr))
+                           : L.conv(cpre, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], w.Y, Tn, 1.0f, nullptr,
+                                    nullptr, 1.0f, 0);
+    if (rc == AB_OK) rc = norm(w.Y, -1, -1, v.norm_w, v.norm_b, w.X, nullptr);
+    // x = x + gamma * pwconv2(gelu(pwconv1(norm(dwconv(x))))) (vocos.py:509-527)
+    for (size_t i = 0; rc == AB_OK && i < v.blocks.size(); ++i) {
+      const VocosBlockRef& blk = v.blocks[i];
+      if (tc) {
+        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, nullptr, Himg);
+        if (rc == AB_OK) rc = pointwise(blk.pw1, AB_PW_GELU, B, Himg, Iimg, nullptr, nullptr, nullptr);
+        if (rc == AB_OK) rc = pointwise(blk.pw2, AB_PW_GAMMA_RESIDUAL, B, Iimg, nullptr, w.X, g->fptr(blk.gamma), nullptr);
+      } else {
+        rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, w.H, nullptr);
+        if (rc == AB_OK) rc = linear_fp32(blk.pw1, B, w.H, w.I, CONV_EPI_GELU, nullptr);
+        if (rc == AB_OK) rc = linear_fp32(blk.pw2, B, w.I, w.X, CONV_EPI_GAMMA_RESIDUAL, g->fptr(blk.gamma));
+      }
+    }
+    // final_layer_norm (:781)
+    if (rc == AB_OK) rc = norm(w.X, -1, -1, v.final_w, v.final_b, tc ? nullptr : w.Y, tc ? Himg : nullptr);
+    return rc;
+  }
+};
+
+// Vocos: the backbone, the head's Linear with S = min(exp(mag), 1e2) (cos p + i sin p) (vocos.py:343-360) and the iSTFT
 int forward_vocos(Launch& L, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3], float* dev_wav,
                   void* dev_workspace) {
   ab_generator* g = L.g;
   const VocosRef& v = g->vocos;
-  const ConvRef& cpre = g->conv_pre;
-  const int C0 = g->cfg.upsample_initial_channel, Tn = (int)T, bins = g->cfg.istft_n_fft / 2 + 1;
-  const bool tc = g->precision != AB_PREC_FP32;
+  const int bins = g->cfg.istft_n_fft / 2 + 1;
   VocosWs w;
   if (vocos_layout(g, B, T, static_cast<char*>(dev_workspace), &w) == 0) return fail(AB_ERR_CUDA, "forward: iSTFT plan: %s", g_err);
-  uint16_t *Himg = reinterpret_cast<uint16_t*>(w.H), *Iimg = reinterpret_cast<uint16_t*>(w.I);
-  const double el = (double)B * T;
-  auto norm = [&](const float* x, int dw_w, int dw_b, int ln_w, int ln_b, float* y, uint16_t* yimg) {
-    return L.norm(B, C0, Tn, x, dw_w, dw_b, ln_w, ln_b, 1e-6f, y, yimg);
-  };
-  // fp32 Linear over channels (k = 1 conv) with the GELU or layer-scale residual epilogue
-  auto linear_fp32 = [&](const ConvRef& c, const float* x, float* y, int epi, const float* gamma) {
-    return L.conv(c, B, x, (int64_t)c.cin * Tn, Tn, 1, y, Tn, 1.0f, epi == CONV_EPI_GAMMA_RESIDUAL ? y : nullptr, nullptr,
-                  1.0f, 0, epi, gamma);
-  };
-  // Linear over channels on the pointwise wgmma GEMM, from the operand image ximg
-  auto pointwise = [&](const ConvRef& c, int epi, const uint16_t* ximg, uint16_t* yimg, float* y, const float* gamma,
-                       float* spec) {
-    TcPwParams p;
-    p.epilogue = epi; p.ximg = ximg; p.w = g->tcptr(c.w); p.bias = g->fptr(c.b); p.gamma = gamma;
-    p.yimg = yimg; p.y = y; p.spec = spec;
-    p.B = (int)B; p.Cin = c.cin; p.Cout = c.cout; p.T = Tn; p.precision = g->precision;
-    const double out = epi == AB_PW_GELU ? 2.0 * el * rup16(c.cout) : epi == AB_PW_GAMMA_RESIDUAL ? 8.0 * el * c.cout
-                                                                                                   : 8.0 * el * (c.cout / 2);
-    return L.timed(5, 2.0 * el * c.cin * c.cout, 2.0 * el * rup16(c.cin) + 2.0 * c.cin * c.cout + out,
-                   [&] { return launch_tc_pointwise(p, L.st); });
-  };
-  // x = norm(embed(x)) (vocos.py:764-772)
-  int rc = L.on_tc(cpre) ? L.tc_conv(cpre, nullptr, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], nullptr, w.Y,
-                                     nullptr, Tn, 1.0f, nullptr, nullptr, 1.0f, 0, Launch::conv_bytes(cpre, B, Tn, nullptr, nullptr))
-                         : L.conv(cpre, B, dev_mel, mel_strides[0], mel_strides[1], mel_strides[2], w.Y, Tn, 1.0f, nullptr,
-                                  nullptr, 1.0f, 0);
-  if (rc == AB_OK) rc = norm(w.Y, -1, -1, v.norm_w, v.norm_b, w.X, nullptr);
-  // x = x + gamma * pwconv2(gelu(pwconv1(norm(dwconv(x))))) (vocos.py:509-527)
-  for (size_t i = 0; rc == AB_OK && i < v.blocks.size(); ++i) {
-    const VocosBlockRef& blk = v.blocks[i];
-    if (tc) {
-      rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, nullptr, Himg);
-      if (rc == AB_OK) rc = pointwise(blk.pw1, AB_PW_GELU, Himg, Iimg, nullptr, nullptr, nullptr);
-      if (rc == AB_OK) rc = pointwise(blk.pw2, AB_PW_GAMMA_RESIDUAL, Iimg, nullptr, w.X, g->fptr(blk.gamma), nullptr);
-    } else {
-      rc = norm(w.X, blk.dw_w, blk.dw_b, blk.ln_w, blk.ln_b, w.H, nullptr);
-      if (rc == AB_OK) rc = linear_fp32(blk.pw1, w.H, w.I, CONV_EPI_GELU, nullptr);
-      if (rc == AB_OK) rc = linear_fp32(blk.pw2, w.I, w.X, CONV_EPI_GAMMA_RESIDUAL, g->fptr(blk.gamma));
-    }
-  }
-  // final_layer_norm (:781), then the head's Linear and S = min(exp(mag), 1e2) (cos p + i sin p) (:343-360)
-  if (rc == AB_OK) rc = norm(w.X, -1, -1, v.final_w, v.final_b, tc ? nullptr : w.Y, tc ? Himg : nullptr);
-  if (rc == AB_OK && tc) rc = pointwise(v.head, AB_PW_SPECTRUM, Himg, nullptr, nullptr, nullptr, w.S);
-  if (rc == AB_OK && !tc) {
-    rc = linear_fp32(v.head, w.Y, w.I, CONV_EPI_NONE, nullptr);
+  VocosForward f(L, B, T, w);
+  int rc = f.backbone(dev_mel, mel_strides);
+  if (rc == AB_OK && f.tc) rc = f.pointwise(v.head, AB_PW_SPECTRUM, B, f.Himg, nullptr, nullptr, nullptr, w.S);
+  if (rc == AB_OK && !f.tc) {
+    rc = f.linear_fp32(v.head, B, w.Y, w.I, CONV_EPI_NONE, nullptr);
     // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart
     for (int64_t b = 0; rc == AB_OK && b < B; ++b) {
       const float* hb = w.I + b * 2 * bins * T;
@@ -1590,6 +1647,24 @@ int forward_vocos(Launch& L, const float* dev_mel, int64_t B, int64_t T, const i
       return ab_istft_forward(g->istft, w.S + b0 * T * bins * 2, nb, T, g->fptr(v.window), dev_wav + b0 * T * g->hop, w.ist,
                               w.ist_bytes, L.st);
     });
+  });
+}
+
+// nn.Sequential(VocosBackbone, nn.Linear) (repcodec_model.py:108-127): the backbone, then y [B, T, out] = Linear(x), on
+// the GEMM's time-major epilogue or, in fp32, the k = 1 conv's; with tail events the Linear runs in the batch chunks
+int forward_vocos_linear(Launch& L, const float* dev_mel, int64_t B, int64_t T, const int64_t mel_strides[3], float* dev_y,
+                         void* dev_workspace) {
+  ab_generator* g = L.g;
+  const ConvRef& head = g->vocos.head;
+  VocosWs w;
+  vocos_layout(g, B, T, static_cast<char*>(dev_workspace), &w);
+  VocosForward f(L, B, T, w);
+  const int rc = f.backbone(dev_mel, mel_strides);
+  const size_t img = tc_act_image_bytes(1, head.cin, T) / sizeof(uint16_t);   // one utterance's operand image
+  return L.tail(B, rc, [&](int64_t b0, int64_t nb) {
+    float* y = dev_y + b0 * T * head.cout;
+    return f.tc ? f.pointwise(head, AB_PW_LINEAR, nb, f.Himg + b0 * img, nullptr, y, nullptr, nullptr)
+                : f.linear_fp32(head, nb, w.Y + b0 * head.cin * T, y, CONV_EPI_LINEAR, nullptr);
   });
 }
 
@@ -1899,6 +1974,7 @@ int forward_generator(Launch& L, const float* dev_mel, int64_t B, int64_t T, con
   int rc = check_forward(g, dev_mel, B, T, mel_strides, dev_g, g_batch_stride, dev_wav, dev_workspace, workspace_bytes);
   if (rc != AB_OK) return rc;
   if (g->cfg.kind == AB_GEN_VOCOS) return forward_vocos(L, dev_mel, B, T, mel_strides, dev_wav, dev_workspace);
+  if (g->cfg.kind == AB_GEN_VOCOS_LINEAR) return forward_vocos_linear(L, dev_mel, B, T, mel_strides, dev_wav, dev_workspace);
   GanWs w;
   gan_layout(g, B, T, static_cast<char*>(dev_workspace), &w);
   GanForward f(L, B, T, w);
@@ -2490,7 +2566,7 @@ int ab_rvq_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides
                     void* stream) {
   int rc = rvq_check(g, B, T, n_quantizers, "rvq_quantize");
   if (rc != AB_OK) return rc;
-  if (!dev_x || !x_strides || !dev_quantized_out || !dev_codes_out || !dev_layers_out)
+  if (!dev_x || !x_strides || !dev_quantized_out || !dev_codes_out)
     return fail(AB_ERR_ARG, "rvq_quantize: null argument");
   const int C = g->cfg.n_mel, D = g->cfg.vq_codebook_dim;
   FacRvqParams p;
@@ -2513,8 +2589,9 @@ int ab_rvq_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides
   Launch L{g, static_cast<cudaStream_t>(stream)};
   const double el = (double)B * T, n = n_quantizers, rows = (double)g->cfg.vq_codebook_size;
   rc = L.timed(12, 4.0 * el * n * C * D + 2.0 * el * n * rows * D,
-               4.0 * el * C * (2 + n) + 8.0 * el * n + 4.0 * n * rows * (FAC_MAX_CODEBOOK_DIM + 1) + 8.0 * n * C * D,
-               [&] { return launch_facodec_rvq(p, L.st, nullptr, dev_layers_out); });
+               4.0 * el * C * (2 + (dev_layers_out ? n : 0)) + 8.0 * el * n + 4.0 * n * rows * (FAC_MAX_CODEBOOK_DIM + 1) +
+                   8.0 * n * C * D,
+               [&] { return launch_facodec_rvq(p, L.st, nullptr, dev_layers_out, true); });
   return L.done(rc);
 }
 
@@ -2733,7 +2810,7 @@ int ab_vocos_norm_forward(const float* dev_x, const float* dev_dw_w, const float
 }
 
 static_assert(AB_VOCOS_PW_GELU == AB_PW_GELU && AB_VOCOS_PW_GAMMA == AB_PW_GAMMA_RESIDUAL &&
-                  AB_VOCOS_PW_SPECTRUM == AB_PW_SPECTRUM,
+                  AB_VOCOS_PW_SPECTRUM == AB_PW_SPECTRUM && AB_VOCOS_PW_LINEAR == AB_PW_LINEAR,
               "the public pointwise epilogues name launch_tc_pointwise's");
 
 size_t ab_vocos_pointwise_workspace_bytes(int32_t epilogue, int64_t B, int64_t cin, int64_t cout, int64_t T,
@@ -2752,7 +2829,7 @@ int ab_vocos_pointwise_forward(int32_t epilogue, const float* dev_x, const uint1
                                const float* dev_bias, const float* dev_gamma, float* dev_y, uint16_t* dev_yimg,
                                float* dev_spec, int64_t B, int64_t cin, int64_t cout, int64_t T, int32_t precision,
                                void* ws, size_t ws_bytes, void* stream) {
-  if (epilogue < AB_VOCOS_PW_GELU || epilogue > AB_VOCOS_PW_SPECTRUM)
+  if (epilogue < AB_VOCOS_PW_GELU || epilogue > AB_VOCOS_PW_LINEAR)
     return fail(AB_ERR_ARG, "vocos_pointwise: unknown epilogue %d", epilogue);
   if (precision != AB_PREC_FP32 && precision != AB_PREC_TC_F16 && precision != AB_PREC_TC_BF16)
     return fail(AB_ERR_ARG, "vocos_pointwise: unknown precision %d", precision);
@@ -2762,8 +2839,12 @@ int ab_vocos_pointwise_forward(int32_t epilogue, const float* dev_x, const uint1
     return fail(AB_ERR_ARG, "vocos_pointwise: precision %d takes its input as %s", precision, tc ? "ximg" : "x");
   const bool out_ok = epilogue == AB_VOCOS_PW_GELU ? (tc ? dev_yimg != nullptr : dev_y != nullptr)
                       : epilogue == AB_VOCOS_PW_GAMMA ? dev_y && dev_gamma
-                                                      : dev_spec != nullptr;
+                      : epilogue == AB_VOCOS_PW_LINEAR ? dev_y != nullptr
+                                                       : dev_spec != nullptr;
   if (!out_ok) return fail(AB_ERR_ARG, "vocos_pointwise: epilogue %d: missing output or gamma", epilogue);
+  if (epilogue == AB_VOCOS_PW_LINEAR && (dev_gamma || dev_yimg || dev_spec))
+    return fail(AB_ERR_ARG, "vocos_pointwise: epilogue %d (Linear) writes y alone: gamma, yimg and spec must be NULL",
+                epilogue);
   if (epilogue == AB_VOCOS_PW_SPECTRUM && (cout & 1))
     return fail(AB_ERR_ARG, "vocos_pointwise: the spectrum needs an even C_out (magnitude and phase halves), got %lld",
                 (long long)cout);
@@ -2796,7 +2877,8 @@ int ab_vocos_pointwise_forward(int32_t epilogue, const float* dev_x, const uint1
   p.y = epilogue == AB_VOCOS_PW_SPECTRUM ? head : dev_y;
   p.B = (int)B; p.Cin = (int)cin; p.Cout = (int)cout; p.T = (int)T; p.k = 1; p.d = 1;
   p.pre_slope = 1.0f; p.out_div = 1.0f; p.post_tanh = 0;
-  p.epi = epilogue == AB_VOCOS_PW_GELU ? CONV_EPI_GELU : epilogue == AB_VOCOS_PW_GAMMA ? CONV_EPI_GAMMA_RESIDUAL : CONV_EPI_NONE;
+  p.epi = epilogue == AB_VOCOS_PW_GELU ? CONV_EPI_GELU : epilogue == AB_VOCOS_PW_GAMMA ? CONV_EPI_GAMMA_RESIDUAL
+          : epilogue == AB_VOCOS_PW_LINEAR ? CONV_EPI_LINEAR : CONV_EPI_NONE;
   p.gamma = dev_gamma;
   rc = launch_conv1d_fp32(p, st);
   // [B, 2 bins, T]: the magnitude and phase halves of one utterance are bins * T apart (forward_vocos)

@@ -61,10 +61,11 @@ struct ConvParams {
   int reflect = 0;      // 1: ReflectionPad1d((k-1)*d/2) in place of zero padding (MelGAN, melgan.py:39-40,59-66,90-95)
   // Vocos' pointwise layers (vocos.py:509-527), replacing residual / acc_prev / out_div / tanh:
   //   CONV_EPI_GELU: y = gelu(bias + W x) (exact erf);  CONV_EPI_GAMMA_RESIDUAL: y = residual + gamma * (bias + W x)
+  //   CONV_EPI_LINEAR (k = 1 only): y = W x + bias written time-major, y[b, t, co] of a contiguous [B, T, Cout]
   int epi = 0;
   const float* gamma = nullptr;   // [Cout]
 };
-enum { CONV_EPI_NONE = 0, CONV_EPI_GELU = 1, CONV_EPI_GAMMA_RESIDUAL = 2 };
+enum { CONV_EPI_NONE = 0, CONV_EPI_GELU = 1, CONV_EPI_GAMMA_RESIDUAL = 2, CONV_EPI_LINEAR = 3 };
 
 struct ConvTParams {
   const float* x;       // contiguous [B, Cin, Tin]
@@ -272,9 +273,10 @@ struct FacRvqParams {       // quantize (facodec.py:408-445) for one tile of fra
 int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows, int D, cudaStream_t s);
 // prosody == nullptr: FACodecDecoder's RVQ (every group reads x); else FACodecDecoderV2's (facodec.py:1027-1094): the
 // prosody group reads prosody [B, C, T] (contiguous), the content group x, the residual group x - (prosody + content).
-// layers != nullptr: the codec's ResidualVQ, one group (ngroups 1, emb unused): quantized [B, C, T] is its sum and
-// layers [n_used, B, C, T] each layer's term
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody = nullptr, float* layers = nullptr);
+// one_group: the codec's ResidualVQ, one group (ngroups 1, emb unused, C <= AB_RVQ_MAX_INPUT_DIM): quantized [B, C, T]
+// is its sum and layers, when given, [n_used, B, C, T] each layer's term
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody = nullptr, float* layers = nullptr,
+                       bool one_group = false);
 // softmax(q k^T / 8) v per (utterance, head) from qkv [B, 3 * 256, T] (q, k, v rows; time fastest) -> y fp32 [B, 256, T]
 // or the operand image yimg [B][32][T][8]
 int launch_facodec_attention(const float* qkv, float* y, uint16_t* yimg, int bf16, int B, int T, cudaStream_t s);

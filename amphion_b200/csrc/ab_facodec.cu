@@ -197,18 +197,25 @@ __global__ void __launch_bounds__(256) facodec_cbnorm_kernel(const float* __rest
 // V1's code holds neither of the others' sources: RVQ_FACODEC; RVQ_PROSODY (FACodecDecoderV2, facodec.py:1027-1094): the
 // prosody group's residual starts from the prosody transformer's output instead of x, the content and residual groups
 // and the positional add are V1's; RVQ_LAYERS (the codec's ResidualVQ, amphion_codec/quantize/residual_vq.py:69-134):
-// one group, whose sum ((0 + q_0) + q_1) + ... is quantized_out, and each layer's q also written to its plane of `layers`.
+// one group, whose sum ((0 + q_0) + q_1) + ... is quantized_out, and each layer's q also written to its plane of `layers`
+// when that is given.  With one group x is needed only once, so RVQ_LAYERS loads it straight into the residual and keeps
+// two [C][TT] planes (residual, sum) where the FACodec modes keep four: 128 C + 19,584 bytes, which fits C <= 1447
+// (RepCodec's 1024-wide features) in the 200 KB the launch allows.  Its arithmetic is the other modes'.
 constexpr int RVQ_TT = 16;
 constexpr int RVQ_THREADS = 256;
 constexpr int RVQ_CH = 256;
 constexpr int RVQ_LANES = RVQ_THREADS / RVQ_TT;   // threads scanning one frame's codebook
-
-size_t rvq_smem_bytes(int C) {
-  return sizeof(float) * ((size_t)4 * C * RVQ_TT + RVQ_CH * (FAC_MAX_CODEBOOK_DIM + 1) +
-                          RVQ_TT * (2 * FAC_MAX_CODEBOOK_DIM + 1)) + sizeof(int) * RVQ_TT;
-}
+constexpr int RVQ_SMEM_MAX = 200 * 1024;
 
 enum RvqMode { RVQ_FACODEC = 0, RVQ_PROSODY = 1, RVQ_LAYERS = 2 };
+
+constexpr size_t rvq_smem_bytes(int C, bool layers) {
+  return sizeof(float) * ((size_t)(layers ? 2 : 4) * C * RVQ_TT + RVQ_CH * (FAC_MAX_CODEBOOK_DIM + 1) +
+                          RVQ_TT * (2 * FAC_MAX_CODEBOOK_DIM + 1)) + sizeof(int) * RVQ_TT;
+}
+static_assert(rvq_smem_bytes(AB_RVQ_MAX_INPUT_DIM, true) <= RVQ_SMEM_MAX &&
+                  rvq_smem_bytes(AB_RVQ_MAX_INPUT_DIM + 1, true) > RVQ_SMEM_MAX,
+              "AB_RVQ_MAX_INPUT_DIM is the widest input RVQ_LAYERS' shared memory holds");
 struct FacRvqProsodyParams : FacRvqParams {
   const float* prosody;     // [B, C, T], the prosody transformer's output
 };
@@ -224,11 +231,12 @@ template <int MODE>
 __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<MODE> p, int tiles) {
   extern __shared__ __align__(16) float qsm[];
   const int C = p.C, D = p.D, tid = threadIdx.x;
+  constexpr bool ONE = MODE == RVQ_LAYERS;   // one group: x is the first residual, no x or s01 plane
   float* xs = qsm;                          // [C][TT] x
-  float* rs = xs + C * RVQ_TT;              // [C][TT] residual
+  float* rs = ONE ? qsm : xs + C * RVQ_TT;  // [C][TT] residual
   float* gs = rs + C * RVQ_TT;              // [C][TT] current group's sum
   float* s01 = gs + C * RVQ_TT;             // [C][TT] prosody, then prosody + content
-  float* cbs = s01 + C * RVQ_TT;            // [RVQ_CH][16] normalised codebook chunk
+  float* cbs = ONE ? s01 : s01 + C * RVQ_TT;   // [RVQ_CH][16] normalised codebook chunk
   float* cb2s = cbs + RVQ_CH * FAC_MAX_CODEBOOK_DIM;    // [RVQ_CH]
   float* zes = cb2s + RVQ_CH;               // [TT][16] z_e, then z_q
   float* es = zes + RVQ_TT * FAC_MAX_CODEBOOK_DIM;      // [TT][16] normalised z_e
@@ -237,23 +245,37 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<MOD
   const int b = blockIdx.x / tiles, t0 = (blockIdx.x - b * tiles) * RVQ_TT;
   const int n = C * RVQ_TT;
   const float* xb = p.x + (int64_t)b * p.xsb;
-  for (int i = tid; i < n; i += RVQ_THREADS) {
-    const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
-    float v = 0.f;
-    if (t < p.T) {
-      v = __ldg(xb + c * p.xsc + (int64_t)t * p.xst);
-      // transformer.py:43-45 on the batch-first stream: utterance b adds row b of pe at every time step
-      if (p.stream) p.stream[((int64_t)b * C + c) * p.T + t] = __fadd_rn(v, __ldg(p.pe + (int64_t)b * C + c));
+  if constexpr (ONE) {
+    // residual = x, sum = 0.  The walk follows x's smaller stride, so that both [B, C, T] and the [B, T, C] view
+    // RepCodec's encoder hands over are read in runs along memory
+    const bool cfast = p.xsc < p.xst;
+    for (int i = tid; i < n; i += RVQ_THREADS) {
+      const int q = cfast ? i / C : i / RVQ_TT, r = cfast ? i - q * C : i - q * RVQ_TT;
+      const int c = cfast ? r : q, u = cfast ? q : r, t = t0 + u;
+      rs[c * RVQ_TT + u] = t < p.T ? __ldg(xb + c * p.xsc + (int64_t)t * p.xst) : 0.f;
+      gs[c * RVQ_TT + u] = 0.f;
     }
-    xs[i] = v;
+  } else {
+    for (int i = tid; i < n; i += RVQ_THREADS) {
+      const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
+      float v = 0.f;
+      if (t < p.T) {
+        v = __ldg(xb + c * p.xsc + (int64_t)t * p.xst);
+        // transformer.py:43-45 on the batch-first stream: utterance b adds row b of pe at every time step
+        if (p.stream) p.stream[((int64_t)b * C + c) * p.T + t] = __fadd_rn(v, __ldg(p.pe + (int64_t)b * C + c));
+      }
+      xs[i] = v;
+    }
   }
   const int fu = tid / RVQ_LANES, lane = tid % RVQ_LANES;   // search: frame fu, rows lane, lane + RVQ_LANES, ...
-  for (int g = 0; g < 3; ++g) {
+  for (int g = 0; g < (ONE ? 1 : 3); ++g) {
     if (p.nused[g] == 0) continue;
     __syncthreads();
-    for (int i = tid; i < n; i += RVQ_THREADS) {
-      rs[i] = g < 2 ? xs[i] : __fsub_rn(xs[i], s01[i]);   // facodec.py:436: x - (prosody + content)
-      gs[i] = 0.f;
+    if constexpr (!ONE) {
+      for (int i = tid; i < n; i += RVQ_THREADS) {
+        rs[i] = g < 2 ? xs[i] : __fsub_rn(xs[i], s01[i]);   // facodec.py:436: x - (prosody + content)
+        gs[i] = 0.f;
+      }
     }
     if constexpr (MODE == RVQ_PROSODY) {
       if (g == 0) {   // facodec.py:1038-1042: the prosody group quantizes melspec_encoder's output
@@ -352,9 +374,9 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<MOD
         a = __fadd_rn(a, __ldg(p.b_out[q] + c));
         rs[i] = __fsub_rn(rs[i], a);
         gs[i] = __fadd_rn(gs[i], a);
-        if constexpr (MODE == RVQ_LAYERS) {
+        if constexpr (ONE) {
           const int t = t0 + u;
-          if (t < p.T) p.layers[(((int64_t)q * p.B + b) * C + c) * p.T + t] = a;
+          if (p.layers && t < p.T) p.layers[(((int64_t)q * p.B + b) * C + c) * p.T + t] = a;
         }
       }
     }
@@ -363,11 +385,12 @@ __global__ void __launch_bounds__(RVQ_THREADS, 1) facodec_rvq_kernel(RvqArgs<MOD
       const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
       const float v = gs[i];
       if (t < p.T) p.quantized[(((int64_t)g * p.B + b) * C + c) * p.T + t] = v;
+      if (ONE) continue;
       if (g == 0) s01[i] = v;
       else if (g == 1) s01[i] = __fadd_rn(s01[i], v);
       else if (t < p.T) p.emb[((int64_t)b * C + c) * p.T + t] = __fadd_rn(s01[i], v);
     }
-    if (g == 1 && p.nused[2] == 0) {
+    if (!ONE && g == 1 && p.nused[2] == 0) {
       for (int i = tid; i < n; i += RVQ_THREADS) {
         const int c = i / RVQ_TT, t = t0 + (i - c * RVQ_TT);
         if (t < p.T) p.emb[((int64_t)b * C + c) * p.T + t] = s01[i];
@@ -658,16 +681,17 @@ int launch_facodec_cbnorm(const float* cb, float* cbn, float* cbn2, int64_t rows
   return AB_OK;
 }
 
-int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody, float* layers) {
-  // layers: the codec's single group, which writes quantized_out through `quantized` and no emb
-  if (!p.x || (!layers && !p.emb) || !p.codes || !p.quantized || (!p.pe) != (!p.stream) || (prosody && layers))
+int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* prosody, float* layers, bool one_group) {
+  // one_group: the codec's single group, which writes quantized_out through `quantized`, no emb and no stream
+  if (!p.x || (!one_group && !p.emb) || !p.codes || !p.quantized || (!p.pe) != (!p.stream) ||
+      (one_group && (prosody || p.stream)) || (layers && !one_group))
     return fail(AB_ERR_ARG, "facodec rvq: null argument");
-  const bool groups_ok = layers ? p.ngroups == 1 && p.nused[1] == 0 && p.nused[2] == 0
-                                : p.nused[1] > 0 && p.ngroups >= 2 && p.ngroups <= 3;
+  const bool groups_ok = one_group ? p.ngroups == 1 && p.nused[1] == 0 && p.nused[2] == 0
+                                   : p.nused[1] > 0 && p.ngroups >= 2 && p.ngroups <= 3;
   if (p.B <= 0 || p.C <= 0 || p.T <= 0 || p.D <= 0 || p.D > FAC_MAX_CODEBOOK_DIM || p.nused[0] <= 0 || !groups_ok)
     return fail(AB_ERR_ARG, "facodec rvq: bad shape");
-  const size_t smem = rvq_smem_bytes(p.C);
-  if (smem > 200 * 1024) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: %d channels do not fit shared memory", p.C);
+  const size_t smem = rvq_smem_bytes(p.C, one_group);
+  if (smem > RVQ_SMEM_MAX) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: %d channels do not fit shared memory", p.C);
   const int64_t tiles = ceil_div(p.T, RVQ_TT), grid = (int64_t)p.B * tiles;
   if (grid > 0x7fffffffll) return fail(AB_ERR_UNSUPPORTED, "facodec rvq: grid too large");
   if (prosody) {
@@ -681,7 +705,7 @@ int launch_facodec_rvq(const FacRvqParams& p, cudaStream_t s, const float* proso
     AB_LAUNCH_CHECK("facodec_rvq_kernel<RVQ_PROSODY>");
     return AB_OK;
   }
-  if (layers) {
+  if (one_group) {
     static DeviceOnce configured;
     if (smem > 48 * 1024 && configured.need())
       AB_CUDA_TRY(cudaFuncSetAttribute(facodec_rvq_kernel<RVQ_LAYERS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));

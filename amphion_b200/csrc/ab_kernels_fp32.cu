@@ -86,6 +86,30 @@ __global__ void __launch_bounds__(NT) conv1d_fp32_kernel(ConvParams p) {
     __syncthreads();
   }
 
+  if constexpr (EPI == CONV_EPI_LINEAR) {
+    // y[b, t, co] = acc + bias: the thread's 4 channels of a time step are one 16-byte store when C_out % 4 == 0
+    // and y is 16-byte aligned
+    const int cb = co0 + ty * 4;
+    const bool vec = !(p.Cout & 3) && !(reinterpret_cast<uintptr_t>(p.y) & 15);
+    float bv[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) bv[c] = cb + c < p.Cout ? __ldg(p.bias + cb + c) : 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int t = t0 + tx + 16 * i;
+      if (t >= p.T) continue;
+      float* y = p.y + ((int64_t)b * p.T + t) * p.Cout + cb;
+      const float v[4] = {acc[0][i] + bv[0], acc[1][i] + bv[1], acc[2][i] + bv[2], acc[3][i] + bv[3]};
+      if (vec && cb < p.Cout) {
+        *reinterpret_cast<float4*>(y) = make_float4(v[0], v[1], v[2], v[3]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (cb + c < p.Cout) y[c] = v[c];
+      }
+    }
+    return;
+  }
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     const int co = co0 + ty * 4 + c;
@@ -357,8 +381,10 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
   if (p.reflect && halo / 2 >= p.T)
     return fail(AB_ERR_ARG, "conv1d: reflection padding %d needs more than %d samples", halo / 2, p.T);
   if (p.epi != CONV_EPI_NONE) {
-    if (p.reflect || (p.epi == CONV_EPI_GAMMA_RESIDUAL && (!p.residual || !p.gamma)) || p.epi > CONV_EPI_GAMMA_RESIDUAL)
-      return fail(AB_ERR_ARG, "conv1d: epilogue %d needs zero padding (and residual + gamma for the layer scale)", p.epi);
+    if (p.reflect || (p.epi == CONV_EPI_GAMMA_RESIDUAL && (!p.residual || !p.gamma)) || p.epi > CONV_EPI_LINEAR ||
+        (p.epi == CONV_EPI_LINEAR && (p.k != 1 || !p.bias)))
+      return fail(AB_ERR_ARG, "conv1d: epilogue %d needs zero padding (residual + gamma for the layer scale; k = 1 and "
+                              "a bias for the Linear)", p.epi);
   } else if (p.Cout == 1 && p.k == 7 && p.d == 1 && !p.residual && !p.acc_prev && p.out_div == 1.0f) {
     dim3 grid((unsigned)ceil_div(p.T, PT), 1, (unsigned)p.B);
     const bool vec = p.xst == 1 && (p.T & 3) == 0 && (p.xsc & 3) == 0 && (p.xsb & 3) == 0 &&
@@ -388,9 +414,10 @@ int launch_conv1d_fp32(const ConvParams& p, cudaStream_t s) {
   const size_t smem = sizeof(float) * ((size_t)CI_T * (TT + halo) + (size_t)CI_T * p.k * CO_T);
   if (smem > 200 * 1024)
     return fail(AB_ERR_UNSUPPORTED, "conv1d: k=%d dilation=%d needs %zu B of shared memory", p.k, p.d, smem);
-  static DeviceOnce configured[4];
+  static DeviceOnce configured[5];
   auto kern = p.epi == CONV_EPI_GELU ? conv1d_fp32_kernel<0, CONV_EPI_GELU>
               : p.epi == CONV_EPI_GAMMA_RESIDUAL ? conv1d_fp32_kernel<0, CONV_EPI_GAMMA_RESIDUAL>
+              : p.epi == CONV_EPI_LINEAR ? conv1d_fp32_kernel<0, CONV_EPI_LINEAR>
               : p.reflect ? conv1d_fp32_kernel<1> : conv1d_fp32_kernel<0>;
   if (smem > 48 * 1024 && configured[p.epi ? 1 + p.epi : (p.reflect ? 1 : 0)].need()) {
     AB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));

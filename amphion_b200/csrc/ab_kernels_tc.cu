@@ -1122,8 +1122,14 @@ __device__ __forceinline__ void epilogue_convt(const HcArgs& p, const HcGeom& g,
 //   PW_GAMMA:    y = y + gamma * (acc + b), fp32 in place            (pwconv2, layer scale and residual, vocos.py:509-527)
 //   PW_SPECTRUM: columns 2j, 2j + 1 hold bin j's log-magnitude and phase (launch_tc_pack_head_weight):
 //                spec[b T + t][j] = min(exp(m), 1e2) (cos p, sin p)  (ISTFTHead, vocos.py:343-361)
+//   PW_LINEAR:   y[b, t, co] = acc + b, fp32 time-major [B, T, C_out]  (nn.Linear after a VocosBackbone, RepCodec's
+//                encoder and decoder): a thread's two adjacent columns are one 8-byte store, so a quad of threads
+//                writes 32 contiguous bytes of a row; an odd C_out (or a y that is not 8-byte aligned) takes scalar
+//                stores
 // ITEM_CONVT selects hitem_kernel's ConvTranspose epilogue, epilogue_convt.
-enum ItemEpi : int { PW_GELU = AB_PW_GELU, PW_GAMMA = AB_PW_GAMMA_RESIDUAL, PW_SPECTRUM = AB_PW_SPECTRUM, ITEM_CONVT };
+enum ItemEpi : int {
+  PW_GELU = AB_PW_GELU, PW_GAMMA = AB_PW_GAMMA_RESIDUAL, PW_SPECTRUM = AB_PW_SPECTRUM, PW_LINEAR = AB_PW_LINEAR, ITEM_CONVT
+};
 struct PwArgs {
   const float* gamma;   // PW_GAMMA: [C_out]
   float2* spec;         // PW_SPECTRUM: [B*T][C_out / 2]
@@ -1159,6 +1165,16 @@ __device__ __forceinline__ void epilogue_pw(const HcArgs& p, const HcGeom& g, co
             const float v = (q ? a1 : a0) + bias_s[co + q];
             float* y = p.y + ((int64_t)b * p.Cout + co + q) * g.Tout + t;
             *y = __fadd_rn(*y, __fmul_rn(__ldg(e.gamma + co + q), v));
+          }
+        } else if constexpr (EPI == PW_LINEAR) {
+          if (co >= p.Cout) continue;
+          float* y = p.y + ((int64_t)b * g.Tout + t) * p.Cout + co;
+          const float v0 = a0 + bias_s[co], v1 = a1 + bias_s[co + 1];   // bias_s is zero beyond C_out
+          if (!(p.Cout & 1) && !(reinterpret_cast<uintptr_t>(p.y) & 7)) {
+            *reinterpret_cast<float2*>(y) = make_float2(v0, v1);
+          } else {
+            y[0] = v0;
+            if (co + 1 < p.Cout) y[1] = v1;
           }
         } else {
           static_assert(EPI == PW_SPECTRUM, "pointwise epilogue");
@@ -1699,7 +1715,7 @@ int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s) {
   if (p.B <= 0 || p.T <= 0 || p.Cin <= 0 || p.Cout <= 0) return fail(AB_ERR_ARG, "tc pointwise: bad shape");
   if (p.precision != AB_PREC_TC_F16 && p.precision != AB_PREC_TC_BF16) return fail(AB_ERR_ARG, "tc pointwise: bad precision");
   if ((p.epilogue == AB_PW_GELU && !p.yimg) || (p.epilogue == AB_PW_GAMMA_RESIDUAL && (!p.y || !p.gamma)) ||
-      (p.epilogue == AB_PW_SPECTRUM && (!p.spec || (p.Cout & 1))))
+      (p.epilogue == AB_PW_SPECTRUM && (!p.spec || (p.Cout & 1))) || (p.epilogue == AB_PW_LINEAR && !p.y))
     return fail(AB_ERR_ARG, "tc pointwise: epilogue %d: missing output or odd C_out", p.epilogue);
   HcGeom g;
   int rc = make_geom(0, p.Cin, p.Cout, 1, 1, p.T, true, g);   // k = 1 conv tiles
@@ -1720,6 +1736,7 @@ int launch_tc_pointwise(const TcPwParams& p, cudaStream_t s) {
     case AB_PW_GELU: return run(IntC<PW_GELU>());
     case AB_PW_GAMMA_RESIDUAL: return run(IntC<PW_GAMMA>());
     case AB_PW_SPECTRUM: return run(IntC<PW_SPECTRUM>());
+    case AB_PW_LINEAR: return run(IntC<PW_LINEAR>());
   }
   return fail(AB_ERR_ARG, "tc pointwise: unknown epilogue %d", p.epilogue);
 }

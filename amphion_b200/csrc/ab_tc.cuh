@@ -83,7 +83,8 @@ int launch_tc_chain(const TcChainParams& p, cudaStream_t s);
 //   AB_PW_GAMMA_RESIDUAL:  y = y + gamma * (W x + b), fp32 [B, C_out, T]    (pwconv2, layer scale, residual)
 //   AB_PW_SPECTRUM:        spec [B*T][C_out/2] complex = min(exp(m), 1e2) (cos p + i sin p), m / p the two halves of
 //                          W x + b (ISTFTHead); w from launch_tc_pack_head_weight
-enum { AB_PW_GELU = 0, AB_PW_GAMMA_RESIDUAL = 1, AB_PW_SPECTRUM = 2 };
+//   AB_PW_LINEAR:          y = W x + b, fp32 time-major [B, T, C_out]       (nn.Linear's output layout)
+enum { AB_PW_GELU = 0, AB_PW_GAMMA_RESIDUAL = 1, AB_PW_SPECTRUM = 2, AB_PW_LINEAR = 3 };
 struct TcPwParams {
   int epilogue = AB_PW_GELU;
   const uint16_t* ximg = nullptr;   // [B][ceil16(Cin)/8][T][8], padding channels zero
@@ -91,7 +92,7 @@ struct TcPwParams {
   const float* bias = nullptr;      // [Cout]
   const float* gamma = nullptr;     // AB_PW_GAMMA_RESIDUAL
   uint16_t* yimg = nullptr;         // AB_PW_GELU: [B][ceil16(Cout)/8][T][8] (padding channels written as zero)
-  float* y = nullptr;               // AB_PW_GAMMA_RESIDUAL
+  float* y = nullptr;               // AB_PW_GAMMA_RESIDUAL [B, C_out, T]; AB_PW_LINEAR [B, T, C_out]
   float* spec = nullptr;            // AB_PW_SPECTRUM: interleaved (re, im)
   int B = 0, Cin = 0, Cout = 0, T = 0;
   int precision = AB_PREC_TC_F16;

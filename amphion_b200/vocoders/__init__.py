@@ -10,6 +10,7 @@ from .nsfhifigan import NSFHiFiGAN
 from .vocos import Vocos
 from .facodec import FACodecDecoder, FACodecDecoderV2, FACodecEncoder, FACodecEncoderV2, FACodecRedecoder
 from .amphion_codec import CodecDecoder, CodecEncoder
+from .repcodec import RepCodec
 from .gan_vocoder_inference import synthesis_audios, synthesize_to_files
 from .gan_vocoder_inference import vocoder_inference as _gan_vocoder_inference
 
@@ -21,9 +22,9 @@ _vocoders["diffwave"] = DiffWave
 _vocoder_forward_funcs["diffwave"] = diffusion_vocoder_inference.vocoder_inference
 _vocoder_infer_funcs["diffwave"] = diffusion_vocoder_inference.synthesis_audios
 
-# Vocos, the FACodec classes and the codec's CodecEncoder / CodecDecoder are not in the registry: the reference has no entry for them, and their constructors take
+# Vocos, the FACodec classes, the codec's CodecEncoder / CodecDecoder and RepCodec are not in the registry: the reference has no entry for them, and their constructors take
 # keyword arguments, not cfg
-__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "DiffWave", "NSFHiFiGAN", "MelGAN", "APNet", "Vocos", "FACodecDecoder", "FACodecEncoder", "FACodecRedecoder", "FACodecEncoderV2", "FACodecDecoderV2", "CodecEncoder", "CodecDecoder", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
+__all__ = ["HiFiGAN", "HiFiGAN_vits", "BigVGAN", "DiffWave", "NSFHiFiGAN", "MelGAN", "APNet", "Vocos", "FACodecDecoder", "FACodecEncoder", "FACodecRedecoder", "FACodecEncoderV2", "FACodecDecoderV2", "CodecEncoder", "CodecDecoder", "RepCodec", "ISTFT", "ISTFTHead", "synthesis_audios", "synthesize_to_files", "_vocoders",
            "_vocoder_forward_funcs", "_vocoder_infer_funcs"]
 
 # `amphion_b200.vocoders.vocoder_inference` is the MODULE (synthesis, load_nnvocoder), as

@@ -219,6 +219,12 @@ class ResidualVQ(NativeGenerator):
         history; the losses are the zeros the reference returns in eval."""
         _refuse_training(self, "the ResidualVQ", "quantizer dropout, commitment losses", _SERVED)
         n = self._n(n_quantizers, "ResidualVQ.forward")
+        out, codes, layers = self._quantize(z, n, True)
+        zeros = torch.zeros(n, dtype=torch.float32, device=out.device)
+        return out, codes, zeros, zeros.clone(), layers
+
+    def _quantize(self, z, n, with_layers):
+        """quantized_out, codes and, with ``with_layers``, all_quantized (else None: nothing is written for it)."""
         if not isinstance(z, torch.Tensor) or z.dim() != 3 or z.shape[1] != self.input_dim:
             got = tuple(z.shape) if isinstance(z, torch.Tensor) else type(z).__name__
             raise ValueError(f"ResidualVQ expects z of shape [B, {self.input_dim}, T], got {got}")
@@ -231,12 +237,11 @@ class ResidualVQ(NativeGenerator):
         with self._launch(dev) as h:
             out = torch.empty(B, D, T, dtype=torch.float32, device=dev)
             codes = torch.empty(n, B, T, dtype=torch.int64, device=dev)
-            layers = torch.empty(n, B, D, T, dtype=torch.float32, device=dev)
+            layers = torch.empty(n, B, D, T, dtype=torch.float32, device=dev) if with_layers else None
             _capi.check(_capi.lib.ab_rvq_quantize(h, _capi.ptr(z), _capi.shape_array(z.stride()), B, T, n, _capi.ptr(out),
                                                   _capi.ptr(codes), _capi.ptr(layers), _capi.stream_ptr()),
                         "ab_rvq_quantize")
-        zeros = torch.zeros(n, dtype=torch.float32, device=dev)
-        return out, codes, zeros, zeros.clone(), layers
+        return out, codes, layers
 
     def vq2emb(self, vq, n_quantizers=None):
         """codes [>= n, B, T] (integer, any strides) -> [B, input_dim, T] fp32 on the codes' device."""

@@ -69,6 +69,16 @@ extern "C" {
  * reference's state-dict names ("backbone.embed.weight", "backbone.convnext.3.pwconv1.weight" [out, in], ".gamma",
  * "backbone.final_layer_norm.bias", "head.out.weight", "head.istft.window", ...).  Output: wav [B, 1, T * istft_hop];
  * with tail events the iSTFT runs in the batch chunks.
+ * AB_GEN_VOCOS_LINEAR: nn.Sequential(VocosBackbone, nn.Linear(dim, out)), RepCodec's encoder and decoder
+ * (models/codec/kmeans/repcodec_model.py:108-127, vocos.py:719-783): AB_GEN_VOCOS's backbone, then y = Linear(x)
+ * (fp32 accumulation, then the bias) in place of the ISTFTHead.  Config fields: n_mel = input_channels,
+ * upsample_initial_channel = dim, ffn_channels = intermediate_dim, num_layers, trunk_out_channels = out_features;
+ * every other field 0.  Tensors keep the Sequential's names: "0.embed.weight", "0.norm.*", "0.convnext.{i}.{dwconv,
+ * norm,pwconv1,pwconv2}.*", "0.convnext.{i}.gamma", "0.final_layer_norm.*", "1.weight" [out, dim], "1.bias".  Input
+ * [B, input_channels, T] with any strides (ab_generator_forward); output y [B, T, out] fp32 contiguous, the layout
+ * nn.Linear returns.  The embed conv runs on the tensor cores iff input_channels <= 512 (AB_GEN_VOCOS's routing), the
+ * Linear on the pointwise GEMM's AB_VOCOS_PW_LINEAR epilogue at 16 bits; with tail events the Linear runs in the batch
+ * chunks.
  * AB_GEN_DIFFWAVE: DiffWave.forward (models/vocoders/diffusion/diffwave/diffwave.py:130-183): x = relu(input_projection(
  * audio)); per residual layer i (dilation 2^(i % dilation_cycle)): y = dilated_conv(x + diffusion_projection(emb)) +
  * conditioner_projection(up(mel)), z = sigmoid(y[:C]) tanh(y[C:]), (r, s) = output_projection(z), x = (x + r) / sqrt(2),
@@ -115,7 +125,8 @@ extern "C" {
  * AB_GEN_RVQ: the codec's ResidualVQ of FactorizedVectorQuantize layers (models/codec/amphion_codec/quantize/residual_vq.py,
  * factorized_vector_quantize.py, quantizer_type "fvq", use_l2_normlize = True), alone.  Config fields: n_mel = input_dim,
  * vq_num_q[0] = num_quantizers (1..AB_FACODEC_MAX_Q), vq_codebook_size (any size >= 1), vq_codebook_dim (1..16, !=
- * input_dim); every other field 0.  Tensors keep the reference's names: "quantizers.{i}.in_project.weight" [codebook_dim,
+ * input_dim); every other field 0.  input_dim above AB_RVQ_MAX_INPUT_DIM (1447) fails with AB_ERR_UNSUPPORTED at
+ * ab_generator_create.  Tensors keep the reference's names: "quantizers.{i}.in_project.weight" [codebook_dim,
  * input_dim, 1] (weight norm over every dim but 0) / ".bias", "quantizers.{i}.out_project.weight" [input_dim, codebook_dim,
  * 1] / ".bias", "quantizers.{i}.codebook.weight" [codebook_size, codebook_dim].  Runs through ab_rvq_*.
  * AB_GEN_FACODEC_REDECODER: NaturalSpeech 3's FACodecRedecoder (models/codec/ns3_codec/facodec.py:602-769), the README's
@@ -131,9 +142,11 @@ extern "C" {
  * The reference's forward (:691-732) transposes the [B, T, d] sum before timbre_norm and is not served. */
 enum ab_generator_kind {
   AB_GEN_HIFIGAN = 0, AB_GEN_BIGVGAN = 1, AB_GEN_NSFHIFIGAN = 2, AB_GEN_TRUNK = 3, AB_GEN_MELGAN = 4, AB_GEN_VOCOS = 5,
-  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8, AB_GEN_FACODEC_REDECODER = 9, AB_GEN_RVQ = 10
+  AB_GEN_DIFFWAVE = 6, AB_GEN_FACODEC = 7, AB_GEN_FACODEC_ENCODER = 8, AB_GEN_FACODEC_REDECODER = 9, AB_GEN_RVQ = 10,
+  AB_GEN_VOCOS_LINEAR = 11
 };
 #define AB_FACODEC_MAX_Q 32   /* most codebook layers over the three ResidualVQs */
+#define AB_RVQ_MAX_INPUT_DIM 1447   /* widest AB_GEN_RVQ input_dim (the quantize kernel's two shared-memory planes) */
 enum ab_activation { AB_ACT_LRELU = 0, AB_ACT_SNAKE = 1, AB_ACT_SNAKEBETA = 2, AB_ACT_SNAKE1D = 3 };
 /* arithmetic of the k-tap channel-mixing convolutions */
 enum ab_precision {
@@ -403,7 +416,8 @@ int ab_facodec_redecoder_vq2emb(ab_generator* g, const int64_t* dev_codes, const
  * quantized_out = ((0 + q_0) + q_1) + ..., the reference's order.  No workspace.
  * ---------------------------------------------------------------------- */
 /* x [B, input_dim, T] fp32 with any element strides -> quantized_out [B, input_dim, T], codes_out int64 [n, B, T] and
- * layers_out [n, B, input_dim, T] (each layer's q, the reference's all_quantized), all contiguous.  One launch. */
+ * layers_out [n, B, input_dim, T] (each layer's q, the reference's all_quantized), all contiguous.  layers_out may be
+ * NULL: nothing is written in its place.  One launch. */
 int ab_rvq_quantize(ab_generator* g, const float* dev_x, const int64_t x_strides[3], int64_t batch, int64_t frames,
                     int32_t n_quantizers, float* dev_quantized_out, int64_t* dev_codes_out, float* dev_layers_out,
                     void* stream);
@@ -534,6 +548,9 @@ int ab_facodec_prosody_input_forward(const float* dev_x, const int64_t x_strides
  *     AB_VOCOS_PW_GAMMA:    y = y + gamma * (W x + b) in place, fp32 [B, C_out, T] (tc: from ximg; fp32: from x)
  *     AB_VOCOS_PW_SPECTRUM: spec [B*T][C_out/2] complex (interleaved re, im) = min(exp(m), 1e2) (cos p + i sin p), m and
  *                           p the first and second halves of W x + b (Vocos' ISTFTHead; even C_out)
+ *     AB_VOCOS_PW_LINEAR:   y = W x + b written time-major, fp32 [B, T, C_out] (nn.Linear's layout; tc: from ximg;
+ *                           fp32: from x, acc = fma(w[co][ci], x[ci], acc) for ci ascending from 0, then + b[co]);
+ *                           gamma, yimg and spec must be NULL
  *   At AB_PREC_TC_F16 / TC_BF16 the input is the operand image ximg [B][ceil16(C_in)/8][T][8] and one pointwise wgmma
  *   GEMM launch runs; at AB_PREC_FP32 the input is x and the CUDA-core conv kernel runs with k = 1 (SPECTRUM: into the
  *   workspace, then ab_spectral_head_forward per utterance).  The other input and the outputs an epilogue does not
@@ -542,6 +559,7 @@ int ab_facodec_prosody_input_forward(const float* dev_x, const int64_t x_strides
 #define AB_VOCOS_PW_GELU 0
 #define AB_VOCOS_PW_GAMMA 1
 #define AB_VOCOS_PW_SPECTRUM 2
+#define AB_VOCOS_PW_LINEAR 3
 int ab_vocos_norm_forward(const float* dev_x, const float* dev_dw_w, const float* dev_dw_b, const float* dev_ln_w,
                           const float* dev_ln_b, float eps, float* dev_y, uint16_t* dev_yimg, int32_t precision,
                           int64_t batch, int64_t channels, int64_t length, void* stream);
